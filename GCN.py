@@ -1,7 +1,7 @@
 """Drop-in replacement for the reference's top-level ``GCN`` module (import name fixed by ``Main.py:5``).
 
 Exports ``GCN`` (reference ``GCN.py:7-46``) and ``Adj_Preprocessor`` (reference ``GCN.py:50-135``) with the
-reference's signatures; the arithmetic runs in ``libstmgcn_b200.so`` (hand-written sm_100a CUDA, C ABI in
+reference's signatures; the arithmetic runs in ``libstmgcn_b200.so`` (hand-written sm_90a CUDA, C ABI in
 ``include/stmgcn_b200.h``).  Implementation: ``st-mgcn_b200/stmgcn_b200/{modules,preprocess}.py``.
 """
 import os as _os

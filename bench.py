@@ -1,19 +1,21 @@
 #!/usr/bin/env python
 """bench.py -- region-timesteps/s of the ST-MGCN hot path (fwd + MSE + bwd [+ gradient all-reduce]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl ours|reference] [--dump-outputs DIR]
 
 Contract (driver): prints ONE JSON line on rank 0.  ``value`` = whole-job region-timesteps/s with the inputs
 resident in HBM; ``e2e`` = the same metric through the public module API with HOST (pinned) inputs, the
 host->device copies and a device->host read of the loss inside the timed region; ``roofline`` = the
 Chebyshev SpMM (the forward's 18 recurrence launches at cfg3) timed alone with CUDA events against the
-measured HBM peak; ``cpu_baseline`` = the UNMODIFIED reference modules (``baseline/_ref``, staged by build(); the
-oracle port if absent) on this box's host cores on a bounded sample.  ``--impl reference`` times only that CPU path.
+measured HBM peak; ``cpu_baseline`` = the UNMODIFIED reference modules (``oracle/_ref``, byte-compiled by build(); the
+oracle port if absent) on the host cores, on a bounded sample.  ``--impl reference`` times only that CPU path.
 
 Default workload: cfg3 = BASELINE.json configs[2] (4096 regions, 3 graphs, K=3, seq_len=12, batch 64 per
 GPU, fp32) -- the configuration BASELINE.json's metric quotes the SpMM HBM figure on, and the largest fp32
 single-GPU configuration; with N GPUs the per-GPU batch stays 64 (weak scaling; N=8 is cfg4's 512 windows).
-A step's working set (tens of GB of LSTM tape) is far larger than the 126 MB L2, so no explicit L2 flush.
+A step's working set (GBs of LSTM tape) is far larger than the H100's 50 MB L2, so no explicit L2 flush.
+``--dump-outputs DIR`` writes what the last timed step computed -- the prediction, the loss and every parameter gradient,
+as float32 ``DIR/<name>.npy`` -- so that two builds can be compared output for output on identical seeded inputs.
 """
 from __future__ import annotations
 
@@ -50,6 +52,9 @@ def parse_args():
     ap.add_argument("--cuda-graph", action="store_true",
                     help="replay the step from a captured CUDA graph (stmgcn_b200.graphs.GraphedStep); measured gain "
                          "at cfg3 is ~1 %% -- the step is GPU-bound, not launch-bound -- so eager is the default")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last timed step's prediction, loss and parameter gradients "
+                         "(rank 0) as float32 DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -61,11 +66,12 @@ def peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return json.load(fh), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "sm_max_mhz": 1965.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16, 1980 MHz boost clock
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "sm_max_mhz": 1980.0}, "datasheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries, 100 ms apart)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -120,6 +126,36 @@ class ClockSampler:
         return out
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, out, loss, model, limit=DUMP_LIMIT_BYTES, seed=0):
+    """What the last timed step computed, as a caller of the step receives it: prediction (B, N, C), scalar loss and the
+    gradient of every parameter (float32 .npy).  Above ``limit`` bytes in all, the prediction is replaced by a fixed,
+    seeded sample of its flat elements (``out_sample.npy``; their flat indices, exact in float64, in
+    ``out_sample_index.npy``)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss.detach().reshape(())}
+    for name, prm in model.named_parameters():
+        if prm.grad is not None:
+            arrays["grad." + name] = prm.grad.detach()
+    rest = sum(t.numel() for t in arrays.values()) * 4
+    flat = out.detach().reshape(-1)
+    if rest + flat.numel() * 4 <= limit:
+        arrays["out"] = out.detach()
+    else:
+        # 4 B value + 8 B index per sampled element; 64 KB kept free for the .npy headers
+        n_keep = max(1, min(flat.numel(), (limit - rest - (64 << 10)) // 12))
+        gen = torch.Generator().manual_seed(seed)
+        idx = torch.randperm(flat.numel(), generator=gen)[:n_keep].sort().values
+        arrays["out_sample"] = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, "out_sample_index.npy"), idx.numpy().astype(np.float64))
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.float().cpu().numpy())
+
+
 def spmm_algorithmic_bytes(n, nnz, f_total, k_order, elem=4):
     """SURVEY.md section 8(d): per GCN call K*CSR + N*F*e*(3K-1)."""
     csr = nnz * 8 + (n + 1) * 4
@@ -129,19 +165,22 @@ def spmm_algorithmic_bytes(n, nnz, f_total, k_order, elem=4):
 # ---------------------------------------------------------------------------------------------------
 # reference arm: the oracle port (dense supports + nn.LSTM, the reference's algorithm) on host cores
 # ---------------------------------------------------------------------------------------------------
-REF_DIR = os.path.join(REPO, "baseline", "_ref")
+REF_DIR = os.path.join(REPO, "oracle", "_ref")
 
 
 def _reference_modules():
-    """The UNMODIFIED reference's ``GCN`` / ``STMGCN`` modules from ``baseline/_ref`` (staged by
-    ``__graft_entry__.build()``), imported under private names so they can never shadow the repo's drop-in modules.
-    Returns None when the directory was not staged (then the oracle port is timed instead)."""
-    if not os.path.exists(os.path.join(REF_DIR, "STMGCN.py")):
+    """The UNMODIFIED reference's ``GCN`` / ``STMGCN`` modules, byte-compiled into ``oracle/_ref`` by
+    ``__graft_entry__.build()`` (``oracle/stage_reference.py``), imported under private names so they can never shadow
+    the repo's drop-in modules.  Returns None when the directory was not built (then the oracle port is timed instead)."""
+    if not all(os.path.exists(os.path.join(REF_DIR, n + ".pyc")) for n in ("GCN", "STMGCN")):
         return None
+    import importlib.machinery
     import importlib.util
 
     def load(name):
-        spec = importlib.util.spec_from_file_location(f"_stmgcn_ref_{name}", os.path.join(REF_DIR, name + ".py"))
+        path = os.path.join(REF_DIR, name + ".pyc")
+        loader = importlib.machinery.SourcelessFileLoader(f"_stmgcn_ref_{name}", path)
+        spec = importlib.util.spec_from_file_location(f"_stmgcn_ref_{name}", path, loader=loader)
         mod = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(mod)
         return mod
@@ -162,17 +201,15 @@ def _reference_modules():
 def cpu_reference_run(w, steps, warmup, sample_batch=None, log=None, step_budget_s=6.0):
     """Time the reference's CPU implementation of the path on the host cores.
 
-    kind "reference": the unmodified reference modules from ``baseline/_ref`` -- ``Adj_Preprocessor.process`` (dense
+    kind "reference": the unmodified reference modules from ``oracle/_ref`` -- ``Adj_Preprocessor.process`` (dense
     supports, GCN.py:57-97), ``ST_MGCN.forward`` (STMGCN.py:100-119), ``nn.MSELoss``, ``backward`` -- exactly the step of
     ``Model_Trainer.py:35-41`` without the optimizer.  kind "port": the oracle's dense restatement (same algorithm, same
-    torch ops) when ``baseline/_ref`` is absent.
+    torch ops) when ``oracle/_ref`` was not built.
 
-    Thread count: "all the host threads it can use" is calibrated, not assumed -- on the GPU boxes os.cpu_count()
-    reports 128 logical CPUs but running 128 intra-op threads is ~50x SLOWER than 16-32 (measured: 64 s vs 1.1 s for a
-    2-window step), so candidates are tried smallest-first on a 1-window step and the fastest is used; `cores` in the
-    result is the number of threads actually used.  The sample batch is then sized to ~step_budget_s per step."""
+    Thread count: "all the host threads it can use" is calibrated, not assumed -- on large hosts running one intra-op
+    thread per logical CPU can be far slower than 16-32 threads, so candidates are tried smallest-first on a 1-window
+    step and the fastest is used; `cores` in the result is the number of threads actually used.  The sample batch is then sized to ~step_budget_s per step."""
     import torch
-    from torch import nn
     from stmgcn_b200 import synth
     ncpu = os.cpu_count() or 1
     torch.set_num_threads(min(ncpu, 16))
@@ -185,6 +222,7 @@ def cpu_reference_run(w, steps, warmup, sample_batch=None, log=None, step_budget
         pre = ref_gcn.Adj_Preprocessor("chebyshev", w.cheb_order)
         import contextlib
         import io
+        from torch import nn
         with contextlib.redirect_stdout(io.StringIO()):        # GCN.py:119-121 prints its lambda_max fallback notice
             sups = [pre.process(a) for a in adjs]              # GCN.py:57-97 (dense polynomials, once)
         torch.manual_seed(0)
@@ -241,9 +279,9 @@ def cpu_reference_run(w, steps, warmup, sample_batch=None, log=None, step_budget
         model_name = [l.split(":")[1].strip() for l in open("/proc/cpuinfo") if l.startswith("model name")][0]
     except Exception:
         model_name = "unknown"
-    what = ("the UNMODIFIED reference modules (baseline/_ref: Adj_Preprocessor.process dense supports, ST_MGCN.forward, "
+    what = ("the UNMODIFIED reference modules (oracle/_ref: Adj_Preprocessor.process dense supports, ST_MGCN.forward, "
             "MSELoss, backward)" if kind == "reference" else
-            "the oracle port (dense supports + nn.LSTM, as the reference executes; baseline/_ref not staged)")
+            "the oracle port (dense supports + nn.LSTM, as the reference executes; oracle/_ref not built)")
     return dict(value=value, unit=UNIT, cores=best_c, kind=kind,
                 sample=f"{w.name} shapes with batch {sample_batch} (of {w.batch}), {steps} timed step(s) after "
                        f"{warmup} warm-up, fwd+MSE+bwd through {what}, "
@@ -270,7 +308,7 @@ def workload_config(w, world, per_gpu_batch, arith="fp32"):
                         f"seq_len={w.seq_len}, batch={per_gpu_batch}/GPU x {world} GPU(s), {arith}, H={w.lstm_hidden} "
                         f"L={w.lstm_layers} G={w.gcn_hidden} C={w.input_dim}, graph density {w.density}",
             "global_batch": per_gpu_batch * world, "parallelism": f"dp{world}",
-            "l2": "per-step working set (GBs of activations) exceeds the 126 MB L2; no explicit flush",
+            "l2": "per-step working set (GBs of activations) exceeds the 50 MB L2; no explicit flush",
             "step": "forward + MSELoss + backward (+ one gradient all-reduce when world > 1); optimizer excluded",
             "cuda_graph": None}
 
@@ -309,6 +347,7 @@ def run_ours(args, w):
 
     use_graph = args.cuda_graph
     launches_per_step = None
+    last_out = [None]                      # the prediction of the most recent step (for --dump-outputs)
     if use_graph:
         # one eager step to count this library's launches, then capture fwd + loss + bwd (+ all-reduce) once
         l0 = _lib.launch_count()
@@ -321,6 +360,7 @@ def run_ours(args, w):
         def step(x, y):
             loss = gstep(x, y)
             bucket.all_reduce_mean_()          # the one collective of the step stays outside the graph (NCCL, eager)
+            last_out[0] = gstep.out
             return loss
     else:
         def step(x, y):
@@ -329,6 +369,7 @@ def run_ours(args, w):
             loss = crit(out, y)
             loss.backward()
             bucket.all_reduce_mean_()
+            last_out[0] = out
             return loss
 
     ms_step_local = [0.0]                  # this rank's own device time per step of the last timed() call
@@ -359,7 +400,14 @@ def run_ours(args, w):
     if sampler:
         sampler.start()
     l0 = _lib.launch_count()
-    ms_total = timed(lambda: step(x_d, y_d), args.steps)
+    last_loss = [None]
+
+    def timed_step():
+        last_loss[0] = step(x_d, y_d)
+
+    ms_total = timed(timed_step, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out[0], last_loss[0], model)
     launches = (_lib.launch_count() - l0) // args.steps if launches_per_step is None else launches_per_step
     clocks = sampler.stop() if sampler else None
     ms_step = ms_total / args.steps
@@ -473,28 +521,9 @@ def run_ours(args, w):
             achieved = (sum(alg_dom) * (k_ord - 1)) / (ms_dom * 1e-3) / 1e9
         else:
             us_launch, achieved = ms_spmm * 1e3 / max(n_launch, 1), alg / (ms_spmm * 1e-3) / 1e9
-        # DRAM bytes per launch of this launch type: read from the committed summary of this round's `ncu --set full`
-        # capture of exactly this launch (tools/ncu_spmm.sh -> tools/ncu_summary.py -> profiles/r2_spmm_ncu.json); only
-        # valid for the shape it was captured on (cfg3, batch 64)
-        traffic, traffic_src = None, None
-        tpath = os.path.join(REPO, "profiles", "r2_spmm_ncu.json")
-        if w.name == "cfg3" and b == 64 and os.path.exists(tpath):
-            with open(tpath) as fh:
-                tj = json.load(fh)
-            try:
-                mb = float(tj["dram__bytes_read.sum"]) + float(tj["dram__bytes_write.sum"])
-                traffic = mb * 1e6
-                traffic_src = ("profiles/r2_spmm_ncu.json: dram__bytes_read.sum + dram__bytes_write.sum of one launch "
-                               f"({tj['dram__bytes_read.sum']} + {tj['dram__bytes_write.sum']} MB), ncu --set full")
-            except (KeyError, ValueError):
-                pass
         roofline = {"bound": "hbm", "kernel": "spmm_row_gather_kernel<4> (Chebyshev recurrence step, spatial, k>=2)",
-                    "achieved": achieved, "peak": pk["hbm_gbs"], "peak_kind": f"{pk_kind} (MEASURED_PEAKS.json hbm_gbs)",
-                    "unit": "GB/s", "frac": achieved / pk["hbm_gbs"], "traffic": traffic, "traffic_source": traffic_src,
-                    "gather_ceiling": {"measured_gather_GBps": 17900, "source": "profiles/r2_gather_probe.log (tools/gather_probe.cu: "
-                                       "512-byte row-segment gathers through L2/L1, same N / F / degree)",
-                                       "note": "the launch gathers nnz*F*4 B = 2.87 GB against 0.2 GB of algorithmic HBM bytes; "
-                                               "at the measured gather rate that alone is 160 us"},
+                    "achieved": achieved, "peak": pk["hbm_gbs"], "peak_kind": f"{pk_kind} hbm_gbs",
+                    "unit": "GB/s", "frac": achieved / pk["hbm_gbs"],
                     "algorithmic_bytes_per_launch": sum(alg_dom) / len(alg_dom), "avg_us_per_launch": us_launch,
                     "launches_timed": n_dom,
                     "forward_all": {"algorithmic_bytes": alg, "launches": n_launch, "ms": ms_spmm,

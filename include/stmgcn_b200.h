@@ -1,5 +1,5 @@
 /*
- * stmgcn_b200.h -- C ABI of libstmgcn_b200.so: the B200 (sm_100a) ST-MGCN hot path.
+ * stmgcn_b200.h -- C ABI of libstmgcn_b200.so: the H100 (sm_90a) ST-MGCN hot path.
  *
  * The reference (underdoc-wang/ST-MGCN) has NO plugin / FFI / operator interface: its boundary is the
  * Python nn.Module surface (GCN.py:7-46, STMGCN.py:7-119).  This header is therefore the boundary a
@@ -98,9 +98,9 @@ int32_t stmgcn_obs_to_node_major(const float* obs, float* xo, float* xt, int64_t
 int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t rows, int32_t p,
                         const float* w, const float* bias, int32_t q, int32_t act, float* out,
                         float* pool, int64_t b_inner, const float* wimg, void* stream);
-/* Tensor-core operand images of W (ks*64, 64) for p = q = 64, ks <= 8 (3xTF32: every fp32 operand split into tf32 hi + lo, three tcgen05 passes):
+/* Tensor-core operand images of W (ks*64, 64) for p = q = 64, ks <= 8 (3xTF32: every fp32 operand split into tf32 hi + lo, three wgmma passes):
  * img_fwd: ks*64*64*2 floats; img_bwd (may be NULL): one 2*2*256*32-float image per group of 4 supports (two images
- * when ks > 4), ZERO-FILLED by the caller (rows beyond ks*64 stay zero).  Passing wimg / wimg_t != NULL to stmgcn_proj_fwd / _bwd selects the tcgen05 kernels when
+ * when ks > 4), ZERO-FILLED by the caller (rows beyond ks*64 stay zero).  Passing wimg / wimg_t != NULL to stmgcn_proj_fwd / _bwd selects the wgmma kernels when
  * p = q = 64 (and, for the backward, a full d_out and u are given); otherwise the exact-FFMA kernels run. */
 int32_t stmgcn_proj_pack_tc(const float* w, int32_t ks, float* img_fwd, float* img_bwd, void* stream);
 /* backward of the projection.  dZ = dOut (.) [out > 0] (act = RELU) with dOut either a full (rows, q)

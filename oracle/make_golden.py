@@ -1,8 +1,9 @@
-"""Generate ``tests/golden/*.npz`` by running the UNMODIFIED reference (``/root/reference``) on CPU fp32.
+"""Generate ``tests/golden/*.npz`` by running the UNMODIFIED reference ST-MGCN checkout on CPU fp32.
 
-TEST INFRASTRUCTURE.  Run in the build container only (the reference does not travel to the GPU box):
+TEST INFRASTRUCTURE.  Needs a checkout of the reference (its ``GCN.py`` / ``STMGCN.py``); the fixtures it writes are
+committed, so the tests never need the reference itself:
 
-    python oracle/make_golden.py
+    python oracle/make_golden.py /path/to/reference
 
 Each fixture stores: the adjacency matrices, the reference's supports ``Adj_Preprocessor.process``
 (``GCN.py:57-97``), the reference model's ``state_dict`` after ``torch.manual_seed(seed)`` construction,
@@ -21,7 +22,7 @@ from torch import nn
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
-REF = "/root/reference"
+REF = os.environ.get("STMGCN_REFERENCE_DIR", "")     # set from the command line, see __main__
 
 
 def import_reference():
@@ -75,6 +76,9 @@ def build_case(name, n, m, k, t, b, c, hid, layers, gcn_hid, density, seed, weig
 
 
 if __name__ == "__main__":
+    REF = os.path.abspath(sys.argv[1]) if len(sys.argv) > 1 else REF
+    if not os.path.exists(os.path.join(REF, "STMGCN.py")):
+        sys.exit("usage: python oracle/make_golden.py /path/to/reference  (the directory with GCN.py and STMGCN.py)")
     torch.set_num_threads(1)
     # BASELINE.json configs[0]: 64 regions, 1 graph, K=2, seq_len=4, batch=8, H=G=64, L=3, C=1.
     build_case("cfg1_ref", 64, 1, 2, 4, 8, 1, 64, 3, 64, 0.10, seed=0)
@@ -83,3 +87,6 @@ if __name__ == "__main__":
     # BASELINE.json configs[1]/[2] hyper-parameters (3 graphs, K=3, seq_len=12, H=G=64, L=3, C=1) at a size the reference
     # finishes in seconds: 96 regions x batch 6 = 576 LSTM rows (4.5 tiles of 128: ragged last tile on the GPU).
     build_case("cfg3_small_ref", 96, 3, 3, 12, 6, 1, 64, 3, 64, 0.05, seed=2)
+    # two graphs, two LSTM layers, narrow hidden sizes (H=16, G=8): pins the oracle's dense restatement to the reference
+    # modules away from the H=64 shapes of the other fixtures.
+    build_case("small_ref", 30, 2, 3, 5, 2, 1, 16, 2, 8, 0.2, seed=3)

@@ -4,7 +4,7 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline``
 legs may import this file.  Nothing under ``st-mgcn_b200/``, ``GCN.py`` or ``STMGCN.py`` does, and the
 product path raises if the CUDA library is missing rather than falling back to anything in here.
 
-Two independent restatements of the reference algorithm (all citations into ``/root/reference``):
+Two independent restatements of the reference algorithm (all citations into the reference ST-MGCN sources):
 
 * **dense** (``dense_*`` functions, torch CPU): the algorithm exactly as the reference executes it --
   K+1 dense ``N x N`` supports multiplied into the features one by one (``GCN.py:34-36``), concatenated
@@ -22,7 +22,7 @@ Two independent restatements of the reference algorithm (all citations into ``/r
 
 Parity pin: the reference has no tests, golden vectors or fixtures of its own (SURVEY.md section 4) --
 "parity unpinned" by the reference's own tests.  The pin used here is the reference code itself,
-imported from ``/root/reference`` in the build container (``oracle/make_golden.py`` ->
+imported from a reference checkout (``oracle/make_golden.py`` ->
 ``tests/golden/*.npz``; ``tests/test_oracle.py::test_dense_matches_reference_modules``).
 """
 from __future__ import annotations

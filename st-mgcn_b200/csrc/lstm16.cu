@@ -1,26 +1,20 @@
 // K3b, second generation (H = 64): the shared LSTM of CG_LSTM (reference STMGCN.py:21-22, :47-50; nn.LSTM semantics)
-// on tcgen05 with bf16 hi/lo PLANES ("3xBF16", see tc16.cuh) and NO gate tape.
+// on the Hopper tensor cores (wgmma) with bf16 hi/lo PLANES ("3xBF16", see tc16.cuh) and NO gate tape.
 //
 // Tape written by the forward (all the backward needs; it recomputes the gates from it):
 //   hp : (L, T, P, rows, 64) bf16  -- the hidden state of every layer-step as P planes (P = 2: hi | lo, fp32-grade
 //        arithmetic; P = 1: hi only, the bf16 mode).  A 128-row x 64-column piece of a plane IS a K-major, 128-byte
-//        swizzled tcgen05 operand tile once a TMA tensor load has put it into shared memory -- no splitter warps, no
-//        per-thread loads, no proxy fences on the operand path.
-//   cs : (L, T, rows_pad, 64) fp32, tile-blocked ([tile][unit/4][128 rows][4 units], see below): the 32 lanes of a warp
-//        (32 consecutive rows, the same 4 units) touch ONE contiguous 512-byte run per access.  (With 8-unit groups every
-//        access was 16 bytes at a 32-byte stride: 32 half-used sectors and ~22 L1 data-pipe wavefronts per request; ncu
-//        showed the L1 data pipe -- tensor-core operand reads + LSU -- at 77 % (forward) / 90 % (backward) of its peak.)
-// 4 + 4 bytes per (row, unit, layer-step) instead of 4 + 4 + 16 with the gate tape of the first generation
-// (lstm_tc.cu): 4.8 GB instead of 14.5 GB per graph branch at BASELINE configs[2], and configs[4] fits.
+//        swizzled wgmma operand tile once a TMA tensor load has put it into shared memory.
+//   cs : (L, T, rows_pad, 64) fp32, tile-blocked ([tile][unit/4][128 rows][4 units], see below).
+// 4 + 4 bytes per (row, unit, layer-step) instead of 4 + 4 + 16 with a gate tape.
 //
 // forward kernel (one launch per layer-step, persistent, one CTA per SM):
 //   producer warp : loads the layer's weight image ONCE (resident for the whole launch: [256 gate cols][64 k] bf16 tiles,
 //                   hi and lo, per K segment = 128 KB) and streams the A planes of every tile through a ring of 16 KB
 //                   stages with TMA tensor loads (h_below hi, h_below lo, h_prev hi, h_prev lo)
-//   MMA warp      : per tile 8 (P = 1) or 24 (P = 2) tcgen05.mma kind::f16 (M 128, N 256, K 16) into one of two TMEM
-//                   accumulators: Ahi.Whi + Ahi.Wlo + Alo.Whi
-//   16 epilogue warps: TMEM -> registers -> bias (+ layer 0: x*s . W_ih in exact fp32) -> gates -> c, h -> h split into
-//                   bf16 planes -> coalesced global stores.  Nothing of the gates leaves the SM.
+//   2 warpgroups  : per tile and warpgroup (64 rows) 8 (P = 1) or 24 (P = 2) wgmma m64n256k16 into registers:
+//                   Ahi.Whi + Ahi.Wlo + Alo.Whi, then bias (+ layer 0: x*s . W_ih in exact fp32) -> gates -> c, h ->
+//                   h split into bf16 planes -> global stores.  Nothing of the gates leaves the SM.
 #include "tc16.cuh"
 #include <cuda.h>
 #include <stdlib.h>
@@ -84,17 +78,16 @@ __device__ __forceinline__ void lstm_cell_gates8(float ai, float af, float ag, f
     tc = (1.f - ec) * rcp_ftz_(1.f + ec);
 }
 
-// L2 prefetch of a tensor-map box (no shared memory, no barrier): the later TMA load of the same box finds it in L2
-__device__ __forceinline__ void tma_prefetch_3d(const void* tmap, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
-                 :: "l"(tmap), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-
 // =====================================================================================================
 // forward
 // =====================================================================================================
-constexpr int kFEpiWarps = 16;
-constexpr int kFThreads = (kFEpiWarps + 2) * 32;       // + MMA warp + producer warp
+// CTA = two consumer warpgroups + one producer warp, persistent over 128-row tiles.  Warpgroup w owns rows 64w .. 64w+63
+// of a tile and accumulates its [64 x 256] gate pre-activations in registers (wgmma m64n256k16).  Accumulator fragment
+// (wgmma.cuh): thread holds columns 8j + 2(lane%4) + {0,1} of rows r0 and r0 + 8; with gate-interleaved columns
+// n = 4 unit + gate that is gates (i, f) (lane%4 even) or (g, o) (odd) of unit 2j + (lane%4)/2.  Partner lanes (lane ^ 1)
+// swap one row's pair, after which the even lane owns the cell (r0, unit) and the odd lane the cell (r0 + 8, unit).
+constexpr int kFWarpgroups = 2;
+constexpr int kFThreads = kFWarpgroups * 128 + 32;     // + producer warp
 constexpr int kFStages = 5;
 
 struct F16Tail {
@@ -102,10 +95,7 @@ struct F16Tail {
     float wih[kMaxC * kGateCols];
     uint64_t full[kFStages];
     uint64_t empty[kFStages];
-    uint64_t tmem_full[2];
-    uint64_t tmem_empty[2];
     uint64_t w_full;
-    uint32_t tmem_base;
 };
 constexpr size_t kFSmem = 1024 + 4 * (size_t)kWTileBytes + (size_t)kFStages * kATileBytes + sizeof(F16Tail);
 static_assert(kFSmem <= 232448, "lstm16 forward kernel exceeds the 227 KB shared-memory limit");
@@ -130,6 +120,10 @@ struct Fwd16Params {
     int n_tiles;
 };
 
+__device__ __forceinline__ uint16_t bf16_bits(float v) {
+    return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+}
+
 // CIN: 0 = not layer 0; 1 = layer 0 with one input channel (the reference's input_dim, compile-time: no predicated-off
 // W_ih FMAs / loads in the cell loop); kMaxC = layer 0 with a runtime channel count <= kMaxC
 template <int PLANES, int CIN>
@@ -137,8 +131,6 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
     constexpr bool L0 = CIN > 0;
     constexpr int kC = (CIN == 1) ? 1 : kMaxC;
     extern __shared__ uint8_t smem_raw[];
-    // 1024-byte alignment by pointer arithmetic on the __shared__ array (an integer round trip would make every access through
-    // `smem` a generic LD/ST/ATOM instead of LDS/STS/ATOMS: ncu showed the bias loads as long-scoreboard stalls)
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* wsm = smem;                                           // resident weight tiles
     uint8_t* stages = smem + 4 * (size_t)kWTileBytes;
@@ -146,34 +138,24 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const int lane = tid & 31;
-    constexpr int kMmaWarp = kFEpiWarps;
-    constexpr int kProdWarp = kFEpiWarps + 1;
+    constexpr int kProdWarp = kFWarpgroups * 4;
 
     if (tid == 0) {
         for (int s = 0; s < kFStages; ++s) {
             mbar_init(&tail->full[s], 1);
-            mbar_init(&tail->empty[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tail->tmem_full[a], 1);
-            mbar_init(&tail->tmem_empty[a], kFEpiWarps);       // one arrival per epilogue warp
+            mbar_init(&tail->empty[s], kFWarpgroups);          // one arrival per consumer warpgroup
         }
         mbar_init(&tail->w_full, 1);
         fence_barrier_init();
     }
-    if (warp == kMmaWarp) tmem_alloc(&tail->tmem_base, 512);
     for (int i = tid; i < kGateCols; i += kFThreads) tail->bias[i] = p.bias[i] * gate_scale(i);
     if (L0)
         for (int i = tid; i < p.c_in * kGateCols; i += kFThreads) tail->wih[i] = p.wih[i] * gate_scale(i);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tail->tmem_base;
     const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
     if (warp == kProdWarp) {
         // ===================== producer: resident weights once, then the A planes of every tile =====================
-        TC_PROF_DECL
         const bool leader = elect_one_sync();
         if (leader && p.nseg > 0) {
             mbar_arrive_expect_tx(&tail->w_full, (uint32_t)(p.nseg * PLANES * kWTileBytes));
@@ -197,196 +179,100 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
                     }
             }
         }
-        TC_PROF_FLUSH(0, leader)
-    } else if (warp == kMmaWarp) {
-        // ===================== MMA issuer =====================
-        TC_PROF_DECL
-        const bool leader = elect_one_sync();
-        if (p.nseg > 0) {
-            constexpr uint32_t idesc = idesc_bf16(kTileM, kGateCols);
-            mbar_wait_p(&tail->w_full, 0, 0);
-            tc_fence_after();
-            uint32_t it = 0;
-            for (int i = 0; i < my_tiles; ++i) {
-                const int a = i & 1;
-                const uint32_t aph = (uint32_t)(i >> 1) & 1;
-                mbar_wait_p(&tail->tmem_empty[a], aph ^ 1, 2);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)a * kGateCols;
-                for (int s = 0; s < p.nseg; ++s) {
-                    const uint64_t w_hi = desc16_k(smem_u32(wsm + (size_t)(s * 2) * kWTileBytes));
-                    const uint64_t w_lo = desc16_k(smem_u32(wsm + (size_t)(s * 2 + 1) * kWTileBytes));
-                    {   // hi plane of the segment: against W hi (and W lo)
-                        const int stg = it % kFStages;
-                        const uint32_t ph = (it / kFStages) & 1;
-                        mbar_wait_p(&tail->full[stg], ph, 1);
-                        tc_fence_after();
-                        if (leader) {
-                            const uint64_t a_d = desc16_k(smem_u32(stages + (size_t)stg * kATileBytes));
-                            if (PLANES == 2) {
-                                // per k-step: A_hi . W_hi keeps A in the collector, A_hi . W_lo re-uses it (one A read, not two)
+        return;
+    }
+    // ===================== consumers: gate GEMM (wgmma) + LSTM cell =====================
+    const int wg = tid >> 7;
+    const int q = lane & 3;
+    const bool odd = (q & 1) != 0;
+    const uint32_t row_in_tile = (uint32_t)(64 * wg + 16 * (warp & 3) + (lane >> 2) + (odd ? 8 : 0));
+    const uint32_t rows32 = (uint32_t)p.rows;
+    const uint32_t w_u = smem_u32(wsm), a_u = smem_u32(stages) + (uint32_t)wg * 64u * 128u;
+    float acc[128];
 #pragma unroll
-                                for (int kk = 0; kk < 4; ++kk) {
-                                    mma_bf16_keep_a(d_tmem, a_d + (uint64_t)(2 * kk), w_hi + (uint64_t)(2 * kk), idesc, (s > 0 || kk > 0) ? 1u : 0u);
-                                    mma_bf16_reuse_a(d_tmem, a_d + (uint64_t)(2 * kk), w_lo + (uint64_t)(2 * kk), idesc, 1u);
-                                }
-                            } else {
-#pragma unroll
-                                for (int kk = 0; kk < 4; ++kk)
-                                    mma_bf16(d_tmem, a_d + (uint64_t)(2 * kk), w_hi + (uint64_t)(2 * kk), idesc, (s > 0 || kk > 0) ? 1u : 0u);
-                            }
-                            mma_commit(&tail->empty[stg]);
-                        }
-                        __syncwarp();
-                        ++it;
-                    }
-                    if (PLANES == 2) {   // lo plane of the segment: against W hi
-                        const int stg = it % kFStages;
-                        const uint32_t ph = (it / kFStages) & 1;
-                        mbar_wait_p(&tail->full[stg], ph, 1);
-                        tc_fence_after();
-                        if (leader) {
-                            const uint64_t a_d = desc16_k(smem_u32(stages + (size_t)stg * kATileBytes));
-#pragma unroll
-                            for (int kk = 0; kk < 4; ++kk)
-                                mma_bf16(d_tmem, a_d + (uint64_t)(2 * kk), w_hi + (uint64_t)(2 * kk), idesc, 1u);
-                            mma_commit(&tail->empty[stg]);
-                        }
-                        __syncwarp();
-                        ++it;
-                    }
-                }
-                if (leader) mma_commit(&tail->tmem_full[a]);
-                __syncwarp();
-            }
-        }
-        TC_PROF_FLUSH(1, leader)
-    } else {
-        // ===================== epilogue: LSTM cell =====================
-        TC_PROF_DECL
-        // TMEM lane quadrant q = warp & 3 (rows 32q .. 32q+31 of the tile), column quarter part = warp >> 2
-        // (gate columns 64*part .. +63 = units 16*part .. +15), four pieces of 16 columns = 4 units each
-        const int q = warp & 3, part = warp >> 2;
-        constexpr bool l0 = L0;
-        // c_{t-1} of this thread's row (16 units) lives in registers; the four floats a piece has just consumed are
-        // reloaded at once with the NEXT tile's values, so the loads are in flight for most of a tile (loading all 16 at the
-        // end of a tile exposed the full DRAM latency at the top of the next one: ncu showed 21 % of the samples there)
-        float cpv[16];
-        float xs[kMaxC], xs_next[kMaxC], sv_next = 0.f;    // xs_next: raw x of the next tile; scaled by sv_next at the swap
-        // 32-bit element offsets (rows <= 2^25 is checked on the host): 64-bit address pairs cost registers, and the few
-        // that spilled were re-read from local memory in the tile loop at full L1-miss latency (ncu: 18 % of the samples)
-        const uint32_t row_in_tile = (uint32_t)(q * 32 + lane);
-        const uint32_t rows32 = (uint32_t)p.rows;
-        // tile-blocked (rows_pad x 64): element (tile, row, unit) at tile*8192 + (unit/4)*512 + row*4 + unit%4
-        const uint32_t thr_c = row_in_tile * 4u + (uint32_t)part * 2048u;
-        auto load_c4 = [&](int tile_n, int j) {
-            const uint32_t rn = (uint32_t)tile_n * kTileM + row_in_tile;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.c_prev != nullptr && tile_n < p.n_tiles && rn < rows32)
-                v = *reinterpret_cast<const float4*>(p.c_prev + ((uint32_t)tile_n * 8192u + thr_c + (uint32_t)j * 512u));
-            cpv[4 * j] = v.x; cpv[4 * j + 1] = v.y; cpv[4 * j + 2] = v.z; cpv[4 * j + 3] = v.w;
-        };
-        // loads only: the product x * s is formed when the tile starts (multiplying here waited for the loads on the spot:
-        // 14 % of the layer-0 kernel's stall samples)
-        auto load_xs = [&](int tile_n) {
-            const uint32_t rn = (uint32_t)tile_n * kTileM + row_in_tile;
-            const bool ok = tile_n < p.n_tiles && rn < rows32;
-            sv_next = 0.f;
-            if (ok) sv_next = p.sg[(rn % (uint32_t)p.b_inner) * (uint32_t)p.t_len + (uint32_t)p.t];    // (32-bit: a 64-bit % is a call)
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    if (p.nseg > 0) mbar_wait(&tail->w_full, 0, 0);
+    uint32_t it = 0;
+    for (int i = 0; i < my_tiles; ++i) {
+        const int tile = (int)blockIdx.x + i * (int)gridDim.x;
+        const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
+        const bool valid = r < rows32;
+        // layer 0: x * s of this thread's row (loaded before the MMAs: the latency hides behind them)
+        float xs[kMaxC];
+        if (L0) {
+            const float sv = valid ? p.sg[(r % (uint32_t)p.b_inner) * (uint32_t)p.t_len + (uint32_t)p.t] : 0.f;
 #pragma unroll
             for (int c = 0; c < kMaxC; ++c)
-                xs_next[c] = (c < kC && ok && (CIN == 1 || c < p.c_in)) ? p.xo[((int64_t)rn * p.t_len + p.t) * p.c_in + c] : 0.f;
-        };
-#pragma unroll
-        for (int j = 0; j < 4; ++j) load_c4((int)blockIdx.x, j);
-        if (l0) {
-            load_xs((int)blockIdx.x);
-#pragma unroll
-            for (int c = 0; c < kMaxC; ++c) xs[c] = xs_next[c] * sv_next;
+                xs[c] = (c < kC && valid && (CIN == 1 || c < p.c_in)) ? p.xo[((int64_t)r * p.t_len + p.t) * p.c_in + c] * sv : 0.f;
         }
-        const int gstep = (int)gridDim.x;
-        int tile = (int)blockIdx.x;                // carried in a register: re-reading %ctaid every tile is a long-scoreboard stall
-        for (int i = 0; i < my_tiles; ++i, tile += gstep) {
-            const int a = i & 1;
-            const uint32_t aph = (uint32_t)(i >> 1) & 1;
-            const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
-            const bool valid = r < rows32;
-            if (p.nseg > 0) {
-                mbar_wait(&tail->tmem_full[a], aph, 3);
-                tc_fence_after();
-            }
-            const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)a * kGateCols + (uint32_t)part * 64;
-            // (measured and rejected: software-pipelining the tcgen05.ld of the next piece under this piece's arithmetic with
-            //  per-piece 8-byte h stores -- 3.77 ms per branch forward against 2.86 ms for this load-then-wait form)
-            uint32_t hi[8], lo[8];
+        wg_fence_regs(acc);
+        for (int s = 0; s < p.nseg; ++s) {
+            const uint64_t w_hi = desc16_k(w_u + (uint32_t)(s * 2) * kWTileBytes);
+            const uint64_t w_lo = desc16_k(w_u + (uint32_t)(s * 2 + 1) * kWTileBytes);
 #pragma unroll
-            for (int pc = 0; pc < 4; ++pc) {
-                uint32_t v[16];
-                if (p.nseg > 0) {
-                    tmem_ld16(t_row + pc * 16, v);
-                    tmem_ld_wait();
-                } else {
+            for (int pl = 0; pl < PLANES; ++pl, ++it) {
+                const int stg = it % kFStages;
+                mbar_wait(&tail->full[stg], (it / kFStages) & 1, 1);
+                const uint64_t a_d = desc16_k(a_u + (uint32_t)stg * kATileBytes);
+                wg_fence();
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] = 0u;
+                for (int kk = 0; kk < 4; ++kk) {
+                    // hi plane: A_hi . W_hi (+ A_hi . W_lo); lo plane: A_lo . W_hi
+                    wgmma_bf16_n256_t00(acc, a_d + (uint64_t)(2 * kk), w_hi + (uint64_t)(2 * kk), (s > 0 || pl > 0 || kk > 0) ? 1u : 0u);
+                    if (PLANES == 2 && pl == 0) wgmma_bf16_n256_t00(acc, a_d + (uint64_t)(2 * kk), w_lo + (uint64_t)(2 * kk), 1u);
                 }
-                const int unit0 = part * 16 + pc * 4;
-                float hn[4], cn[4];
+                wg_commit();
+                wg_wait<0>();
+                wg_fence_regs(acc);
+                // the stage has been read: one arrival per warpgroup
+                asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+                if ((tid & 127) == 0) mbar_arrive(&tail->empty[stg]);
+            }
+        }
+        if (p.nseg == 0) {
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int col = 4 * (unit0 + u);
-                    const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
-                    float pi = fmaf(__uint_as_float(v[4 * u + 0]), -1.4426950408889634f, bv.x);
-                    float pf = fmaf(__uint_as_float(v[4 * u + 1]), -1.4426950408889634f, bv.y);
-                    float pg = fmaf(__uint_as_float(v[4 * u + 2]), -2.8853900817779268f, bv.z);
-                    float po = fmaf(__uint_as_float(v[4 * u + 3]), -1.4426950408889634f, bv.w);
-                    if (l0) {
+            for (int k = 0; k < 128; ++k) acc[k] = 0.f;
+        }
+        // ---- LSTM cell: 32 cells per thread, row row_in_tile, units 2j + q/2 ----
+        const uint32_t cbase = (uint32_t)tile * 8192u + row_in_tile * 4u;
 #pragma unroll
-                        for (int c = 0; c < kC; ++c)
-                            if (CIN == 1 || c < p.c_in) {
-                                const float4 wv = *reinterpret_cast<const float4*>(&tail->wih[c * kGateCols + col]);
-                                pi = fmaf(xs[c], wv.x, pi); pf = fmaf(xs[c], wv.y, pf);
-                                pg = fmaf(xs[c], wv.z, pg); po = fmaf(xs[c], wv.w, po);
-                            }
+        for (int j = 0; j < 32; ++j) {
+            const float s0 = odd ? acc[4 * j + 0] : acc[4 * j + 2];
+            const float s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+            const float o0 = __shfl_xor_sync(0xffffffffu, s0, 1);
+            const float o1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+            const float vi = odd ? o0 : acc[4 * j + 0], vf = odd ? o1 : acc[4 * j + 1];
+            const float vg = odd ? acc[4 * j + 2] : o0, vo = odd ? acc[4 * j + 3] : o1;
+            const int unit = 2 * j + (q >> 1);
+            const int col = 4 * unit;
+            const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
+            float pi = fmaf(vi, -1.4426950408889634f, bv.x);
+            float pf = fmaf(vf, -1.4426950408889634f, bv.y);
+            float pg = fmaf(vg, -2.8853900817779268f, bv.z);
+            float po = fmaf(vo, -1.4426950408889634f, bv.w);
+            if (L0) {
+#pragma unroll
+                for (int c = 0; c < kC; ++c)
+                    if (CIN == 1 || c < p.c_in) {
+                        const float4 wv = *reinterpret_cast<const float4*>(&tail->wih[c * kGateCols + col]);
+                        pi = fmaf(xs[c], wv.x, pi); pf = fmaf(xs[c], wv.y, pf);
+                        pg = fmaf(xs[c], wv.z, pg); po = fmaf(xs[c], wv.w, po);
                     }
-                    lstm_cell_fwd8(pi, pf, pg, po, cpv[4 * pc + u], cn[u], hn[u]);
-                }
-                if (PLANES == 2) {
-                    split_bf16x2(hn[0], hn[1], hi[2 * pc], lo[2 * pc]);
-                    split_bf16x2(hn[2], hn[3], hi[2 * pc + 1], lo[2 * pc + 1]);
-                } else {
-                    hi[2 * pc] = pack_bf16x2(hn[0], hn[1]);
-                    hi[2 * pc + 1] = pack_bf16x2(hn[2], hn[3]);
-                }
-                if (valid) {
-                    *reinterpret_cast<float4*>(p.c_out + ((uint32_t)tile * 8192u + thr_c + (uint32_t)pc * 512u)) =
-                        make_float4(cn[0], cn[1], cn[2], cn[3]);
-                    if (p.h_f32 != nullptr)
-                        *reinterpret_cast<float4*>(p.h_f32 + (r * (uint32_t)kHid + (uint32_t)unit0)) = make_float4(hn[0], hn[1], hn[2], hn[3]);
-                }
-                load_c4(tile + gstep, pc);                      // this piece's registers are free: next tile's values
-                if (l0 && pc == 0) load_xs(tile + gstep);
             }
-            if (p.nseg > 0) {          // all TMEM reads of this accumulator are done (one mbarrier arrival per warp: 512
-                tc_fence_before();     // per-thread arrivals are 512 serialised shared-memory atomics per tile)
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tail->tmem_empty[a]);
-            }
+            const uint32_t co = cbase + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
+            const float cp = (p.c_prev != nullptr && valid) ? p.c_prev[co] : 0.f;
+            float cn, hn;
+            lstm_cell_fwd8(pi, pf, pg, po, cp, cn, hn);
             if (valid) {
-                // 16 bf16 = 32 bytes per row and plane: one 256-bit store (a full sector) instead of two 128-bit ones
-                st_global_v8(p.h_hi + (r * (uint32_t)kHid + (uint32_t)part * 16u), hi);
-                if (PLANES == 2) st_global_v8(p.h_lo + (r * (uint32_t)kHid + (uint32_t)part * 16u), lo);
-            }
-            if (l0) {
-#pragma unroll
-                for (int c = 0; c < kMaxC; ++c) xs[c] = xs_next[c] * sv_next;
+                p.c_out[co] = cn;
+                const uint32_t ho = r * (uint32_t)kHid + (uint32_t)unit;
+                const __nv_bfloat16 hb = __float2bfloat16_rn(hn);
+                p.h_hi[ho] = __bfloat16_as_ushort(hb);
+                if (PLANES == 2) p.h_lo[ho] = bf16_bits(hn - __bfloat162float(hb));
+                if (p.h_f32 != nullptr) p.h_f32[ho] = hn;
             }
         }
-        TC_PROF_FLUSH(2, tid == 0)
     }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == kMmaWarp) tmem_dealloc(tmem_base, 512);
 }
 
 // ---- weight image packer: nn.LSTM parameters of one layer -> resident operand tiles + interleaved bias / W_ih^T ----
@@ -419,55 +305,35 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
 
 // =====================================================================================================
 // backward: gate recompute + BPTT pointwise + data gradient + weight gradient in ONE kernel, time-fused per layer
-// (a launch = one layer x a run of timesteps, see Bwd16Params; "tile" below = one (step, tile) work item)
+// (a launch = one layer x a run of timesteps, see Bwd16Params; "item" below = one (step, tile) work item)
 // =====================================================================================================
-// Per 128-row tile, the 256 gate columns are processed as four chunks of 64 (16 units x i,f,g,o):
-//   R_c : recompute the chunk's pre-activations  G_c[128 x 64] = [h_below | h_prev] . Wp[:, chunk]     (TMEM, 64 columns)
-//   P_c : 16 compute warps: TMEM -> gates -> c_t, tanh(c_t) -> BPTT pointwise -> dA_c (fp32) -> bf16 hi/lo planes in a
-//         128-byte-swizzled shared-memory tile; dc in place
-//   W_c : weight gradient   dWp[:, chunk] += [h_below | h_prev]^T . dA_c   -- BOTH operands are the MN-major view of tiles
-//         that are already in shared memory (the A planes, dA_c); one 256-column TMEM accumulator lives for the launch
-//   D_c : data gradient     [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T  -- B is the MN-major view of the weight chunk
-//         R_c used; 128-column TMEM accumulator, drained by the compute warps at the start of the next tile
-//   B_c : bias gradient     db[chunk] += dA_c^T . ones   -- 8 small MMAs (M = 64 hi + 64 lo columns, N = 16) on the W warp
-// dA never leaves the SM; the gates are never stored.  HBM traffic per tile: A planes 64 KB + c_prev, dh_in, dh_rec, dc
-// (4 x 32 KB) in, dc, dh_rec, dx_below (3 x 32 KB) out = 288 KB (the first-generation pair of kernels moved 640 KB).
-// Weight chunks stream from L2 twice, into one single-buffered slot for R_c and one for D_c (see the producer).
-// Partial weight gradients: every CTA adds its TMEM accumulator into its OWN slice of a scratch buffer (vector reductions,
-// no contention; the slice layout is the accumulator's register layout); stmgcn_lstm16_wgrad_reduce sums the slices once
-// per layer and writes nn.LSTM-native gradients.
-// The kernel is bound by the L1 / shared-memory data pipe (ncu: 94 %: tensor-core operand reads 61 % + LSU 33 %).
-constexpr int kBCompWarps = 16;
-constexpr int kBThreads = (kBCompWarps + 2) * 32;       // + MMA-issuing warp + producer warp
-constexpr int kBWStages = 2;                            // two single-buffered slots: the recompute's and the data gradient's copy
-constexpr int kBWChunkTile = 64 * 128;                  // [64 gate cols][64 k] bf16 = 8 KB
-constexpr int kBWStageBytes = 4 * kBWChunkTile;         // (seg0 hi | seg0 lo | seg1 hi | seg1 lo) = 32 KB
-constexpr int kBSgMax = 1024;
+// CTA = two consumer warpgroups (warpgroup w: rows 64w .. 64w+63 of a tile) + one producer warp.  The layer's weight image
+// stays resident in shared memory; the producer streams the A planes ([h_below | h_prev], hi and lo) of each item with
+// TMA.  Per item the 256 gate columns are processed as four chunks of 64 (16 units x i,f,g,o):
+//   R_c : recompute  G_c[64 x 64] = [h_below | h_prev] . Wp[:, chunk]                      (registers, m64n64)
+//   P_c : gates -> c_t, tanh(c_t) -> BPTT pointwise -> dA_c (fp32) -> bf16 hi/lo planes in a 128-byte-swizzled
+//         shared-memory tile; dc in place
+//   W_c : weight gradient  dWp[kd, chunk] = A^T . dA_c, warpgroup w: kd rows 64w .. (both operands: MN-major views of
+//         tiles already in shared memory), added into this CTA's own slice of a scratch buffer with vector reductions
+//   B_c : bias gradient    db[chunk] += ones . dA_c (warpgroup 0, A = a register fragment of ones), summed in shared memory
+//   D_c : data gradient    [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T  (B: MN-major view of the resident weights;
+//         accumulated in registers over the four chunks, stored at the end of the item)
+// dA never leaves the SM; the gates are never stored.  stmgcn_lstm16_wgrad_reduce sums the slices once per layer and
+// writes nn.LSTM-native gradients.
+constexpr int kBWarpgroups = 2;
+constexpr int kBThreads = kBWarpgroups * 128 + 32;      // + producer warp
+constexpr int kBATiles = 4;                             // (seg0 | seg1) x (hi | lo); layer 0: seg 1 = the auxiliary [x*s] tile
 
 struct B16Tail {
-    uint16_t ones[1024];                       // [16][64] bf16 tile of 1.0: B operand of the bias-gradient MMA (first member:
-                                               // the tail starts 1024-byte aligned, as a swizzled K-major operand must)
-    float bias[kGateCols];
-    float wih[kMaxC * kGateCols];
-    float s_ds[kBSgMax];
-    uint64_t ahi_full[2], ahi_empty[2];        // A hi planes: double-buffered by tile parity
-    uint64_t alo_full, alo_empty;              // A lo planes: single buffer
-    uint64_t w_full[kBWStages], w_empty[kBWStages];
-    uint64_t r_full, r_empty;
-    uint64_t d_full, d_empty;
-    uint64_t g_full, g_empty;
-    uint64_t done;
-    uint32_t tmem_base;
+    float db[kGateCols];
+    uint64_t a_full, a_empty, w_full;
 };
-constexpr int kBATiles = 6;                             // hi planes of two tiles (2 x 2 segments) + lo planes of one (2 segments)
-constexpr size_t kBSmem = 1024 + kBATiles * (size_t)kATileBytes + (size_t)kBWStages * kBWStageBytes + 2 * (size_t)kATileBytes + sizeof(B16Tail);
+constexpr size_t kBSmem = 1024 + 4 * (size_t)kWTileBytes + kBATiles * (size_t)kATileBytes + 2 * (size_t)kATileBytes + sizeof(B16Tail);
 static_assert(kBSmem <= 232448, "lstm16 backward kernel exceeds the 227 KB shared-memory limit");
 
-// One launch = one LAYER, all timesteps T-1 .. 0 (the tiles of a CTA are its own through time: rows never mix).  A step
-// of a tile needs what the SAME CTA produced for that tile one step later (dh_rec, dc: global, in place), so nothing but
-// the launch order of the layers (top down) synchronises; what a per-step launch paid 36 times per branch -- prologue,
-// first-tile latency, the 128 KB weight-gradient flush per CTA, the launch gap: 22 us of a 169 us launch, measured by
-// scaling the row count -- is paid 3 times.
+// One launch = one LAYER, a run of timesteps from T-1 down (the tiles of a CTA are its own through time: rows never mix).
+// A step of a tile needs what the SAME CTA produced for that tile one step later (dh_rec, dc: global, in place), so nothing
+// but the launch order of the layers (top down) synchronises.
 constexpr int kBMaxSteps = 64;
 struct Bwd16Step {
     int32_t slice[2];          // plane slice of K segment s in its tensor map (hi plane; lo = + 1)
@@ -493,616 +359,338 @@ struct Bwd16Params {
     float* dh_rec;             // blocked, in (unless first) / out, in place through the steps
     float* dc;                 // blocked, in (unless first) / out, in place through the steps
     float* dbp;                // (256) +=  gate-interleaved bias gradient
-    float* dw_slice;           // gridDim.x slices of 128*256 floats (accumulator register layout)
-    int dw_first;              // 1: first launch of this layer: slices are written, not accumulated
+    float* dw_slice;           // gridDim.x slices of 128 x 256 floats (row-major [kd][gate column]), +=
     int64_t rows;
     int n_tiles;
     Bwd16Step steps[kBMaxSteps];   // in execution order: steps[0] is t = T-1
 };
 static_assert(sizeof(Bwd16Params) <= 4096, "kernel parameter block exceeds 4 KB");
 
+__device__ __forceinline__ void cons_sync(int n_threads) { asm volatile("bar.sync 1, %0;" ::"r"(n_threads) : "memory"); }
+
 template <int PLANES, int CIN>                                  // CIN: see lstm16_fwd_kernel
 __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_constant__ Bwd16Params p) {
     constexpr bool L0 = CIN > 0;
     constexpr int kC = (CIN == 1) ? 1 : kMaxC;
+    constexpr int kNseg = L0 ? 1 : 2;
     extern __shared__ uint8_t smem_raw[];
-    // 1024-byte alignment by pointer arithmetic on the __shared__ array (an integer round trip would make every access through
-    // `smem` a generic LD/ST/ATOM instead of LDS/STS/ATOMS: ncu showed the bias loads as long-scoreboard stalls)
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    // A planes: tiles [hi buffer 0: seg0, seg1 (aux)] [hi buffer 1: seg0, seg1 (aux)] [lo: seg0, seg1 (aux)].  The hi planes
-    // of the NEXT tile load while this tile is processed; the lo planes (needed by one of three passes) are single-buffered
-    // and released by the FIRST pass of the tile's last weight-gradient MMA group.  Fully single-buffered planes cost the
-    // compute warps 16 % of their lifetime waiting for the first recompute of every tile (role accounting, profiles/).
-    uint8_t* a_sm = smem;
-    uint8_t* w_sm = a_sm + kBATiles * (size_t)kATileBytes;         // weight chunk ring
-    uint8_t* da_sm = w_sm + (size_t)kBWStages * kBWStageBytes;     // dA chunk: hi tile | lo tile
+    uint8_t* w_sm = smem;                                          // resident weights: tiles (seg*2 + plane) of 32 KB
+    uint8_t* a_sm = w_sm + 4 * (size_t)kWTileBytes;                // A planes: tiles (seg*2 + plane) of 16 KB
+    uint8_t* da_sm = a_sm + kBATiles * (size_t)kATileBytes;        // dA chunk: hi tile | lo tile
     B16Tail* tail = (B16Tail*)(da_sm + 2 * (size_t)kATileBytes);
+    // layer 0 has one weight segment: the pre-scaled W_ih^T lives in the unused seg-1 weight slot
+    float* wih_s = reinterpret_cast<float*>(w_sm + 2 * (size_t)kWTileBytes);
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const int lane = tid & 31;
-    constexpr int kMmaWarp = kBCompWarps;
-    constexpr int kProdWarp = kBCompWarps + 1;
-    // TMEM columns: weight grad (256) | data grad (128) | recompute (64, single buffer: the compute warps hold it only for
-    // the TMEM -> register copy at the start of a chunk) | bias grad (4 chunks x 16)
-    constexpr uint32_t kWgCol = 0, kDgCol = 256, kRcCol = 384, kDbCol = 448;
+    constexpr int kProdWarp = kBWarpgroups * 4;
+    constexpr int kCons = kBWarpgroups * 128;
 
     if (tid == 0) {
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&tail->ahi_full[b], 1);
-            mbar_init(&tail->ahi_empty[b], 1);
-        }
-        mbar_init(&tail->alo_full, 1);
-        mbar_init(&tail->alo_empty, 1);
-        for (int s = 0; s < kBWStages; ++s) {
-            mbar_init(&tail->w_full[s], 1);
-            mbar_init(&tail->w_empty[s], 1);
-        }
-        mbar_init(&tail->r_full, 1);
-        mbar_init(&tail->r_empty, kBCompWarps);                // one arrival per compute warp
-        mbar_init(&tail->d_full, kBCompWarps);
-        mbar_init(&tail->d_empty, 1);
-        mbar_init(&tail->g_full, 1);
-        mbar_init(&tail->g_empty, kBCompWarps);
-        mbar_init(&tail->done, 1);
+        mbar_init(&tail->a_full, 1);
+        mbar_init(&tail->a_empty, kBWarpgroups);
+        mbar_init(&tail->w_full, 1);
         fence_barrier_init();
     }
-    if (warp == kMmaWarp) tmem_alloc(&tail->tmem_base, 512);
-    for (int i = tid; i < kGateCols; i += kBThreads) tail->bias[i] = p.bias[i] * gate_scale(i);
-    for (int i = tid; i < 1024; i += kBThreads) tail->ones[i] = 0x3f80u;           // bf16 1.0 (layout-invariant)
+    for (int i = tid; i < kGateCols; i += kBThreads) tail->db[i] = 0.f;
     if (L0) {
-        for (int i = tid; i < p.c_in * kGateCols; i += kBThreads) tail->wih[i] = p.wih[i] * gate_scale(i);
-        for (int i = tid; i < kBSgMax; i += kBThreads) tail->s_ds[i] = 0.f;
+        for (int i = tid; i < p.c_in * kGateCols; i += kBThreads) wih_s[i] = p.wih[i] * gate_scale(i);
+        // auxiliary tiles (seg-1 slots): zero once; columns 0..C-1 are rewritten per item
+        for (int i = tid; i < 2 * kATileBytes / 16; i += kBThreads)
+            reinterpret_cast<uint4*>(a_sm + 2 * (size_t)kATileBytes)[i] = make_uint4(0u, 0u, 0u, 0u);
     }
-    fence_proxy_async_smem();                   // the ones tile is read by the tensor pipe (async proxy)
-    tc_fence_before();
+    fence_proxy_async_smem();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tail->tmem_base;
     const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    const bool have_aux = L0;
-    // K segments of the gate GEMM: layers > 0: [h_below | h_prev]; layer 0: [h_prev] (at t = 0 without an initial state the
-    // h_prev tiles are loaded as zeros: every step of a layer has the same operand geometry and accumulates into the same
-    // weight-gradient rows)
-    constexpr int kNseg = L0 ? 1 : 2;
     const int n_items = my_tiles * p.n_steps;                      // work items (step, tile), step-major
-    // operand tiles of the weight-gradient GEMM (MN-major view): atom 0 and atom 1 along M = kd
-    // layers > 0: atom 0 = h_below, atom 1 = h_prev;  layer 0: atom 0 = h_prev, atom 1 = auxiliary [x*s] tile
-    constexpr uint32_t wg_a0 = 0u;                                 // segment slot of atom 0
-    constexpr uint32_t wg_lbo = kATileBytes;
 
     if (warp == kProdWarp) {
         // ===================== producer =====================
-        TC_PROF_DECL
         const bool leader = elect_one_sync();
         if (leader && n_items > 0) {
-            const int first = (int)blockIdx.x, gstep = (int)gridDim.x;
-            // work item w = (step w / my_tiles, tile first + (w % my_tiles) * gstep)
-            auto seg_load = [&](uint8_t* dst, const Bwd16Step& sp, int sg, int plane, int tile, uint64_t* bar) {
-                if (sp.src[sg] == 2) bulk_g2s(dst, p.zero_tile, kATileBytes, bar);
-                else tma_load_3d(dst, &p.maps[sp.src[sg]], 0, tile * kTileM, sp.slice[sg] + plane, bar);
-            };
-            auto load_hi = [&](int w) {                 // hi planes of item w -> hi buffer w & 1
-                const int b = w & 1;
-                const int st = w / my_tiles, tile = first + (w - st * my_tiles) * gstep;
+            mbar_arrive_expect_tx(&tail->w_full, (uint32_t)(kNseg * PLANES * kWTileBytes));
+            for (int sg = 0; sg < kNseg; ++sg)
+                for (int pl = 0; pl < PLANES; ++pl)
+                    bulk_g2s(w_sm + (size_t)(sg * 2 + pl) * kWTileBytes, p.wimg + (size_t)(sg * 2 + pl) * kWTileBytes, kWTileBytes,
+                             &tail->w_full);
+            for (int w = 0; w < n_items; ++w) {
+                const int st = w / my_tiles, tile = (int)blockIdx.x + (w - st * my_tiles) * (int)gridDim.x;
                 const Bwd16Step& sp = p.steps[st];
-                if (w >= 2) mbar_wait_p(&tail->ahi_empty[b], (uint32_t)((w >> 1) - 1) & 1, 1);
-                mbar_arrive_expect_tx(&tail->ahi_full[b], (uint32_t)(kNseg * kATileBytes));
+                mbar_wait_p(&tail->a_empty, (uint32_t)(w & 1) ^ 1u, 0);
+                mbar_arrive_expect_tx(&tail->a_full, (uint32_t)(kNseg * PLANES * kATileBytes));
                 for (int sg = 0; sg < kNseg; ++sg)
-                    seg_load(a_sm + (size_t)(b * 2 + sg) * kATileBytes, sp, sg, 0, tile, &tail->ahi_full[b]);
-            };
-            auto load_lo = [&](int w) {                 // lo planes of item w -> the single lo buffer
-                const int st = w / my_tiles, tile = first + (w - st * my_tiles) * gstep;
-                const Bwd16Step& sp = p.steps[st];
-                if (w >= 1) mbar_wait_p(&tail->alo_empty, (uint32_t)(w - 1) & 1, 1);
-                mbar_arrive_expect_tx(&tail->alo_full, (uint32_t)(kNseg * kATileBytes));
-                for (int sg = 0; sg < kNseg; ++sg)
-                    seg_load(a_sm + (size_t)(4 + sg) * kATileBytes, sp, sg, 1, tile, &tail->alo_full);
-            };
-            auto load_w = [&](int stg, uint32_t wc) {   // weight chunk wc & 3 -> buffer stg (0: the recompute's copy, 1: the
-                const int c = wc & 3;                   // data gradient's copy); use wc of a buffer waits for release wc - 1
-                mbar_wait_p(&tail->w_empty[stg], (wc & 1) ^ 1, 0);
-                mbar_arrive_expect_tx(&tail->w_full[stg], (uint32_t)(kNseg * PLANES * kBWChunkTile));
-                for (int sg = 0; sg < kNseg; ++sg)
-                    for (int pl = 0; pl < PLANES; ++pl)
-                        bulk_g2s(w_sm + (size_t)stg * kBWStageBytes + (size_t)(sg * 2 + pl) * kBWChunkTile,
-                                 p.wimg + (size_t)(sg * 2 + pl) * kWTileBytes + (size_t)c * kBWChunkTile, kBWChunkTile, &tail->w_full[stg]);
-            };
-            auto prefetch_next = [&](int w) {           // item w's lo planes and per-row inputs -> L2
-                const int st = w / my_tiles, tile = first + (w - st * my_tiles) * gstep;
-                const Bwd16Step& sp = p.steps[st];
-                if (PLANES == 2)
-                    for (int sg = 0; sg < kNseg; ++sg)
-                        if (sp.src[sg] != 2) tma_prefetch_3d(&p.maps[sp.src[sg]], 0, tile * kTileM, sp.slice[sg] + 1);
-                // the compute warps' per-row inputs (a tile is one contiguous 32 KB run in every workspace): their
-                // one-chunk-ahead register prefetch then costs an L2 hit, not a DRAM round trip
+                    for (int pl = 0; pl < PLANES; ++pl) {
+                        uint8_t* dst = a_sm + (size_t)(sg * 2 + pl) * kATileBytes;
+                        if (sp.src[sg] == 2) bulk_g2s(dst, p.zero_tile, kATileBytes, &tail->a_full);
+                        else tma_load_3d(dst, &p.maps[sp.src[sg]], 0, tile * kTileM, sp.slice[sg] + pl, &tail->a_full);
+                    }
+                // the per-row inputs of this item -> L2 (a tile is one contiguous 32 KB run in every workspace)
                 const int64_t o = (int64_t)tile * kTileM * kHid;
                 constexpr uint32_t kB = kTileM * kHid * 4;
                 if (sp.c_prev) prefetch_l2(sp.c_prev + o, kB);
                 if (sp.dh_in) prefetch_l2(sp.dh_in + o, kB);
-                if (!sp.first && my_tiles > 2) {         // (written by this CTA more than a tile-time ago)
-                    prefetch_l2(p.dh_rec + o, kB);
-                    prefetch_l2(p.dc + o, kB);
-                }
-            };
-            // Every weight chunk is loaded TWICE (L2 hits), into two single-buffered slots: one copy for the recompute R_c, one
-            // for the data gradient D_c.  With one shared ring a stage was held from R_c until D_c (a whole chunk-time later), so
-            // R_{c+2} had to wait for D_c + a reload + its own MMAs inside one chunk-time: the recompute warp spent 40 % of its
-            // life waiting for weights and the compute warps 11 % waiting for the recompute.  Now R_{c+1} only needs the compute
-            // warps to have copied G_c out of TMEM.
-            // Flat schedule: every wait below is on an event that lies in the PAST of what the consumers need next, in time
-            // order: R(g+2) is released at the start of chunk-time g+1, D(g+1)'s buffer at the end of chunk-time g.
-            load_hi(0);
-            if (PLANES == 2) load_lo(0);
-            load_w(0, 0);
-            load_w(1, 0);
-            load_w(0, 1);
-            for (int i = 0; i < n_items; ++i) {
-                const bool more = i + 1 < n_items;
-                const uint32_t g0 = 4u * (uint32_t)i;
-                if (more) {
-                    load_hi(i + 1);
-                    prefetch_next(i + 1);
-                }
-                load_w(0, g0 + 2);
-                load_w(1, g0 + 1);
-                load_w(0, g0 + 3);
-                load_w(1, g0 + 2);
-                if (more) load_w(0, g0 + 4);
-                load_w(1, g0 + 3);
-                if (more) {
-                    if (PLANES == 2) load_lo(i + 1);
-                    load_w(0, g0 + 5);
-                    load_w(1, g0 + 4);
-                }
             }
         }
-        TC_PROF_FLUSH(5, leader)
-    } else if (warp == kMmaWarp) {
-        // ===================== the MMA issuer: recompute (R) | weight gradient (W) | bias gradient | data gradient (D) =====================
-        // ONE thread issues every tcgen05.mma of the CTA, in the order the work becomes ready:
-        //     R_{g+1} (hi passes [+ lo pass])  ->  W_g lo pass, D_g, W_g hi passes, bias gradient  ->  [tile boundary: R_{g+1} lo pass]
-        // R_{g+1} is released when the compute warps have copied G_g out of TMEM (start of chunk-time g), W_g / D_g when dA_g is in
-        // shared memory (its end).  (An earlier version used three issuing warps because an issue cost ~90 cycles -- that was the
-        // ELECT / BRA.U.ANY loop ptxas wraps around `lane == 0`-guarded UTCHMMAs, gone with elect.sync.)  A single in-order issuer
-        // is what makes the A-operand collector usable: in the 3xBF16 scheme the products A_hi.B_hi and A_hi.B_lo share A, so
-        // the second MMA of each pair takes A from the tensor core's collector buffer instead of re-reading 4 KB of shared memory
-        // -- the kernel is bound by the shared-memory data pipe (ncu: 94 %, 61 % of it tensor-core operand reads).
-        // Everything that does not change is hoisted into 64-bit descriptor constants; a k-step is one add on the descriptor's
-        // address field (encoded address = bytes >> 4; all operands live below 256 KB: no carry).
-        TC_PROF_DECL
-        const bool leader = elect_one_sync();
-        constexpr uint32_t idesc_rc = idesc_bf16(kTileM, 64);              // recompute: A K-major, B K-major, N = 64
-        constexpr uint32_t idesc_wg = idesc_bf16(kTileM, 64, 1, 1);        // weight gradient: both MN-major, M = kd (128), N = 64
-        constexpr uint32_t idesc_db = idesc_bf16(kTileM, 16, 1, 0);        // bias gradient: A = dA^T (hi | lo atoms), B = ones
-        constexpr uint32_t idesc_dg = idesc_bf16(kTileM, 64 * kNseg, 0, 1);   // data gradient: B MN-major, N = 64 * nseg
-        const uint32_t a_u = smem_u32(a_sm), w_u = smem_u32(w_sm), da_u = smem_u32(da_sm);
-        constexpr uint64_t kStepK = 2;                                     // K-major: 16 bf16 = 32 bytes
-        constexpr uint64_t kStepMN = 2048 >> 4;                            // MN-major: 16 rows of 128 bytes
-        constexpr uint64_t kTileEnc = kATileBytes >> 4, kChunkEnc = kBWChunkTile >> 4, kStageEnc = kBWStageBytes >> 4;
-        constexpr int nseg = kNseg;
-        const uint64_t rc_a = desc16_k(a_u);                               // hi: + (buffer*2 + s) * kTileEnc; lo: + (4 + s) * kTileEnc
-        const uint64_t rc_b = desc16_k(w_u);                               // buffer 0 (the recompute's copy): + (s*2 + plane) * kChunkEnc
-        const uint64_t wg_hi0 = desc16_mn(a_u + wg_a0 * kATileBytes, wg_lbo);              // hi buffer 0; buffer 1: + 2 * kTileEnc
-        const uint64_t wg_lo = desc16_mn(a_u + (4 + wg_a0) * kATileBytes, wg_lbo);         // lo planes
-        const uint64_t wg_b = desc16_mn(da_u, kATileBytes);                                  // dA hi; lo: + kTileEnc
-        const uint64_t db_b = desc16_k(smem_u32(tail->ones));
-        const uint64_t dg_a = desc16_k(da_u);                              // dA hi; lo: + kTileEnc
-        const uint64_t dg_b = desc16_mn(w_u, 2 * kBWChunkTile) + kStageEnc;   // buffer 1 (the data gradient's copy) (+ kChunkEnc: lo plane)
-        const uint32_t t_rc = tmem_base + kRcCol, t_wg = tmem_base + kWgCol, t_db = tmem_base + kDbCol, t_dg = tmem_base + kDgCol;
-        const bool a_sync = nseg > 0 || L0;          // someone waits for the A buffers (producer and / or the aux-tile writers)
-        const uint32_t total = 4u * (uint32_t)n_items;    // chunks; "tile" below = work item (step, tile): the hand-offs do
-                                                          // not care which timestep an item belongs to
+        return;
+    }
 
-        // hi-plane passes of the recompute of chunk wc (tile wc >> 2): G = A_hi . (W_hi + W_lo)
-        auto issue_r_hi = [&](uint32_t wc) {
-            const int ab = (int)((wc >> 2) & 1);
+    // ===================== consumers =====================
+    const int wg = tid >> 7;
+    const int q = lane & 3;
+    const bool odd = (q & 1) != 0;
+    const uint32_t rw0 = (uint32_t)(64 * wg + 16 * (warp & 3) + (lane >> 2));   // fragment row (and rw0 + 8)
+    const uint32_t row_in_tile = rw0 + (odd ? 8u : 0u);                          // this thread's cell row
+    const uint32_t rows32 = (uint32_t)p.rows;
+    const uint32_t w_u = smem_u32(w_sm), a_u = smem_u32(a_sm), da_u = smem_u32(da_sm);
+    const uint32_t a_rows = (uint32_t)wg * 64u * 128u;             // this warpgroup's rows inside a 128-row tile
+    constexpr uint32_t kStepMN = 2048;                             // MN-major k16 step: 16 rows of 128 bytes
+    // layer 0: when b_inner divides the tile height, a thread's row belongs to the same window b in every tile: its share of
+    // d_s is summed in a register and added once per step
+    const bool ds_fixed = L0 && (kTileM % (uint32_t)p.b_inner) == 0u;
+    float ds_acc = 0.f;
+    float* slice = p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols);
+    uint32_t ones[4];
 #pragma unroll
-            for (int s = 0; s < 2; ++s) {
-                if (s < nseg) {
-                    const uint64_t a_hi = rc_a + (uint64_t)(ab * 2 + s) * kTileEnc;
-                    const uint64_t b_hi = rc_b + (uint64_t)(s * 2) * kChunkEnc, b_lo = b_hi + kChunkEnc;
-#pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) {
-                        const uint32_t acc = (s > 0 || kk > 0) ? 1u : 0u;
-                        if (PLANES == 2) {
-                            mma_bf16_keep_a(t_rc, a_hi + kk * kStepK, b_hi + kk * kStepK, idesc_rc, acc);
-                            mma_bf16_reuse_a(t_rc, a_hi + kk * kStepK, b_lo + kk * kStepK, idesc_rc, 1u);
-                        } else {
-                            mma_bf16(t_rc, a_hi + kk * kStepK, b_hi + kk * kStepK, idesc_rc, acc);
-                        }
-                    }
-                }
-            }
-        };
-        // lo-plane pass (PLANES == 2): G += A_lo . W_hi; then the chunk's weight slot and the accumulator are handed over
-        auto issue_r_lo_and_commit = [&]() {
-            if (PLANES == 2) {
-#pragma unroll
-                for (int s = 0; s < 2; ++s) {
-                    if (s < nseg) {
-                        const uint64_t a_lo = rc_a + (uint64_t)(4 + s) * kTileEnc;
-                        const uint64_t b_hi = rc_b + (uint64_t)(s * 2) * kChunkEnc;
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk) mma_bf16(t_rc, a_lo + kk * kStepK, b_hi + kk * kStepK, idesc_rc, 1u);
-                    }
-                }
-            }
-            mma_commit(&tail->w_empty[0]);
-            mma_commit(&tail->r_full);
-        };
+    for (int k = 0; k < 4; ++k) ones[k] = 0x3f803f80u;                // bf16 pair (1, 1)
+    mbar_wait(&tail->w_full, 0, 0);
 
-        if (n_items > 0) {                           // R_0
-            mbar_wait_p(&tail->ahi_full[0], 0, 3);
-            mbar_wait_p(&tail->w_full[0], 0, 0);
-            if (PLANES == 2) mbar_wait_p(&tail->alo_full, 0, 3);
-            tc_fence_after();
-            if (leader) {
-                issue_r_hi(0);
-                issue_r_lo_and_commit();
+    for (int w = 0; w < n_items; ++w) {
+        const int st = w / my_tiles, tile = (int)blockIdx.x + (w - st * my_tiles) * (int)gridDim.x;
+        const Bwd16Step& sp = p.steps[st];
+        const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
+        const bool valid = r < rows32;
+        const bool last_of_step = (w - st * my_tiles) == my_tiles - 1;
+        float xs[kMaxC], xraw[kMaxC], dxs[kMaxC];
+        if (L0) {
+            const float sv = valid ? p.sg[(r % (uint32_t)p.b_inner) * (uint32_t)p.t_len + (uint32_t)sp.t] : 0.f;
+#pragma unroll
+            for (int c = 0; c < kMaxC; ++c) {
+                xraw[c] = (c < kC && valid && (CIN == 1 || c < p.c_in)) ? p.xo[((int64_t)r * p.t_len + sp.t) * p.c_in + c] : 0.f;
+                xs[c] = xraw[c] * sv;
+                dxs[c] = 0.f;
             }
-            __syncwarp();
         }
-        for (uint32_t g = 0; g < total; ++g) {
-            const int i = (int)(g >> 2), c = (int)(g & 3);
-            const bool have_next = nseg > 0 && g + 1 < total;
-            // ---- (1) recompute of the next chunk ----
-            if (have_next) {
-                const uint32_t wc = g + 1;
-                mbar_wait_p(&tail->w_full[0], wc & 1, 0);
-                if (c == 3) mbar_wait_p(&tail->ahi_full[(i + 1) & 1], (uint32_t)((i + 1) >> 1) & 1, 3);
-                mbar_wait_p(&tail->r_empty, (wc & 1) ^ 1, 2);
-                tc_fence_after();
-                if (leader) {
-                    issue_r_hi(wc);
-                    if (c != 3) issue_r_lo_and_commit();         // (c == 3: the next tile's lo planes land after W_g's lo pass)
-                }
-                __syncwarp();
-            }
-            // ---- (2) dA_g is in shared memory: weight gradient, data gradient, bias gradient ----
-            if (nseg > 0) mbar_wait_p(&tail->w_full[1], g & 1, 0);
-            mbar_wait_p(&tail->d_full, g & 1, 1);
-            if (c == 0 && nseg > 0 && i > 0) mbar_wait_p(&tail->g_empty, (uint32_t)(i - 1) & 1, 2);
-            tc_fence_after();
-            if (leader) {
-                const uint64_t wg_hi = wg_hi0 + (uint64_t)((i & 1) * 2) * kTileEnc;
-                const uint32_t d_wg = t_wg + (uint32_t)c * 64;
-                const uint32_t acc0 = (i > 0) ? 1u : 0u;
-                if (PLANES == 2) {                   // W_g, lo-plane pass first: the tile's last one releases the single lo buffer a.s.a.p.
-                    mma_bf16(d_wg, wg_lo, wg_b, idesc_wg, acc0);
+        // the previous item's stores (dh_rec, dc of other threads' cells) and its reads of the shared tiles are complete
+        cons_sync(kCons);
+        if (L0 && (q >> 1) == 0) {
+            // auxiliary weight-gradient operand (seg-1 slots): row = this thread's row, columns 0..C-1 = x*s (hi / lo split)
+            uint32_t hi[2], lo[2];
+            split_bf16x2(xs[0], xs[1], hi[0], lo[0]);
+            split_bf16x2(xs[2], xs[3], hi[1], lo[1]);
+            const uint32_t off = row_in_tile * 128u + ((0u ^ (row_in_tile & 7u)) << 4);
+            *reinterpret_cast<uint2*>(a_sm + 2 * (size_t)kATileBytes + off) = make_uint2(hi[0], hi[1]);
+            *reinterpret_cast<uint2*>(a_sm + 3 * (size_t)kATileBytes + off) = make_uint2(lo[0], lo[1]);
+        }
+        mbar_wait(&tail->a_full, (uint32_t)w & 1u, 1);
+        float dacc[32 * kNseg];                                    // [dx_below | dh_prev] (layer 0: [dh_prev])
 #pragma unroll
-                    for (int ks = 1; ks < 8; ++ks) mma_bf16(d_wg, wg_lo + ks * kStepMN, wg_b + ks * kStepMN, idesc_wg, 1u);
-                    if (c == 3 && a_sync) mma_commit(&tail->alo_empty);
-                }
-                if (nseg > 0) {                      // D_g: [dx_below | dh_prev] += (dA_hi + dA_lo) . W_hi^T + dA_hi . W_lo^T
+        for (int k = 0; k < 32 * kNseg; ++k) dacc[k] = 0.f;
+        for (int c = 0; c < 4; ++c) {
+            // ---- R_c ----
+            float g[32];
 #pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) {
-                        const uint32_t acc = (c > 0 || kk > 0) ? 1u : 0u;
-                        if (PLANES == 2) {
-                            mma_bf16_keep_a(t_dg, dg_a + kk * kStepK, dg_b + kk * kStepMN, idesc_dg, acc);
-                            mma_bf16_reuse_a(t_dg, dg_a + kk * kStepK, dg_b + kChunkEnc + kk * kStepMN, idesc_dg, 1u);
-                        } else {
-                            mma_bf16(t_dg, dg_a + kk * kStepK, dg_b + kk * kStepMN, idesc_dg, acc);
-                        }
+            for (int k = 0; k < 32; ++k) g[k] = 0.f;
+            wg_fence_regs(g);
+            wg_fence();
+#pragma unroll
+            for (int s = 0; s < kNseg; ++s) {
+                const uint64_t a_hi = desc16_k(a_u + (uint32_t)(s * 2) * kATileBytes + a_rows);
+                const uint64_t a_lo = desc16_k(a_u + (uint32_t)(s * 2 + 1) * kATileBytes + a_rows);
+                const uint64_t b_hi = desc16_k(w_u + (uint32_t)(s * 2) * kWTileBytes + (uint32_t)c * 8192u);
+                const uint64_t b_lo = desc16_k(w_u + (uint32_t)(s * 2 + 1) * kWTileBytes + (uint32_t)c * 8192u);
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    wgmma_bf16_n64_t00(g, a_hi + 2 * kk, b_hi + 2 * kk, (s > 0 || kk > 0) ? 1u : 0u);
+                    if (PLANES == 2) {
+                        wgmma_bf16_n64_t00(g, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
+                        wgmma_bf16_n64_t00(g, a_lo + 2 * kk, b_hi + 2 * kk, 1u);
                     }
-#pragma unroll
-                    for (int kk = 0; kk < 4; ++kk)                       // dA lo plane: always (it never leaves the SM)
-                        mma_bf16(t_dg, dg_a + kTileEnc + kk * kStepK, dg_b + kk * kStepMN, idesc_dg, 1u);
-                    mma_commit(&tail->w_empty[1]);
-                    if (c == 3) mma_commit(&tail->g_full);
                 }
-                // W_g, hi planes: A_hi^T . (dA_hi + dA_lo); dA always has its lo plane: in the single-plane (bf16 storage) mode
-                // only the STORED operands are rounded to bf16
+            }
+            wg_commit();
+            wg_wait<0>();
+            wg_fence_regs(g);
+            // ---- P_c: 8 cells per thread (row row_in_tile, units 16c + 2j + q/2) ----
+            uint32_t dhi[8], dlo[8];
+            const uint32_t bo = (uint32_t)tile * 8192u + row_in_tile * 4u;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const float s0 = odd ? g[4 * j + 0] : g[4 * j + 2];
+                const float s1 = odd ? g[4 * j + 1] : g[4 * j + 3];
+                const float o0 = __shfl_xor_sync(0xffffffffu, s0, 1);
+                const float o1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+                const float vi = odd ? o0 : g[4 * j + 0], vf = odd ? o1 : g[4 * j + 1];
+                const float vg = odd ? g[4 * j + 2] : o0, vo = odd ? g[4 * j + 3] : o1;
+                const int unit = 16 * c + 2 * j + (q >> 1);
+                const int col = 4 * unit;
+                const float4 bv = *reinterpret_cast<const float4*>(p.bias + col);
+                float pi = fmaf(vi, -1.4426950408889634f, bv.x * -1.4426950408889634f);
+                float pf = fmaf(vf, -1.4426950408889634f, bv.y * -1.4426950408889634f);
+                float pg = fmaf(vg, -2.8853900817779268f, bv.z * -2.8853900817779268f);
+                float po = fmaf(vo, -1.4426950408889634f, bv.w * -1.4426950408889634f);
+                if (L0) {
+#pragma unroll
+                    for (int cc = 0; cc < kC; ++cc)
+                        if (CIN == 1 || cc < p.c_in) {
+                            const float4 wv = *reinterpret_cast<const float4*>(&wih_s[cc * kGateCols + col]);
+                            pi = fmaf(xs[cc], wv.x, pi); pf = fmaf(xs[cc], wv.y, pf);
+                            pg = fmaf(xs[cc], wv.z, pg); po = fmaf(xs[cc], wv.w, po);
+                        }
+                }
+                const uint32_t o = bo + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
+                float cp = 0.f, dh = 0.f, dci = 0.f;
+                if (valid) {
+                    if (sp.c_prev) cp = sp.c_prev[o];
+                    if (sp.dh_in) dh = sp.dh_in[o];
+                    if (!sp.first) {
+                        dh += p.dh_rec[o];
+                        dci = p.dc[o];
+                    }
+                }
+                float gi, gf, gg, go, tc_;
+                lstm_cell_gates8(pi, pf, pg, po, cp, gi, gf, gg, go, tc_);
+                // rows past the end: dh = dci = 0, so dA = 0
+                const float dcv = fmaf(dh * go, 1.f - tc_ * tc_, dci);
+                const float da0 = dcv * gg * gi * (1.f - gi);
+                const float da1 = dcv * cp * gf * (1.f - gf);
+                const float da2 = dcv * gi * (1.f - gg * gg);
+                const float da3 = dh * tc_ * go * (1.f - go);
+                if (valid) p.dc[o] = dcv * gf;
+                if (L0) {
+#pragma unroll
+                    for (int cc = 0; cc < kC; ++cc)
+                        if (CIN == 1 || cc < p.c_in) {
+                            // W_ih is stored pre-scaled: undo -log2(e) (and the g gate's extra factor 2)
+                            const float4 wv = *reinterpret_cast<const float4*>(&wih_s[cc * kGateCols + col]);
+                            dxs[cc] = fmaf(da0 * wv.x + da1 * wv.y + 0.5f * (da2 * wv.z) + da3 * wv.w, -0.6931471805599453f, dxs[cc]);
+                        }
+                }
+                split_bf16x2(da0, da1, dhi[j], dlo[j]);
+                uint32_t h2, l2;
+                split_bf16x2(da2, da3, h2, l2);
+                const uint32_t off = row_in_tile * 128u + ((((uint32_t)j) ^ (row_in_tile & 7u)) << 4) + (uint32_t)(q >> 1) * 8u;
+                if (j == 0) cons_sync(kCons);                      // W / D / B of the previous chunk have read the dA tile
+                *reinterpret_cast<uint2*>(da_sm + off) = make_uint2(dhi[j], h2);
+                *reinterpret_cast<uint2*>(da_sm + kATileBytes + off) = make_uint2(dlo[j], l2);
+            }
+            fence_proxy_async_smem();
+            cons_sync(kCons);                                      // the dA tile (both row halves) is complete
+            // ---- W_c: dWp[kd rows 64 wg .., chunk] = A^T . dA_c ----
+            float wgr[32];
+#pragma unroll
+            for (int k = 0; k < 32; ++k) wgr[k] = 0.f;
+            float bgr[32];
+#pragma unroll
+            for (int k = 0; k < 32; ++k) bgr[k] = 0.f;
+            wg_fence_regs(wgr);
+            wg_fence_regs(bgr);
+            wg_fence_regs(dacc);
+            wg_fence();
+            {
+                const uint32_t wa_hi = a_u + (uint32_t)(wg * 2) * kATileBytes, wa_lo = wa_hi + kATileBytes;
 #pragma unroll
                 for (int ks = 0; ks < 8; ++ks) {
-                    mma_bf16_keep_a(d_wg, wg_hi + ks * kStepMN, wg_b + ks * kStepMN, idesc_wg, (PLANES == 2 || ks > 0) ? 1u : acc0);
-                    mma_bf16_reuse_a(d_wg, wg_hi + ks * kStepMN, wg_b + kTileEnc + ks * kStepMN, idesc_wg, 1u);
+                    const uint64_t ah = desc16_mn(wa_hi + ks * kStepMN, kATileBytes);
+                    const uint64_t al = desc16_mn(wa_lo + ks * kStepMN, kATileBytes);
+                    const uint64_t bh = desc16_mn(da_u + ks * kStepMN, kATileBytes);
+                    const uint64_t bl = desc16_mn(da_u + kATileBytes + ks * kStepMN, kATileBytes);
+                    // dA always has its lo plane; in the single-plane mode only the STORED operands are rounded to bf16
+                    wgmma_bf16_n64_t11(wgr, ah, bh, ks > 0 ? 1u : 0u);
+                    wgmma_bf16_n64_t11(wgr, ah, bl, 1u);
+                    if (PLANES == 2) wgmma_bf16_n64_t11(wgr, al, bh, 1u);
+                    // (both warpgroups issue it -- only warpgroup 0's result is used -- so that no wgmma sits on a
+                    // warpgroup-dependent branch, which would make ptxas serialise every wgmma of the kernel)
+                    wgmma_bf16_n64_rs_t1(bgr, ones, bh, ks > 0 ? 1u : 0u);
+                    wgmma_bf16_n64_rs_t1(bgr, ones, bl, 1u);
                 }
-                if (c == 3 && a_sync) mma_commit(&tail->ahi_empty[i & 1]);       // this tile's hi buffer may be refilled
-                // bias gradient on the tensor pipe: D[128 x 16] += dA_c^T (MN-major A, M = 64 columns of the hi plane | 64 of the
-                // lo plane: the two planes are the two 64-element atoms, LBO = one tile) . ones[K = 16 rows][16].  Lane m < 64 of
-                // the accumulator holds sum_rows hi(dA)[:, m], lane 64 + m the lo plane's sum; all 16 columns are equal.
-#pragma unroll
-                for (int ks = 0; ks < 8; ++ks)
-                    mma_bf16(t_db + (uint32_t)c * 16, wg_b + ks * kStepMN, db_b, idesc_db, (i > 0 || ks > 0) ? 1u : 0u);
-                mma_commit(&tail->d_empty);
             }
-            __syncwarp();
-            // ---- (3) tile boundary: the next tile's lo planes were requested when W_g's lo pass released the buffer ----
-            if (have_next && c == 3) {
-                if (PLANES == 2) {
-                    mbar_wait_p(&tail->alo_full, (uint32_t)(i + 1) & 1, 3);
-                    tc_fence_after();
+            // ---- D_c: [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T ----
+            {
+                const uint64_t ah = desc16_k(da_u + a_rows), al = desc16_k(da_u + kATileBytes + a_rows);
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    const uint32_t wb = w_u + (uint32_t)c * 8192u + (uint32_t)kk * kStepMN;
+                    const uint64_t bh = desc16_mn(wb, 2 * kWTileBytes), bl = desc16_mn(wb + kWTileBytes, 2 * kWTileBytes);
+                    if constexpr (kNseg == 2) {
+                        wgmma_bf16_n128_t01(dacc, ah + 2 * kk, bh, 1u);
+                        if (PLANES == 2) wgmma_bf16_n128_t01(dacc, ah + 2 * kk, bl, 1u);
+                        wgmma_bf16_n128_t01(dacc, al + 2 * kk, bh, 1u);
+                    } else {
+                        wgmma_bf16_n64_t01(dacc, ah + 2 * kk, bh, 1u);
+                        if (PLANES == 2) wgmma_bf16_n64_t01(dacc, ah + 2 * kk, bl, 1u);
+                        wgmma_bf16_n64_t01(dacc, al + 2 * kk, bh, 1u);
+                    }
                 }
-                if (leader) issue_r_lo_and_commit();
-                __syncwarp();
+            }
+            wg_commit();
+            wg_wait<0>();
+            wg_fence_regs(wgr);
+            wg_fence_regs(bgr);
+            wg_fence_regs(dacc);
+            // weight-gradient fragment -> this CTA's slice (row-major [kd][256]); bias sums: row 0 of warpgroup 0
+            {
+                const uint32_t m0 = rw0;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const uint32_t n = (uint32_t)(64 * c + 8 * j + 2 * q);
+                    red_add_f32x2(slice + (size_t)m0 * kGateCols + n, wgr[4 * j], wgr[4 * j + 1]);
+                    red_add_f32x2(slice + (size_t)(m0 + 8) * kGateCols + n, wgr[4 * j + 2], wgr[4 * j + 3]);
+                }
+                if (wg == 0 && m0 == 0) {
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        tail->db[64 * c + 8 * j + 2 * q] += bgr[4 * j];
+                        tail->db[64 * c + 8 * j + 2 * q + 1] += bgr[4 * j + 1];
+                    }
+                }
             }
         }
-        if (leader && n_items > 0) mma_commit(&tail->done);
-        __syncwarp();
-        TC_PROF_FLUSH(4, leader)
-    } else {
-        // ===================== compute warps =====================
-        TC_PROF_DECL
-        // TMEM lane quadrant q = warp & 3 (row 32q + lane of the tile), part = warp >> 2: units 4*part .. +3 of every chunk
-        const int q = warp & 3, part = warp >> 2;
-        const int ctid = tid;
-        (void)ctid;
-        float xs[kMaxC], xraw[kMaxC], dxs[kMaxC];
-        uint32_t dcount = 0, rcount = 0;
-        // raw inputs of one chunk: c_prev, dh_in, dh_rec, dc of this thread's 4 units
-        struct Raw { float4 cp, dhi, dhr, dcv; };
-        // tile-blocked workspaces: element (tile, row, unit) at tile*8192 + (unit/4)*512 + row*4 + unit%4
-        const uint32_t row_in_tile = (uint32_t)(q * 32 + lane);
-        const uint32_t rows32 = (uint32_t)p.rows;       // (rows <= 2^25 is checked on the host: 32-bit element offsets)
-        const uint32_t thr_off = row_in_tile * 4u + (uint32_t)part * 512u;
-        float xraw_next[kMaxC], sv_next = 0.f;      // layer 0: x and gate value of the next tile, loaded a chunk ahead
-        // layer 0: when b_inner divides the tile height, a thread's row belongs to the same window b in every tile: its share
-        // of d_s is summed in a register and added once (one shared-memory float atomic = a CAS loop; 16 per address and tile
-        // were 6 % of the layer-0 kernel's stall samples)
-        const bool ds_fixed = L0 && (kTileM % (uint32_t)p.b_inner) == 0u;
-        const bool ds_smem = L0 && (int64_t)p.n_steps * p.b_inner <= kBSgMax;    // s_ds holds [step][window]
-        float ds_acc = 0.f;
-        // (st, tile): step index and tile of a work item; a step index >= n_steps marks "no such item"
-        auto load_x = [&](int st, int tile_n) {
-            const uint32_t rn = (uint32_t)tile_n * kTileM + row_in_tile;
-            const bool ok = st < p.n_steps && rn < rows32;
-            const uint32_t t = ok ? (uint32_t)p.steps[st].t : 0u;
-            sv_next = 0.f;
-            if (ok) sv_next = p.sg[(rn % (uint32_t)p.b_inner) * (uint32_t)p.t_len + t];      // (32-bit: a 64-bit % is a call)
+        // the A planes of this item have been read by every MMA: one arrival per warpgroup
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+        if ((tid & 127) == 0) mbar_arrive(&tail->a_empty);
+        // ---- [dx_below | dh_prev] fragment -> tile-blocked workspaces ----
 #pragma unroll
-            for (int c = 0; c < kMaxC; ++c)
-                xraw_next[c] = (c < kC && ok && (CIN == 1 || c < p.c_in)) ? p.xo[((int64_t)rn * p.t_len + t) * p.c_in + c] : 0.f;
-        };
-        auto load_raw = [&](int st, int tile, int c, Raw& rw) {
-            const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
-            const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-            rw.cp = rw.dhi = rw.dhr = rw.dcv = z;
-            if (st < p.n_steps && r < rows32) {
-                const Bwd16Step& sp = p.steps[st];
-                const uint32_t o = (uint32_t)tile * 8192u + (uint32_t)c * 2048u + thr_off;
-                if (sp.c_prev) rw.cp = *reinterpret_cast<const float4*>(sp.c_prev + o);
-                if (sp.dh_in) rw.dhi = *reinterpret_cast<const float4*>(sp.dh_in + o);
-                if (!sp.first) {
-                    rw.dhr = *reinterpret_cast<const float4*>(p.dh_rec + o);
-                    rw.dcv = *reinterpret_cast<const float4*>(p.dc + o);
-                }
-            }
-        };
-        // [dx_below | dh_prev] of work item w_prev (step st_prev, tile tile_prev): TMEM -> tile-blocked workspaces
-        auto drain = [&](int w_prev, int st_prev, int tile_prev) {
-            const uint32_t r = (uint32_t)tile_prev * kTileM + row_in_tile;
-            const Bwd16Step& sp = p.steps[st_prev];
-            mbar_wait(&tail->g_full, (uint32_t)w_prev & 1, 2);
-            tc_fence_after();
-            constexpr int ncols = 64 * kNseg;
-            if (part * 32 < ncols) {
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + kDgCol + (uint32_t)part * 32, v);
-                tmem_ld_wait();
-                const int col = part * 32;
+        for (int h = 0; h < 2; ++h) {
+            const uint32_t rr = rw0 + 8u * h;
+            if ((uint32_t)tile * kTileM + rr >= rows32) continue;
+#pragma unroll
+            for (int j = 0; j < 8 * kNseg; ++j) {
+                const int col = 8 * j + 2 * q;
                 // layers > 0: columns [0,64) = dx_below, [64,128) = dh_prev; layer 0: [0,64) = dh_prev
                 const bool is_dx = !L0 && col < 64;
                 float* base = is_dx ? sp.dx_out : p.dh_rec;
-                const int unit0 = col & 63;
-                if (r < rows32 && base != nullptr && (is_dx || sp.store_dh)) {
-                    const uint32_t o = (uint32_t)tile_prev * 8192u + row_in_tile * 4u + (uint32_t)(unit0 >> 2) * 512u;
-#pragma unroll
-                    for (int k = 0; k < 8; ++k)          // units unit0 + 4k .. +3: the warp writes one contiguous 512-byte run
-                        *reinterpret_cast<uint4*>(base + (o + (uint32_t)k * 512u)) = make_uint4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-                }
+                if (base == nullptr || !(is_dx || sp.store_dh)) continue;
+                const int unit = col & 63;
+                *reinterpret_cast<float2*>(base + (uint32_t)tile * 8192u + (uint32_t)(unit >> 2) * 512u + rr * 4u + (uint32_t)(unit & 3)) =
+                    make_float2(dacc[4 * j + 2 * h], dacc[4 * j + 2 * h + 1]);
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tail->g_empty);
-        };
-        Raw cur, nxt;              // (measured and rejected: loading two chunks ahead -- the 16 extra registers at the 96-register
-                                   //  cap cost more than the covered latency gained: 8.43 -> 8.68 ms per branch)
-        const int gstep = (int)gridDim.x;
-        // work items in step-major order: (st, i) = (step index, this CTA's i-th tile); (st_n, tile_n) = the item after it
-        int st = 0, i = 0, tile = (int)blockIdx.x;
-        if (n_items == 0) st = p.n_steps;
-        load_raw(st, tile, 0, nxt);
-        if (L0) load_x(st, tile);
-        for (int w = 0; w < n_items; ++w) {
-            const bool last_of_step = (i + 1 == my_tiles);
-            const int st_n = last_of_step ? st + 1 : st;
-            const int tile_n = last_of_step ? (int)blockIdx.x : tile + gstep;
-            const int st_p = (i == 0) ? st - 1 : st;                                   // the item before this one
-            const int tile_p = (i == 0) ? (int)blockIdx.x + (my_tiles - 1) * gstep : tile - gstep;
-            const Bwd16Step& sp = p.steps[st];
-            const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
-            const bool valid = r < rows32;
-            if (L0) {
-#pragma unroll
-                for (int c = 0; c < kMaxC; ++c) {
-                    xraw[c] = xraw_next[c];
-                    xs[c] = xraw[c] * sv_next;
-                    dxs[c] = 0.f;
-                }
-            }
-            // (the drain sits in the tile-boundary bubble: the first recompute of this tile cannot finish before the lo planes
-            // have been reloaded; moved behind chunk 0 it cost 2.3 k cycles of real time per tile, measured)
-            if (w > 0) drain(w - 1, st_p, tile_p);
-            if (i == 0 && w > 0) {
-                // step boundary: this step reads the dh_rec the CTA's own drains wrote during the previous step (other threads'
-                // stores): a barrier of the 512 compute threads orders them, and the first chunk's inputs -- not prefetched
-                // across the boundary (with one tile per CTA they did not exist yet) -- are loaded behind it
-                asm volatile("bar.sync 1, %0;" ::"n"(kBCompWarps * 32) : "memory");
-                load_raw(st, tile, 0, nxt);
-            }
-            if (have_aux && part == 0) {
-                // auxiliary weight-gradient operand: the seg-1 slot of this tile's hi buffer and of the lo buffer; row = this
-                // thread's row, columns 0..C-1 = x*s (hi / lo split)
-                if (w >= 2) mbar_wait(&tail->ahi_empty[w & 1], (uint32_t)((w >> 1) - 1) & 1, 3);
-                uint32_t hi[2], lo[2];
-                split_bf16x2(xs[0], xs[1], hi[0], lo[0]);
-                split_bf16x2(xs[2], xs[3], hi[1], lo[1]);
-                const uint32_t row = (uint32_t)(q * 32 + lane);
-                const uint32_t off = row * 128u + ((0u ^ (row & 7u)) << 4);
-                *reinterpret_cast<uint4*>(a_sm + (size_t)((w & 1) * 2 + 1) * kATileBytes + off) = make_uint4(hi[0], hi[1], 0u, 0u);
-                if (PLANES == 2) {
-                    if (w >= 1) mbar_wait(&tail->alo_empty, (uint32_t)(w - 1) & 1, 3);
-                    *reinterpret_cast<uint4*>(a_sm + (size_t)5 * kATileBytes + off) = make_uint4(lo[0], lo[1], 0u, 0u);
-                }
-            }
-            for (int c = 0; c < 4; ++c, ++dcount) {
-                cur = nxt;
-                uint32_t v[16];
-                {
-                    mbar_wait(&tail->r_full, rcount & 1, c == 0 ? 3 : 1);      // (profile builds: class 3 = first chunk of a tile)
-                    tc_fence_after();
-                    tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + kRcCol + (uint32_t)part * 16, v);
-                    tmem_ld_wait();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tail->r_empty);
-                    ++rcount;
-                }
-                const int unit0 = 16 * c + 4 * part;
-                const float cp[4] = {cur.cp.x, cur.cp.y, cur.cp.z, cur.cp.w};
-                const float dhi[4] = {cur.dhi.x, cur.dhi.y, cur.dhi.z, cur.dhi.w};
-                const float dhr[4] = {cur.dhr.x, cur.dhr.y, cur.dhr.z, cur.dhr.w};
-                const float dci[4] = {cur.dcv.x, cur.dcv.y, cur.dcv.z, cur.dcv.w};
-                float da[16], dcn[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int col = 4 * (unit0 + u);
-                    const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
-                    float pi = fmaf(__uint_as_float(v[4 * u + 0]), -1.4426950408889634f, bv.x);
-                    float pf = fmaf(__uint_as_float(v[4 * u + 1]), -1.4426950408889634f, bv.y);
-                    float pg = fmaf(__uint_as_float(v[4 * u + 2]), -2.8853900817779268f, bv.z);
-                    float po = fmaf(__uint_as_float(v[4 * u + 3]), -1.4426950408889634f, bv.w);
-                    if (L0) {
-#pragma unroll
-                        for (int cc = 0; cc < kC; ++cc)
-                            if (CIN == 1 || cc < p.c_in) {
-                                const float4 wv = *reinterpret_cast<const float4*>(&tail->wih[cc * kGateCols + col]);
-                                pi = fmaf(xs[cc], wv.x, pi); pf = fmaf(xs[cc], wv.y, pf);
-                                pg = fmaf(xs[cc], wv.z, pg); po = fmaf(xs[cc], wv.w, po);
-                            }
-                    }
-                    float gi, gf, gg, go, tc_;
-                    lstm_cell_gates8(pi, pf, pg, po, cp[u], gi, gf, gg, go, tc_);
-                    // rows past the end: load_raw returned zeros for dh_rec / dh_in / dc, so dh = dcv = 0 and dA = 0 without selects
-                    const float dh = dhr[u] + dhi[u];
-                    const float dcv = fmaf(dh * go, 1.f - tc_ * tc_, dci[u]);
-                    da[4 * u + 0] = dcv * gg * gi * (1.f - gi);
-                    da[4 * u + 1] = dcv * cp[u] * gf * (1.f - gf);
-                    da[4 * u + 2] = dcv * gi * (1.f - gg * gg);
-                    da[4 * u + 3] = dh * tc_ * go * (1.f - go);
-                    dcn[u] = dcv * gf;
-                    if (L0) {
-#pragma unroll
-                        for (int cc = 0; cc < kC; ++cc)
-                            if (CIN == 1 || cc < p.c_in) {
-                                // W_ih is stored pre-scaled: undo -log2(e) (and the g gate's extra factor 2)
-                                const float4 wv = *reinterpret_cast<const float4*>(&tail->wih[cc * kGateCols + col]);
-                                dxs[cc] = fmaf(da[4 * u] * wv.x + da[4 * u + 1] * wv.y + 0.5f * (da[4 * u + 2] * wv.z) + da[4 * u + 3] * wv.w,
-                                               -0.6931471805599453f, dxs[cc]);
-                            }
-                    }
-                }
-                // dA chunk -> bf16 planes, 128-byte-swizzled tile: row = this thread's row, columns 16*part .. +15
-                uint32_t hi[8], lo[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) split_bf16x2(da[2 * j], da[2 * j + 1], hi[j], lo[j]);
-                if (dcount > 0) mbar_wait(&tail->d_empty, (dcount - 1) & 1, 0);     // W_{c-1}, D_{c-1} have read the dA tile
-                {
-                    const uint32_t row = (uint32_t)(q * 32 + lane);
-                    const uint32_t o0 = row * 128u + ((((uint32_t)(2 * part)) ^ (row & 7u)) << 4);
-                    const uint32_t o1 = row * 128u + ((((uint32_t)(2 * part + 1)) ^ (row & 7u)) << 4);
-                    *reinterpret_cast<uint4*>(da_sm + o0) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                    *reinterpret_cast<uint4*>(da_sm + o1) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-                    *reinterpret_cast<uint4*>(da_sm + kATileBytes + o0) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                    *reinterpret_cast<uint4*>(da_sm + kATileBytes + o1) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                }
-                fence_proxy_async_smem();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tail->d_full);
-                // next chunk's inputs: issued AFTER the proxy fence -- fence.proxy.async implies MEMBAR.ALL.CTA, which waits for
-                // every outstanding load of the thread, so a prefetch issued before it is simply waited for at the fence
-                if (c < 3) load_raw(st, tile, c + 1, nxt);
-                else {
-                    // (across a step boundary the first chunk is loaded behind the step's barrier, see above)
-                    if (!last_of_step) load_raw(st_n, tile_n, 0, nxt);
-                    if (L0) load_x(st_n, tile_n);
-                }
-                if (valid)
-                    *reinterpret_cast<float4*>(p.dc + ((uint32_t)tile * 8192u + (uint32_t)c * 2048u + thr_off)) =
-                        make_float4(dcn[0], dcn[1], dcn[2], dcn[3]);
-            }
-            if (L0 && valid) {
-                // gate adjoint: d s[b, t] += sum_c dxmod[r, c] * xo[r, t, c]   (STMGCN.py:44)
-                float contrib = 0.f;
-#pragma unroll
-                for (int cc = 0; cc < kC; ++cc) contrib += dxs[cc] * xraw[cc];
-                if (ds_fixed) {
-                    ds_acc += contrib;
-                } else {
-                    const int64_t b = (int64_t)(r % (uint32_t)p.b_inner);
-                    if (ds_smem) atomicAdd(&tail->s_ds[(int64_t)st * p.b_inner + b], contrib);
-                    else atomicAdd(&p.d_s[b * p.t_len + sp.t], contrib);
-                }
-            }
-            if (L0 && ds_fixed && last_of_step) {       // this thread's share of d_s[b, t] for the step that ends here
-                const int64_t b = (int64_t)(row_in_tile % (uint32_t)p.b_inner);
-                if (ds_smem) atomicAdd(&tail->s_ds[(int64_t)st * p.b_inner + b], ds_acc);
-                else atomicAdd(&p.d_s[b * p.t_len + sp.t], ds_acc);
-                ds_acc = 0.f;
-            }
-            // next work item
-            if (last_of_step) { st = st + 1; i = 0; tile = (int)blockIdx.x; }
-            else { ++i; tile += gstep; }
         }
-        if (n_items > 0) drain(n_items - 1, p.n_steps - 1, (int)blockIdx.x + (my_tiles - 1) * gstep);
-        TC_PROF_FLUSH(3, tid == 0)
-        // ---- weight-gradient accumulator -> this CTA's scratch slice (register layout: [part][piece][vec][row m][4]) ----
-        if (n_items > 0) {
-            mbar_wait_raw(&tail->done, 0);
-            tc_fence_after();
-            float* slice = p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols);
-            const int m = q * 32 + lane;
-            if (part == 0) {                       // bias gradient: lanes [0,64) hold the hi-plane sums, [64,128) the lo-plane sums
-                uint32_t v[16];
-#pragma unroll 1
-                for (int c = 0; c < 4; ++c) {
-                    tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + kDbCol + (uint32_t)c * 16, v);
-                    tmem_ld_wait();
-                    atomicAdd(&p.dbp[64 * c + (m & 63)], __uint_as_float(v[0]));
-                }
-            }
-#pragma unroll 1
-            for (int j = 0; j < 4; ++j) {
-                uint32_t v[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + kWgCol + (uint32_t)part * 64 + (uint32_t)j * 16, v);
-                tmem_ld_wait();
+        if (L0) {
+            // gate adjoint: d s[b, t] += sum_c dxmod[r, c] * xo[r, t, c]   (STMGCN.py:44); this thread has half the row's units
+            float contrib = 0.f;
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    float4* dst = reinterpret_cast<float4*>(slice + ((size_t)((part * 4 + j) * 4 + e) * kTileM + m) * 4);
-                    float4 acc = make_float4(__uint_as_float(v[4 * e]), __uint_as_float(v[4 * e + 1]), __uint_as_float(v[4 * e + 2]),
-                                             __uint_as_float(v[4 * e + 3]));
-                    // later launches of the layer add with a fire-and-forget vector reduction (the slice is private to this
-                    // CTA: no contention, no read latency at the end of the launch)
-                    if (p.dw_first) *dst = acc;
-                    else red_add_f32x4(dst, acc);
-                }
+            for (int cc = 0; cc < kC; ++cc) contrib += dxs[cc] * xraw[cc];
+            contrib += __shfl_xor_sync(0xffffffffu, contrib, 2);
+            if ((q >> 1) == 0 && valid) {
+                if (ds_fixed) ds_acc += contrib;
+                else atomicAdd(&p.d_s[(int64_t)(r % (uint32_t)p.b_inner) * p.t_len + sp.t], contrib);
+            }
+            if (ds_fixed && last_of_step) {
+                if ((q >> 1) == 0 && ds_acc != 0.f)
+                    atomicAdd(&p.d_s[(int64_t)(row_in_tile % (uint32_t)p.b_inner) * p.t_len + sp.t], ds_acc);
+                ds_acc = 0.f;
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == kMmaWarp) tmem_dealloc(tmem_base, 512);
-    if (L0 && (int64_t)p.n_steps * p.b_inner <= kBSgMax)
-        for (int e = tid; e < p.n_steps * (int)p.b_inner; e += kBThreads) {
-            const int st = e / (int)p.b_inner, b = e - st * (int)p.b_inner;
-            atomicAdd(&p.d_s[(int64_t)b * p.t_len + p.steps[st].t], tail->s_ds[e]);
-        }
+    cons_sync(kCons);
+    for (int i = tid; i < kGateCols; i += kCons)
+        if (n_items > 0) atomicAdd(&p.dbp[i], tail->db[i]);
 }
 
 // Sum the per-CTA weight-gradient slices of one layer and write nn.LSTM-native gradients:
 //   d_w_ih (256, in), d_w_hh (256, 64), d_b_ih = d_b_hh (256); native row of gate-interleaved column n: (n & 3) * 64 + (n >> 2).
-// Accumulator row m = kd index: layers > 0: m < 64 -> W_ih[:, m], m >= 64 -> W_hh[:, m - 64]; layer 0: m < 64 -> W_hh[:, m],
+// Slice row m = kd index: layers > 0: m < 64 -> W_ih[:, m], m >= 64 -> W_hh[:, m - 64]; layer 0: m < 64 -> W_hh[:, m],
 // m = 64 + c -> W_ih[:, c].
 __global__ void lstm16_wgrad_reduce_kernel(const float* __restrict__ slices, int n_slices, int layer, int c_in,
                                            const float* __restrict__ dbp, float* __restrict__ d_w_ih,
@@ -1111,8 +699,7 @@ __global__ void lstm16_wgrad_reduce_kernel(const float* __restrict__ slices, int
     if (e < kTileM * kGateCols) {
         float s = 0.f;
         for (int i = 0; i < n_slices; ++i) s += slices[(size_t)i * (kTileM * kGateCols) + e];
-        const int x = e & 3, m = (e >> 2) & 127, rest = e >> 9;    // rest = (part*4 + j)*4 + vec
-        const int n = (rest >> 2) * 16 + (rest & 3) * 4 + x;       // gate-interleaved column
+        const int m = e / kGateCols, n = e % kGateCols;
         const int nat = (n & 3) * kHid + (n >> 2);
         if (layer > 0) {
             if (m < 64) d_w_ih[(size_t)nat * kHid + m] = s;
@@ -1316,19 +903,15 @@ extern "C" int32_t stmgcn_lstm16_layer_bwd(int32_t layer, int32_t t_len, int32_t
     p.dbp = dbp;
     p.dw_slice = dw_scratch;
     p.rows = rows;
+    // every CTA adds into its own slice: start from zero
+    STMGCN_CUDA(cudaMemsetAsync(dw_scratch, 0, (size_t)grid * kTileM * kGateCols * sizeof(float), st));
     p.n_tiles = n_tiles;
-    // Steps per launch: the weight-gradient accumulator of a CTA lives in TMEM for the whole launch, and the tensor core's fp32
-    // accumulation loses precision with the length of the chain (all T steps of cfg5's 7 tiles per CTA = 21.5 k rows in one
-    // chain put 1.3e-4 into the LSTM weight gradients, measured; per-step launches, 1.8 k rows: 1.4e-5).  A launch therefore
-    // covers at most kMaxChainItems (step, tile) items per CTA; the slices are summed across launches in fp32 memory.
-    constexpr int kMaxChainItems = 48;                             // 6144 rows per accumulation chain
-    const int tiles_per_cta = (int)ceil_div(n_tiles, grid);
-    int steps_per_launch = kMaxChainItems / tiles_per_cta;
-    if (steps_per_launch < 1) steps_per_launch = 1;
+    // one launch covers all timesteps of the layer (t_len <= kBMaxSteps); the weight-gradient partials of every chunk are
+    // added into fp32 memory, so the length of the run does not lengthen any tensor-core accumulation chain
+    const int steps_per_launch = t_len;
     for (int s0 = 0; s0 < t_len; s0 += steps_per_launch) {
         const int ns_launch = (t_len - s0 < steps_per_launch) ? (t_len - s0) : steps_per_launch;
         p.n_steps = ns_launch;
-        p.dw_first = (s0 == 0) ? 1 : 0;
         for (int sj = 0; sj < ns_launch; ++sj) {
             const int si = s0 + sj;
             const int t = t_len - 1 - si;
@@ -1373,16 +956,3 @@ extern "C" int32_t stmgcn_lstm16_wgrad_reduce(int32_t layer, int32_t c_in, int32
     count_launch();
     return check_launch("lstm16_wgrad_reduce");
 }
-
-#ifdef STMGCN_TC_PROFILE
-// per-role wait accounting of THIS translation unit's kernels (see tc_common.cuh); instrumented builds only
-extern "C" int32_t stmgcn_dbg_tc_prof16(unsigned long long* host_out, int32_t reset) {
-    cudaDeviceSynchronize();
-    cudaMemcpyFromSymbol(host_out, stmgcn::tc::g_tc_prof, sizeof(unsigned long long) * 64);
-    if (reset) {
-        unsigned long long z[64] = {0};
-        cudaMemcpyToSymbol(stmgcn::tc::g_tc_prof, z, sizeof(z));
-    }
-    return 0;
-}
-#endif

@@ -195,7 +195,7 @@ int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     STMGCN_REQUIRE(rows > 0 && p > 0 && q > 0, STMGCN_ERR_SHAPE, "proj_fwd: bad shape");
     STMGCN_REQUIRE(act == STMGCN_ACT_NONE || act == STMGCN_ACT_RELU, STMGCN_ERR_ARG, "proj_fwd: act=%d", act);
     cudaStream_t st = (cudaStream_t)stream;
-    if (wimg && !pool && proj_tc_applicable(ks, p, q, s, out, nullptr) && stride_k % 4 == 0)   // tcgen05 path (proj_tc.cu)
+    if (wimg && !pool && proj_tc_applicable(ks, p, q, s, out, nullptr) && stride_k % 4 == 0)   // wgmma path (proj_tc.cu)
         return launch_proj_fwd_tc(s, stride_k, ks, rows, wimg, bias, act, out, st);
     ASegs a{};
     a.nseg = ks;
@@ -238,7 +238,7 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     cudaStream_t st = (cudaStream_t)stream;
     if (wimg_t && u && d_out && proj_tc_applicable(ks, p, q, s, out, d_out) && aligned16(dz_work) && aligned16(u) &&
         stride_k % 4 == 0 && stride_u % 4 == 0) {
-        // tcgen05 path: dZ + bias gradient + U in one kernel, then dW per 128-row block of W (proj_tc.cu, lstm_tc.cu)
+        // wgmma path: dZ + bias gradient + U in one kernel, then dW per 128-row block of W (proj_tc.cu, wgrad_tc.cu)
         // U has 64*ks columns; one launch produces up to 256 of them (supports 0..3), a second one the rest (it re-forms
         // dZ in its loader but neither stores it nor accumulates the bias gradient again)
         if (int32_t rc = launch_proj_bwd_tc(d_out, out, act, rows, ks < 4 ? ks : 4, wimg_t, dz_work, dbias, u, stride_u, st)) return rc;

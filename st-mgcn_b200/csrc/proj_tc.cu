@@ -1,10 +1,14 @@
-// K2 on the 5th-gen tensor cores (p = q = 64, the reference's lstm_hidden_dim / gcn_hidden_dim, Main.py:62-63):
+// K2 on the Hopper tensor cores (p = q = 64, the reference's lstm_hidden_dim / gcn_hidden_dim, Main.py:62-63):
 //   forward : out[128 x 64]  = act( [T_0X | T_1X | ... | T_KX][128 x Ks*64] . W[Ks*64 x 64] + b )   (GCN.py:37-42)
 //             -- the A operand is read segment by segment straight from the Chebyshev stack the SpMM steps wrote
-//             (no torch.cat), split to tf32 hi/lo in the loader, accumulated in TMEM (3xTF32, tc_common.cuh)
+//             (no torch.cat), split to tf32 hi/lo on its way to shared memory, accumulated in registers by wgmma
+//             (3xTF32, tc_common.cuh)
 //   backward: dZ = dOut (.) [out > 0] is formed in the loader (and written out for the weight-gradient kernel, with
 //             the bias gradient as a by-product);  U[128 x Ks*64] = dZ[128 x 64] . W^T  -> U_k segments
-// Same CTA anatomy as lstm_tc.cu: 8 loader warps (register ping-pong), 1 MMA warp, 4 or 8 epilogue warps.
+// CTA = two warpgroups, one 128-row tile at a time (persistent over tiles); warpgroup w owns rows 64w .. 64w+63 of the
+// tile.  Per 32-wide k-block every thread loads its share of A (and the pre-packed weight image), the block stores both
+// into one shared-memory stage, and each warpgroup issues 3 x 4 wgmma (k8) into its accumulator; the global loads of
+// the next k-block are in flight while those run.
 #include "tc_pipeline.cuh"
 
 using namespace stmgcn;
@@ -12,27 +16,22 @@ using namespace stmgcn::tc;
 
 namespace {
 
-constexpr int kPLoaderWarps = 8;
-constexpr int kPLoaders = kPLoaderWarps * 32;
+constexpr int kPThreads = 256;
+constexpr int kPWarps = kPThreads / 32;
 constexpr int kMaxSeg = 8;
 
 template <int N>
 struct PCfg {
-    static constexpr int kEpiWarps = (N == 64) ? 4 : 8;
-    static constexpr int kThreads = (kEpiWarps + kPLoaderWarps + 1) * 32;
     static constexpr int kBBytes = N * kKB * 4;
     static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
-    static constexpr int kStages = (N == 64) ? 4 : 2;
-    static constexpr int kTmemCols = (2 * N < 32) ? 32 : 2 * N;
 };
 
 struct PTail {
     float bias[64];
-    float s_db[kPLoaderWarps][64];
-    Barriers bar;
+    float s_db[kPWarps][64];
 };
 template <int N>
-constexpr size_t psmem() { return 1024 + (size_t)PCfg<N>::kStages * PCfg<N>::kStageBytes + sizeof(PTail); }
+constexpr size_t psmem() { return 1024 + (size_t)PCfg<N>::kStageBytes + sizeof(PTail); }
 
 struct PParams {
     const float* seg[kMaxSeg];   // forward: A segments (rows x 64)
@@ -53,45 +52,56 @@ struct PParams {
     int n_tiles;
 };
 
+template <int N>
+__device__ __forceinline__ void proj_mma(float (&acc)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                         bool first) {
+#pragma unroll
+    for (int pass = 0; pass < 3; ++pass) {
+        const uint64_t da = smem_desc_k_sw128(pass == 1 ? a_lo : a_hi);
+        const uint64_t db = smem_desc_k_sw128(pass == 2 ? b_lo : b_hi);
+#pragma unroll
+        for (int k = 0; k < kKB / 8; ++k) {
+            const uint32_t sc = (!first || pass > 0 || k > 0) ? 1u : 0u;
+            if constexpr (N == 64) wgmma_tf32_n64(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), sc);
+            else wgmma_tf32_n256(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), sc);
+        }
+    }
+}
+
 template <int N, bool DZ>
-__global__ void __launch_bounds__(PCfg<N>::kThreads, 1) proj_rows_tc_kernel(const __grid_constant__ PParams p) {
+__global__ void __launch_bounds__(kPThreads, 1) proj_rows_tc_kernel(const __grid_constant__ PParams p) {
     using Cfg = PCfg<N>;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // keeps the __shared__ address space (LDS/STS, not generic LD/ST)
-    PTail* tail = (PTail*)(smem + (size_t)Cfg::kStages * Cfg::kStageBytes);
-    Barriers* bar = &tail->bar;
+    uint8_t* st = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // keeps the __shared__ address space
+    PTail* tail = (PTail*)(st + (size_t)Cfg::kStageBytes);
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const int lane = tid & 31;
-    constexpr int kMmaWarp = Cfg::kEpiWarps + kPLoaderWarps;
+    const int wg = tid >> 7;                             // warpgroup: rows 64 wg .. 64 wg + 63 of the tile
 
-    if (tid == 0) init_barriers(bar, Cfg::kStages, Cfg::kEpiWarps * 32, kPLoaders / 2);   // one loader group per k-block
-    if (warp == kMmaWarp) tmem_alloc(&bar->tmem_base, Cfg::kTmemCols);
-    for (int i = tid; i < 64; i += Cfg::kThreads) tail->bias[i] = (!DZ && p.bias) ? p.bias[i] : 0.f;
-    for (int i = tid; i < kPLoaderWarps * 64; i += Cfg::kThreads) (&tail->s_db[0][0])[i] = 0.f;
-    tc_fence_before();
+    for (int i = tid; i < 64; i += kPThreads) tail->bias[i] = (!DZ && p.bias) ? p.bias[i] : 0.f;
+    for (int i = tid; i < kPWarps * 64; i += kPThreads) (&tail->s_db[0][0])[i] = 0.f;
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = bar->tmem_base;
 
-    if (warp >= Cfg::kEpiWarps && warp < kMmaWarp) {
-        // ===================== loaders: two groups alternate k-blocks (see lstm_tc.cu on the proxy fence) ==========
-        TC_PROF_DECL
-        constexpr int kGroups = 2, kGT = kPLoaders / kGroups, kPer = 1024 / kGT;
-        const int ltid = tid - Cfg::kEpiWarps * 32;
-        const int grp = ltid / kGT, gtid = ltid % kGT;
-        const int c = gtid & 7, rsub = gtid >> 3, lwarp = ltid >> 5;
-        const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-        const int total = my_tiles * p.nkb;
-        for (int j = grp; j < total; j += kGroups) {
-            const int tile = blockIdx.x + (j / p.nkb) * gridDim.x, kb = j % p.nkb;
+    constexpr int kPer = 1024 / kPThreads;               // float4 of the 128 x 32 A block per thread
+    constexpr int kBVec = 2 * Cfg::kBBytes / 16 / kPThreads;
+    const int c = tid & 7, rsub = tid >> 3;
+    const uint32_t s_u = smem_u32(st);
+    const uint32_t a_hi = s_u + (uint32_t)wg * 64u * 128u, a_lo = a_hi + kABytes;
+    const uint32_t b_hi = s_u + 2 * kABytes, b_lo = b_hi + Cfg::kBBytes;
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+
+    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+        for (int kb = 0; kb < p.nkb; ++kb) {
             const int koff = (kb & 1) * kKB + c * 4;
             float4 v[kPer];
             if (DZ) {
                 float4 sb = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
                 for (int i = 0; i < kPer; ++i) {
-                    const int64_t r = (int64_t)tile * kTileM + rsub + (kGT / 8) * i;
+                    const int64_t r = (int64_t)tile * kTileM + rsub + 32 * i;
                     float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
                     if (r < p.rows) {
                         d = *reinterpret_cast<const float4*>(p.d_out + r * 64 + koff);
@@ -112,106 +122,77 @@ __global__ void __launch_bounds__(PCfg<N>::kThreads, 1) proj_rows_tc_kernel(cons
                     sb.z += __shfl_xor_sync(0xffffffffu, sb.z, o); sb.w += __shfl_xor_sync(0xffffffffu, sb.w, o);
                 }
                 if (lane < 8) {
-                    float4* acc = reinterpret_cast<float4*>(&tail->s_db[lwarp][koff]);
-                    float4 t = *acc;
+                    float4* a = reinterpret_cast<float4*>(&tail->s_db[warp][koff]);
+                    float4 t = *a;
                     t.x += sb.x; t.y += sb.y; t.z += sb.z; t.w += sb.w;
-                    *acc = t;
+                    *a = t;
                 }
             } else {
                 const float* seg = p.seg[kb >> 1];
 #pragma unroll
                 for (int i = 0; i < kPer; ++i) {
-                    const int64_t r = (int64_t)tile * kTileM + rsub + (kGT / 8) * i;
+                    const int64_t r = (int64_t)tile * kTileM + rsub + 32 * i;
                     v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
                     if (seg != nullptr && r < p.rows) v[i] = *reinterpret_cast<const float4*>(seg + r * 64 + koff);
                 }
             }
-            const int s = j % Cfg::kStages;
-            const uint32_t ph = (j / Cfg::kStages) & 1;
-            mbar_wait(&bar->empty[s], ph ^ 1, 0);
-            uint8_t* st = smem + (size_t)s * Cfg::kStageBytes;
-            if (gtid == 0) {
-                mbar_arrive_expect_tx(&bar->full[s], 2 * Cfg::kBBytes);
-                const float* src = p.wimg + (size_t)kb * (2 * Cfg::kBBytes / 4);
-                bulk_g2s(st + 2 * kABytes, src, Cfg::kBBytes, &bar->full[s]);
-                bulk_g2s(st + 2 * kABytes + Cfg::kBBytes, src + Cfg::kBBytes / 4, Cfg::kBBytes, &bar->full[s]);
-            }
+            const uint4* wsrc = reinterpret_cast<const uint4*>(p.wimg + (size_t)kb * (2 * Cfg::kBBytes / 4));
+            uint4 wv[kBVec];
+#pragma unroll
+            for (int i = 0; i < kBVec; ++i) wv[i] = wsrc[tid + i * kPThreads];
+            wg_wait<0>();                                     // this warpgroup's MMAs of the previous k-block are done
+            __syncthreads();                                  // ... and the other warpgroup's: the stage may be overwritten
 #pragma unroll
             for (int i = 0; i < kPer; ++i) {
-                const int row = rsub + (kGT / 8) * i;
+                const int row = rsub + 32 * i;
                 split_store(st, (uint32_t)row * 128u + (uint32_t)((c ^ (row & 7)) << 4), v[i]);
             }
+#pragma unroll
+            for (int i = 0; i < kBVec; ++i) reinterpret_cast<uint4*>(st + 2 * kABytes)[tid + i * kPThreads] = wv[i];
             fence_proxy_async_smem();
-            mbar_arrive(&bar->full[s]);
-            if (DZ) {          // dZ tape for the weight-gradient kernel, stored after the hand-off (see lstm_tc.cu)
+            __syncthreads();
+            wg_fence_regs(acc);
+            wg_fence();
+            proj_mma<N>(acc, a_hi, a_lo, b_hi, b_lo, kb == 0);
+            wg_commit();
+            if (DZ && p.dz_out != nullptr) {   // dZ tape for the weight-gradient kernel
 #pragma unroll
                 for (int i = 0; i < kPer; ++i) {
-                    const int64_t r = (int64_t)tile * kTileM + rsub + (kGT / 8) * i;
-                    if (r < p.rows && p.dz_out != nullptr) *reinterpret_cast<float4*>(p.dz_out + r * 64 + koff) = v[i];
+                    const int64_t r = (int64_t)tile * kTileM + rsub + 32 * i;
+                    if (r < p.rows) *reinterpret_cast<float4*>(p.dz_out + r * 64 + koff) = v[i];
                 }
             }
         }
-        TC_PROF_FLUSH(11, ltid == 0)
-    } else if (warp == kMmaWarp) {
-        mma_issuer<N, Cfg::kStages, 4>(bar, smem, Cfg::kStageBytes, Cfg::kBBytes, p.nkb, p.n_tiles, tmem_base, lane);
-    } else {
-        // ===================== epilogue =====================
-        TC_PROF_DECL
-        const int q = warp & 3, part = warp >> 2;          // N = 256: two column halves
-        uint32_t tcount = 0;
-        for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x, ++tcount) {
-            const int a = tcount & 1;
-            const uint32_t aph = (tcount >> 1) & 1;
-            const int64_t r = (int64_t)tile * kTileM + q * 32 + lane;
-            const bool valid = r < p.rows;
-            mbar_wait(&bar->tmem_full[a], aph, 3);
-            tc_fence_after();
-            const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)a * N;
-            constexpr int kChunksPerWarp = (N == 64) ? 2 : 4;
-#pragma unroll 1
-            for (int ci = 0; ci < kChunksPerWarp; ++ci) {
-                const int chunk = part * kChunksPerWarp + ci;
-                uint32_t v[32];
-                tmem_ld32(t_row + chunk * 32, v);
-                tmem_ld_wait();
-                if (!valid) continue;
+        wg_wait<0>();
+        wg_fence_regs(acc);
+        // ===================== epilogue: accumulator fragment -> global =====================
+        const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t r = (int64_t)tile * kTileM + r0 + 8 * h;
+            if (r >= p.rows) continue;
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) {
+                const int col = 8 * j + c0;
+                float2 o = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
                 if (N == 64) {
-                    float* dst = p.out + r * 64 + chunk * 32;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float4 o;
-                        o.x = __uint_as_float(v[4 * j + 0]) + tail->bias[chunk * 32 + 4 * j + 0];
-                        o.y = __uint_as_float(v[4 * j + 1]) + tail->bias[chunk * 32 + 4 * j + 1];
-                        o.z = __uint_as_float(v[4 * j + 2]) + tail->bias[chunk * 32 + 4 * j + 2];
-                        o.w = __uint_as_float(v[4 * j + 3]) + tail->bias[chunk * 32 + 4 * j + 3];
-                        if (p.act == STMGCN_ACT_RELU) {
-                            o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-                        }
-                        *reinterpret_cast<float4*>(dst + 4 * j) = o;
-                    }
+                    o.x += tail->bias[col];
+                    o.y += tail->bias[col + 1];
+                    if (p.act == STMGCN_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                    *reinterpret_cast<float2*>(p.out + r * 64 + col) = o;
                 } else {
-                    const int col = chunk * 32;                    // U_k, k = col / 64
-                    if ((col >> 6) >= p.ks_out) continue;
-                    float* dst = p.u + (int64_t)(col >> 6) * p.stride_u + r * 64 + (col & 63);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        *reinterpret_cast<uint4*>(dst + 4 * j) = make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+                    if ((col >> 6) >= p.ks_out) continue;      // U_k, k = col / 64
+                    *reinterpret_cast<float2*>(p.u + (int64_t)(col >> 6) * p.stride_u + r * 64 + (col & 63)) = o;
                 }
             }
-            tc_fence_before();
-            mbar_arrive(&bar->tmem_empty[a]);
         }
-        TC_PROF_FLUSH(12, tid == 0)
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (warp == kMmaWarp) tmem_dealloc(tmem_base, Cfg::kTmemCols);
     if (DZ && p.dbias != nullptr) {
-        for (int i = tid; i < 64; i += Cfg::kThreads) {
+        for (int i = tid; i < 64; i += kPThreads) {
             float v = 0.f;
 #pragma unroll
-            for (int w = 0; w < kPLoaderWarps; ++w) v += tail->s_db[w][i];
+            for (int w = 0; w < kPWarps; ++w) v += tail->s_db[w][i];
             atomicAdd(&p.dbias[i], v);
         }
     }
@@ -240,7 +221,7 @@ int32_t launch_proj_fwd_tc(const float* s, int64_t stride_k, int ks, int64_t row
     p.rows = rows;
     p.n_tiles = (int)ceil_div(rows, kTileM);
     const int grid = p.n_tiles < sm_count() ? p.n_tiles : sm_count();
-    kern<<<grid, PCfg<64>::kThreads, psmem<64>(), st>>>(p);
+    kern<<<grid, kPThreads, psmem<64>(), st>>>(p);
     count_launch();
     return check_launch("proj_fwd_tc");
 }
@@ -265,7 +246,7 @@ int32_t launch_proj_bwd_tc(const float* d_out, const float* out_act, int act, in
     p.rows = rows;
     p.n_tiles = (int)ceil_div(rows, kTileM);
     const int grid = p.n_tiles < sm_count() ? p.n_tiles : sm_count();
-    kern<<<grid, PCfg<256>::kThreads, psmem<256>(), st>>>(p);
+    kern<<<grid, kPThreads, psmem<256>(), st>>>(p);
     count_launch();
     return check_launch("proj_bwd_tc");
 }

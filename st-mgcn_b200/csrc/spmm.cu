@@ -5,12 +5,8 @@
 // fully coalesced 512 B gather of the neighbour's feature run.  The grid is column-tile-major (blockIdx.y = column tile)
 // so the CTAs resident at any moment share one column tile of X (N x 512 B = 2 MB at N=4096): gathers are served by
 // L2/L1, HBM sees X, Z, U once and Y once.
-// Why there is no shared-memory-staged variant: the kernel's time is its gather volume nnz*F*4 B (2.87 GB per launch at
-// BASELINE configs[2]) divided by what an on-chip level can serve for RANDOM row gathers.  tools/gather_probe.cu measures
-// exactly that on B200 (profiles/r2_gather_probe.log): 512-byte segment gathers through L2/L1 17.9 TB/s (165 us for this
-// launch's volume), an unstructured shared-memory strip 7.4-8.7 TB/s (bank conflicts), a persistent L1-resident 128-byte
-// column tile 13.6-15.1 TB/s.  A round-1 strip kernel with a bank-aware sliced ELL reached 228 us.  This kernel runs at
-// 170-187 us = 88-97 % of the best measured gather rate; the 70 %-of-HBM target would need 65 TB/s of gather bandwidth.
+// The kernel's time is its gather volume nnz*F*4 B (2.87 GB per launch at BASELINE configs[2]) divided by what the
+// on-chip levels can serve for RANDOM row gathers, not its algorithmic HBM bytes (bench.py reports both).
 #include "common.cuh"
 #include <stdlib.h>
 

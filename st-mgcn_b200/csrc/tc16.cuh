@@ -1,24 +1,23 @@
-// 16-bit (bf16) operand helpers for the tcgen05 kernels: kind::f16 MMA, instruction descriptor, the 128-byte-swizzled
-// tile layout shared by K-major and MN-major operands, and the bf16 hi/lo split.
+// 16-bit (bf16) operand helpers for the wgmma kernels: the 128-byte-swizzled tile layout shared by K-major and MN-major
+// operands, its descriptors, and the bf16 hi/lo split.
 //
 // Precision scheme "3xBF16": every fp32 operand v is stored as TWO bf16 planes, hi = bf16(v) (round to nearest) and
-// lo = bf16(v - hi); v = hi + lo up to 2^-18 relative.  A.B is accumulated in fp32 TMEM as Ahi.Bhi + Alo.Bhi + Ahi.Blo
-// (the dropped Alo.Blo term is ~2^-18 relative).  Emulated through the whole 3-layer, 12-step LSTM forward + BPTT this
-// stays within 2.5e-6 (forward) / 7.4e-6 (weight gradients) of exact arithmetic -- the 1e-4 parity bar (BASELINE.json)
-// has >10x headroom -- at HALF the tensor-pipe time and HALF the shared-memory / L2 operand bytes of 3xTF32, and the
-// planes cost the same 4 bytes per value in HBM as the fp32 number they replace.  A single pass over the hi planes is
-// the bf16 arithmetic mode of the bf16-quoted configurations (BASELINE.json configs[1], [3], [4]).
+// lo = bf16(v - hi); v = hi + lo up to 2^-18 relative.  A.B is accumulated in fp32 registers as Ahi.Bhi + Alo.Bhi + Ahi.Blo
+// (the dropped Alo.Blo term is ~2^-18 relative), inside the 1e-4 parity bar (BASELINE.json) at half the tensor-pipe time
+// and half the shared-memory / L2 operand bytes of 3xTF32; the planes cost the same 4 bytes per value in HBM as the fp32
+// number they replace.  A single pass over the hi planes is the bf16 arithmetic mode of the bf16-quoted configurations
+// (BASELINE.json configs[1], [3], [4]).
 //
 // One tile layout for everything: a [rows][64 bf16] tile, 128 bytes per row, 8-row groups of 1024 bytes, 16-byte
 // chunk index XORed with (row & 7) -- the TMA SWIZZLE_128B pattern.  Read with a K-major descriptor it is an operand
-// whose K runs along the 64 columns (M/N = rows); read with an MN-major descriptor (canonical layout
-// ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units, cute/atom/mma_traits_sm100.hpp) it is the TRANSPOSED operand: M/N
-// runs along the 64 columns (one 64-element atom; further atoms LBO bytes apart), K along the rows (8-row atoms, SBO =
-// 1024 bytes apart).  So the same shared-memory image of [h_below | h_prev] feeds the gate GEMM (K-major A) and the
-// weight-gradient GEMM (MN-major A), and one image of dA feeds the data-gradient GEMM (K-major A) and the weight
-// gradient GEMM (MN-major B).
+// whose K runs along the 64 columns (M/N = rows); read with an MN-major descriptor (canonical layout ((64,n),(8,k)),
+// tc_common.cuh) it is the TRANSPOSED operand: M/N runs along the 64 columns (one 64-element atom; further atoms LBO
+// bytes apart), K along the rows (8-row atoms, SBO = 1024 bytes apart).  So the same shared-memory image of
+// [h_below | h_prev] feeds the gate GEMM (K-major A) and the weight-gradient GEMM (MN-major A), and one image of dA
+// feeds the data-gradient GEMM (K-major A) and the weight-gradient GEMM (MN-major B).
 #pragma once
 #include "tc_common.cuh"
+#include "wgmma.cuh"
 #include <cuda_bf16.h>
 
 namespace stmgcn {
@@ -32,59 +31,13 @@ __host__ __device__ __forceinline__ uint32_t sw128_off16(uint32_t row, uint32_t 
     return row * 128u + ((((col >> 3) ^ (row & 7u)) & 7u) << 4) + ((col & 7u) << 1);
 }
 
-// kind::f16 instruction descriptor, bf16 inputs, fp32 accumulate.  a_mn / b_mn: 1 = the operand is MN-major.
-__host__ __device__ constexpr uint32_t idesc_bf16(int m, int n, int a_mn = 0, int b_mn = 0) {
-    return (1u << 4)                               // c_format = F32
-           | (1u << 7)                             // a_format = BF16
-           | (1u << 10)                            // b_format = BF16
-           | ((uint32_t)(a_mn & 1) << 15) | ((uint32_t)(b_mn & 1) << 16)
-           | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-
-// K-major 128B-swizzled tile: same descriptor as the fp32 tiles (rows of 128 B, 8-row groups 1024 B apart); one MMA
-// consumes K = 16 bf16 = 32 bytes: advance the start address by 32 B (+2 in the encoded field) per k-step.
+// K-major 128B-swizzled tile: rows of 128 B, 8-row groups 1024 B apart; one k16 MMA consumes 32 bytes of the row:
+// advance the start address by 32 B (+2 in the encoded field) per k-step.
 __device__ __forceinline__ uint64_t desc16_k(uint32_t smem_addr) { return smem_desc_k_sw128(smem_addr); }
 // MN-major view of the same tile: K = 16 rows per MMA = two 8-row atoms (SBO = 1024 B); advance by 2048 B per k-step.
 // lbo_bytes: distance between 64-element atoms along M/N (unused when the operand is 64 wide).
 __device__ __forceinline__ uint64_t desc16_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
-    return smem_desc_mn_sw128(smem_addr, lbo_bytes, 1024u, 2);
-}
-
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        :
-        : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// Two consecutive MMAs of ONE issuing thread that share their A operand: the first keeps A in the tensor core's collector
-// buffer (SASS: A_KEEP), the second takes it from there (A_REUSE) instead of reading the 4 KB from shared memory again.
-// In the 3xBF16 scheme the pairs (A_hi . B_hi, A_hi . B_lo) share A: one of three A reads disappears -- these kernels are
-// bound by the shared-memory data pipe the operand reads go through (ncu: l1tex data pipe 94 % in the backward).
-// Only valid when no other thread issues MMAs in between (single MMA-issuing thread per CTA).
-__device__ __forceinline__ void mma_bf16_keep_a(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16.collector::a::fill [%0], %1, %2, %3, p;\n\t}"
-        :
-        : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void mma_bf16_reuse_a(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16.collector::a::lastuse [%0], %1, %2, %3, p;\n\t}"
-        :
-        : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+    return smem_desc_mn_sw128(smem_addr, lbo_bytes, 1024u);
 }
 
 // ---- bf16 hi / lo split ------------------------------------------------------------------------------------

@@ -1,12 +1,11 @@
-// Blackwell (sm_100a) primitives used by the tensor-core kernels: mbarrier, 1-D bulk async copy (TMA unit,
-// SASS UBLKCP), tcgen05 (alloc / mma kind::tf32 / commit / ld / fences), UMMA descriptors.
+// Hopper (sm_90a) primitives used by the tensor-core kernels: mbarrier, 1-D bulk async copy and TMA tensor loads,
+// wgmma shared-memory matrix descriptors (the instructions themselves: wgmma.cuh).
 //
 // Precision scheme "3xTF32": every fp32 operand v is split into hi = v with the low 13 mantissa bits cleared
 // (exactly representable in tf32, so the tensor core's own fp32->tf32 conversion cannot change it) and
 // lo = v - hi (exact in fp32; <= 13 significant bits, again masked to tf32).  A.B is accumulated in fp32
-// TMEM as Ahi.Bhi + Alo.Bhi + Ahi.Blo; the dropped Alo.Blo term is ~2^-22 relative.  Measured against the
-// fp64 oracle this keeps the LSTM within ~2e-6 of the exact-fp32 path (the 1e-4 parity bar forbids
-// single-pass TF32, SURVEY.md section 0.5).
+// registers as Ahi.Bhi + Alo.Bhi + Ahi.Blo; the dropped Alo.Blo term is ~2^-22 relative, well inside the 1e-4
+// parity bar that rules out single-pass TF32 (SURVEY.md section 0.5).
 #pragma once
 #include "common.cuh"
 
@@ -70,33 +69,11 @@ __device__ __forceinline__ void mbar_wait_polite(uint64_t* bar, uint32_t parity)
     }
     __trap();
 }
-// Optional wait-time accounting (built with -DSTMGCN_TC_PROFILE): cycles each role spends blocked on each barrier
-// class, summed per launch into g_tc_prof[slot]; slot = role*4 + barrier class.  Read with stmgcn_dbg_tc_prof().
-#ifdef STMGCN_TC_PROFILE
-__device__ unsigned long long g_tc_prof[64];
-struct WaitProf {
-    unsigned long long acc[4] = {0, 0, 0, 0};
-    long long t_start;
-    __device__ WaitProf() { t_start = clock64(); }
-    __device__ void flush(int role, bool leader) {
-        if (leader) {
-            for (int i = 0; i < 4; ++i) atomicAdd(&g_tc_prof[role * 4 + i], acc[i]);
-            atomicAdd(&g_tc_prof[48 + role], (unsigned long long)(clock64() - t_start));
-        }
-    }
-};
-#define TC_PROF_DECL WaitProf _wp;
-#define TC_PROF_FLUSH(role, leader) _wp.flush(role, leader);
-#define mbar_wait(bar, parity, cls) do { long long _t0 = clock64(); mbar_wait_raw(bar, parity); _wp.acc[cls] += clock64() - _t0; } while (0)
-#define mbar_wait_p(bar, parity, cls) do { long long _t0 = clock64(); mbar_wait_polite(bar, parity); _wp.acc[cls] += clock64() - _t0; } while (0)
-#else
-#define TC_PROF_DECL
-#define TC_PROF_FLUSH(role, leader)
+// (the third argument names the barrier class a wait belongs to; it documents the call site)
 #define mbar_wait(bar, parity, cls) mbar_wait_raw(bar, parity)
 #define mbar_wait_p(bar, parity, cls) mbar_wait_polite(bar, parity)
-#endif
 
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma / bulk copies read smem through it)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / bulk copies read smem through it)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- 1-D bulk async copy global -> shared, completion on an mbarrier (TMA unit; SASS: UBLKCP) -----------
@@ -107,40 +84,22 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                  : "memory");
 }
 
-// L2 prefetch of a contiguous global range (no registers, no shared memory; SASS UBLKPF)
-// One elected lane of a fully converged warp.  Guarding the single-thread tcgen05 / TMA / mbarrier instructions with this
-// instead of `lane == 0` matters: ptxas cannot prove `lane == 0` selects one thread, and wraps EVERY uniform-datapath
-// instruction (UTCHMMA, UTCBAR, UBLKCP, UTMALDG) in an ELECT / BRA.U.ANY serialisation loop -- ~10 extra instructions and
-// a branch per MMA, measured as ~90 cycles per issued tcgen05.mma.  After elect.sync the instructions issue back to back.
-// The elected lane is the same on every call of a converged warp, so MMAs and their tcgen05.commit come from one thread.
+// One elected lane of a fully converged warp, for the single-thread TMA / mbarrier instructions (ptxas can prove that
+// elect.sync selects one thread; a `lane == 0` guard gets wrapped in a serialisation loop).
 __device__ __forceinline__ bool elect_one_sync() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-// 256-bit global store / load (sm_100: STG.E.ENL2.256 / LDG.E.ENL2.256): 8 consecutive 32-bit words, 32-byte aligned
-__device__ __forceinline__ void st_global_v8(void* dst, const uint32_t* v) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-                 "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
+// fire-and-forget 8-byte reduction into global memory (the add happens in L2, nothing returns)
+__device__ __forceinline__ void red_add_f32x2(float* dst, float a, float b) {
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
 }
-// fire-and-forget 16-byte reduction into global memory (REDG.E.ADD.F32x4: the add happens in L2, nothing returns)
-__device__ __forceinline__ void red_add_f32x4(float4* dst, const float4& v) {
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
+// L2 prefetch of a contiguous global range (no registers, no shared memory)
 __device__ __forceinline__ void prefetch_l2(const void* gmem, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem), "r"(bytes) : "memory");
 }
 
-// ---- tcgen05 --------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {   // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {      // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
 // ---- TMA tensor stores (shared -> global through a CUtensorMap, bulk async-group completion) ----
 __device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t smem_addr, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
@@ -156,95 +115,33 @@ __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bul
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// programmatic dependent launch: the next kernel of the stream may start its prologue (barrier init, TMEM allocation)
+// programmatic dependent launch: the next kernel of the stream may start its prologue (barrier init)
 // on SMs this grid has already left; pdl_wait() blocks until the previous grid has completed and flushed its memory
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] . B[smem], tf32 inputs, fp32 accumulate; one thread issues for the CTA.
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        :
-        : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all previously issued MMAs of this thread complete -> one arrival on the mbarrier
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets row (lane base + i), columns [c, c+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
-        "[%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- UMMA descriptors (field layout: cute/arch/mma_sm100_desc.hpp in the vendored CUTLASS tree) --------------
-// K-major operand tile, 128-byte swizzle: rows of 128 B (32 fp32 along K), 8-row groups 1024 B apart.
+// ---- wgmma shared-memory matrix descriptors (sm_90: start >> 4 [0,14), LBO >> 4 [16,30), SBO >> 4 [32,46),
+// layout type [62,64) with 1 = 128-byte swizzle).  Tiles are 1024-byte aligned, so the base-offset field stays 0.
+// K-major operand, 128-byte swizzle: rows of 128 B along K, 8-row groups 1024 B apart (SBO); LBO is unused.
+// A k-step inside the 128-byte row is an add on the start address (32 B = +2 encoded for k16 bf16 / k8 tf32).
 __device__ __forceinline__ uint64_t smem_desc_k_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3fff);          // start address  [0,14)
-    d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major) [16,30)
-    d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset: 8 rows x 128 B [32,46)
-    d |= (uint64_t)1 << 46;                              // descriptor version 1 (Blackwell) [46,48)
-    d |= (uint64_t)2 << 61;                              // layout type SWIZZLE_128B [61,64)
+    d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// kind::tf32, fp32 accumulate, M x N tile; mn_major = 0: A and B K-major, 1: both MN-major
-__host__ __device__ constexpr uint32_t idesc_tf32(int m, int n, int mn_major = 0) {
-    return (1u << 4)                               // c_format  = F32
-           | (2u << 7)                             // a_format  = TF32
-           | (2u << 10)                            // b_format  = TF32
-           | ((uint32_t)(mn_major & 1) << 15)      // a_major
-           | ((uint32_t)(mn_major & 1) << 16)      // b_major
-           | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-// MN-major operand, 128-byte swizzle.  Canonical layout (cute/atom/mma_traits_sm100.hpp, in 16-byte units):
-// ((8,n),(8,k)) : ((1,LBO),(8,SBO)) -- a 1024-byte atom holds 32 consecutive M/N elements (one 128-byte row)
-// for each of 8 consecutive K; LBO = byte distance between atoms along M/N, SBO = between atoms along K.
-__device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                       uint32_t layout_type = 2) {
+// MN-major operand (16-bit types only), 128-byte swizzle: canonical layout ((64, n), (8, k)) in elements -- an atom of
+// 1024 B holds 64 consecutive M/N elements (one 128-byte row) for each of 8 consecutive K; LBO = byte distance between
+// atoms along M/N, SBO = between atoms along K.
+__device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)layout_type << 61;
+    d |= (uint64_t)1 << 62;
     return d;
-}
-// MN-major tile for 32-bit operands: layout type SWIZZLE_128B_BASE32B (1), Swizzle<2,5,2> on the byte address:
-// atoms of 128 B (32 consecutive M/N elements) x 4 K-rows = 512 B; inside an atom the 32-byte chunk index is XORed
-// with the K-row index.  Atoms are laid out [mn atom][k atom]: LBO = (k_rows/4)*512 bytes, SBO = 512 bytes.
-__host__ __device__ __forceinline__ uint32_t mn32_offset(uint32_t q /*float4 index along M/N*/, uint32_t k,
-                                                         uint32_t k_rows) {
-    const uint32_t atom_mn = q >> 3, c16 = q & 7;            // 8 float4 per 128-byte row
-    const uint32_t atom_k = k >> 2, kr = k & 3;
-    return atom_mn * (k_rows >> 2) * 512u + atom_k * 512u + kr * 128u + ((((c16 >> 1) ^ kr) & 3u) << 5) + ((c16 & 1u) << 4);
 }
 
 // byte offset of element (row, k) inside a [rows][32 fp32] K-major tile with the 128-byte swizzle

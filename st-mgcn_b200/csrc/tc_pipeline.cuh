@@ -1,7 +1,8 @@
-// Shared pieces of the tcgen05 kernels: tile constants, the mbarrier set, the single-thread MMA issuer, the tf32 hi/lo
-// split + swizzled store helpers and the weight-image packer.  Included by lstm_tc.cu and proj_tc.cu.
+// Shared pieces of the 3xTF32 wgmma kernels: tile constants, the tf32 hi/lo split + swizzled store helpers and the
+// weight-image packer.  Included by proj_tc.cu and wgrad_tc.cu.
 #pragma once
 #include "tc_common.cuh"
+#include "wgmma.cuh"
 
 namespace stmgcn {
 namespace tc {
@@ -10,75 +11,7 @@ constexpr int kTileM = 128;
 constexpr int kKB = 32;              // k-block: one 128-byte swizzle row of fp32
 constexpr int kHid = 64;
 constexpr int kGateCols = 256;       // 4H
-constexpr int kMaxStages = 4;
-constexpr int kAccs = 2;
-constexpr int kABytes = kTileM * kKB * 4;            // 16 KB per hi or lo A tile
-
-struct Barriers {
-    uint64_t full[kMaxStages];
-    uint64_t empty[kMaxStages];
-    uint64_t tmem_full[kAccs];
-    uint64_t tmem_empty[kAccs];
-    uint32_t tmem_base;
-};
-
-__device__ __forceinline__ void init_barriers(Barriers* b, int stages, int n_epi_threads, int n_loaders) {
-    for (int s = 0; s < stages; ++s) {
-        mbar_init(&b->full[s], n_loaders + 1);
-        mbar_init(&b->empty[s], 1);
-    }
-    for (int a = 0; a < kAccs; ++a) {
-        mbar_init(&b->tmem_full[a], 1);
-        mbar_init(&b->tmem_empty[a], n_epi_threads);
-    }
-    fence_barrier_init();
-}
-
-// The MMA warp: for every tile, for every k-block: wait operands, issue 3 x 4 MMAs, release the stage.
-template <int N, int STAGES, int PROF_KERNEL>
-__device__ __forceinline__ void mma_issuer(Barriers* bar, uint8_t* smem, int stage_bytes, int b_bytes, int nkb,
-                                           int n_tiles, uint32_t tmem_base, int lane) {
-    constexpr uint32_t idesc = idesc_tf32(kTileM, N);
-    TC_PROF_DECL
-    (void)lane;
-    const bool leader = elect_one_sync();      // (not `leader`: see elect_one_sync in tc_common.cuh)
-    uint32_t it = 0, tcount = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-        const int a = tcount & 1;
-        const uint32_t aph = (tcount >> 1) & 1;
-        mbar_wait(&bar->tmem_empty[a], aph ^ 1, 2);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)a * N;
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-            const int s = it % STAGES;
-            const uint32_t ph = (it / STAGES) & 1;
-            mbar_wait(&bar->full[s], ph, 1);
-            tc_fence_after();
-            if (leader) {
-                const uint32_t st = smem_u32(smem + (size_t)s * stage_bytes);
-                const uint64_t a_hi = smem_desc_k_sw128(st);
-                const uint64_t a_lo = smem_desc_k_sw128(st + kABytes);
-                const uint64_t b_hi = smem_desc_k_sw128(st + 2 * kABytes);
-                const uint64_t b_lo = smem_desc_k_sw128(st + 2 * kABytes + b_bytes);
-#pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {
-                    const uint64_t da = (pass == 1) ? a_lo : a_hi;
-                    const uint64_t db = (pass == 2) ? b_lo : b_hi;
-#pragma unroll
-                    for (int k = 0; k < kKB / 8; ++k) {
-                        const uint32_t acc = (kb > 0 || pass > 0 || k > 0) ? 1u : 0u;
-                        mma_tf32(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, acc);
-                    }
-                }
-                mma_commit(&bar->empty[s]);
-            }
-            __syncwarp();
-        }
-        if (leader) mma_commit(&bar->tmem_full[a]);
-        __syncwarp();
-    }
-    TC_PROF_FLUSH(PROF_KERNEL * 3 + 1, leader)
-}
+constexpr int kABytes = kTileM * kKB * 4;            // 16 KB per hi or lo A tile of 128 rows
 
 __device__ __forceinline__ void split_store(uint8_t* st, uint32_t off, const float4& v) {
     float4 hi, lo;

@@ -1,7 +1,7 @@
-// Weight gradient of the stacked-K projection on the 5th-gen tensor cores (tcgen05, TMEM accumulator, 3xTF32 -- see
+// Weight gradient of the stacked-K projection on the Hopper tensor cores (wgmma, register accumulators, 3xTF32 -- see
 // tc_common.cuh):  dW[kd x 64] += [T_kX | T_{k+1}X]^T . dZ  per 128-row block of W (reference: the autograd of GCN.py:39).
-// (The shared LSTM's own weight gradient is fused into lstm16_bwd_kernel, lstm16.cu; this kernel was the LSTM's
-// first-generation weight-gradient reduction and keeps its generic two-segment form.)
+// (The shared LSTM's own weight gradient is fused into lstm16_bwd_kernel, lstm16.cu; this kernel keeps the generic
+// two-segment form.)
 #include "tc_pipeline.cuh"
 #include <stdlib.h>
 #include <string.h>
@@ -11,34 +11,20 @@ using namespace stmgcn::tc;
 
 namespace {
 
-constexpr int kWgLoaderWarps = 16;
-
 // =====================================================================================================
-// weight gradients:  dWp[kd x 256] += sum over (t, r) of [h_below_t | h_{t-1}][r, :]^T . dA_t[r, :]
-// M = kd index (padded to 128), N = 256 gate columns, K = rows.  Both operands are row-major in HBM, i.e. K is the slow
-// dimension: they are MN-major operands.  The loaders copy rows with coalesced float4 loads and store them as MN-major
-// atoms with the 32-byte-base 128B swizzle (layout type SWIZZLE_128B_BASE32B = 1, see mn32_offset in tc_common.cuh;
-// with the plain SWIZZLE_128B type and the MN-major descriptor bits the tf32 MMA returns zeros).  One TMEM
-// accumulator lives for the whole kernel and is flushed with red.add.
+// dW[kd x N] += sum over rows r of [seg0 | seg1][r, :]^T . da[r, :]
+// M = kd index (padded to 128; warpgroup w owns kd rows 64w .. 64w+63), N = 64, K = rows, 32 rows per k-block.  Both
+// operands are row-major in HBM (K is the slow dimension) and tf32 wgmma reads K-major operands only, so the loaders
+// transpose on their way to shared memory: element (row r, m) lands at sw128_offset(m, r) of a [m][32 k] tile.  The
+// accumulators live for the whole launch and are flushed with atomics once.
 // =====================================================================================================
-constexpr int kWgStages = 2;
-constexpr int kWgRows = 32;                                        // K per stage
-constexpr int kWgABytes = 128 * kWgRows * 4;                       // 16 KB  [128 m][32 k] K-major
+constexpr int kWgRows = 32;                                        // K per k-block
+constexpr int kWgThreads = 256;
 template <int N> struct WgCfg {
     static constexpr int kBBytes = N * kWgRows * 4;                // [N][32 k] K-major
-    static constexpr int kStageBytes = 2 * kWgABytes + 2 * kBBytes;
-    static constexpr size_t kSmem = 1024 + (size_t)kWgStages * kStageBytes + 64;
-    static constexpr int kTmemCols = N < 32 ? 32 : N;
+    static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
+    static constexpr size_t kSmem = 1024 + (size_t)kStageBytes;
 };
-constexpr int kWgThreads = (kWgLoaderWarps + 1) * 32;              // 544
-
-struct WgTail {
-    uint64_t full[kWgStages];
-    uint64_t empty[kWgStages];
-    uint64_t done;
-    uint32_t tmem_base;
-};
-static_assert(sizeof(WgTail) <= 64, "WgTail");
 
 struct WgParams {
     const float* seg0;       // h_below tape base for this layer: (T, rows, 64) or nullptr (layer 0)
@@ -57,147 +43,90 @@ struct WgParams {
 template <int N>
 __global__ void __launch_bounds__(kWgThreads, 1) lstm_wgrad_tc_kernel(const __grid_constant__ WgParams p) {
     using Cfg = WgCfg<N>;
-    constexpr int kWgBBytes = Cfg::kBBytes;
-    constexpr int kWgStageBytes = Cfg::kStageBytes;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // keeps the __shared__ address space (LDS/STS, not generic LD/ST)
-    WgTail* tail = (WgTail*)(smem + (size_t)kWgStages * kWgStageBytes);
+    uint8_t* st = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // keeps the __shared__ address space
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const int lane = tid & 31;
-    constexpr int kMmaWarp = kWgLoaderWarps;
-    constexpr int kLoaders = kWgLoaderWarps * 32;
+    const int wg = tid >> 7;
+    constexpr int kNA = 1024 / kWgThreads, kNB = (kWgRows * N / 4) / kWgThreads;
+    static_assert(kNB >= 1, "loader mapping");
+    const uint32_t s_u = smem_u32(st);
+    const uint32_t a_hi = s_u + (uint32_t)wg * 64u * 128u, a_lo = a_hi + kABytes;
+    const uint32_t b_hi = s_u + 2 * kABytes, b_lo = b_hi + Cfg::kBBytes;
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    bool first = true;
 
-        if (tid == 0) {
-        for (int s = 0; s < kWgStages; ++s) {
-            mbar_init(&tail->full[s], kLoaders / 2);       // one loader group per chunk
-            mbar_init(&tail->empty[s], 1);
+    for (int64_t chunk = blockIdx.x; chunk < p.total_chunks; chunk += gridDim.x) {
+        const int t = (int)(chunk / p.chunks_per_t);
+        const int64_t r0 = (chunk % p.chunks_per_t) * kWgRows;
+        const float* s0 = p.seg0 ? p.seg0 + (int64_t)t * p.rows * kHid : nullptr;
+        const float* s1 = p.shift1 ? ((t > 0) ? p.seg1 + (int64_t)(t - 1) * p.rows * kHid : p.h0)
+                                    : p.seg1 + (int64_t)t * p.rows * kHid;
+        const float* dt = p.da + (int64_t)t * p.rows * N;
+        float4 va[kNA], vb[kNB];
+#pragma unroll
+        for (int i = 0; i < kNA; ++i) {                   // A': 32 rows x 32 float4 (128 kd values), coalesced
+            const int idx = tid + i * kWgThreads;
+            const int row = idx >> 5, q = idx & 31;
+            const int64_t r = r0 + row;
+            // kd = 128: m 0..63 from seg0 (h_below), 64..127 from seg1 (h_prev); kd = 64: m 0..63 from seg1
+            const float* src = (p.kd == 128) ? (q < 16 ? s0 : s1) : (q < 16 ? s1 : nullptr);
+            va[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (src != nullptr && r < p.rows) va[i] = *reinterpret_cast<const float4*>(src + r * kHid + (q & 15) * 4);
         }
-        mbar_init(&tail->done, 1);
-        fence_barrier_init();
+#pragma unroll
+        for (int i = 0; i < kNB; ++i) {                   // B': 32 rows x N/4 float4, coalesced
+            const int idx = tid + i * kWgThreads;
+            const int row = idx / (N / 4), q = idx % (N / 4);
+            const int64_t r = r0 + row;
+            vb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (r < p.rows) vb[i] = *reinterpret_cast<const float4*>(dt + r * N + q * 4);
+        }
+        wg_wait<0>();
+        __syncthreads();                                  // both warpgroups are done with the stage
+#pragma unroll
+        for (int i = 0; i < kNA; ++i) {
+            const int idx = tid + i * kWgThreads;
+            split_store_t(st, st + kABytes, (idx & 31) * 4, idx >> 5, va[i]);
+        }
+#pragma unroll
+        for (int i = 0; i < kNB; ++i) {
+            const int idx = tid + i * kWgThreads;
+            split_store_t(st + 2 * kABytes, st + 2 * kABytes + Cfg::kBBytes, (idx % (N / 4)) * 4, idx / (N / 4), vb[i]);
+        }
+        fence_proxy_async_smem();
+        __syncthreads();
+        wg_fence_regs(acc);
+        wg_fence();
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+            const uint64_t da = smem_desc_k_sw128(pass == 1 ? a_lo : a_hi);
+            const uint64_t db = smem_desc_k_sw128(pass == 2 ? b_lo : b_hi);
+#pragma unroll
+            for (int k = 0; k < kWgRows / 8; ++k)
+                wgmma_tf32_n64(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (!first || pass > 0 || k > 0) ? 1u : 0u);
+        }
+        wg_commit();
+        first = false;
     }
-    if (warp == kMmaWarp) tmem_alloc(&tail->tmem_base, Cfg::kTmemCols);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tail->tmem_base;
-    const bool has_work = (int64_t)blockIdx.x < p.total_chunks;
-
-    if (warp < kMmaWarp) {
-        // ===================== loaders: HBM rows -> tf32 hi/lo -> MN-major swizzled atoms =====================
-        TC_PROF_DECL
-        // two loader groups alternate row chunks (see the note in lstm_cell_tc_kernel about the proxy fence)
-        constexpr int kGroups = 2, kGT = kLoaders / kGroups;
-        constexpr int kNA = 1024 / kGT, kNB = (32 * N / 4) / kGT;
-        static_assert(kNB >= 1, "loader mapping");
-        const int ltid = tid;
-        const int grp = ltid / kGT, gtid = ltid % kGT;
-        const int64_t my_chunks = (p.total_chunks - (int64_t)blockIdx.x + gridDim.x - 1) / gridDim.x;
-        for (int64_t j = grp; j < my_chunks; j += kGroups) {
-            const int64_t chunk = blockIdx.x + j * gridDim.x;
-            const int t = (int)(chunk / p.chunks_per_t);
-            const int64_t r0 = (chunk % p.chunks_per_t) * kWgRows;
-            const float* s0 = p.seg0 ? p.seg0 + (int64_t)t * p.rows * kHid : nullptr;
-            const float* s1 = p.shift1 ? ((t > 0) ? p.seg1 + (int64_t)(t - 1) * p.rows * kHid : p.h0)
-                                        : p.seg1 + (int64_t)t * p.rows * kHid;
-            const float* dt = p.da + (int64_t)t * p.rows * N;
-            float4 va[kNA], vb[kNB];
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    if (first) return;                                    // no chunk: nothing accumulated
+    // ===================== accumulator fragment (rows = kd index) -> atomics into dWp =====================
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-            for (int i = 0; i < kNA; ++i) {                   // A': 32 rows x 32 float4 (128 kd values), coalesced
-                const int idx = gtid + i * kGT;
-                const int row = idx >> 5, q = idx & 31;
-                const int64_t r = r0 + row;
-                // kd = 128: m 0..63 from seg0 (h_below), 64..127 from seg1 (h_prev); kd = 64: m 0..63 from seg1
-                const float* src = (p.kd == 128) ? (q < 16 ? s0 : s1) : (q < 16 ? s1 : nullptr);
-                va[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (src != nullptr && r < p.rows) va[i] = *reinterpret_cast<const float4*>(src + r * kHid + (q & 15) * 4);
-            }
+    for (int h = 0; h < 2; ++h) {
+        const int m = r0 + 8 * h;
+        if (m >= p.kd) continue;
 #pragma unroll
-            for (int i = 0; i < kNB; ++i) {                   // B': 32 rows x N/4 float4, coalesced
-                const int idx = gtid + i * kGT;
-                const int row = idx / (N / 4), q = idx % (N / 4);
-                const int64_t r = r0 + row;
-                vb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (r < p.rows) vb[i] = *reinterpret_cast<const float4*>(dt + r * N + q * 4);
-            }
-            const int s = (int)(j % kWgStages);
-            const uint32_t ph = (uint32_t)(j / kWgStages) & 1;
-            mbar_wait(&tail->empty[s], ph ^ 1, 0);
-            uint8_t* st = smem + (size_t)s * kWgStageBytes;
-#pragma unroll
-            for (int i = 0; i < kNA; ++i) {
-                const int idx = gtid + i * kGT;
-                split_store(st, mn32_offset(idx & 31, idx >> 5, kWgRows), va[i]);      // hi at st, lo at st + kWgABytes
-            }
-#pragma unroll
-            for (int i = 0; i < kNB; ++i) {
-                const int idx = gtid + i * kGT;
-                const uint32_t off = mn32_offset(idx % (N / 4), idx / (N / 4), kWgRows);
-                float4 hi, lo;
-                const float4 v = vb[i];
-                hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
-                lo.x = tf32_lo(v.x, hi.x); lo.y = tf32_lo(v.y, hi.y); lo.z = tf32_lo(v.z, hi.z); lo.w = tf32_lo(v.w, hi.w);
-                *reinterpret_cast<float4*>(st + 2 * kWgABytes + off) = hi;
-                *reinterpret_cast<float4*>(st + 2 * kWgABytes + kWgBBytes + off) = lo;
-            }
-            fence_proxy_async_smem();
-            mbar_arrive(&tail->full[s]);
+        for (int j = 0; j < N / 8; ++j) {
+            atomicAdd(p.dwp + (int64_t)m * N + 8 * j + c0, acc[4 * j + 2 * h]);
+            atomicAdd(p.dwp + (int64_t)m * N + 8 * j + c0 + 1, acc[4 * j + 2 * h + 1]);
         }
-        TC_PROF_FLUSH(9, ltid == 0)
-        // ===================== epilogue (warps 0-3): accumulator rows = kd index -> red.add into dWp =====================
-        if (warp < 4 && has_work) {
-            mbar_wait(&tail->done, 0, 3);
-            tc_fence_after();
-            const int m = warp * 32 + lane;
-            const uint32_t t_row = tmem_base + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
-            for (int chunk32 = 0; chunk32 < N / 32; ++chunk32) {
-                uint32_t v[32];
-                tmem_ld32(t_row + chunk32 * 32, v);
-                tmem_ld_wait();
-                if (m < p.kd) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) atomicAdd(p.dwp + (int64_t)m * N + chunk32 * 32 + j, __uint_as_float(v[j]));
-                }
-            }
-        }
-    } else {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = idesc_tf32(128, N, 1);          // both operands MN-major
-        constexpr uint32_t kLbo = (kWgRows / 4) * 512, kSbo = 512;
-        TC_PROF_DECL
-        const bool leader = elect_one_sync();      // (not `leader`: see elect_one_sync in tc_common.cuh)
-        uint32_t it = 0;
-        for (int64_t chunk = blockIdx.x; chunk < p.total_chunks; chunk += gridDim.x, ++it) {
-            const int s = it % kWgStages;
-            const uint32_t ph = (it / kWgStages) & 1;
-            mbar_wait(&tail->full[s], ph, 1);
-            tc_fence_after();
-            if (leader) {
-                const uint32_t st = smem_u32(smem + (size_t)s * kWgStageBytes);
-#pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {
-                    const uint32_t a_base = st + ((pass == 1) ? kWgABytes : 0);
-                    const uint32_t b_base = st + 2 * kWgABytes + ((pass == 2) ? kWgBBytes : 0);
-#pragma unroll
-                    for (int ks = 0; ks < kWgRows / 8; ++ks) {      // one MMA consumes K = 8 rows = two 4-row atoms
-                        const uint64_t da = smem_desc_mn_sw128(a_base + ks * 2 * kSbo, kLbo, kSbo, 1);
-                        const uint64_t db = smem_desc_mn_sw128(b_base + ks * 2 * kSbo, kLbo, kSbo, 1);
-                        mma_tf32(tmem_base, da, db, idesc, (it > 0 || pass > 0 || ks > 0) ? 1u : 0u);
-                    }
-                }
-                mma_commit(&tail->empty[s]);
-            }
-            __syncwarp();
-        }
-        if (leader && has_work) mma_commit(&tail->done);
-        __syncwarp();
-        TC_PROF_FLUSH(10, leader)
     }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == kMmaWarp) tmem_dealloc(tmem_base, Cfg::kTmemCols);
 }
 
 

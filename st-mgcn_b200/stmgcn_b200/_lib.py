@@ -63,7 +63,7 @@ def _load() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: the ST-MGCN hot path has no CPU fallback. Build it with "
-            f"`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a).")
+            f"`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a).")
     lib = ctypes.CDLL(LIB_PATH)
     for name, res, args in SIGNATURES:
         fn = getattr(lib, name)          # AttributeError here == header/library mismatch: fail loudly

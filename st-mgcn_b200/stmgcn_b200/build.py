@@ -1,7 +1,7 @@
-"""Build ``libstmgcn_b200.so`` in-tree with nvcc for sm_100a (and nothing else).
+"""Build ``libstmgcn_b200.so`` in-tree with nvcc for sm_90a (H100; and nothing else).
 
 ``python -m stmgcn_b200.build`` (with ``st-mgcn_b200/`` on ``sys.path``) or ``__graft_entry__.build()``.
-The shared object lands in ``st-mgcn_b200/lib/`` -- git-ignored, but shipped to the GPU box by gpurun.
+The shared object lands in ``st-mgcn_b200/lib/`` (git-ignored build output).
 Objects are rebuilt only when a source or header is newer.
 """
 from __future__ import annotations
@@ -17,16 +17,14 @@ ROOT = os.path.dirname(PKG_DIR)                      # st-mgcn_b200/
 REPO = os.path.dirname(ROOT)
 CSRC = os.path.join(ROOT, "csrc")
 LIB_DIR = os.path.join(ROOT, "lib")
-_PROF = bool(os.environ.get("STMGCN_TC_PROFILE"))       # instrumented build (per-role wait accounting): separate objects and .so
-OBJ_DIR = os.path.join(ROOT, "build_prof" if _PROF else "build")
-LIB_PATH = os.path.join(LIB_DIR, "libstmgcn_b200_prof.so" if _PROF else "libstmgcn_b200.so")
+OBJ_DIR = os.path.join(ROOT, "build")
+LIB_PATH = os.path.join(LIB_DIR, "libstmgcn_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",   # the long form: `-arch=sm_100a` drops the `a` features
+    "-gencode", "arch=compute_90a,code=sm_90a",     # the long form: `-arch=sm_90a` drops the `a` features (wgmma)
     "-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O3",
     "-Xptxas", "-v",
-] + (["-DSTMGCN_TC_PROFILE"] if os.environ.get("STMGCN_TC_PROFILE") else []) + [
 ]
 # --use_fast_math is deliberately NOT applied blindly: see below (we keep IEEE div/sqrt, only fast exp).
 NVCC_FLAGS.remove("--use_fast_math")

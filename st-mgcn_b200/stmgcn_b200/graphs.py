@@ -47,6 +47,7 @@ class GraphedStep:
         loss.backward()
         if self.all_reduce:
             self.bucket.all_reduce_mean_()
+        self.out = out.detach()         # after capture: the static buffer of the replayed step's prediction
         return loss
 
     def __call__(self, x: Optional[torch.Tensor] = None, y: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -61,6 +62,7 @@ class GraphedStep:
             loss.backward()
             if self.all_reduce:
                 self.bucket.all_reduce_mean_()
+            self.out = out.detach()
             return loss
         if x is not None:
             self.x.copy_(x, non_blocking=True)

@@ -1,9 +1,9 @@
 """Host-side mirror of the reference's ``nn.Module`` surface (the drop-in boundary, SURVEY.md section 8(b)).
 
 Same class names, constructor signatures, parameter names / shapes / creation order / init, ``forward``
-signatures and ``state_dict`` keys as ``/root/reference/GCN.py`` and ``/root/reference/STMGCN.py`` -- so
+signatures and ``state_dict`` keys as the reference's ``GCN.py`` and ``STMGCN.py`` -- so
 ``Main.py`` and ``Model_Trainer.py`` run unchanged and checkpoints interchange -- but every ``forward``
-runs the sm_100a kernels of ``libstmgcn_b200.so`` (no torch einsum / nn.LSTM execution, no CPU path).
+runs the sm_90a kernels of ``libstmgcn_b200.so`` (no torch einsum / nn.LSTM execution, no CPU path).
 """
 from __future__ import annotations
 

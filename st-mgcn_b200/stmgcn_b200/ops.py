@@ -34,7 +34,7 @@ _LSTM_PATH = os.environ.get("STMGCN_LSTM_PATH", "tc")
 
 
 def lstm_path() -> str:
-    """"tc": tcgen05 kernels where shapes allow (LSTM: H = 64, C <= 4; projection: p = q = 64); "fma": exact-fp32 FFMA kernels."""
+    """"tc": tensor-core (wgmma) kernels where shapes allow (LSTM: H = 64, C <= 4; projection: p = q = 64); "fma": exact-fp32 FFMA kernels."""
     return _LSTM_PATH
 
 
@@ -166,7 +166,7 @@ _PROJ_CACHE: "OrderedDict" = OrderedDict()
 
 
 def _proj_images(w: torch.Tensor, ks: int, p: int, need_bwd: bool):
-    """tcgen05 operand images of the projection weights (p = q = 64, ks <= 8), or (None, None).  Cached on the
+    """Tensor-core operand images of the projection weights (p = q = 64, ks <= 8), or (None, None).  Cached on the
     parameter's storage + in-place version (re-packed only after an optimizer step; bypassed during CUDA-graph capture so
     the pack kernels are part of the graph)."""
     if lstm_path() != "tc" or p != 64 or w.shape[1] != 64 or ks > 8:
@@ -538,7 +538,7 @@ class SharedLSTM(torch.autograd.Function):
     Returns (h_top, h_n (L,R,H), c_n (L,R,H)); the last two are not differentiable.
 
     Two kernel families (include/stmgcn_b200.h):
-    * H = 64, C <= 4, T <= 64 (the reference's configuration, Main.py:62) and ``lstm_path() == "tc"``: the tcgen05 bf16-plane
+    * H = 64, C <= 4, T <= 64 (the reference's configuration, Main.py:62) and ``lstm_path() == "tc"``: the tensor-core bf16-plane
       kernels of lstm16.cu -- tape = hidden-state planes + cell state, no gate tape, fused recompute backward;
     * anything else, or ``lstm_path() == "fma"``: the exact-fp32 CUDA-core kernels of lstm.cu with their own tape
       (hs, cs, gates); their backward overwrites the gate tape in place, so it can run only once per forward.

@@ -1,8 +1,8 @@
 """pytest configuration: ``gpu`` marker + import paths.
 
 ``-m "not gpu"`` runs here (no GPU): oracle vs golden vectors, host logic, C-ABI load/export checks.
-``-m gpu`` runs on a B200: parity of the CUDA path (through the C ABI) against the oracle / fixtures.
-Nothing in the ``gpu`` tests reads ``/root/reference`` (it does not exist on the GPU box).
+``-m gpu`` runs on an H100: parity of the CUDA path (through the C ABI) against the oracle / fixtures.
+Every test is self-contained: what came from the reference project is stored under ``tests/golden/``.
 """
 import os
 import sys
@@ -18,7 +18,7 @@ GOLDEN = os.path.join(REPO, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):

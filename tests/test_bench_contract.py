@@ -1,4 +1,4 @@
-"""bench.py contract checks that need no GPU: the reference arm (the unmodified reference from baseline/_ref, or the oracle port, timed on host cores) prints one JSON
+"""bench.py contract checks that need no GPU: the reference arm (the unmodified reference modules from oracle/_ref, or the oracle port, timed on host cores) prints one JSON
 line with the keys the driver reads, non-zero ranks of a multi-process launch stay silent, and the product arm refuses
 to run without a CUDA device instead of falling back to anything on the CPU."""
 import json
@@ -29,9 +29,9 @@ def test_reference_arm_prints_the_contract_line():
     for key in ("metric", "value", "n_gpus", "steps", "warmup", "ms_per_step", "scaling", "dtype", "data", "config",
                 "cpu_baseline", "e2e"):
         assert key in d, key
-    staged = os.path.exists(os.path.join(ROOT, "baseline", "_ref", "STMGCN.py"))
+    staged = os.path.exists(os.path.join(ROOT, "oracle", "_ref", "STMGCN.pyc"))
     assert d["value"] > 0 and d["cpu_baseline"]["cores"] >= 1
-    # the unmodified reference (staged by build()) when present, else the oracle port
+    # the unmodified reference (built by build()) when present, else the oracle port
     assert d["cpu_baseline"]["kind"] == ("reference" if staged else "port")
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0
     assert d["e2e"]["value"] == d["value"] == d["cpu_baseline"]["value"]

@@ -129,7 +129,7 @@ def test_cfg5_shapes_vs_fp64_oracle_on_one_window(relu):
 
 
 def test_lstm_tensor_core_vs_exact_fp32_at_cfg3_size():
-    """tcgen05 LSTM forward + BPTT + weight gradients against the exact-FFMA kernels ON DEVICE at cfg3's 262 144 rows."""
+    """tensor-core (wgmma) LSTM forward + BPTT + weight gradients against the exact-FFMA kernels ON DEVICE at cfg3's 262 144 rows."""
     from stmgcn_b200 import ops
     n, b, t, hid, lyr = 4096, 64, 12, 64, 3
     gen = torch.Generator().manual_seed(5)

@@ -216,7 +216,7 @@ def test_errors_are_loud():
 
 @pytest.mark.parametrize("rows_n,b,t,c", [(5, 60, 3, 1), (3, 50, 2, 2), (40, 64, 4, 1), (7, 36, 8, 1), (2, 1100, 4, 1)])
 def test_lstm_tensor_core_path_matches_exact_fp32_path(rows_n, b, t, c):
-    """tcgen05 3xTF32 LSTM forward vs the exact-FFMA kernels on the same inputs (ragged 128-row tiles)."""
+    """tensor-core (wgmma) LSTM forward vs the exact-FFMA kernels on the same inputs (ragged 128-row tiles)."""
     from stmgcn_b200 import ops
     hid, lyr = 64, 3
     gen = torch.Generator().manual_seed(rows_n * 100 + t)
@@ -247,7 +247,7 @@ def test_lstm_tensor_core_path_matches_exact_fp32_path(rows_n, b, t, c):
 # column (global-atomic adjoint path)
 @pytest.mark.parametrize("rows_n,b,t,c", [(5, 60, 3, 1), (40, 64, 4, 1), (3, 50, 2, 2), (7, 36, 8, 1), (2, 1100, 4, 1)])
 def test_lstm_tensor_core_backward_matches_exact_fp32_path(rows_n, b, t, c):
-    """tcgen05 fused BPTT kernel (pointwise in the loader + dA.Wp^T) vs the exact-FFMA kernels: d_s and all
+    """tensor-core (wgmma) fused BPTT kernel (pointwise in the loader + dA.Wp^T) vs the exact-FFMA kernels: d_s and all
     LSTM weight gradients (C=2 exercises the mixed case: layer 0 on FFMA, layers > 0 on tensor cores)."""
     from stmgcn_b200 import ops
     hid, lyr = 64, 3
@@ -327,7 +327,7 @@ def test_training_loop_like_model_trainer(tmp_path):
 
 @pytest.mark.parametrize("ks", [1, 3, 4, 6])
 def test_projection_tensor_core_path_matches_exact_fp32_path(ks):
-    """tcgen05 projection (fwd, dZ/U, dW) vs the exact-FFMA kernels; ks = 3 exercises the odd 64-row tail block of dW."""
+    """tensor-core (wgmma) projection (fwd, dZ/U, dW) vs the exact-FFMA kernels; ks = 3 exercises the odd 64-row tail block of dW."""
     from stmgcn_b200 import ops
     from stmgcn_b200.graph import GraphHandle, SupportSet
     n, b, p, q = 37, 9, 64, 64                                  # 333 rows: ragged 128-row tiles
