@@ -110,6 +110,75 @@ def lstm_explicit(x: torch.Tensor, layers: Sequence[Tuple[torch.Tensor, ...]],
     return seq, (torch.stack(h_n), torch.stack(c_n))
 
 
+def round_bf16(v: torch.Tensor) -> torch.Tensor:
+    """``v`` rounded to bf16 (round-to-nearest-even, from its fp32 value) in ``v``'s dtype; the gradient passes straight
+    through, like the kernels' bf16 stores."""
+    return v + (v.float().to(torch.bfloat16).to(v.dtype) - v).detach()
+
+
+def lstm_planes_reference(x: torch.Tensor, layers: Sequence[Tuple[torch.Tensor, ...]], planes: int = 2,
+                          h0: Optional[torch.Tensor] = None, c0: Optional[torch.Tensor] = None,
+                          tape: Optional[Dict[str, torch.Tensor]] = None):
+    """The arithmetic of the bf16-plane tensor-core LSTM (``lstm16.cu``) in the dtype of ``x`` (fp64 for tests),
+    differentiable by autograd.  Same contract as :func:`lstm_explicit`; ``x:(R,T,C)`` is the modulated input ``xo * s``.
+
+    ``planes = 2`` (hi + lo operand planes): exact operands, i.e. :func:`lstm_explicit`.  ``planes = 1`` (one bf16 plane):
+    the operands of the tensor-core products are rounded to bf16 -- the hidden states (h_below, h_prev, h0) and the MMA
+    weights (``W_hh`` of every layer, ``W_ih`` of layers > 0).  Layer 0's input term ``x W_ih^T``, the biases and the
+    cell state are not rounded (the kernels add them with fp32 FMAs).
+
+    ``tape`` (optional): the kernel's own tape as values of ``x``'s dtype -- ``h (L,T,R,H)`` (the hidden-state planes
+    summed), ``c (L,T,R,H)`` and, with an initial state, ``h0 (L,R,H)`` (its planes summed).  Every step then takes the
+    VALUES of h_below, h_prev and c_prev from the tape but routes their GRADIENT through this function's own h and c
+    (``operand = tape + (computed - computed.detach())``): the forward consumes what the kernel consumed, so a rounding
+    boundary that fp32 and fp64 see on different sides cannot propagate, and the autograd backward has the kernel
+    backward's semantics (gates recomputed from the tape, straight through the bf16 stores).
+
+    Returns ``(top-layer outputs (R,T,H), (h_n, c_n), (hs, cs))``; ``hs[l][t]`` / ``cs[l][t]`` are the computed states
+    of every layer-step (with a tape: step-local, i.e. one step of the recurrence from the kernel's own inputs).
+    """
+    if planes not in (1, 2):
+        raise ValueError(planes)
+    rnd = round_bf16 if planes == 1 else (lambda v: v)
+
+    def forced(computed, l, t, key):
+        if tape is None:
+            return computed
+        return (tape[key][l] if t is None else tape[key][l, t]) + (computed - computed.detach())
+
+    r, t_len, _ = x.shape
+    hid = layers[0][1].shape[1]
+    seq = x
+    h_n, c_n, hs_all, cs_all = [], [], [], []
+    for l, (w_ih, w_hh, b_ih, b_hh) in enumerate(layers):
+        w_in = w_ih if l == 0 else rnd(w_ih)
+        w_rec = rnd(w_hh)
+        h = x.new_zeros(r, hid) if h0 is None else h0[l]
+        c = x.new_zeros(r, hid) if c0 is None else c0[l]
+        if h0 is not None:
+            h = forced(h, l, None, "h0")
+        hs, cs = [], []
+        for t in range(t_len):
+            x_t = seq[t] if l > 0 else x[:, t]
+            if l > 0:
+                x_t = rnd(forced(x_t, l - 1, t, "h"))
+            h_op = rnd(h if t == 0 else forced(h, l, t - 1, "h"))
+            c_op = c if t == 0 else forced(c, l, t - 1, "c")
+            gates = x_t @ w_in.t() + h_op @ w_rec.t() + (b_ih + b_hh)
+            i, f, g, o = gates.split(hid, dim=1)
+            i, f, g, o = torch.sigmoid(i), torch.sigmoid(f), torch.tanh(g), torch.sigmoid(o)
+            c = f * c_op + i * g
+            h = o * torch.tanh(c)
+            hs.append(h)
+            cs.append(c)
+        seq = hs
+        h_n.append(h)
+        c_n.append(c)
+        hs_all.append(hs)
+        cs_all.append(cs)
+    return torch.stack(seq, dim=1), (torch.stack(h_n), torch.stack(c_n)), (hs_all, cs_all)
+
+
 def lstm_library(x: torch.Tensor, layers: Sequence[Tuple[torch.Tensor, ...]],
                  h0: Optional[torch.Tensor] = None, c0: Optional[torch.Tensor] = None):
     """Same contract as :func:`lstm_explicit` through ``torch.nn.LSTM`` -- the library call the
@@ -231,16 +300,22 @@ class SparseOracle:
     ``laplacians`` are scipy CSR matrices ``L~_m`` (``supports[1]`` of the reference, taken verbatim
     so a non-unit ``lambda_max`` or an asymmetric graph is handled, SURVEY.md section 0.3).
     Internal layout mirrors the CUDA path: node-major ``(N, B, p)`` feature rows.
+
+    ``relu_masks`` (optional, ReLU only): the ReLU masks to use instead of ``z > 0``, one boolean ``(N, B, q)`` array per
+    GCN in the order temporal graph 0, spatial graph 0, temporal graph 1, ...  With the masks a GPU run took, the oracle
+    follows the same branch of every ReLU, so a pre-activation within rounding distance of the kink cannot move the
+    gradients.
     """
 
     def __init__(self, params: Dict[str, np.ndarray], laplacians, n_supports: int, relu: bool = True,
-                 dtype=np.float64):
+                 dtype=np.float64, relu_masks=None):
         self.dt = np.dtype(dtype)
         self.p = {k: np.asarray(v, dtype=self.dt) for k, v in params.items()}
         self.lap = [l.astype(self.dt).tocsr() for l in laplacians]
         self.lap_t = [l.T.tocsr() for l in self.lap]
         self.ks = n_supports
         self.relu = relu
+        self.relu_masks = relu_masks
         self.m = len(self.lap)
         n = 0
         while f"rnn_list.0.lstm.weight_ih_l{n}" in self.p:
@@ -259,18 +334,31 @@ class SparseOracle:
             out.append(2.0 * (lap @ out[-1]) - out[-2])
         return np.stack(out).reshape((self.ks,) + x.shape)
 
-    def _gcn_fwd(self, lap, x, w, b):
+    def _gcn_pre(self, lap, x, w, b):
+        """-> (pre-activation z, stack)."""
         s = self._cheb_stack(lap, x)
         p = x.shape[-1]
         z = sum(s[k] @ w[k * p:(k + 1) * p] for k in range(self.ks))
         if b is not None:
             z = z + b
+        return z, s
+
+    def _gcn_fwd(self, lap, x, w, b):
+        z, s = self._gcn_pre(lap, x, w, b)
         return (np.maximum(z, 0) if self.relu else z), s
 
-    def _gcn_bwd(self, lap_t, s, out, d_out, w, need_dx: bool):
-        """Spec in SURVEY.md section 8(a) "Backward"."""
+    def _gcn_fwd_masked(self, lap, x, w, b, mask):
+        """:meth:`_gcn_fwd` with a given ReLU mask in place of ``z > 0``: ``out = z * mask``."""
+        z, s = self._gcn_pre(lap, x, w, b)
+        return z * mask, s
+
+    def _gcn_bwd(self, lap_t, s, out, d_out, w, need_dx: bool, mask=None):
+        """Spec in SURVEY.md section 8(a) "Backward".  ReLU mask: ``mask`` if given, else ``out > 0``."""
         p = s.shape[-1]
-        dz = d_out * (out > 0) if self.relu else d_out
+        if self.relu:
+            dz = d_out * (mask if mask is not None else (out > 0))
+        else:
+            dz = d_out
         db = dz.reshape(-1, dz.shape[-1]).sum(0)
         dw = np.concatenate([np.tensordot(s[k], dz, axes=([0, 1], [0, 1])) for k in range(self.ks)], 0)
         dx = None
@@ -362,7 +450,9 @@ class SparseOracle:
         for m in range(self.m):
             pre = f"rnn_list.{m}."
             wt, bt = self.p[pre + "gconv_temporal_feats.W"], self.p.get(pre + "gconv_temporal_feats.b")
-            gt, st = self._gcn_fwd(self.lap[m], xt, wt, bt)           # STMGCN.py:40
+            mt, ms = self.relu_masks[2 * m:2 * m + 2] if self.relu and self.relu_masks is not None else (None, None)
+            gt, st = (self._gcn_fwd(self.lap[m], xt, wt, bt) if mt is None            # STMGCN.py:40
+                      else self._gcn_fwd_masked(self.lap[m], xt, wt, bt, mt))
             z = (xt + gt).sum(0) / n                                  # :41-42  (B,T)
             fw, fb = self.p[pre + "fc.weight"], self.p[pre + "fc.bias"]
             a1 = z @ fw.T + fb
@@ -372,10 +462,11 @@ class SparseOracle:
             h_top, saved = self._lstm_fwd(rows, pre + "lstm.")        # :48-50
             hm = h_top.reshape(n, b_sz, -1)
             ws, bs = self.p[f"gcn_list.{m}.W"], self.p.get(f"gcn_list.{m}.b")
-            gs, ss = self._gcn_fwd(self.lap[m], hm, ws, bs)           # :114
+            gs, ss = (self._gcn_fwd(self.lap[m], hm, ws, bs) if ms is None            # :114
+                      else self._gcn_fwd_masked(self.lap[m], hm, ws, bs, ms))
             fused = gs if fused is None else fused + gs               # :116
             if keep:
-                tape.append(dict(st=st, gt=gt, z=z, a1=a1, r1=r1, s=s, saved=saved, ss=ss, gs=gs))
+                tape.append(dict(st=st, gt=gt, mt=mt, z=z, a1=a1, r1=r1, s=s, saved=saved, ss=ss, gs=gs, ms=ms))
         y = fused @ self.p["fc.weight"].T + self.p["fc.bias"]        # :118  (N,B,C)
         if keep:
             self._tape = dict(obs_nm=xo, fused=fused, per_graph=tape)
@@ -395,7 +486,7 @@ class SparseOracle:
             t = tp["per_graph"][m]
             pre = f"rnn_list.{m}."
             ws = self.p[f"gcn_list.{m}.W"]
-            dws, dbs, d_h = self._gcn_bwd(self.lap_t[m], t["ss"], t["gs"], d_fused, ws, True)
+            dws, dbs, d_h = self._gcn_bwd(self.lap_t[m], t["ss"], t["gs"], d_fused, ws, True, t["ms"])
             grads[f"gcn_list.{m}.W"] = dws
             if f"gcn_list.{m}.b" in self.p:
                 grads[f"gcn_list.{m}.b"] = dbs
@@ -414,7 +505,7 @@ class SparseOracle:
             d_z = d_a1 @ fw                                           # (B,T)
             d_gt = np.broadcast_to(d_z[None] / n, t["gt"].shape)
             wt = self.p[pre + "gconv_temporal_feats.W"]
-            dwt, dbt, _ = self._gcn_bwd(self.lap_t[m], t["st"], t["gt"], d_gt, wt, False)
+            dwt, dbt, _ = self._gcn_bwd(self.lap_t[m], t["st"], t["gt"], d_gt, wt, False, t["mt"])
             grads[pre + "gconv_temporal_feats.W"] = dwt
             if pre + "gconv_temporal_feats.b" in self.p:
                 grads[pre + "gconv_temporal_feats.b"] = dbt

@@ -396,9 +396,13 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     for (int i = tid; i < kGateCols; i += kBThreads) tail->db[i] = 0.f;
     if (L0) {
         for (int i = tid; i < p.c_in * kGateCols; i += kBThreads) wih_s[i] = p.wih[i] * gate_scale(i);
-        // auxiliary tiles (seg-1 slots): zero once; columns 0..C-1 are rewritten per item
+        // auxiliary tiles (seg-1 slots): zero once; columns 0..C-1 are rewritten per item.  One plane: the h_prev lo slot is
+        // never loaded; zeroed, it lets both warpgroups issue the lo-plane weight-gradient pass (see W_c)
         for (int i = tid; i < 2 * kATileBytes / 16; i += kBThreads)
             reinterpret_cast<uint4*>(a_sm + 2 * (size_t)kATileBytes)[i] = make_uint4(0u, 0u, 0u, 0u);
+        if (PLANES == 1)
+            for (int i = tid; i < kATileBytes / 16; i += kBThreads)
+                reinterpret_cast<uint4*>(a_sm + (size_t)kATileBytes)[i] = make_uint4(0u, 0u, 0u, 0u);
     }
     fence_proxy_async_smem();
     __syncthreads();
@@ -595,10 +599,12 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                     const uint64_t al = desc16_mn(wa_lo + ks * kStepMN, kATileBytes);
                     const uint64_t bh = desc16_mn(da_u + ks * kStepMN, kATileBytes);
                     const uint64_t bl = desc16_mn(da_u + kATileBytes + ks * kStepMN, kATileBytes);
-                    // dA always has its lo plane; in the single-plane mode only the STORED operands are rounded to bf16
+                    // dA always has its lo plane; in the single-plane mode only the STORED operands are rounded to bf16.
+                    // Layer 0's warpgroup 1 multiplies the auxiliary x*s tile, which is not stored: it keeps its lo plane in
+                    // both modes, as the forward's fp32 FMAs do (warpgroup 0's lo slot is zero then, and adds nothing)
                     wgmma_bf16_n64_t11(wgr, ah, bh, ks > 0 ? 1u : 0u);
                     wgmma_bf16_n64_t11(wgr, ah, bl, 1u);
-                    if (PLANES == 2) wgmma_bf16_n64_t11(wgr, al, bh, 1u);
+                    if (PLANES == 2 || L0) wgmma_bf16_n64_t11(wgr, al, bh, 1u);
                     // (both warpgroups issue it -- only warpgroup 0's result is used -- so that no wgmma sits on a
                     // warpgroup-dependent branch, which would make ptxas serialise every wgmma of the kernel)
                     wgmma_bf16_n64_rs_t1(bgr, ones, bh, ks > 0 ? 1u : 0u);

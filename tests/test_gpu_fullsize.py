@@ -47,30 +47,12 @@ def _build(w, batch, seed_x=100, relu=True):
     return model.to(DEV), [s.to(DEV) for s in sups_cpu], [_csr_of(s) for s in sups_cpu], params, x, y
 
 
-class _KinkAwareOracle(O.SparseOracle):
-    """SparseOracle that records, per GCN call, how close the closest pre-activation is to the ReLU kink."""
-
-    def __init__(self, *a, **k):
-        super().__init__(*a, **k)
-        self.kink = []                          # per _gcn_fwd call (order: temporal m0, spatial m0, temporal m1, ...)
-
-    def _gcn_fwd(self, lap, x, w, b):
-        s = self._cheb_stack(lap, x)
-        p = x.shape[-1]
-        z = sum(s[k] @ w[k * p:(k + 1) * p] for k in range(self.ks))
-        if b is not None:
-            z = z + b
-        self.kink.append(float(np.min(np.abs(z)) / max(float(np.max(np.abs(z))), 1e-30)))
-        return (np.maximum(z, 0) if self.relu else z), s
-
-
 def _check_subbatch(w, batch, picks, tol=TOL, relu=True):
-    """ReLU note.  With only a few windows carrying gradient, ONE pre-activation of a GCN that lands within rounding
-    distance of zero flips its ReLU mask between fp32 and fp64 and moves every gradient of that graph branch by ~1e-3
-    (one element out of ~10^6 active ones; measured: the same flip appears with the first- and the second-generation
-    kernels on different inputs, never in a full batch).  The fp32 reference itself has the same property.  So the ReLU
-    variant checks forward + loss strictly and the gradients of a branch strictly only when the oracle finds no
-    pre-activation closer than 1e-5 (relative) to the kink; the variant without activation (smooth) checks everything."""
+    """ReLU: the oracle takes the ReLU masks of the GPU's own grad-enabled forward (its GCN outputs > 0, picked windows
+    only).  With a few windows carrying gradient, one pre-activation within rounding distance of zero would otherwise flip
+    its mask between fp32 and fp64 and move every gradient of that graph branch by ~1e-3; with the GPU's masks the oracle
+    follows the same branch of every ReLU, and every gradient is held to ``tol``."""
+    from stmgcn_b200 import ops
     model, sups, laps, params, x, y = _build(w, batch, relu=relu)
     crit = nn.MSELoss(reduction="mean")
     xd = x.to(DEV)
@@ -79,29 +61,34 @@ def _check_subbatch(w, batch, picks, tol=TOL, relu=True):
     # targets: the run's own output everywhere except the picked windows
     y2 = out0.detach().clone()
     y2[picks] = y[picks].to(DEV)
-    out = model(obs_seq=xd, sta_adj_list=sups)
+    gcn_outs = []                       # per GCN call: temporal graph 0, spatial graph 0, temporal graph 1, ...
+    real_proj_fwd = ops._proj_fwd
+
+    def recording_proj_fwd(*a, **k):
+        out_ = real_proj_fwd(*a, **k)
+        gcn_outs.append(out_)
+        return out_
+    ops._proj_fwd = recording_proj_fwd
+    try:
+        out = model(obs_seq=xd, sta_adj_list=sups)
+    finally:
+        ops._proj_fwd = real_proj_fwd
+    assert len(gcn_outs) == 2 * w.n_graphs
     loss = crit(out, y2)
     loss.backward()
     torch.cuda.synchronize()
-    orc = _KinkAwareOracle(params, laps, w.n_supports, relu=relu, dtype=np.float64)
+    masks = [(g[:, picks] > 0).cpu().numpy() for g in gcn_outs] if relu else None
+    del gcn_outs
+    orc = O.SparseOracle(params, laps, w.n_supports, relu=relu, dtype=np.float64, relu_masks=masks)
     o_ref, l_ref, g_ref = orc.loss_and_grads(x[picks].numpy(), y[picks].numpy())
     scale = len(picks) / float(batch)
     errs = {"out": O.max_rel_err(out.detach()[picks].cpu().numpy(), o_ref),
             "loss": abs(loss.item() - l_ref * scale) / abs(l_ref * scale)}
     for key, p in model.named_parameters():
         errs["grad " + key] = O.max_rel_err(p.grad.cpu().numpy(), g_ref[key] * scale)
-    # a branch is "near a kink" if any of its two GCNs has a pre-activation within 1e-5 of zero (relative to max |z|)
-    near = [relu and min(orc.kink[2 * m], orc.kink[2 * m + 1]) < 1e-5 for m in range(w.n_graphs)]
-    print(f"{w.name} B={batch} relu={relu} windows {picks}: kink distance per branch "
-          f"{[f'{min(orc.kink[2 * m], orc.kink[2 * m + 1]):.1e}' for m in range(w.n_graphs)]}; max-norm relative errors vs "
-          f"the fp64 oracle: " + ", ".join(f"{k} {v:.2e}" for k, v in sorted(errs.items(), key=lambda kv: -kv[1])[:6]))
-
-    def tol_of(key):
-        for m in range(w.n_graphs):
-            if near[m] and (f"rnn_list.{m}." in key or f"gcn_list.{m}." in key):
-                return 5e-2
-        return tol
-    bad = {k: v for k, v in errs.items() if not (v <= tol_of(k))}
+    print(f"{w.name} B={batch} relu={relu} planes={ops.lstm_planes()} windows {picks}: max-norm relative errors vs the "
+          f"fp64 oracle: " + ", ".join(f"{k} {v:.2e}" for k, v in sorted(errs.items(), key=lambda kv: -kv[1])[:6]))
+    bad = {k: v for k, v in errs.items() if not (v <= tol)}
     assert not bad, f"{w.name} B={batch}: above tolerance: {bad}"
     assert bool(torch.isfinite(out).all())                  # every window, not only the picked ones
     return errs
@@ -126,6 +113,23 @@ def test_cfg5_shapes_vs_fp64_oracle_on_one_window(relu):
     """BASELINE configs[4] shapes: 16384 regions, 3 graphs at 1 % density, K=5 (six supports), T=24; batch 8 of 32."""
     from stmgcn_b200 import synth
     _check_subbatch(synth.WORKLOADS["cfg5"], 8, [5], relu=relu)
+
+
+@pytest.mark.parametrize("cfg,batch,picks", [("cfg2", 32, [0, 17, 31]), ("cfg5", 8, [5])])
+def test_bf16_mode_at_the_quoted_sizes_vs_fp64_oracle(cfg, batch, picks):
+    """BASELINE configs[1] and [4] are quoted in the bf16 arithmetic mode (ops.set_lstm_planes(1): one bf16 hidden-state
+    plane in the tensor-core LSTM, bf16 gather copies in the spatial Chebyshev recurrence, spmm_step16): the whole model at
+    those sizes against the fp64 oracle at the bf16 tolerance 2e-2 (SURVEY.md section 8(d)).  The model without the GCN
+    activation, as in test_gpu_parity.py: bf16-level noise flips ReLU masks, which says nothing about the kernels.
+    tests/test_gpu_lstm16.py is the tight check of the LSTM arithmetic in this mode; this is the end-to-end bound."""
+    from stmgcn_b200 import ops, synth
+    old = ops.lstm_planes()
+    try:
+        ops.set_lstm_planes(1)
+        errs = _check_subbatch(synth.WORKLOADS[cfg], batch, picks, tol=2e-2, relu=False)
+    finally:
+        ops.set_lstm_planes(old)
+    assert errs["out"] > 1e-6, "the bf16 mode produced fp32-grade results: the single-plane path did not run"
 
 
 def test_lstm_tensor_core_vs_exact_fp32_at_cfg3_size():

@@ -137,3 +137,138 @@ def test_dense_matches_reference_modules():
     assert set(g2) >= set(grads) and len(grads) > 0
     for key in grads:
         assert_close(g2[key].numpy(), grads[key], f"grad {key}", 2e-5)
+
+
+def _rand_lstm(seed, c_in, hid, n_layers, rows, t_len, scale=0.3):
+    gen = torch.Generator().manual_seed(seed)
+    layers = []
+    for l in range(n_layers):
+        in_l = c_in if l == 0 else hid
+        layers.append(tuple((torch.randn(*s, generator=gen, dtype=torch.float64) * scale).requires_grad_(True)
+                            for s in ((4 * hid, in_l), (4 * hid, hid), (4 * hid,), (4 * hid,))))
+    x = torch.randn(rows, t_len, c_in, generator=gen, dtype=torch.float64).requires_grad_(True)
+    return gen, layers, x
+
+
+def test_round_bf16_is_bf16_rounding_with_a_straight_through_gradient():
+    v = (torch.randn(1000, dtype=torch.float64) * 3).requires_grad_(True)
+    r = O.round_bf16(v)
+    assert torch.equal(r.detach(), v.detach().float().to(torch.bfloat16).double())
+    err = (r - v).detach().abs()
+    assert 0 < float(err.max()) and bool((err <= v.detach().abs() * 2.0 ** -8).all())      # half an ulp: 8 significant bits
+    r.backward(torch.arange(1000, dtype=torch.float64))
+    assert torch.equal(v.grad, torch.arange(1000, dtype=torch.float64))
+
+
+def test_lstm_planes_reference_two_planes_equals_the_lstm_oracles():
+    """Two planes, no tape: the reference of the tensor-core LSTM is plain nn.LSTM arithmetic -- outputs equal
+    lstm_explicit (with an initial state), autograd gradients equal SparseOracle's hand-written BPTT, to fp64 rounding."""
+    hid, lyr, rows, t_len, c_in = 8, 3, 5, 6, 2
+    gen, layers, x = _rand_lstm(0, c_in, hid, lyr, rows, t_len)
+    h0, c0 = (torch.randn(lyr, rows, hid, generator=gen, dtype=torch.float64) * 0.3 for _ in range(2))
+    seq, (hn, cn), (hs, cs) = O.lstm_planes_reference(x, layers, 2, h0, c0)
+    seq_e, (hn_e, cn_e) = O.lstm_explicit(x, layers, h0, c0)
+    for a, b, what in ((seq, seq_e, "seq"), (hn, hn_e, "h_n"), (cn, cn_e, "c_n"),
+                       (torch.stack(hs[-1], 1), seq_e, "hs"), (torch.stack([c[-1] for c in cs]), cn_e, "cs")):
+        assert_close(a.detach().numpy(), b.detach().numpy(), what, 1e-14)
+    # gradients (no initial state: the sparse oracle's LSTM starts from zeros)
+    seq, _, _ = O.lstm_planes_reference(x, layers, 2)
+    d_top = torch.randn(rows, hid, generator=gen, dtype=torch.float64)
+    flat = [w for layer in layers for w in layer]
+    got = torch.autograd.grad((seq[:, -1] * d_top).sum(), [x] + flat)
+    pre = "rnn_list.0.lstm."
+    params = {}
+    for l, layer in enumerate(layers):
+        for name, w in zip(("weight_ih", "weight_hh", "bias_ih", "bias_hh"), layer):
+            params[f"{pre}{name}_l{l}"] = w.detach().numpy()
+    orc = O.SparseOracle(params, [], 1)
+    h_top, saved = orc._lstm_fwd(x.detach().numpy(), pre)
+    assert_close(seq[:, -1].detach().numpy(), h_top, "h_top vs SparseOracle", 1e-14)
+    grads = {}
+    dx = orc._lstm_bwd(d_top.numpy(), saved, pre, grads)
+    assert_close(got[0].numpy(), dx, "dx vs SparseOracle", 1e-12)
+    for i, g in enumerate(got[1:]):
+        l, j = divmod(i, 4)
+        name = ("weight_ih", "weight_hh", "bias_ih", "bias_hh")[j]
+        assert_close(g.numpy(), grads[f"{pre}{name}_l{l}"], f"{name}_l{l} vs SparseOracle", 1e-12)
+
+
+@pytest.mark.parametrize("planes", [1, 2])
+def test_lstm_planes_reference_tape_forcing_with_its_own_states_changes_nothing(planes):
+    """Forcing the reference with a tape of its own states leaves outputs and autograd gradients unchanged: tape forcing
+    only replaces VALUES, the gradient still flows through the computed states."""
+    hid, lyr, rows, t_len, c_in = 8, 2, 4, 5, 3
+    gen, layers, x = _rand_lstm(1, c_in, hid, lyr, rows, t_len)
+    h0, c0 = (torch.randn(lyr, rows, hid, generator=gen, dtype=torch.float64) * 0.3 for _ in range(2))
+    d_top = torch.randn(rows, hid, generator=gen, dtype=torch.float64)
+    flat = [x] + [w for layer in layers for w in layer]
+    seq, _, (hs, cs) = O.lstm_planes_reference(x, layers, planes, h0, c0)
+    ref = torch.autograd.grad((seq[:, -1] * d_top).sum(), flat)
+    tape = dict(h=torch.stack([torch.stack(v) for v in hs]).detach(), c=torch.stack([torch.stack(v) for v in cs]).detach(),
+                h0=h0)
+    seq_f, _, (hs_f, cs_f) = O.lstm_planes_reference(x, layers, planes, h0, c0, tape=tape)
+    got = torch.autograd.grad((seq_f[:, -1] * d_top).sum(), flat)
+    assert torch.allclose(seq_f, seq, rtol=0, atol=1e-15)
+    for a, b in zip(got, ref):
+        assert torch.allclose(a, b, rtol=1e-13, atol=1e-15)
+    # one plane: the operands of the tensor-core products are bf16 -- a bf16-level change, far above fp64 rounding
+    if planes == 1:
+        seq2, _, _ = O.lstm_planes_reference(x, layers, 2, h0, c0)
+        assert 1e-4 < O.max_rel_err(seq.detach().numpy(), seq2.detach().numpy()) < 2e-2
+
+
+def test_lstm_planes_reference_rounds_only_the_tensor_core_operands():
+    """One plane: h operands, W_hh and W_ih of layers > 0 are rounded to bf16; layer 0's W_ih (the fp32 FMA input term)
+    and the biases are not.  A change far below one bf16 ulp moves the output only through the unrounded operands."""
+    hid, lyr, rows, t_len, c_in = 8, 2, 3, 2, 1
+    _, layers, x = _rand_lstm(2, c_in, hid, lyr, rows, t_len)
+    def cells(ls):                     # the cell states of every layer-step (a change in h can vanish in its rounding)
+        _, _, (_, cs) = O.lstm_planes_reference(x, ls, 1)
+        return torch.stack([torch.stack(c) for c in cs])
+
+    base = cells(layers)
+    for l, j, moves in ((0, 0, True), (0, 1, False), (0, 2, True), (1, 0, False), (1, 1, False), (1, 3, True)):
+        pert = [list(layer) for layer in layers]
+        pert[l][j] = pert[l][j] + 1e-9 * torch.sign(pert[l][j].detach())
+        assert bool((cells(pert) != base).any()) == moves, (l, j)
+
+
+def test_sparse_oracle_relu_masks():
+    """SparseOracle(relu_masks=...): the oracle's own masks (z > 0) change nothing; a flipped mask entry is followed in
+    the forward (out = z * mask) and in the backward.  Without an activation the masks are ignored."""
+    from stmgcn_b200 import synth
+    n, m, k, t, b, c, hid, lyr, g = 15, 2, 2, 4, 2, 1, 8, 2, 6
+    gen = torch.Generator().manual_seed(3)
+    sups = [O.chebyshev_supports_dense(synth.make_adjacency(n, i, 0.3), k) for i in range(m)]
+    params = {k_: v.numpy() for k_, v in O.init_params(m, t, c, hid, lyr, g, k + 1, seed=3).items()}
+    x, y = torch.randn(b, t, n, c, generator=gen).numpy(), torch.randn(b, n, c, generator=gen).numpy()
+    laps = [O.laplacian_csr_from_supports(s) for s in sups]
+
+    class Recording(O.SparseOracle):
+        def _gcn_fwd(self, lap, x_, w, b_):
+            z, s = self._gcn_pre(lap, x_, w, b_)
+            self.z.append(z)
+            return super()._gcn_fwd(lap, x_, w, b_)
+
+    rec = Recording(params, laps, k + 1)
+    rec.z = []
+    o0, l0, g0 = rec.loss_and_grads(x, y)
+    masks = [z > 0 for z in rec.z]
+    o1, l1, g1 = O.SparseOracle(params, laps, k + 1, relu_masks=masks).loss_and_grads(x, y)
+    assert np.array_equal(o0, o1) and l0 == l1 and all(np.array_equal(g0[key], g1[key]) for key in g0)
+    # flip the mask entry with the smallest |z| of graph 1's spatial GCN: the output moves by exactly that entry's change
+    # (max(z, 0) -> z * mask) through the output layer, and the gradients follow the flipped branch
+    z = rec.z[3]
+    idx = np.unravel_index(np.argmin(np.abs(z)), z.shape)
+    flipped = [mk.copy() for mk in masks]
+    flipped[3][idx] = ~flipped[3][idx]
+    o2, _, g2 = O.SparseOracle(params, laps, k + 1, relu_masks=flipped).loss_and_grads(x, y)
+    want = o0.copy()
+    delta = z[idx] * (1.0 if flipped[3][idx] else -1.0)            # out[idx] goes from max(z, 0) to z * mask
+    fc_w = params["fc.weight"].astype(np.float64)
+    want[idx[1], idx[0], :] += delta * fc_w[:, idx[2]]
+    assert np.allclose(o2, want, rtol=0, atol=1e-12)
+    assert any(not np.array_equal(g0[key], g2[key]) for key in g0)
+    o3, _, g3 = O.SparseOracle(params, laps, k + 1, relu=False, relu_masks=flipped).loss_and_grads(x, y)
+    o4, _, g4 = O.SparseOracle(params, laps, k + 1, relu=False).loss_and_grads(x, y)
+    assert np.array_equal(o3, o4) and all(np.array_equal(g3[key], g4[key]) for key in g3)
