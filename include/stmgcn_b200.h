@@ -183,8 +183,7 @@ int32_t stmgcn_lstm16_step_fwd(int32_t t, int32_t t_len, int32_t n_layers, int64
 int32_t stmgcn_lstm16_grid(int64_t rows);
 /* BPTT of ONE layer through all timesteps T-1 .. 0 (call the layers top-down): recomputes the gates from hp, forms dA,
  * accumulates the weight and bias gradients and propagates [dx_below | dh_prev].  A tile's rows never mix with other
- * tiles', so each CTA walks its own tiles through time inside a launch; a launch covers as many consecutive timesteps as
- * keep a CTA's weight-gradient accumulation chain within 6144 rows (cfg3: 3 steps, 4 launches per layer).  T <= 64.
+ * tiles', so each CTA walks its own tiles through time inside the layer's one launch.  T <= 64.
  * Workspaces (tile-blocked, R_pad = ceil(R/128)*128 rows; none needs initialisation):
  *   dh_in : top layer: d_top (R_pad,64), the gradient of the top layer's last hidden state; other layers: the dx_out
  *           (T,R_pad,64) the layer above wrote;      dx_out: (T,R_pad,64), NULL for layer 0;

@@ -323,11 +323,7 @@ inline int32_t launch_tall(const ASegs& a, int64_t rows, int kd, const float* bm
                            const Epi& epi, cudaStream_t st, const char* what) {
     using Cfg = TallCfg<TN>;
     auto kern = tall_gemm_kernel<TN, VEC, Epi>;
-    static bool attr_done = false;      // per instantiation
-    if (!attr_done) {
-        STMGCN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        attr_done = true;
-    }
+    if (int32_t rc = ensure_dyn_smem((const void*)kern, Cfg::SMEM)) return rc;
     dim3 grid((unsigned)ceil_div(rows, Cfg::TM), (unsigned)ceil_div(nc, TN));
     kern<<<grid, kGemmThreads, Cfg::SMEM, st>>>(a, rows, kd, bmat, ldb, nc, epi);
     count_launch();
@@ -339,11 +335,7 @@ inline int32_t launch_reduce(const ASegs& a, const ReduceTime& tm, int64_t rows,
                              int64_t ldd, int nc, float* gout, int ldg, cudaStream_t st, const char* what) {
     using Cfg = ReduceCfg<TN>;
     auto kern = reduce_gemm_kernel<TN, VEC>;
-    static bool attr_done = false;
-    if (!attr_done) {
-        STMGCN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        attr_done = true;
-    }
+    if (int32_t rc = ensure_dyn_smem((const void*)kern, Cfg::SMEM)) return rc;
     const int64_t total_chunks = ceil_div(rows, kKC) * tm.n_t;
     const int panels = (int)(ceil_div(kd, Cfg::TMK) * ceil_div(nc, TN));
     int64_t gx = (int64_t)sm_count() / (panels > 0 ? panels : 1);

@@ -33,23 +33,28 @@ int32_t check_launch(const char* what) {
     return 0;
 }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+// SMs of the current device.  If the device query fails, the H100 SXM's 132: only grid sizes depend on it, and the
+// launch that follows reports the device error itself.
 int sm_count() {
+    constexpr int kFallback = 132;
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kFallback;
     if (cached[dev] == 0) {
         int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = kFallback;
         cached[dev] = v;
     }
     return cached[dev];
 }
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a PER-DEVICE attribute: remember (kernel, device) pairs, not a
-// process-wide flag, so a model moved to another GPU of the same process still launches (ADVICE r1); mutex: the forward
-// thread and the autograd thread may both get here first.
+// process-wide flag, so a model moved to another GPU of the same process still launches; mutex: the forward thread and
+// the autograd thread may both get here first.  The library registers 37 kernels: 12 lstm16 forward / backward variants,
+// 3 in proj_tc.cu, 18 tall_gemm_kernel and 4 reduce_gemm_kernel instances; a kernel past the table would set the
+// attribute on every launch.
 int32_t ensure_dyn_smem(const void* kernel, size_t bytes) {
-    constexpr int kMaxKernels = 32, kMaxDev = 64;
+    constexpr int kMaxKernels = 64, kMaxDev = 64;
     static std::mutex mu;
     static const void* kernels[kMaxKernels] = {};
     static bool done[kMaxKernels][kMaxDev] = {};

@@ -78,6 +78,36 @@ __device__ __forceinline__ void lstm_cell_gates8(float ai, float af, float ag, f
     tc = (1.f - ec) * rcp_ftz_(1.f + ec);
 }
 
+// ---- pieces of the cell epilogue shared by the forward and the backward kernel ----------------------------------
+// Accumulator values d[4j .. 4j+3] (gate-interleaved columns, see the forward kernel) -> pre-activations (i, f, g, o) of
+// this thread's cell: partner lanes (lane ^ 1) swap one row's pair.
+template <int R>
+__device__ __forceinline__ float4 frag_to_gates(const float (&d)[R], int j, bool odd) {
+    const float s0 = odd ? d[4 * j + 0] : d[4 * j + 2];
+    const float s1 = odd ? d[4 * j + 1] : d[4 * j + 3];
+    const float o0 = __shfl_xor_sync(0xffffffffu, s0, 1);
+    const float o1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+    return make_float4(odd ? o0 : d[4 * j + 0], odd ? o1 : d[4 * j + 1], odd ? d[4 * j + 2] : o0, odd ? d[4 * j + 3] : o1);
+}
+// exponent arguments of (i, f, g, o): pre-activation times the gate's exponent factor plus the scaled bias b, and on
+// layer 0 plus x*s . W_ih (wih: the scaled, gate-interleaved (C, 256) W_ih^T in shared memory)
+template <int CIN>
+__device__ __forceinline__ float4 gate_args(float4 v, float4 b, const float (&xs)[kMaxC], const float* wih, int col, int c_in) {
+    constexpr int kC = (CIN == 1) ? 1 : kMaxC;
+    float4 a = make_float4(fmaf(v.x, -1.4426950408889634f, b.x), fmaf(v.y, -1.4426950408889634f, b.y),
+                           fmaf(v.z, -2.8853900817779268f, b.z), fmaf(v.w, -1.4426950408889634f, b.w));
+    if (CIN > 0) {
+#pragma unroll
+        for (int c = 0; c < kC; ++c)
+            if (CIN == 1 || c < c_in) {
+                const float4 wv = *reinterpret_cast<const float4*>(&wih[c * kGateCols + col]);
+                a.x = fmaf(xs[c], wv.x, a.x); a.y = fmaf(xs[c], wv.y, a.y);
+                a.z = fmaf(xs[c], wv.z, a.z); a.w = fmaf(xs[c], wv.w, a.w);
+            }
+    }
+    return a;
+}
+
 // =====================================================================================================
 // forward
 // =====================================================================================================
@@ -172,7 +202,7 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
                     for (int pl = 0; pl < PLANES; ++pl, ++it) {
                         const int stg = it % kFStages;
                         const uint32_t ph = (it / kFStages) & 1;
-                        mbar_wait_p(&tail->empty[stg], ph ^ 1, 0);
+                        mbar_wait_polite(&tail->empty[stg], ph ^ 1);
                         mbar_arrive_expect_tx(&tail->full[stg], kATileBytes);
                         tma_load_3d(stages + (size_t)stg * kATileBytes, &p.amap[s], 0, tile * kTileM, p.aslice[s] + pl,
                                     &tail->full[stg]);
@@ -191,7 +221,7 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
     float acc[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    if (p.nseg > 0) mbar_wait(&tail->w_full, 0, 0);
+    if (p.nseg > 0) mbar_wait_raw(&tail->w_full, 0);
     uint32_t it = 0;
     for (int i = 0; i < my_tiles; ++i) {
         const int tile = (int)blockIdx.x + i * (int)gridDim.x;
@@ -212,7 +242,7 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
 #pragma unroll
             for (int pl = 0; pl < PLANES; ++pl, ++it) {
                 const int stg = it % kFStages;
-                mbar_wait(&tail->full[stg], (it / kFStages) & 1, 1);
+                mbar_wait_raw(&tail->full[stg], (it / kFStages) & 1);
                 const uint64_t a_d = desc16_k(a_u + (uint32_t)stg * kATileBytes);
                 wg_fence();
 #pragma unroll
@@ -237,32 +267,15 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
         const uint32_t cbase = (uint32_t)tile * 8192u + row_in_tile * 4u;
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
-            const float s0 = odd ? acc[4 * j + 0] : acc[4 * j + 2];
-            const float s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
-            const float o0 = __shfl_xor_sync(0xffffffffu, s0, 1);
-            const float o1 = __shfl_xor_sync(0xffffffffu, s1, 1);
-            const float vi = odd ? o0 : acc[4 * j + 0], vf = odd ? o1 : acc[4 * j + 1];
-            const float vg = odd ? acc[4 * j + 2] : o0, vo = odd ? acc[4 * j + 3] : o1;
+            const float4 v = frag_to_gates(acc, j, odd);
             const int unit = 2 * j + (q >> 1);
             const int col = 4 * unit;
             const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
-            float pi = fmaf(vi, -1.4426950408889634f, bv.x);
-            float pf = fmaf(vf, -1.4426950408889634f, bv.y);
-            float pg = fmaf(vg, -2.8853900817779268f, bv.z);
-            float po = fmaf(vo, -1.4426950408889634f, bv.w);
-            if (L0) {
-#pragma unroll
-                for (int c = 0; c < kC; ++c)
-                    if (CIN == 1 || c < p.c_in) {
-                        const float4 wv = *reinterpret_cast<const float4*>(&tail->wih[c * kGateCols + col]);
-                        pi = fmaf(xs[c], wv.x, pi); pf = fmaf(xs[c], wv.y, pf);
-                        pg = fmaf(xs[c], wv.z, pg); po = fmaf(xs[c], wv.w, po);
-                    }
-            }
+            const float4 a = gate_args<CIN>(v, bv, xs, tail->wih, col, p.c_in);
             const uint32_t co = cbase + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
             const float cp = (p.c_prev != nullptr && valid) ? p.c_prev[co] : 0.f;
             float cn, hn;
-            lstm_cell_fwd8(pi, pf, pg, po, cp, cn, hn);
+            lstm_cell_fwd8(a.x, a.y, a.z, a.w, cp, cn, hn);
             if (valid) {
                 p.c_out[co] = cn;
                 const uint32_t ho = r * (uint32_t)kHid + (uint32_t)unit;
@@ -305,7 +318,7 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
 
 // =====================================================================================================
 // backward: gate recompute + BPTT pointwise + data gradient + weight gradient in ONE kernel, time-fused per layer
-// (a launch = one layer x a run of timesteps, see Bwd16Params; "item" below = one (step, tile) work item)
+// (a launch = one layer x all its timesteps, see Bwd16Params; "item" below = one (step, tile) work item)
 // =====================================================================================================
 // CTA = two consumer warpgroups (warpgroup w: rows 64w .. 64w+63 of a tile) + one producer warp.  The layer's weight image
 // stays resident in shared memory; the producer streams the A planes ([h_below | h_prev], hi and lo) of each item with
@@ -331,7 +344,7 @@ struct B16Tail {
 constexpr size_t kBSmem = 1024 + 4 * (size_t)kWTileBytes + kBATiles * (size_t)kATileBytes + 2 * (size_t)kATileBytes + sizeof(B16Tail);
 static_assert(kBSmem <= 232448, "lstm16 backward kernel exceeds the 227 KB shared-memory limit");
 
-// One launch = one LAYER, a run of timesteps from T-1 down (the tiles of a CTA are its own through time: rows never mix).
+// One launch = one LAYER, its timesteps from T-1 down (the tiles of a CTA are its own through time: rows never mix).
 // A step of a tile needs what the SAME CTA produced for that tile one step later (dh_rec, dc: global, in place), so nothing
 // but the launch order of the layers (top down) synchronises.
 constexpr int kBMaxSteps = 64;
@@ -421,7 +434,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             for (int w = 0; w < n_items; ++w) {
                 const int st = w / my_tiles, tile = (int)blockIdx.x + (w - st * my_tiles) * (int)gridDim.x;
                 const Bwd16Step& sp = p.steps[st];
-                mbar_wait_p(&tail->a_empty, (uint32_t)(w & 1) ^ 1u, 0);
+                mbar_wait_polite(&tail->a_empty, (uint32_t)(w & 1) ^ 1u);
                 mbar_arrive_expect_tx(&tail->a_full, (uint32_t)(kNseg * PLANES * kATileBytes));
                 for (int sg = 0; sg < kNseg; ++sg)
                     for (int pl = 0; pl < PLANES; ++pl) {
@@ -457,7 +470,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     uint32_t ones[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) ones[k] = 0x3f803f80u;                // bf16 pair (1, 1)
-    mbar_wait(&tail->w_full, 0, 0);
+    mbar_wait_raw(&tail->w_full, 0);
 
     for (int w = 0; w < n_items; ++w) {
         const int st = w / my_tiles, tile = (int)blockIdx.x + (w - st * my_tiles) * (int)gridDim.x;
@@ -486,7 +499,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             *reinterpret_cast<uint2*>(a_sm + 2 * (size_t)kATileBytes + off) = make_uint2(hi[0], hi[1]);
             *reinterpret_cast<uint2*>(a_sm + 3 * (size_t)kATileBytes + off) = make_uint2(lo[0], lo[1]);
         }
-        mbar_wait(&tail->a_full, (uint32_t)w & 1u, 1);
+        mbar_wait_raw(&tail->a_full, (uint32_t)w & 1u);
         float dacc[32 * kNseg];                                    // [dx_below | dh_prev] (layer 0: [dh_prev])
 #pragma unroll
         for (int k = 0; k < 32 * kNseg; ++k) dacc[k] = 0.f;
@@ -520,28 +533,13 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             const uint32_t bo = (uint32_t)tile * 8192u + row_in_tile * 4u;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const float s0 = odd ? g[4 * j + 0] : g[4 * j + 2];
-                const float s1 = odd ? g[4 * j + 1] : g[4 * j + 3];
-                const float o0 = __shfl_xor_sync(0xffffffffu, s0, 1);
-                const float o1 = __shfl_xor_sync(0xffffffffu, s1, 1);
-                const float vi = odd ? o0 : g[4 * j + 0], vf = odd ? o1 : g[4 * j + 1];
-                const float vg = odd ? g[4 * j + 2] : o0, vo = odd ? g[4 * j + 3] : o1;
+                const float4 v = frag_to_gates(g, j, odd);
                 const int unit = 16 * c + 2 * j + (q >> 1);
                 const int col = 4 * unit;
-                const float4 bv = *reinterpret_cast<const float4*>(p.bias + col);
-                float pi = fmaf(vi, -1.4426950408889634f, bv.x * -1.4426950408889634f);
-                float pf = fmaf(vf, -1.4426950408889634f, bv.y * -1.4426950408889634f);
-                float pg = fmaf(vg, -2.8853900817779268f, bv.z * -2.8853900817779268f);
-                float po = fmaf(vo, -1.4426950408889634f, bv.w * -1.4426950408889634f);
-                if (L0) {
-#pragma unroll
-                    for (int cc = 0; cc < kC; ++cc)
-                        if (CIN == 1 || cc < p.c_in) {
-                            const float4 wv = *reinterpret_cast<const float4*>(&wih_s[cc * kGateCols + col]);
-                            pi = fmaf(xs[cc], wv.x, pi); pf = fmaf(xs[cc], wv.y, pf);
-                            pg = fmaf(xs[cc], wv.z, pg); po = fmaf(xs[cc], wv.w, po);
-                        }
-                }
+                const float4 bv = *reinterpret_cast<const float4*>(p.bias + col);     // scaled here (gate_scale)
+                const float4 a = gate_args<CIN>(v, make_float4(bv.x * -1.4426950408889634f, bv.y * -1.4426950408889634f,
+                                                               bv.z * -2.8853900817779268f, bv.w * -1.4426950408889634f),
+                                                xs, wih_s, col, p.c_in);
                 const uint32_t o = bo + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
                 float cp = 0.f, dh = 0.f, dci = 0.f;
                 if (valid) {
@@ -553,7 +551,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                     }
                 }
                 float gi, gf, gg, go, tc_;
-                lstm_cell_gates8(pi, pf, pg, po, cp, gi, gf, gg, go, tc_);
+                lstm_cell_gates8(a.x, a.y, a.z, a.w, cp, gi, gf, gg, go, tc_);
                 // rows past the end: dh = dci = 0, so dA = 0
                 const float dcv = fmaf(dh * go, 1.f - tc_ * tc_, dci);
                 const float da0 = dcv * gg * gi * (1.f - gi);
@@ -755,7 +753,37 @@ bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t sl
               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static int32_t set_smem_attr(const void* fn, size_t bytes) { return ensure_dyn_smem(fn, bytes); }
+// The K segments of layer l at step t, in the order of the weight image's segments, and the cell state the step continues:
+// layers > 0 first read h of the layer below at step t; then h_prev: hp at t - 1, at t = 0 the initial state h0p if
+// there is one, else nothing (zeros, STMGCN.py:53-57).
+enum SegSrc { kSegHp = 0, kSegH0p = 1, kSegAbsent = 2 };     // = Bwd16Step::src
+struct StepSegs {
+    int nseg;                  // layers > 0: 2 (h_below, h_prev); layer 0: 1 (h_prev)
+    int src[2];                // SegSrc
+    int slice[2];              // the segment's hi-plane slice in its tensor (lo = + 1); 0 when absent
+    const float* c_prev;       // blocked or nullptr (zeros)
+};
+static StepSegs step_segs(int l, int t, int t_len, int planes, bool has_h0, const float* cs, const float* c0,
+                          int64_t cslice) {
+    StepSegs g{};
+    if (l > 0) {
+        g.src[g.nseg] = kSegHp;
+        g.slice[g.nseg] = ((l - 1) * t_len + t) * planes;
+        ++g.nseg;
+    }
+    if (t > 0) {
+        g.src[g.nseg] = kSegHp;
+        g.slice[g.nseg] = (l * t_len + t - 1) * planes;
+    } else if (has_h0) {
+        g.src[g.nseg] = kSegH0p;
+        g.slice[g.nseg] = l * planes;
+    } else {
+        g.src[g.nseg] = kSegAbsent;
+    }
+    ++g.nseg;
+    g.c_prev = t > 0 ? cs + (int64_t)(l * t_len + t - 1) * cslice : (c0 ? c0 + (int64_t)l * cslice : nullptr);
+    return g;
+}
 
 // kernel variant for (planes, cin): cin = 0 (not layer 0), 1 (layer 0, one input channel), kMaxC (layer 0, runtime count)
 using FwdFn = void (*)(const Fwd16Params);
@@ -798,8 +826,8 @@ extern "C" int32_t stmgcn_lstm16_step_fwd(int32_t t, int32_t t_len, int32_t n_la
     const int64_t plane_elems = rows * kHid;                       // bf16 elements per plane
     const int64_t cslice = rows_pad * kHid;
     const FwdFn fn0 = fwd_kernel_for(planes, c_in == 1 ? 1 : kMaxC), fn1 = fwd_kernel_for(planes, 0);
-    if (int32_t rc = set_smem_attr((const void*)fn0, kFSmem)) return rc;
-    if (int32_t rc = set_smem_attr((const void*)fn1, kFSmem)) return rc;
+    if (int32_t rc = ensure_dyn_smem((const void*)fn0, kFSmem)) return rc;
+    if (int32_t rc = ensure_dyn_smem((const void*)fn1, kFSmem)) return rc;
     CUtensorMap hp_map, h0_map;
     STMGCN_REQUIRE(make_plane_map(&hp_map, hp, rows, (int64_t)n_layers * t_len * planes), STMGCN_ERR_STATE,
                    "lstm16_step_fwd: cuTensorMapEncodeTiled failed (hp)");
@@ -811,24 +839,15 @@ extern "C" int32_t stmgcn_lstm16_step_fwd(int32_t t, int32_t t_len, int32_t n_la
         STMGCN_REQUIRE(wimg[l] && bias[l], STMGCN_ERR_ARG, "lstm16_step_fwd: wimg/bias[%d] null", l);
         Fwd16Params p;
         memset(&p, 0, sizeof(p));
-        int ns = 0;
-        if (l > 0) {                                               // segment: h of the layer below at this step
-            p.amap[ns] = hp_map;
-            p.aslice[ns] = ((l - 1) * t_len + t) * planes;
-            ++ns;
+        const StepSegs g = step_segs(l, t, t_len, planes, h0p != nullptr, cs, c0, cslice);
+        // the weight image holds [seg0 hi | seg0 lo | seg1 hi | seg1 lo]; an absent h_prev segment is the last one and is
+        // dropped: layers > 0 then use only seg 0 (W_ih), layer 0 has no MMA at all
+        for (int s = 0; s < g.nseg; ++s) {
+            if (g.src[s] == kSegAbsent) continue;
+            p.amap[p.nseg] = g.src[s] == kSegHp ? hp_map : h0_map;
+            p.aslice[p.nseg] = g.slice[s];
+            ++p.nseg;
         }
-        if (t > 0) {                                               // segment: this layer's h of the previous step
-            p.amap[ns] = hp_map;
-            p.aslice[ns] = (l * t_len + t - 1) * planes;
-            ++ns;
-        } else if (h0p != nullptr) {
-            p.amap[ns] = h0_map;
-            p.aslice[ns] = l * planes;
-            ++ns;
-        }
-        p.nseg = ns;
-        // the weight image holds [seg0 hi | seg0 lo | seg1 hi | seg1 lo]; at t = 0 without h0 the h_prev segment is absent:
-        // layers > 0 then use only seg 0 (W_ih), layer 0 has no MMA at all
         p.wimg = (const uint8_t*)wimg[l];
         p.bias = bias[l];
         p.wih = (l == 0) ? wih_t : nullptr;
@@ -838,7 +857,7 @@ extern "C" int32_t stmgcn_lstm16_step_fwd(int32_t t, int32_t t_len, int32_t n_la
         p.t = t;
         p.t_len = t_len;
         p.b_inner = b_inner;
-        p.c_prev = t > 0 ? cs + (int64_t)(l * t_len + t - 1) * cslice : (c0 ? c0 + (int64_t)l * cslice : nullptr);
+        p.c_prev = g.c_prev;
         p.c_out = cs + (int64_t)(l * t_len + t) * cslice;
         uint16_t* hbase = (uint16_t*)hp + (int64_t)(l * t_len + t) * planes * plane_elems;
         p.h_hi = hbase;
@@ -884,7 +903,7 @@ extern "C" int32_t stmgcn_lstm16_layer_bwd(int32_t layer, int32_t t_len, int32_t
     const int64_t cslice = (int64_t)n_tiles * kTileM * kHid;
     const int l = layer;
     const BwdFn fn = bwd_kernel_for(planes, l == 0 ? (c_in == 1 ? 1 : kMaxC) : 0);
-    if (int32_t rc = set_smem_attr((const void*)fn, kBSmem)) return rc;
+    if (int32_t rc = ensure_dyn_smem((const void*)fn, kBSmem)) return rc;
     Bwd16Params p;
     memset(&p, 0, sizeof(p));
     STMGCN_REQUIRE(make_plane_map(&p.maps[0], hp, rows, (int64_t)n_layers * t_len * planes), STMGCN_ERR_STATE,
@@ -914,42 +933,25 @@ extern "C" int32_t stmgcn_lstm16_layer_bwd(int32_t layer, int32_t t_len, int32_t
     p.n_tiles = n_tiles;
     // one launch covers all timesteps of the layer (t_len <= kBMaxSteps); the weight-gradient partials of every chunk are
     // added into fp32 memory, so the length of the run does not lengthen any tensor-core accumulation chain
-    const int steps_per_launch = t_len;
-    for (int s0 = 0; s0 < t_len; s0 += steps_per_launch) {
-        const int ns_launch = (t_len - s0 < steps_per_launch) ? (t_len - s0) : steps_per_launch;
-        p.n_steps = ns_launch;
-        for (int sj = 0; sj < ns_launch; ++sj) {
-            const int si = s0 + sj;
-            const int t = t_len - 1 - si;
-            Bwd16Step& sp = p.steps[sj];
-            int ns = 0;
-            if (l > 0) {                                               // K segment: h of the layer below at this step
-                sp.src[ns] = 0;
-                sp.slice[ns] = ((l - 1) * t_len + t) * planes;
-                ++ns;
-            }
-            if (t > 0) {                                               // K segment: this layer's h of the previous step
-                sp.src[ns] = 0;
-                sp.slice[ns] = (l * t_len + t - 1) * planes;
-            } else if (h0p != nullptr) {
-                sp.src[ns] = 1;
-                sp.slice[ns] = l * planes;
-            } else {
-                sp.src[ns] = 2;                                        // zeros (STMGCN.py:53-57)
-                sp.slice[ns] = 0;
-            }
-            sp.t = t;
-            sp.first = (t == t_len - 1) ? 1 : 0;
-            sp.store_dh = (t > 0 || h0p != nullptr) ? 1 : 0;
-            sp.c_prev = t > 0 ? cs + (int64_t)(l * t_len + t - 1) * cslice : (c0 ? c0 + (int64_t)l * cslice : nullptr);
-            sp.dh_in = top ? (t == t_len - 1 ? dh_in : nullptr) : dh_in + (int64_t)t * cslice;
-            sp.dx_out = l > 0 ? dx_out + (int64_t)t * cslice : nullptr;
+    p.n_steps = t_len;
+    for (int si = 0; si < t_len; ++si) {
+        const int t = t_len - 1 - si;
+        Bwd16Step& sp = p.steps[si];
+        const StepSegs g = step_segs(l, t, t_len, planes, h0p != nullptr, cs, c0, cslice);
+        for (int s = 0; s < g.nseg; ++s) {                         // an absent h_prev segment reads the zero tile
+            sp.src[s] = (int8_t)g.src[s];
+            sp.slice[s] = g.slice[s];
         }
-        fn<<<grid, kBThreads, kBSmem, st>>>(p);
-        count_launch();
-        if (int32_t rc = check_launch("lstm16_layer_bwd")) return rc;
+        sp.t = t;
+        sp.first = (t == t_len - 1) ? 1 : 0;
+        sp.store_dh = (t > 0 || h0p != nullptr) ? 1 : 0;
+        sp.c_prev = g.c_prev;
+        sp.dh_in = top ? (t == t_len - 1 ? dh_in : nullptr) : dh_in + (int64_t)t * cslice;
+        sp.dx_out = l > 0 ? dx_out + (int64_t)t * cslice : nullptr;
     }
-    return 0;
+    fn<<<grid, kBThreads, kBSmem, st>>>(p);
+    count_launch();
+    return check_launch("lstm16_layer_bwd");
 }
 
 extern "C" int32_t stmgcn_lstm16_wgrad_reduce(int32_t layer, int32_t c_in, int32_t n_slices, const float* slices,

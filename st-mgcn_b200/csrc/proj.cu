@@ -5,19 +5,26 @@
 
 using namespace stmgcn;
 
-namespace stmgcn {
+namespace stmgcn {   // proj_tc.cu
 bool proj_tc_applicable(int ks, int p, int q, const void* a, const void* b, const void* c);
 int32_t launch_proj_fwd_tc(const float* s, int64_t stride_k, int ks, int64_t rows, const float* wimg, const float* bias,
                            int act, float* out, cudaStream_t st);
-int32_t launch_proj_bwd_tc(const float* d_out, const float* out_act, int act, int64_t rows, int ks, const float* wimg_t,
-                           float* dz_out, float* dbias, float* u, int64_t stride_u, cudaStream_t st);
-int32_t launch_pack_image(const float* src, int n_rows, int k_cols, int64_t rs, int64_t cs, float* img, int tile_rows,
-                          cudaStream_t st);
-int32_t launch_wgrad_tc(const float* seg0, const float* seg1, const float* h0, int shift1, const float* da, int n,
-                        float* dwp, int kd, int t_len, int64_t rows, cudaStream_t st);
+int32_t launch_proj_bwd_tc(const float* s, int64_t stride_k, int ks, int64_t rows, const float* d_out, const float* out_act,
+                           int act, const float* wimg_t, float* dz, float* dbias, float* u, int64_t stride_u, float* dw,
+                           cudaStream_t st);
 }
 
 namespace {
+
+// the Chebyshev stack T_0X .. T_{ks-1}X as the K segments of a GEMM operand
+ASegs stack_segs(const float* s, int64_t stride_k, int ks, int p) {
+    ASegs a{};
+    a.nseg = ks;
+    a.segw = p;
+    a.lda = p;
+    for (int k = 0; k < ks; ++k) a.seg[k] = s + (int64_t)k * stride_k;
+    return a;
+}
 
 struct ProjEpi {
     const float* bias;       // (q) or nullptr
@@ -171,22 +178,6 @@ int32_t launch_tall_auto(const ASegs& a, int64_t rows, int kd, const float* b, i
 
 extern "C" {
 
-int32_t stmgcn_proj_pack_tc(const float* w, int32_t ks, float* img_fwd, float* img_bwd, void* stream) {
-    STMGCN_REQUIRE(w && img_fwd, STMGCN_ERR_ARG, "proj_pack_tc: null pointer");
-    STMGCN_REQUIRE(ks >= 1 && ks <= 8, STMGCN_ERR_SHAPE, "proj_pack_tc: ks=%d (tensor-core path supports 1..8 supports)", ks);
-    cudaStream_t st = (cudaStream_t)stream;
-    // forward operand B[n = out col][k = ks*64 index] = W[k][n]
-    if (int32_t rc = launch_pack_image(w, 64, ks * 64, 1, 64, img_fwd, 64, st)) return rc;
-    // backward operand B[n = k*64+i][k' = out col] = W[n][k'], one 256-row image per group of 4 supports (caller
-    // zero-fills img_bwd: rows beyond the last support stay zero)
-    if (img_bwd) {
-        const int k0 = ks < 4 ? ks : 4;
-        if (int32_t rc = launch_pack_image(w, k0 * 64, 64, 64, 1, img_bwd, 256, st)) return rc;
-        if (ks > 4) return launch_pack_image(w + (int64_t)256 * 64, (ks - 4) * 64, 64, 64, 1, img_bwd + 2 * 2 * 256 * 32, 256, st);
-    }
-    return 0;
-}
-
 int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t rows, int32_t p, const float* w,
                         const float* bias, int32_t q, int32_t act, float* out, float* pool, int64_t b_inner,
                         const float* wimg, void* stream) {
@@ -197,11 +188,7 @@ int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     cudaStream_t st = (cudaStream_t)stream;
     if (wimg && !pool && proj_tc_applicable(ks, p, q, s, out, nullptr) && stride_k % 4 == 0)   // wgmma path (proj_tc.cu)
         return launch_proj_fwd_tc(s, stride_k, ks, rows, wimg, bias, act, out, st);
-    ASegs a{};
-    a.nseg = ks;
-    a.segw = p;
-    a.lda = p;
-    for (int k = 0; k < ks; ++k) a.seg[k] = s + (int64_t)k * stride_k;
+    const ASegs a = stack_segs(s, stride_k, ks, p);
     ProjEpi epi;
     epi.bias = bias;
     epi.act = act;
@@ -237,25 +224,8 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     STMGCN_REQUIRE(!u || wt, STMGCN_ERR_ARG, "proj_bwd: u requested without wt");
     cudaStream_t st = (cudaStream_t)stream;
     if (wimg_t && u && d_out && proj_tc_applicable(ks, p, q, s, out, d_out) && aligned16(dz_work) && aligned16(u) &&
-        stride_k % 4 == 0 && stride_u % 4 == 0) {
-        // wgmma path: dZ + bias gradient + U in one kernel, then dW per 128-row block of W (proj_tc.cu, wgrad_tc.cu)
-        // U has 64*ks columns; one launch produces up to 256 of them (supports 0..3), a second one the rest (it re-forms
-        // dZ in its loader but neither stores it nor accumulates the bias gradient again)
-        if (int32_t rc = launch_proj_bwd_tc(d_out, out, act, rows, ks < 4 ? ks : 4, wimg_t, dz_work, dbias, u, stride_u, st)) return rc;
-        if (ks > 4)
-            if (int32_t rc = launch_proj_bwd_tc(d_out, out, act, rows, ks - 4, wimg_t + 2 * 2 * 256 * 32, nullptr, nullptr,
-                                                u + 4 * stride_u, stride_u, st))
-                return rc;
-        for (int k0 = 0; k0 < ks; k0 += 2) {
-            const bool two = k0 + 1 < ks;
-            const float* s0 = two ? s + (int64_t)k0 * stride_k : nullptr;
-            const float* s1 = s + (int64_t)(two ? k0 + 1 : k0) * stride_k;
-            if (int32_t rc = launch_wgrad_tc(s0, s1, nullptr, 0, dz_work, 64, dw + (int64_t)k0 * 64 * 64, two ? 128 : 64, 1,
-                                             rows, st))
-                return rc;
-        }
-        return 0;
-    }
+        stride_k % 4 == 0 && stride_u % 4 == 0)   // wgmma path (proj_tc.cu)
+        return launch_proj_bwd_tc(s, stride_k, ks, rows, d_out, out, act, wimg_t, dz_work, dbias, u, stride_u, dw, st);
     {
         const int64_t total = rows * q;
         int64_t blocks = ceil_div(total, 256 * 8);
@@ -270,24 +240,15 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     }
     if (ks * p * q <= kSmallThreads * kSmallMaxPerThread && (size_t)kSmallRows * (ks * p + q) * 4 <= 48 * 1024) {
         // small outputs (temporal GCN): dedicated streaming kernel instead of the 512-row-tile reduce GEMM
-        ASegs a{};
-        a.nseg = ks;
-        a.segw = p;
-        a.lda = p;
-        for (int k = 0; k < ks; ++k) a.seg[k] = s + (int64_t)k * stride_k;
         int64_t blocks = ceil_div(rows, kSmallRows);
         const int64_t cap = (int64_t)sm_count() * 4;
         if (blocks > cap) blocks = cap;
         small_wgrad_kernel<<<(unsigned)blocks, kSmallThreads, (size_t)kSmallRows * (ks * p + q) * 4, st>>>(
-            a, rows, ks * p, dz_work, q, dw);
+            stack_segs(s, stride_k, ks, p), rows, ks * p, dz_work, q, dw);
         count_launch();
         if (int32_t rc = check_launch("proj_bwd dW(small)")) return rc;
     } else {   // dW (ks*p, q) += S^T dZ
-        ASegs a{};
-        a.nseg = ks;
-        a.segw = p;
-        a.lda = p;
-        for (int k = 0; k < ks; ++k) a.seg[k] = s + (int64_t)k * stride_k;
+        const ASegs a = stack_segs(s, stride_k, ks, p);
         ReduceTime tm{};
         tm.n_t = 1;
         const int kd = ks * p;

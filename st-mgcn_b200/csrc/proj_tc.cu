@@ -4,21 +4,65 @@
 //             (no torch.cat), split to tf32 hi/lo on its way to shared memory, accumulated in registers by wgmma
 //             (3xTF32, tc_common.cuh)
 //   backward: dZ = dOut (.) [out > 0] is formed in the loader (and written out for the weight-gradient kernel, with
-//             the bias gradient as a by-product);  U[128 x Ks*64] = dZ[128 x 64] . W^T  -> U_k segments
+//             the bias gradient as a by-product);  U[128 x Ks*64] = dZ[128 x 64] . W^T  -> U_k segments;
+//             dW[kd x 64] += [T_kX | T_{k+1}X]^T . dZ per pair of supports (proj_wgrad_tc_kernel)
 // CTA = two warpgroups, one 128-row tile at a time (persistent over tiles); warpgroup w owns rows 64w .. 64w+63 of the
 // tile.  Per 32-wide k-block every thread loads its share of A (and the pre-packed weight image), the block stores both
 // into one shared-memory stage, and each warpgroup issues 3 x 4 wgmma (k8) into its accumulator; the global loads of
 // the next k-block are in flight while those run.
-#include "tc_pipeline.cuh"
+#include "tc_common.cuh"
+#include "wgmma.cuh"
 
 using namespace stmgcn;
 using namespace stmgcn::tc;
 
 namespace {
 
+constexpr int kTileM = 128;
+constexpr int kKB = 32;                              // k-block: one 128-byte swizzle row of fp32
+constexpr int kABytes = kTileM * kKB * 4;            // 16 KB per hi or lo A tile of 128 rows
 constexpr int kPThreads = 256;
 constexpr int kPWarps = kPThreads / 32;
 constexpr int kMaxSeg = 8;
+
+__device__ __forceinline__ void split_store(uint8_t* st, uint32_t off, const float4& v) {
+    float4 hi, lo;
+    hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
+    lo.x = tf32_lo(v.x, hi.x); lo.y = tf32_lo(v.y, hi.y); lo.z = tf32_lo(v.z, hi.z); lo.w = tf32_lo(v.w, hi.w);
+    *reinterpret_cast<float4*>(st + off) = hi;
+    *reinterpret_cast<float4*>(st + kABytes + off) = lo;
+}
+
+// transpose-store one float4 (4 consecutive M/N indices mn..mn+3 of row k) into a K-major swizzled tile pair
+__device__ __forceinline__ void split_store_t(uint8_t* hi_tile, uint8_t* lo_tile, int mn, int k, const float4& v) {
+    const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const uint32_t off = sw128_offset((uint32_t)(mn + j), (uint32_t)k);
+        const float hi = tf32_hi(vv[j]);
+        *reinterpret_cast<float*>(hi_tile + off) = hi;
+        *reinterpret_cast<float*>(lo_tile + off) = tf32_lo(vv[j], hi);
+    }
+}
+
+// K-major hi/lo image of a logical B[n][k] = src[n*rs + k*cs]: per 32-wide k-block [hi | lo], each an [n_rows][32] fp32
+// tile with the 128-byte swizzle.
+__global__ void pack_image_kernel(const float* __restrict__ src, int n_rows, int k_cols, int64_t rs, int64_t cs,
+                                  float* __restrict__ img, int tile_rows) {
+    const int total = n_rows * k_cols;
+    const int tile_floats = tile_rows * kKB;      // tile_rows >= n_rows: extra rows keep what the caller put there (zeros)
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) {
+        const int n = e / k_cols, k = e % k_cols;
+        const float v = src[(int64_t)n * rs + (int64_t)k * cs];
+        const float hi = tf32_hi(v);
+        const float lo = tf32_lo(v, hi);
+        const int kb = k / kKB, kk = k % kKB;
+        const uint32_t off = sw128_offset((uint32_t)n, (uint32_t)kk) / 4;
+        float* base = img + (size_t)kb * (2 * tile_floats);
+        base[off] = hi;
+        base[tile_floats + off] = lo;
+    }
+}
 
 template <int N>
 struct PCfg {
@@ -52,6 +96,7 @@ struct PParams {
     int n_tiles;
 };
 
+// acc (+)= A[64 x 32] . B[32 x N] in 3xTF32: Ahi.Bhi + Alo.Bhi + Ahi.Blo, four k8 steps each; `first` overwrites acc
 template <int N>
 __device__ __forceinline__ void proj_mma(float (&acc)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
                                          bool first) {
@@ -198,6 +243,148 @@ __global__ void __launch_bounds__(kPThreads, 1) proj_rows_tc_kernel(const __grid
     }
 }
 
+// =====================================================================================================
+// dW[kd x 64] += sum over rows r of [S_k | S_{k+1}][r, :]^T . dZ[r, :]   (kd = 128; kd = 64: S_k alone)
+// M = kd index (warpgroup w owns kd rows 64w .. 64w+63), N = 64, K = rows, 32 rows per k-block.  Both operands are
+// row-major in HBM (K is the slow dimension) and tf32 wgmma reads K-major operands only, so the loaders transpose on
+// their way to shared memory: element (row r, m) lands at sw128_offset(m, r) of a [m][32 k] tile.  The accumulators live
+// for the whole launch and are flushed with atomics once.
+// =====================================================================================================
+constexpr int kWgBBytes = 64 * kKB * 4;                            // dZ: [64][32 k] K-major
+constexpr size_t kWgSmem = 1024 + 2 * (size_t)kABytes + 2 * (size_t)kWgBBytes;
+
+struct WgParams {
+    const float* s;          // S_k: (rows, 64)
+    int64_t stride_k;        // S_{k+1} = s + stride_k (kd = 128)
+    const float* dz;         // (rows, 64)
+    float* dw;               // (kd, 64) +=
+    int kd;                  // 128 or 64
+    int64_t rows;
+    int64_t n_chunks;        // ceil(rows / 32)
+};
+
+__global__ void __launch_bounds__(kPThreads, 1) proj_wgrad_tc_kernel(const __grid_constant__ WgParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* st = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // keeps the __shared__ address space
+    const int tid = threadIdx.x;
+    const int warp = tid >> 5;
+    const int lane = tid & 31;
+    const int wg = tid >> 7;
+    constexpr int kNA = 1024 / kPThreads, kNB = (kKB * 64 / 4) / kPThreads;
+    const uint32_t s_u = smem_u32(st);
+    const uint32_t a_hi = s_u + (uint32_t)wg * 64u * 128u, a_lo = a_hi + kABytes;
+    const uint32_t b_hi = s_u + 2 * kABytes, b_lo = b_hi + kWgBBytes;
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    bool first = true;
+
+    for (int64_t chunk = blockIdx.x; chunk < p.n_chunks; chunk += gridDim.x) {
+        const int64_t r0 = chunk * kKB;
+        float4 va[kNA], vb[kNB];
+#pragma unroll
+        for (int i = 0; i < kNA; ++i) {                   // A': 32 rows x 32 float4 (128 kd values), coalesced
+            const int idx = tid + i * kPThreads;
+            const int row = idx >> 5, q = idx & 31;
+            const int64_t r = r0 + row;
+            // m 0..63 from S_k, 64..127 from S_{k+1}
+            const float* src = q < 16 ? p.s : (p.kd == 128 ? p.s + p.stride_k : nullptr);
+            va[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (src != nullptr && r < p.rows) va[i] = *reinterpret_cast<const float4*>(src + r * 64 + (q & 15) * 4);
+        }
+#pragma unroll
+        for (int i = 0; i < kNB; ++i) {                   // B': 32 rows x 16 float4, coalesced
+            const int idx = tid + i * kPThreads;
+            const int row = idx >> 4, q = idx & 15;
+            const int64_t r = r0 + row;
+            vb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (r < p.rows) vb[i] = *reinterpret_cast<const float4*>(p.dz + r * 64 + q * 4);
+        }
+        wg_wait<0>();
+        __syncthreads();                                  // both warpgroups are done with the stage
+#pragma unroll
+        for (int i = 0; i < kNA; ++i) {
+            const int idx = tid + i * kPThreads;
+            split_store_t(st, st + kABytes, (idx & 31) * 4, idx >> 5, va[i]);
+        }
+#pragma unroll
+        for (int i = 0; i < kNB; ++i) {
+            const int idx = tid + i * kPThreads;
+            split_store_t(st + 2 * kABytes, st + 2 * kABytes + kWgBBytes, (idx & 15) * 4, idx >> 4, vb[i]);
+        }
+        fence_proxy_async_smem();
+        __syncthreads();
+        wg_fence_regs(acc);
+        wg_fence();
+        proj_mma<64>(acc, a_hi, a_lo, b_hi, b_lo, first);
+        wg_commit();
+        first = false;
+    }
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    if (first) return;                                    // no chunk: nothing accumulated
+    // ===================== accumulator fragment (rows = kd index) -> atomics into dW =====================
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int m = r0 + 8 * h;
+        if (m >= p.kd) continue;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            atomicAdd(p.dw + (int64_t)m * 64 + 8 * j + c0, acc[4 * j + 2 * h]);
+            atomicAdd(p.dw + (int64_t)m * 64 + 8 * j + c0 + 1, acc[4 * j + 2 * h + 1]);
+        }
+    }
+}
+
+int grid_for(int64_t work) { return (int)(work < sm_count() ? work : sm_count()); }
+
+int32_t launch_pack_image(const float* src, int n_rows, int k_cols, int64_t rs, int64_t cs, float* img, int tile_rows,
+                          cudaStream_t st) {
+    pack_image_kernel<<<(n_rows * k_cols + 255) / 256, 256, 0, st>>>(src, n_rows, k_cols, rs, cs, img, tile_rows);
+    count_launch();
+    return check_launch("pack_image");
+}
+
+// dZ = d_out (.) mask (written to dz_out unless null, bias gradient accumulated unless null), U_k = dZ W_k^T for
+// ks <= 4 supports; wimg_t = image of B[n = k*64+i][k' = j] = W[n][j]  (2 k-blocks of [hi|lo] [256][32])
+int32_t launch_rows_bwd(const float* d_out, const float* out_act, int act, int64_t rows, int ks, const float* wimg_t,
+                        float* dz_out, float* dbias, float* u, int64_t stride_u, cudaStream_t st) {
+    auto kern = proj_rows_tc_kernel<256, true>;
+    if (int32_t rc = ensure_dyn_smem((const void*)kern, psmem<256>())) return rc;
+    PParams p{};
+    p.nkb = 2;
+    p.ks_out = ks;
+    p.d_out = d_out;
+    p.out_act = out_act;
+    p.act = act;
+    p.dz_out = dz_out;
+    p.dbias = dbias;
+    p.wimg = wimg_t;
+    p.u = u;
+    p.stride_u = stride_u;
+    p.rows = rows;
+    p.n_tiles = (int)ceil_div(rows, kTileM);
+    kern<<<grid_for(p.n_tiles), kPThreads, psmem<256>(), st>>>(p);
+    count_launch();
+    return check_launch("proj_bwd_tc");
+}
+
+int32_t launch_wgrad(const float* s, int64_t stride_k, int kd, const float* dz, int64_t rows, float* dw, cudaStream_t st) {
+    if (int32_t rc = ensure_dyn_smem((const void*)proj_wgrad_tc_kernel, kWgSmem)) return rc;
+    WgParams p;
+    p.s = s;
+    p.stride_k = stride_k;
+    p.dz = dz;
+    p.dw = dw;
+    p.kd = kd;
+    p.rows = rows;
+    p.n_chunks = ceil_div(rows, kKB);
+    proj_wgrad_tc_kernel<<<grid_for(p.n_chunks), kPThreads, kWgSmem, st>>>(p);
+    count_launch();
+    return check_launch("proj_wgrad_tc");
+}
+
 }  // namespace
 
 namespace stmgcn {
@@ -220,42 +407,43 @@ int32_t launch_proj_fwd_tc(const float* s, int64_t stride_k, int ks, int64_t row
     p.out = out;
     p.rows = rows;
     p.n_tiles = (int)ceil_div(rows, kTileM);
-    const int grid = p.n_tiles < sm_count() ? p.n_tiles : sm_count();
-    kern<<<grid, kPThreads, psmem<64>(), st>>>(p);
+    kern<<<grid_for(p.n_tiles), kPThreads, psmem<64>(), st>>>(p);
     count_launch();
     return check_launch("proj_fwd_tc");
 }
 
-// backward data: dZ = d_out (.) mask (written to dz_out, bias gradient accumulated), U_k = dZ W_k^T (if u != nullptr);
-// wimg_t = image of B[n = k*64+i][k' = j] = W[n][j]  (2 k-blocks of [hi|lo] [ks*64][32])
-int32_t launch_proj_bwd_tc(const float* d_out, const float* out_act, int act, int64_t rows, int ks, const float* wimg_t,
-                           float* dz_out, float* dbias, float* u, int64_t stride_u, cudaStream_t st) {
-    auto kern = proj_rows_tc_kernel<256, true>;
-    if (int32_t rc = ensure_dyn_smem((const void*)kern, psmem<256>())) return rc;
-    PParams p{};
-    p.nkb = 2;
-    p.ks_out = ks;
-    p.d_out = d_out;
-    p.out_act = out_act;
-    p.act = act;
-    p.dz_out = dz_out;
-    p.dbias = dbias;
-    p.wimg = wimg_t;
-    p.u = u;
-    p.stride_u = stride_u;
-    p.rows = rows;
-    p.n_tiles = (int)ceil_div(rows, kTileM);
-    const int grid = p.n_tiles < sm_count() ? p.n_tiles : sm_count();
-    kern<<<grid, kPThreads, psmem<256>(), st>>>(p);
-    count_launch();
-    return check_launch("proj_bwd_tc");
-}
-
-int32_t launch_pack_image(const float* src, int n_rows, int k_cols, int64_t rs, int64_t cs, float* img, int tile_rows,
-                          cudaStream_t st) {
-    pack_image_kernel<<<(n_rows * k_cols + 255) / 256, 256, 0, st>>>(src, n_rows, k_cols, rs, cs, img, tile_rows);
-    count_launch();
-    return check_launch("pack_image");
+// backward: dZ + bias gradient + U in one row-kernel launch per group of 4 supports (the second one re-forms dZ in its
+// loader but neither stores it nor accumulates the bias gradient again), then dW_k = S_k^T dZ, one launch per pair of
+// supports; wimg_t: stmgcn_proj_pack_tc's backward image
+int32_t launch_proj_bwd_tc(const float* s, int64_t stride_k, int ks, int64_t rows, const float* d_out, const float* out_act,
+                           int act, const float* wimg_t, float* dz, float* dbias, float* u, int64_t stride_u, float* dw,
+                           cudaStream_t st) {
+    if (int32_t rc = launch_rows_bwd(d_out, out_act, act, rows, ks < 4 ? ks : 4, wimg_t, dz, dbias, u, stride_u, st)) return rc;
+    if (ks > 4)
+        if (int32_t rc = launch_rows_bwd(d_out, out_act, act, rows, ks - 4, wimg_t + 2 * 2 * 256 * 32, nullptr, nullptr,
+                                         u + 4 * stride_u, stride_u, st))
+            return rc;
+    for (int k0 = 0; k0 < ks; k0 += 2)
+        if (int32_t rc = launch_wgrad(s + (int64_t)k0 * stride_k, stride_k, k0 + 1 < ks ? 128 : 64, dz, rows,
+                                      dw + (int64_t)k0 * 64 * 64, st))
+            return rc;
+    return 0;
 }
 
 }  // namespace stmgcn
+
+extern "C" int32_t stmgcn_proj_pack_tc(const float* w, int32_t ks, float* img_fwd, float* img_bwd, void* stream) {
+    STMGCN_REQUIRE(w && img_fwd, STMGCN_ERR_ARG, "proj_pack_tc: null pointer");
+    STMGCN_REQUIRE(ks >= 1 && ks <= 8, STMGCN_ERR_SHAPE, "proj_pack_tc: ks=%d (tensor-core path supports 1..8 supports)", ks);
+    cudaStream_t st = (cudaStream_t)stream;
+    // forward operand B[n = out col][k = ks*64 index] = W[k][n]
+    if (int32_t rc = launch_pack_image(w, 64, ks * 64, 1, 64, img_fwd, 64, st)) return rc;
+    // backward operand B[n = k*64+i][k' = out col] = W[n][k'], one 256-row image per group of 4 supports (caller
+    // zero-fills img_bwd: rows beyond the last support stay zero)
+    if (img_bwd) {
+        const int k0 = ks < 4 ? ks : 4;
+        if (int32_t rc = launch_pack_image(w, k0 * 64, 64, 64, 1, img_bwd, 256, st)) return rc;
+        if (ks > 4) return launch_pack_image(w + (int64_t)256 * 64, (ks - 4) * 64, 64, 64, 1, img_bwd + 2 * 2 * 256 * 32, 256, st);
+    }
+    return 0;
+}

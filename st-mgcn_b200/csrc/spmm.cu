@@ -189,7 +189,8 @@ extern "C" int32_t stmgcn_to_bf16(const float* x, void* y16, int64_t count, void
     STMGCN_REQUIRE(count > 0 && count % 8 == 0 && aligned16(x) && aligned16(y16), STMGCN_ERR_SHAPE,
                    "to_bf16: count=%lld must be a positive multiple of 8, pointers 16-byte aligned", (long long)count);
     const int64_t n8 = count / 8;
-    const int blocks = (int)(n8 / 256 + 1 < 148 * 16 ? n8 / 256 + 1 : 148 * 16);
+    const int64_t cap = (int64_t)sm_count() * 16;
+    const int blocks = (int)(n8 / 256 + 1 < cap ? n8 / 256 + 1 : cap);
     to_bf16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, (uint16_t*)y16, n8);
     count_launch();
     return check_launch("to_bf16");

@@ -23,7 +23,6 @@
 namespace stmgcn {
 namespace tc {
 
-constexpr int kTile16Cols = 64;                       // bf16 per 128-byte row
 constexpr int kTile16Bytes = 128 * 128;               // [128 rows][64 bf16] = 16 KB
 
 // byte offset of element (row, col) in a [rows][64 bf16] 128B-swizzled tile

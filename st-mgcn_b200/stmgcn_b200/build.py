@@ -22,12 +22,10 @@ LIB_PATH = os.path.join(LIB_DIR, "libstmgcn_b200.so")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",     # the long form: `-arch=sm_90a` drops the `a` features (wgmma)
-    "-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
+    "-O3", "-lineinfo", "-std=c++17",               # no --use_fast_math: IEEE div / sqrt; the fast exp is explicit
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O3",
     "-Xptxas", "-v",
 ]
-# --use_fast_math is deliberately NOT applied blindly: see below (we keep IEEE div/sqrt, only fast exp).
-NVCC_FLAGS.remove("--use_fast_math")
 
 
 def _nvcc() -> str:

@@ -141,6 +141,28 @@ def test_model_matches_sparse_oracle(shape):
         assert_close(p.grad.cpu().numpy(), g_ref[key], f"grad {key}")
 
 
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two CUDA devices")
+def test_second_device_of_the_process_computes_the_same():
+    """The dynamic shared-memory limit is a per-device kernel attribute.  After the H = 128 model (exact-fp32 LSTM and
+    projection: tall GEMMs with more than 48 KB of shared memory) ran on cuda:0, the same model runs on cuda:1 in the
+    same process and gives the same forward and gradients."""
+    shape = dict(n=50, m=2, k=2, t=7, b=5, c=2, hid=128, layers=2, gcn_hid=68)
+    sups, params, x, y = _mid_case(seed=3, **shape)
+    results = []
+    for dev in ("cuda:0", "cuda:1"):
+        with torch.cuda.device(dev):
+            model = build_model(shape, dev)
+            model.load_state_dict(params)
+            out = model(obs_seq=x.to(dev), sta_adj_list=[s.to(dev) for s in sups])
+            nn.MSELoss()(out, y.to(dev)).backward()
+            torch.cuda.synchronize()
+        results.append((out.detach().cpu().numpy(), {k_: p.grad.cpu().numpy() for k_, p in model.named_parameters()}))
+    (out0, grads0), (out1, grads1) = results
+    assert_close(out1, out0, "cuda:1 forward vs cuda:0")
+    for key, g in grads0.items():
+        assert_close(grads1[key], g, f"cuda:1 grad {key} vs cuda:0")
+
+
 def test_gcn_generic_supports_and_no_activation():
     """localpool-style supports (A[0] != I) take the generic path; activation=None; x with odd strides."""
     import GCN

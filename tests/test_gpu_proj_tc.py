@@ -1,5 +1,5 @@
-"""The tensor-core projection of the Chebyshev GCN (proj_tc.cu forward and dZ / bias gradient / U, wgrad_tc.cu dW, the
-weight-image pack) against an fp64 reference, on random stacks: every support count the kernels take (ks = 1..8; ks > 4
+"""The tensor-core projection of the Chebyshev GCN (proj_tc.cu: forward, dZ / bias gradient / U, dW and the weight-image
+pack) against an fp64 reference, on random stacks: every support count the kernels take (ks = 1..8; ks > 4
 splits U over two launches), row counts around the 32-row weight-gradient chunk and the 128-row tile, a multi-wave
 ragged size, ReLU and bias on and off.  Bars: 2e-5 forward, 5e-5 gradients (max-norm relative)."""
 import pytest
