@@ -326,9 +326,10 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
 //   R_c : recompute  G_c[64 x 64] = [h_below | h_prev] . Wp[:, chunk]                      (registers, m64n64)
 //   P_c : gates -> c_t, tanh(c_t) -> BPTT pointwise -> dA_c (fp32) -> bf16 hi/lo planes in a 128-byte-swizzled
 //         shared-memory tile; dc in place
+//   B_c : bias gradient    db[chunk] += column sums of the fp32 dA_c: a reduce-scatter over the 16 lanes of a warp that
+//         hold the same units, then one shared-memory add per warp and column
 //   W_c : weight gradient  dWp[kd, chunk] = A^T . dA_c, warpgroup w: kd rows 64w .. (both operands: MN-major views of
 //         tiles already in shared memory), added into this CTA's own slice of a scratch buffer with vector reductions
-//   B_c : bias gradient    db[chunk] += ones . dA_c (warpgroup 0, A = a register fragment of ones), summed in shared memory
 //   D_c : data gradient    [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T  (B: MN-major view of the resident weights;
 //         accumulated in registers over the four chunks, stored at the end of the item)
 // dA never leaves the SM; the gates are never stored.  stmgcn_lstm16_wgrad_reduce sums the slices once per layer and
@@ -380,6 +381,19 @@ struct Bwd16Params {
 static_assert(sizeof(Bwd16Params) <= 4096, "kernel parameter block exceeds 4 KB");
 
 __device__ __forceinline__ void cons_sync(int n_threads) { asm volatile("bar.sync 1, %0;" ::"r"(n_threads) : "memory"); }
+
+// One reduce-scatter step between lanes l and l ^ mask over v[0 .. 2H): the lane with the mask bit set keeps the upper
+// half, the other the lower half, each adds its partner's copy of that half; the kept half moves to v[0 .. H).
+template <int H>
+__device__ __forceinline__ void col_sums_step(float (&v)[32], int mask, int lane) {
+    const bool up = (lane & mask) != 0;
+#pragma unroll
+    for (int i = 0; i < H; ++i) {
+        const float send = up ? v[i] : v[i + H];
+        const float keep = up ? v[i + H] : v[i];
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, mask);
+    }
+}
 
 template <int PLANES, int CIN>                                  // CIN: see lstm16_fwd_kernel
 __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_constant__ Bwd16Params p) {
@@ -467,9 +481,6 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     const bool ds_fixed = L0 && (kTileM % (uint32_t)p.b_inner) == 0u;
     float ds_acc = 0.f;
     float* slice = p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols);
-    uint32_t ones[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) ones[k] = 0x3f803f80u;                // bf16 pair (1, 1)
     mbar_wait_raw(&tail->w_full, 0);
 
     for (int w = 0; w < n_items; ++w) {
@@ -530,6 +541,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             wg_fence_regs(g);
             // ---- P_c: 8 cells per thread (row row_in_tile, units 16c + 2j + q/2) ----
             uint32_t dhi[8], dlo[8];
+            float bs[32];                                          // dA of this thread's cells: bs[4j + gate]
             const uint32_t bo = (uint32_t)tile * 8192u + row_in_tile * 4u;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -558,6 +570,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 const float da1 = dcv * cp * gf * (1.f - gf);
                 const float da2 = dcv * gi * (1.f - gg * gg);
                 const float da3 = dh * tc_ * go * (1.f - go);
+                bs[4 * j + 0] = da0; bs[4 * j + 1] = da1; bs[4 * j + 2] = da2; bs[4 * j + 3] = da3;
                 if (valid) p.dc[o] = dcv * gf;
                 if (L0) {
 #pragma unroll
@@ -572,9 +585,23 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 uint32_t h2, l2;
                 split_bf16x2(da2, da3, h2, l2);
                 const uint32_t off = row_in_tile * 128u + ((((uint32_t)j) ^ (row_in_tile & 7u)) << 4) + (uint32_t)(q >> 1) * 8u;
-                if (j == 0) cons_sync(kCons);                      // W / D / B of the previous chunk have read the dA tile
+                if (j == 0) cons_sync(kCons);                      // W / D of the previous chunk have read the dA tile
                 *reinterpret_cast<uint2*>(da_sm + off) = make_uint2(dhi[j], h2);
                 *reinterpret_cast<uint2*>(da_sm + kATileBytes + off) = make_uint2(dlo[j], l2);
+            }
+            // ---- B_c: db[chunk] += column sums of dA_c (rows past the end carry dA = 0) ----
+            // Lanes l ^ 1, ^ 4, ^ 8, ^ 16 hold the same units in other rows.  A reduce-scatter over those 16 lanes halves
+            // the list at each step; afterwards lane l holds the sums of bs[i0], bs[i0 + 1] for
+            // i0 = 16 b0 + 8 b2 + 4 b3 + 2 b4 (b = the bits of l), i.e. unit 2 (i0 / 4) + q/2 of the chunk, gates i0 % 4 + {0, 1}.
+            col_sums_step<16>(bs, 1, lane);
+            col_sums_step<8>(bs, 4, lane);
+            col_sums_step<4>(bs, 8, lane);
+            col_sums_step<2>(bs, 16, lane);
+            {
+                const int i0 = 16 * (lane & 1) + 8 * ((lane >> 2) & 1) + 4 * ((lane >> 3) & 1) + 2 * ((lane >> 4) & 1);
+                const int col = 64 * c + 4 * (2 * (i0 >> 2) + (q >> 1)) + (i0 & 3);
+                atomicAdd(&tail->db[col], bs[0]);
+                atomicAdd(&tail->db[col + 1], bs[1]);
             }
             fence_proxy_async_smem();
             cons_sync(kCons);                                      // the dA tile (both row halves) is complete
@@ -582,11 +609,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             float wgr[32];
 #pragma unroll
             for (int k = 0; k < 32; ++k) wgr[k] = 0.f;
-            float bgr[32];
-#pragma unroll
-            for (int k = 0; k < 32; ++k) bgr[k] = 0.f;
             wg_fence_regs(wgr);
-            wg_fence_regs(bgr);
             wg_fence_regs(dacc);
             wg_fence();
             {
@@ -599,14 +622,12 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                     const uint64_t bl = desc16_mn(da_u + kATileBytes + ks * kStepMN, kATileBytes);
                     // dA always has its lo plane; in the single-plane mode only the STORED operands are rounded to bf16.
                     // Layer 0's warpgroup 1 multiplies the auxiliary x*s tile, which is not stored: it keeps its lo plane in
-                    // both modes, as the forward's fp32 FMAs do (warpgroup 0's lo slot is zero then, and adds nothing)
+                    // both modes, as the forward's fp32 FMAs do (warpgroup 0's lo slot is zero then, and adds nothing; both
+                    // warpgroups issue the pass so that no wgmma sits on a warpgroup-dependent branch, which would make
+                    // ptxas serialise every wgmma of the kernel)
                     wgmma_bf16_n64_t11(wgr, ah, bh, ks > 0 ? 1u : 0u);
                     wgmma_bf16_n64_t11(wgr, ah, bl, 1u);
                     if (PLANES == 2 || L0) wgmma_bf16_n64_t11(wgr, al, bh, 1u);
-                    // (both warpgroups issue it -- only warpgroup 0's result is used -- so that no wgmma sits on a
-                    // warpgroup-dependent branch, which would make ptxas serialise every wgmma of the kernel)
-                    wgmma_bf16_n64_rs_t1(bgr, ones, bh, ks > 0 ? 1u : 0u);
-                    wgmma_bf16_n64_rs_t1(bgr, ones, bl, 1u);
                 }
             }
             // ---- D_c: [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T ----
@@ -630,9 +651,8 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             wg_commit();
             wg_wait<0>();
             wg_fence_regs(wgr);
-            wg_fence_regs(bgr);
             wg_fence_regs(dacc);
-            // weight-gradient fragment -> this CTA's slice (row-major [kd][256]); bias sums: row 0 of warpgroup 0
+            // weight-gradient fragment -> this CTA's slice (row-major [kd][256])
             {
                 const uint32_t m0 = rw0;
 #pragma unroll
@@ -640,13 +660,6 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                     const uint32_t n = (uint32_t)(64 * c + 8 * j + 2 * q);
                     red_add_f32x2(slice + (size_t)m0 * kGateCols + n, wgr[4 * j], wgr[4 * j + 1]);
                     red_add_f32x2(slice + (size_t)(m0 + 8) * kGateCols + n, wgr[4 * j + 2], wgr[4 * j + 3]);
-                }
-                if (wg == 0 && m0 == 0) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        tail->db[64 * c + 8 * j + 2 * q] += bgr[4 * j];
-                        tail->db[64 * c + 8 * j + 2 * q + 1] += bgr[4 * j + 1];
-                    }
                 }
             }
         }

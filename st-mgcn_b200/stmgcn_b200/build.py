@@ -7,6 +7,7 @@ Objects are rebuilt only when a source or header is newer.
 from __future__ import annotations
 
 import os
+import re
 import shutil
 import subprocess
 import sys
@@ -26,6 +27,9 @@ NVCC_FLAGS = [
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O3",
     "-Xptxas", "-v",
 ]
+# ptxas C7511 / C7512: every wgmma of the function then waits for the previous one to complete.  Only a warning, but it
+# costs the tensor-core kernels most of their throughput, so the build refuses it.
+_SERIALIZED_WGMMA = re.compile(r"wgmma\.mma_async instructions are serialized .*? function '([^']+)'")
 
 
 def _nvcc() -> str:
@@ -73,6 +77,11 @@ def build(verbose: bool = False, force: bool = False) -> str:
             fh.write(" ".join(cmd) + "\n" + log)
         if res.returncode != 0:
             raise RuntimeError(f"nvcc failed for {src}:\n{log}")
+        serialized = sorted(set(_SERIALIZED_WGMMA.findall(log)))
+        if serialized:
+            os.remove(obj)              # not left behind as up to date
+            raise RuntimeError(f"ptxas serialized the wgmma instructions of {', '.join(serialized)} in {src} "
+                               f"(insufficient register resources):\n{log}")
         return src, log
 
     if jobs:
