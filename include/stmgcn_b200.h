@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define STMGCN_ABI_VERSION 3
+#define STMGCN_ABI_VERSION 4
 
 /* error codes < 0 */
 #define STMGCN_ERR_ARG      (-1)   /* null pointer / bad enum */
@@ -169,15 +169,16 @@ int32_t stmgcn_lstm_wgrad(int32_t layer, int32_t t_len, int32_t n_layers, int64_
  * gate-interleaved (col = 4*unit + gate) and, for layer 0, wih_t (C, 256) = W_ih^T gate-interleaved. */
 int32_t stmgcn_lstm16_pack(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, int32_t layer,
                            int32_t c_in, void* wimg, float* bias, float* wih_t, void* stream);
-/* One timestep, all layers.  h0p: (L, P, R, 64) bf16 planes of the initial hidden state and c0: (L, R_pad, 64) fp32
- * tile-blocked, or both NULL (zeros, STMGCN.py:53-57).  At t = T-1 the fp32 hidden state is also written: every layer
- * into h_n (L, R, 64) when h_n != NULL, else only the top layer into h_top (R, 64) -- the (N,B,H) operand of the
- * spatial GCN (STMGCN.py:50, :114).  C <= 4. */
-int32_t stmgcn_lstm16_step_fwd(int32_t t, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in,
-                               int64_t b_inner, int32_t planes, const float* xo, const float* s_gate,
-                               const void* const* wimg, const float* const* bias, const float* wih_t,
-                               const void* h0p, const float* c0, void* hp, float* cs, float* h_top, float* h_n,
-                               void* stream);
+/* Forward of ONE layer through all timesteps 0 .. T-1 (call the layers bottom-up: layer l reads the hp planes of layer
+ * l - 1).  A tile's rows never mix with other tiles', so each CTA walks its own tiles through time inside the layer's one
+ * launch, keeping h_{t-1} in shared memory.  h0p: (L, P, R, 64) bf16 planes of the initial hidden state and c0:
+ * (L, R_pad, 64) fp32 tile-blocked, or both NULL (zeros, STMGCN.py:53-57).  At t = T-1 the fp32 hidden state is also
+ * written: into h_n[layer] (h_n: (L, R, 64)) when h_n != NULL, else for the top layer into h_top (R, 64) -- the (N,B,H)
+ * operand of the spatial GCN (STMGCN.py:50, :114).  wimg / bias: this layer's operands from stmgcn_lstm16_pack.  C <= 4. */
+int32_t stmgcn_lstm16_layer_fwd(int32_t layer, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in,
+                                int64_t b_inner, int32_t planes, const float* xo, const float* s_gate,
+                                const void* wimg, const float* bias, const float* wih_t, const void* h0p,
+                                const float* c0, void* hp, float* cs, float* h_top, float* h_n, void* stream);
 
 /* grid (CTAs) the lstm16 kernels use for `rows` rows: the number of weight-gradient scratch slices per layer */
 int32_t stmgcn_lstm16_grid(int64_t rows);

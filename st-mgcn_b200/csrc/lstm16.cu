@@ -8,13 +8,14 @@
 //   cs : (L, T, rows_pad, 64) fp32, tile-blocked ([tile][unit/4][128 rows][4 units], see below).
 // 4 + 4 bytes per (row, unit, layer-step) instead of 4 + 4 + 16 with a gate tape.
 //
-// forward kernel (one launch per layer-step, persistent, one CTA per SM):
+// forward kernel (one launch per layer covering all T steps, persistent, one CTA per SM):
 //   producer warp : loads the layer's weight image ONCE (resident for the whole launch: [256 gate cols][64 k] bf16 tiles,
-//                   hi and lo, per K segment = 128 KB) and streams the A planes of every tile through a ring of 16 KB
-//                   stages with TMA tensor loads (h_below hi, h_below lo, h_prev hi, h_prev lo)
-//   2 warpgroups  : per tile and warpgroup (64 rows) 8 (P = 1) or 24 (P = 2) wgmma m64n256k16 into registers:
-//                   Ahi.Whi + Ahi.Wlo + Alo.Whi, then bias (+ layer 0: x*s . W_ih in exact fp32) -> gates -> c, h ->
-//                   h split into bf16 planes -> global stores.  Nothing of the gates leaves the SM.
+//                   hi and lo, per K segment = 128 KB); layers > 0: streams h_below (hp of the layer below) of every
+//                   (tile, step) into one stage per warpgroup with TMA tensor loads
+//   2 warpgroups  : each walks its 64 rows of a tile through t = 0 .. T-1; per step 8 (P = 1) or 24 (P = 2) wgmma
+//                   m64n256k16 into registers: Ahi.Whi + Ahi.Wlo + Alo.Whi, then bias (+ layer 0: x*s . W_ih in exact
+//                   fp32) -> gates -> c, h -> h split into bf16 planes in shared memory, which is both the h_prev operand
+//                   of the next step and the source of a TMA tensor store of the tape.  Nothing of the gates leaves the SM.
 #include "tc16.cuh"
 #include <cuda.h>
 #include <stdlib.h>
@@ -24,7 +25,7 @@ using namespace stmgcn;
 using namespace stmgcn::tc;
 
 namespace stmgcn {
-bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t slices);
+bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t slices, int box_rows);
 }
 
 namespace {
@@ -109,50 +110,73 @@ __device__ __forceinline__ float4 gate_args(float4 v, float4 b, const float (&xs
 }
 
 // =====================================================================================================
-// forward
+// forward: one launch per LAYER over all its timesteps (a tile's rows never mix with other tiles', so a CTA walks its
+// own tiles through time, as the backward does)
 // =====================================================================================================
 // CTA = two consumer warpgroups + one producer warp, persistent over 128-row tiles.  Warpgroup w owns rows 64w .. 64w+63
-// of a tile and accumulates its [64 x 256] gate pre-activations in registers (wgmma m64n256k16).  Accumulator fragment
-// (wgmma.cuh): thread holds columns 8j + 2(lane%4) + {0,1} of rows r0 and r0 + 8; with gate-interleaved columns
-// n = 4 unit + gate that is gates (i, f) (lane%4 even) or (g, o) (odd) of unit 2j + (lane%4)/2.  Partner lanes (lane ^ 1)
-// swap one row's pair, after which the even lane owns the cell (r0, unit) and the odd lane the cell (r0 + 8, unit).
+// of a tile, walks them through t = 0 .. T-1 and accumulates their [64 x 256] gate pre-activations in registers (wgmma
+// m64n256k16).  The warpgroups share nothing but the resident weights, so they run out of phase: one's wgmma overlaps
+// the other's MUFU-bound cell epilogue.
+//   h_prev : never leaves the SM.  The epilogue of step t writes h_t as bf16 planes into the warpgroup's own [64][64]
+//            128-byte-swizzled tiles (one per plane): the K-major A operand of step t + 1, and the source of the TMA
+//            tensor store of hp[l, t].  At t = 0 the tiles are loaded from h0p, or the segment is absent (zeros).
+//   h_below: layers > 0: hp[l - 1, t], written by the previous launch, streamed by the producer into one stage per
+//            warpgroup; released as soon as the step's wgmma have completed, so the next load overlaps the epilogue.
+//   c      : the tile-blocked cs tape; c_{t-1} is read back by the thread that wrote it one step earlier (L2-hot).
+// Accumulator fragment (wgmma.cuh): thread holds columns 8j + 2(lane%4) + {0,1} of rows r0 and r0 + 8; with
+// gate-interleaved columns n = 4 unit + gate that is gates (i, f) (lane%4 even) or (g, o) (odd) of unit 2j + (lane%4)/2.
+// Partner lanes (lane ^ 1) swap one row's pair, after which the even lane owns the cell (r0, unit) and the odd lane the
+// cell (r0 + 8, unit).
 constexpr int kFWarpgroups = 2;
 constexpr int kFThreads = kFWarpgroups * 128 + 32;     // + producer warp
-constexpr int kFStages = 5;
+constexpr int kHTileBytes = 64 * 128;                  // one plane of a warpgroup's rows: [64 rows][64] bf16 = 8 KB
+constexpr int kFWgBytes = 4 * kHTileBytes;             // per warpgroup: h_prev hi | lo, h_below stage hi | lo
 
 struct F16Tail {
     float bias[kGateCols];
-    float wih[kMaxC * kGateCols];
-    uint64_t full[kFStages];
-    uint64_t empty[kFStages];
+    uint64_t full[kFWarpgroups];       // h_below stage of warpgroup w loaded
+    uint64_t empty[kFWarpgroups];      // ... and consumed
+    uint64_t h0_full[kFWarpgroups];    // h_prev tiles of warpgroup w loaded from h0p
     uint64_t w_full;
 };
-constexpr size_t kFSmem = 1024 + 4 * (size_t)kWTileBytes + (size_t)kFStages * kATileBytes + sizeof(F16Tail);
+constexpr size_t kFSmem = 1024 + 4 * (size_t)kWTileBytes + kFWarpgroups * (size_t)kFWgBytes + sizeof(F16Tail);
 static_assert(kFSmem <= 232448, "lstm16 forward kernel exceeds the 227 KB shared-memory limit");
 
 struct Fwd16Params {
-    alignas(64) CUtensorMap amap[2];   // per K segment: (64, rows, slices) bf16 view of a plane tensor, box 64 x 128 x 1, 128B swizzle
-    int aslice[2];                     // slice of the segment's hi plane (lo plane = +1)
-    int nseg;                          // K segments present: layer 0: h_prev; layers > 0: h_below, h_prev (absent at t = 0 without h0)
-    const uint8_t* wimg;               // tiles [(seg*2 + plane)] of 32 KB
+    alignas(64) CUtensorMap hp_map;    // (64, rows, L*T*P) bf16 view of hp, box 64 x 64 x 1, 128B swizzle
+    alignas(64) CUtensorMap h0_map;    // (64, rows, L*P) view of h0p, same box (has_h0)
+    const uint8_t* wimg;               // this layer's tiles [(seg*2 + plane)] of 32 KB
     const float* bias;                 // (256) gate-interleaved b_ih + b_hh
     const float* wih;                  // layer 0: (C, 256) gate-interleaved W_ih^T; else nullptr
     const float* xo;                   // (rows, T, C)
     const float* sg;                   // (B, T)
-    int c_in, t, t_len;
+    int layer, c_in, t_len;
+    int has_h0;                        // h0_map and c0 are set
     int64_t b_inner;
-    const float* c_prev;               // tile-blocked or nullptr (zeros)
-    float* c_out;                      // tile-blocked
-    uint16_t* h_hi;                    // (rows, 64) bf16 plane
-    uint16_t* h_lo;                    // (rows, 64) bf16 plane (PLANES = 2)
-    float* h_f32;                      // (rows, 64) fp32 copy of h or nullptr
+    const float* c0;                   // this layer's initial cell state, tile-blocked, or nullptr (zeros)
+    float* cs;                         // this layer's cell-state tape (T, rows_pad, 64), tile-blocked
+    float* h_f32;                      // (rows, 64) fp32 copy of h at t = T-1, or nullptr
     int64_t rows;
     int n_tiles;
 };
 
-__device__ __forceinline__ uint16_t bf16_bits(float v) {
-    return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+// One K segment of the gate GEMM: A = the PLANES [64][64] tiles at a_u (hi | lo, kHTileBytes apart), W = the segment's
+// resident [256][64] tiles at w_u (hi | lo).  Issue order per plane: hi: Ahi.Whi, Ahi.Wlo per k-step; lo: Alo.Whi.
+template <int PLANES>
+__device__ __forceinline__ void fwd_segment_mma(float (&acc)[128], uint32_t a_u, uint32_t w_u, bool first) {
+    const uint64_t w_hi = desc16_k(w_u), w_lo = desc16_k(w_u + kWTileBytes);
+#pragma unroll
+    for (int pl = 0; pl < PLANES; ++pl) {
+        const uint64_t a_d = desc16_k(a_u + (uint32_t)pl * kHTileBytes);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            wgmma_bf16_n256_t00(acc, a_d + (uint64_t)(2 * kk), w_hi + (uint64_t)(2 * kk), (!first || pl > 0 || kk > 0) ? 1u : 0u);
+            if (PLANES == 2 && pl == 0) wgmma_bf16_n256_t00(acc, a_d + (uint64_t)(2 * kk), w_lo + (uint64_t)(2 * kk), 1u);
+        }
+    }
 }
+
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
 // CIN: 0 = not layer 0; 1 = layer 0 with one input channel (the reference's input_dim, compile-time: no predicated-off
 // W_ih FMAs / loads in the cell loop); kMaxC = layer 0 with a runtime channel count <= kMaxC
@@ -160,132 +184,184 @@ template <int PLANES, int CIN>
 __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_constant__ Fwd16Params p) {
     constexpr bool L0 = CIN > 0;
     constexpr int kC = (CIN == 1) ? 1 : kMaxC;
+    constexpr int kNseg = L0 ? 1 : 2;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* wsm = smem;                                           // resident weight tiles
-    uint8_t* stages = smem + 4 * (size_t)kWTileBytes;
-    F16Tail* tail = (F16Tail*)(stages + (size_t)kFStages * kATileBytes);
+    uint8_t* wsm = smem;                                           // resident weight tiles (seg*2 + plane)
+    uint8_t* hsm = smem + 4 * (size_t)kWTileBytes;                 // per warpgroup: kFWgBytes
+    F16Tail* tail = (F16Tail*)(hsm + kFWarpgroups * (size_t)kFWgBytes);
+    // layer 0 has one weight segment: the pre-scaled W_ih^T lives in the unused seg-1 weight slot
+    float* wih_s = reinterpret_cast<float*>(wsm + 2 * (size_t)kWTileBytes);
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const int lane = tid & 31;
     constexpr int kProdWarp = kFWarpgroups * 4;
 
     if (tid == 0) {
-        for (int s = 0; s < kFStages; ++s) {
-            mbar_init(&tail->full[s], 1);
-            mbar_init(&tail->empty[s], kFWarpgroups);          // one arrival per consumer warpgroup
+        for (int w = 0; w < kFWarpgroups; ++w) {
+            mbar_init(&tail->full[w], 1);
+            mbar_init(&tail->empty[w], 1);
+            mbar_init(&tail->h0_full[w], 1);
         }
         mbar_init(&tail->w_full, 1);
         fence_barrier_init();
     }
     for (int i = tid; i < kGateCols; i += kFThreads) tail->bias[i] = p.bias[i] * gate_scale(i);
     if (L0)
-        for (int i = tid; i < p.c_in * kGateCols; i += kFThreads) tail->wih[i] = p.wih[i] * gate_scale(i);
+        for (int i = tid; i < p.c_in * kGateCols; i += kFThreads) wih_s[i] = p.wih[i] * gate_scale(i);
     __syncthreads();
     const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
     if (warp == kProdWarp) {
-        // ===================== producer: resident weights once, then the A planes of every tile =====================
+        // ===================== producer: resident weights once, then h_below of every (tile, step) =====================
         const bool leader = elect_one_sync();
-        if (leader && p.nseg > 0) {
-            mbar_arrive_expect_tx(&tail->w_full, (uint32_t)(p.nseg * PLANES * kWTileBytes));
-            for (int s = 0; s < p.nseg; ++s)
+        if (leader && my_tiles > 0) {
+            mbar_arrive_expect_tx(&tail->w_full, (uint32_t)(kNseg * PLANES * kWTileBytes));
+            for (int s = 0; s < kNseg; ++s)
                 for (int pl = 0; pl < PLANES; ++pl)
                     bulk_g2s(wsm + (size_t)(s * 2 + pl) * kWTileBytes, p.wimg + (size_t)(s * 2 + pl) * kWTileBytes, kWTileBytes,
                              &tail->w_full);
-            uint32_t it = 0;
-            for (int i = 0; i < my_tiles; ++i) {
-                const int tile = blockIdx.x + i * gridDim.x;
-                if (p.c_prev != nullptr && i + 2 < my_tiles)     // c_{t-1} of the tile after next -> L2 (a tile is contiguous)
-                    prefetch_l2(p.c_prev + (int64_t)(tile + 2 * (int)gridDim.x) * kTileM * kHid, kTileM * kHid * 4);
-                for (int s = 0; s < p.nseg; ++s)
-                    for (int pl = 0; pl < PLANES; ++pl, ++it) {
-                        const int stg = it % kFStages;
-                        const uint32_t ph = (it / kFStages) & 1;
-                        mbar_wait_polite(&tail->empty[stg], ph ^ 1);
-                        mbar_arrive_expect_tx(&tail->full[stg], kATileBytes);
-                        tma_load_3d(stages + (size_t)stg * kATileBytes, &p.amap[s], 0, tile * kTileM, p.aslice[s] + pl,
-                                    &tail->full[stg]);
+            if (!L0) {
+                // the warpgroups drift apart: serve whichever has released its stage instead of alternating
+                const int n_loads = my_tiles * p.t_len;
+                int done[kFWarpgroups] = {0, 0};
+                uint32_t idle = 0;
+                while (done[0] < n_loads || done[1] < n_loads) {
+                    bool issued = false;
+#pragma unroll
+                    for (int w = 0; w < kFWarpgroups; ++w) {
+                        const int n = done[w];
+                        if (n < n_loads && mbar_try_wait(&tail->empty[w], (uint32_t)(n & 1) ^ 1u)) {
+                            const int i = n / p.t_len, t = n - i * p.t_len;
+                            const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * kTileM + 64 * w;
+                            uint8_t* stage = hsm + (size_t)w * kFWgBytes + 2 * (size_t)kHTileBytes;
+                            mbar_arrive_expect_tx(&tail->full[w], (uint32_t)(PLANES * kHTileBytes));
+                            for (int pl = 0; pl < PLANES; ++pl)
+                                tma_load_3d(stage + (size_t)pl * kHTileBytes, &p.hp_map, 0, row0,
+                                            ((p.layer - 1) * p.t_len + t) * PLANES + pl, &tail->full[w]);
+                            done[w] = n + 1;
+                            issued = true;
+                        }
                     }
+                    if (issued) {
+                        idle = 0;
+                    } else {
+                        if (++idle == (1u << 28)) __trap();            // ~20 s without progress: a protocol bug
+                        __nanosleep(40);
+                    }
+                }
             }
         }
         return;
     }
-    // ===================== consumers: gate GEMM (wgmma) + LSTM cell =====================
+    // ===================== consumers: gate GEMM (wgmma) + LSTM cell, step after step =====================
     const int wg = tid >> 7;
     const int q = lane & 3;
     const bool odd = (q & 1) != 0;
-    const uint32_t row_in_tile = (uint32_t)(64 * wg + 16 * (warp & 3) + (lane >> 2) + (odd ? 8 : 0));
+    const bool issuer = (tid & 127) == 0;                          // the warpgroup's TMA / mbarrier thread
+    const uint32_t row_in_wg = (uint32_t)(16 * (warp & 3) + (lane >> 2) + (odd ? 8 : 0));
+    const uint32_t row_in_tile = 64u * (uint32_t)wg + row_in_wg;
     const uint32_t rows32 = (uint32_t)p.rows;
-    const uint32_t w_u = smem_u32(wsm), a_u = smem_u32(stages) + (uint32_t)wg * 64u * 128u;
+    uint8_t* h_sm = hsm + (size_t)wg * kFWgBytes;                  // h_prev: hi | lo
+    const uint32_t w_u = smem_u32(wsm), h_u = smem_u32(h_sm), b_u = h_u + 2u * kHTileBytes;
+    const int64_t cslice = (int64_t)p.n_tiles * kTileM * kHid;
     float acc[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    if (p.nseg > 0) mbar_wait_raw(&tail->w_full, 0);
-    uint32_t it = 0;
+    mbar_wait_raw(&tail->w_full, 0);
+    uint32_t n_below = 0;                                          // h_below stages consumed
     for (int i = 0; i < my_tiles; ++i) {
         const int tile = (int)blockIdx.x + i * (int)gridDim.x;
+        const int row0 = tile * kTileM + 64 * wg;                  // first row of this warpgroup
         const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
         const bool valid = r < rows32;
-        // layer 0: x * s of this thread's row (loaded before the MMAs: the latency hides behind them)
-        float xs[kMaxC];
-        if (L0) {
-            const float sv = valid ? p.sg[(r % (uint32_t)p.b_inner) * (uint32_t)p.t_len + (uint32_t)p.t] : 0.f;
-#pragma unroll
-            for (int c = 0; c < kMaxC; ++c)
-                xs[c] = (c < kC && valid && (CIN == 1 || c < p.c_in)) ? p.xo[((int64_t)r * p.t_len + p.t) * p.c_in + c] * sv : 0.f;
-        }
-        wg_fence_regs(acc);
-        for (int s = 0; s < p.nseg; ++s) {
-            const uint64_t w_hi = desc16_k(w_u + (uint32_t)(s * 2) * kWTileBytes);
-            const uint64_t w_lo = desc16_k(w_u + (uint32_t)(s * 2 + 1) * kWTileBytes);
-#pragma unroll
-            for (int pl = 0; pl < PLANES; ++pl, ++it) {
-                const int stg = it % kFStages;
-                mbar_wait_raw(&tail->full[stg], (it / kFStages) & 1);
-                const uint64_t a_d = desc16_k(a_u + (uint32_t)stg * kATileBytes);
-                wg_fence();
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    // hi plane: A_hi . W_hi (+ A_hi . W_lo); lo plane: A_lo . W_hi
-                    wgmma_bf16_n256_t00(acc, a_d + (uint64_t)(2 * kk), w_hi + (uint64_t)(2 * kk), (s > 0 || pl > 0 || kk > 0) ? 1u : 0u);
-                    if (PLANES == 2 && pl == 0) wgmma_bf16_n256_t00(acc, a_d + (uint64_t)(2 * kk), w_lo + (uint64_t)(2 * kk), 1u);
-                }
-                wg_commit();
-                wg_wait<0>();
-                wg_fence_regs(acc);
-                // the stage has been read: one arrival per warpgroup
-                asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-                if ((tid & 127) == 0) mbar_arrive(&tail->empty[stg]);
-            }
-        }
-        if (p.nseg == 0) {
-#pragma unroll
-            for (int k = 0; k < 128; ++k) acc[k] = 0.f;
-        }
-        // ---- LSTM cell: 32 cells per thread, row row_in_tile, units 2j + q/2 ----
         const uint32_t cbase = (uint32_t)tile * 8192u + row_in_tile * 4u;
+        if (p.has_h0) {
+            if (issuer) {
+                bulk_wait_group_read0();                           // the previous tile's last store has read the tiles
+                mbar_arrive_expect_tx(&tail->h0_full[wg], (uint32_t)(PLANES * kHTileBytes));
+                for (int pl = 0; pl < PLANES; ++pl)
+                    tma_load_3d(h_sm + (size_t)pl * kHTileBytes, &p.h0_map, 0, row0, p.layer * PLANES + pl, &tail->h0_full[wg]);
+            }
+            mbar_wait_raw(&tail->h0_full[wg], (uint32_t)i & 1u);
+        }
+        for (int t = 0; t < p.t_len; ++t) {
+            // layer 0: x * s of this thread's row (loaded before the MMAs: the latency hides behind them)
+            float xs[kMaxC];
+            if (L0) {
+                const float sv = valid ? p.sg[(r % (uint32_t)p.b_inner) * (uint32_t)p.t_len + (uint32_t)t] : 0.f;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            const float4 v = frag_to_gates(acc, j, odd);
-            const int unit = 2 * j + (q >> 1);
-            const int col = 4 * unit;
-            const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
-            const float4 a = gate_args<CIN>(v, bv, xs, tail->wih, col, p.c_in);
-            const uint32_t co = cbase + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
-            const float cp = (p.c_prev != nullptr && valid) ? p.c_prev[co] : 0.f;
-            float cn, hn;
-            lstm_cell_fwd8(a.x, a.y, a.z, a.w, cp, cn, hn);
-            if (valid) {
-                p.c_out[co] = cn;
-                const uint32_t ho = r * (uint32_t)kHid + (uint32_t)unit;
+                for (int c = 0; c < kMaxC; ++c)
+                    xs[c] = (c < kC && valid && (CIN == 1 || c < p.c_in)) ? p.xo[((int64_t)r * p.t_len + t) * p.c_in + c] * sv : 0.f;
+            }
+            // K segments: h_below (layers > 0), then h_prev (absent at t = 0 without an initial state)
+            // (each branch a complete fence .. wait sequence: a segment count known only at run time makes ptxas
+            // serialise every wgmma of the kernel)
+            const int nseg = (L0 ? 0 : 1) + ((t > 0 || p.has_h0) ? 1 : 0);
+            if (nseg > 0) {
+                wg_fence_regs(acc);
+                if (!L0) mbar_wait_raw(&tail->full[wg], n_below & 1u);
+                if (!L0 && nseg == 2) {
+                    wg_fence();
+                    fwd_segment_mma<PLANES>(acc, b_u, w_u, true);
+                    fwd_segment_mma<PLANES>(acc, h_u, w_u + 2u * kWTileBytes, false);
+                    wg_commit();
+                    wg_wait<0>();
+                } else {
+                    wg_fence();
+                    fwd_segment_mma<PLANES>(acc, L0 ? h_u : b_u, w_u, true);
+                    wg_commit();
+                    wg_wait<0>();
+                }
+                wg_fence_regs(acc);
+            } else {
+#pragma unroll
+                for (int k = 0; k < 128; ++k) acc[k] = 0.f;
+            }
+            // every warp's wgmma have read the operands, and the store of h_{t-1} has read the h_prev tiles: the stage
+            // goes back to the producer, and the tiles may be overwritten
+            if (issuer) bulk_wait_group_read0();
+            wg_sync(wg);
+            if (!L0) {
+                if (issuer) mbar_arrive(&tail->empty[wg]);
+                ++n_below;
+            }
+            // ---- LSTM cell: 32 cells per thread, row row_in_tile, units 2j + q/2 ----
+            float* c_out = p.cs + (int64_t)t * cslice;
+            const float* c_prev = t > 0 ? c_out - cslice : p.c0;
+            float* h_f32 = t == p.t_len - 1 ? p.h_f32 : nullptr;
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+                const float4 v = frag_to_gates(acc, j, odd);
+                const int unit = 2 * j + (q >> 1);
+                const int col = 4 * unit;
+                const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
+                const float4 a = gate_args<CIN>(v, bv, xs, wih_s, col, p.c_in);
+                const uint32_t co = cbase + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
+                const float cp = (c_prev != nullptr && valid) ? c_prev[co] : 0.f;
+                float cn, hn;
+                lstm_cell_fwd8(a.x, a.y, a.z, a.w, cp, cn, hn);
+                if (valid) {
+                    c_out[co] = cn;
+                    if (h_f32 != nullptr) h_f32[r * (uint32_t)kHid + (uint32_t)unit] = hn;
+                }
+                // rows past the end are computed too (a row's gates depend on that row alone) and dropped by the store
+                const uint32_t off = sw128_off16(row_in_wg, (uint32_t)unit);
                 const __nv_bfloat16 hb = __float2bfloat16_rn(hn);
-                p.h_hi[ho] = __bfloat16_as_ushort(hb);
-                if (PLANES == 2) p.h_lo[ho] = bf16_bits(hn - __bfloat162float(hb));
-                if (p.h_f32 != nullptr) p.h_f32[ho] = hn;
+                *reinterpret_cast<__nv_bfloat16*>(h_sm + off) = hb;
+                if (PLANES == 2) *reinterpret_cast<__nv_bfloat16*>(h_sm + kHTileBytes + off) = __float2bfloat16_rn(hn - __bfloat162float(hb));
+            }
+            // h_t -> the async proxy (the store below, the next step's wgmma)
+            fence_proxy_async_smem();
+            wg_sync(wg);
+            if (issuer) {
+                for (int pl = 0; pl < PLANES; ++pl)
+                    tma_store_3d(&p.hp_map, h_sm + (size_t)pl * kHTileBytes, 0, row0, (p.layer * p.t_len + t) * PLANES + pl);
+                bulk_commit_group();
             }
         }
     }
+    if (issuer) bulk_wait_group_read0();                           // shared memory outlives the stores' reads
 }
 
 // ---- weight image packer: nn.LSTM parameters of one layer -> resident operand tiles + interleaved bias / W_ih^T ----
@@ -753,13 +829,14 @@ static EncodeTiledFn16 encode_fn16() {
     }
     return fn;
 }
-// (slices, rows, 64) bf16 plane tensor, box = 1 x 128 x 64, 128-byte swizzle (rows past the end read as zeros)
-bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t slices) {
+// (slices, rows, 64) bf16 plane tensor, box = 1 x box_rows x 64, 128-byte swizzle (rows past the end read as zeros;
+// stores drop them)
+bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t slices, int box_rows) {
     EncodeTiledFn16 fn = encode_fn16();
     if (fn == nullptr) return false;
     const cuuint64_t dims[3] = {(cuuint64_t)kHid, (cuuint64_t)rows, (cuuint64_t)slices};
     const cuuint64_t strides[2] = {(cuuint64_t)kHid * 2, (cuuint64_t)rows * kHid * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)kHid, (cuuint32_t)kTileM, 1};
+    const cuuint32_t box[3] = {(cuuint32_t)kHid, (cuuint32_t)box_rows, 1};
     const cuuint32_t estr[3] = {1, 1, 1};
     return fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
@@ -822,71 +899,54 @@ extern "C" int32_t stmgcn_lstm16_pack(const float* w_ih, const float* w_hh, cons
     return check_launch("lstm16_pack");
 }
 
-extern "C" int32_t stmgcn_lstm16_step_fwd(int32_t t, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in,
-                                          int64_t b_inner, int32_t planes, const float* xo, const float* s_gate,
-                                          const void* const* wimg, const float* const* bias, const float* wih_t,
-                                          const void* h0p, const float* c0, void* hp, float* cs, float* h_top,
-                                          float* h_n, void* stream) {
-    STMGCN_REQUIRE(xo && s_gate && wimg && bias && wih_t && hp && cs, STMGCN_ERR_ARG, "lstm16_step_fwd: null pointer");
-    STMGCN_REQUIRE(planes == 1 || planes == 2, STMGCN_ERR_ARG, "lstm16_step_fwd: planes=%d", planes);
-    STMGCN_REQUIRE(t >= 0 && t < t_len && n_layers >= 1 && n_layers <= 8 && rows > 0 && c_in >= 1 && c_in <= kMaxC && b_inner > 0,
-                   STMGCN_ERR_SHAPE, "lstm16_step_fwd: t=%d T=%d L=%d rows=%lld C=%d", t, t_len, n_layers, (long long)rows, c_in);
-    STMGCN_REQUIRE(rows <= (1LL << 25), STMGCN_ERR_SHAPE, "lstm16_step_fwd: rows=%lld too large (32-bit element offsets)", (long long)rows);
-    STMGCN_REQUIRE((h0p == nullptr) == (c0 == nullptr), STMGCN_ERR_ARG, "lstm16_step_fwd: h0p and c0 go together");
+extern "C" int32_t stmgcn_lstm16_layer_fwd(int32_t layer, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in,
+                                           int64_t b_inner, int32_t planes, const float* xo, const float* s_gate,
+                                           const void* wimg, const float* bias, const float* wih_t, const void* h0p,
+                                           const float* c0, void* hp, float* cs, float* h_top, float* h_n, void* stream) {
+    STMGCN_REQUIRE(xo && s_gate && wimg && bias && hp && cs, STMGCN_ERR_ARG, "lstm16_layer_fwd: null pointer");
+    STMGCN_REQUIRE(planes == 1 || planes == 2, STMGCN_ERR_ARG, "lstm16_layer_fwd: planes=%d", planes);
+    STMGCN_REQUIRE(layer >= 0 && layer < n_layers && n_layers <= 8 && t_len >= 1 && rows > 0 && c_in >= 1 && c_in <= kMaxC &&
+                       b_inner > 0,
+                   STMGCN_ERR_SHAPE, "lstm16_layer_fwd: layer=%d L=%d T=%d rows=%lld C=%d", layer, n_layers, t_len,
+                   (long long)rows, c_in);
+    STMGCN_REQUIRE(rows <= (1LL << 25), STMGCN_ERR_SHAPE, "lstm16_layer_fwd: rows=%lld too large (32-bit element offsets)", (long long)rows);
+    STMGCN_REQUIRE((h0p == nullptr) == (c0 == nullptr), STMGCN_ERR_ARG, "lstm16_layer_fwd: h0p and c0 go together");
+    STMGCN_REQUIRE(layer > 0 || wih_t != nullptr, STMGCN_ERR_ARG, "lstm16_layer_fwd: wih_t null");
+    STMGCN_REQUIRE(layer < n_layers - 1 || h_n != nullptr || h_top != nullptr, STMGCN_ERR_ARG, "lstm16_layer_fwd: h_top null");
     cudaStream_t st = (cudaStream_t)stream;
     const int n_tiles = (int)ceil_div(rows, kTileM);
-    const int64_t rows_pad = (int64_t)n_tiles * kTileM;
-    const int64_t plane_elems = rows * kHid;                       // bf16 elements per plane
-    const int64_t cslice = rows_pad * kHid;
-    const FwdFn fn0 = fwd_kernel_for(planes, c_in == 1 ? 1 : kMaxC), fn1 = fwd_kernel_for(planes, 0);
-    if (int32_t rc = ensure_dyn_smem((const void*)fn0, kFSmem)) return rc;
-    if (int32_t rc = ensure_dyn_smem((const void*)fn1, kFSmem)) return rc;
-    CUtensorMap hp_map, h0_map;
-    STMGCN_REQUIRE(make_plane_map(&hp_map, hp, rows, (int64_t)n_layers * t_len * planes), STMGCN_ERR_STATE,
-                   "lstm16_step_fwd: cuTensorMapEncodeTiled failed (hp)");
+    const int64_t cslice = (int64_t)n_tiles * kTileM * kHid;
+    const int l = layer;
+    const FwdFn fn = fwd_kernel_for(planes, l == 0 ? (c_in == 1 ? 1 : kMaxC) : 0);
+    if (int32_t rc = ensure_dyn_smem((const void*)fn, kFSmem)) return rc;
+    Fwd16Params p;
+    memset(&p, 0, sizeof(p));
+    // a warpgroup's 64 rows are one box: its h_below loads, h0 loads and tape stores
+    STMGCN_REQUIRE(make_plane_map(&p.hp_map, hp, rows, (int64_t)n_layers * t_len * planes, 64), STMGCN_ERR_STATE,
+                   "lstm16_layer_fwd: cuTensorMapEncodeTiled failed (hp)");
     if (h0p != nullptr)
-        STMGCN_REQUIRE(make_plane_map(&h0_map, h0p, rows, (int64_t)n_layers * planes), STMGCN_ERR_STATE,
-                       "lstm16_step_fwd: cuTensorMapEncodeTiled failed (h0p)");
+        STMGCN_REQUIRE(make_plane_map(&p.h0_map, h0p, rows, (int64_t)n_layers * planes, 64), STMGCN_ERR_STATE,
+                       "lstm16_layer_fwd: cuTensorMapEncodeTiled failed (h0p)");
     const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
-    for (int l = 0; l < n_layers; ++l) {
-        STMGCN_REQUIRE(wimg[l] && bias[l], STMGCN_ERR_ARG, "lstm16_step_fwd: wimg/bias[%d] null", l);
-        Fwd16Params p;
-        memset(&p, 0, sizeof(p));
-        const StepSegs g = step_segs(l, t, t_len, planes, h0p != nullptr, cs, c0, cslice);
-        // the weight image holds [seg0 hi | seg0 lo | seg1 hi | seg1 lo]; an absent h_prev segment is the last one and is
-        // dropped: layers > 0 then use only seg 0 (W_ih), layer 0 has no MMA at all
-        for (int s = 0; s < g.nseg; ++s) {
-            if (g.src[s] == kSegAbsent) continue;
-            p.amap[p.nseg] = g.src[s] == kSegHp ? hp_map : h0_map;
-            p.aslice[p.nseg] = g.slice[s];
-            ++p.nseg;
-        }
-        p.wimg = (const uint8_t*)wimg[l];
-        p.bias = bias[l];
-        p.wih = (l == 0) ? wih_t : nullptr;
-        p.xo = xo;
-        p.sg = s_gate;
-        p.c_in = c_in;
-        p.t = t;
-        p.t_len = t_len;
-        p.b_inner = b_inner;
-        p.c_prev = g.c_prev;
-        p.c_out = cs + (int64_t)(l * t_len + t) * cslice;
-        uint16_t* hbase = (uint16_t*)hp + (int64_t)(l * t_len + t) * planes * plane_elems;
-        p.h_hi = hbase;
-        p.h_lo = planes == 2 ? hbase + plane_elems : nullptr;
-        p.h_f32 = nullptr;
-        if (t == t_len - 1) {
-            if (h_n != nullptr) p.h_f32 = h_n + (int64_t)l * rows * kHid;
-            else if (l == n_layers - 1) p.h_f32 = h_top;
-        }
-        p.rows = rows;
-        p.n_tiles = n_tiles;
-        (l == 0 ? fn0 : fn1)<<<grid, kFThreads, kFSmem, st>>>(p);
-        count_launch();
-        if (int32_t rc = check_launch("lstm16_fwd")) return rc;
-    }
-    return 0;
+    p.wimg = (const uint8_t*)wimg;
+    p.bias = bias;
+    p.wih = (l == 0) ? wih_t : nullptr;
+    p.xo = xo;
+    p.sg = s_gate;
+    p.layer = l;
+    p.c_in = c_in;
+    p.t_len = t_len;
+    p.has_h0 = h0p != nullptr ? 1 : 0;
+    p.b_inner = b_inner;
+    p.c0 = c0 != nullptr ? c0 + (int64_t)l * cslice : nullptr;
+    p.cs = cs + (int64_t)l * t_len * cslice;
+    if (h_n != nullptr) p.h_f32 = h_n + (int64_t)l * rows * kHid;
+    else if (l == n_layers - 1) p.h_f32 = h_top;
+    p.rows = rows;
+    p.n_tiles = n_tiles;
+    fn<<<grid, kFThreads, kFSmem, st>>>(p);
+    count_launch();
+    return check_launch("lstm16_layer_fwd");
 }
 
 extern "C" int32_t stmgcn_lstm16_grid(int64_t rows) {
@@ -919,10 +979,10 @@ extern "C" int32_t stmgcn_lstm16_layer_bwd(int32_t layer, int32_t t_len, int32_t
     if (int32_t rc = ensure_dyn_smem((const void*)fn, kBSmem)) return rc;
     Bwd16Params p;
     memset(&p, 0, sizeof(p));
-    STMGCN_REQUIRE(make_plane_map(&p.maps[0], hp, rows, (int64_t)n_layers * t_len * planes), STMGCN_ERR_STATE,
+    STMGCN_REQUIRE(make_plane_map(&p.maps[0], hp, rows, (int64_t)n_layers * t_len * planes, kTileM), STMGCN_ERR_STATE,
                    "lstm16_layer_bwd: cuTensorMapEncodeTiled failed (hp)");
     if (h0p != nullptr)
-        STMGCN_REQUIRE(make_plane_map(&p.maps[1], h0p, rows, (int64_t)n_layers * planes), STMGCN_ERR_STATE,
+        STMGCN_REQUIRE(make_plane_map(&p.maps[1], h0p, rows, (int64_t)n_layers * planes, kTileM), STMGCN_ERR_STATE,
                        "lstm16_layer_bwd: cuTensorMapEncodeTiled failed (h0p)");
     const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
     const bool top = (l == n_layers - 1);

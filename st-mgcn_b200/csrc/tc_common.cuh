@@ -1,5 +1,5 @@
-// Hopper (sm_90a) primitives used by the tensor-core kernels: mbarrier, 1-D bulk async copy, wgmma shared-memory matrix
-// descriptors (the instructions themselves: wgmma.cuh).
+// Hopper (sm_90a) primitives used by the tensor-core kernels: mbarrier, 1-D bulk async copy, TMA tensor stores, wgmma
+// shared-memory matrix descriptors (the instructions themselves: wgmma.cuh).
 //
 // Precision scheme "3xTF32": every fp32 operand v is split into hi = v with the low 13 mantissa bits cleared
 // (exactly representable in tf32, so the tensor core's own fp32->tf32 conversion cannot change it) and
@@ -80,6 +80,16 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                  "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
+
+// ---- TMA tensor store shared -> global through a CUtensorMap (rows past the tensor's end are dropped); completion is
+// tracked per issuing thread in bulk async-groups ---------------------------------------------------------------------
+__device__ __forceinline__ void tma_store_3d(const void* tmap, const void* smem_src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 :: "l"(tmap), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the issuing thread's bulk groups have finished READING shared memory (the source tile may be overwritten)
+__device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
 // One elected lane of a fully converged warp, for the single-thread TMA / mbarrier instructions (ptxas can prove that
 // elect.sync selects one thread; a `lane == 0` guard gets wrapped in a serialisation loop).

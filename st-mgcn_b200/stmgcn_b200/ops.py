@@ -430,8 +430,7 @@ def _lstm16_images(weights: Sequence[torch.Tensor], n_layers: int, c_in: int):
             _lib.check(L.stmgcn_lstm16_pack(w_ih.data_ptr(), w_hh.data_ptr(), b_ih.data_ptr(), b_hh.data_ptr(), l, c_in,
                                             wimg[l].data_ptr(), bias[l].data_ptr(), wih_t.data_ptr() if l == 0 else None,
                                             st), "lstm16_pack")
-        return dict(wimg=wimg, bias=bias, wih_t=wih_t, wimg_arr=_lib.ptr_array([v.data_ptr() for v in wimg]),
-                    bias_arr=_lib.ptr_array([v.data_ptr() for v in bias]))
+        return dict(wimg=wimg, bias=bias, wih_t=wih_t)
 
     return _cached_images(weights, ("lstm16", c_in), pack)
 
@@ -463,11 +462,11 @@ def _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes,
         h_n = None
         h_top = torch.empty((rows, 64), device=dev, dtype=torch.float32)
     st = _stream()
-    for t in range(t_len):
-        _lib.check(L.stmgcn_lstm16_step_fwd(t, t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(),
-                                            img["wimg_arr"], img["bias_arr"], img["wih_t"].data_ptr(), _p(h0p), _p(c0b),
-                                            hp.data_ptr(), cs.data_ptr(), h_top.data_ptr(), _p(h_n), st),
-                   "lstm16_step_fwd")
+    for l in range(n_layers):
+        _lib.check(L.stmgcn_lstm16_layer_fwd(l, t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(),
+                                             img["wimg"][l].data_ptr(), img["bias"][l].data_ptr(), img["wih_t"].data_ptr(),
+                                             _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(), h_top.data_ptr(), _p(h_n), st),
+                   "lstm16_layer_fwd")
     if want_state:
         c_n = from_blocked(cs[:, t_len - 1], rows)
     else:
