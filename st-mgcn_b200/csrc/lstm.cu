@@ -1,7 +1,9 @@
 // K3b: the shared-weight LSTM of CG_LSTM (reference STMGCN.py:21-22, :44, :47-50; nn.LSTM semantics: gate
-// order i,f,g,o, b_ih + b_hh, zero initial state STMGCN.py:53-57), exact-fp32 CUDA-core path: every shape the
-// tensor-core kernels of lstm16.cu do not cover (H != 64, C > 4), and the on-device reference the parity tests
-// compare those kernels with.  Own tape: hs, cs (L,T,R,H) and post-activation gates (L,T,R,4H), fp32 row-major.
+// order i,f,g,o, b_ih + b_hh, zero initial state STMGCN.py:53-57), exact-fp32 CUDA-core path: the shapes the
+// tensor-core kernels of lstm16.cu do not cover (H != 64, T > 64) within this file's own limits -- H a multiple of 4
+// and <= 128, C <= 4, L <= 8 (check_dims; larger shapes return STMGCN_ERR_SHAPE, they do not run) -- and the on-device
+// reference the parity tests compare those kernels with.  Own tape: hs, cs (L,T,R,H) and post-activation gates
+// (L,T,R,4H), fp32 row-major.
 //
 // Rows r = n*B + b (node-major) so the top layer's last hidden state IS the (N,B,H) operand of the spatial
 // Chebyshev GCN (STMGCN.py:114) with no permute.  The context-gate modulation obs * s[b,t] (STMGCN.py:44)

@@ -40,18 +40,32 @@ CASES = [
     ("waves_b64", None, 64, 12, 3, 1, False),         # several tiles per CTA, ds_acc carried across items
     ("waves_b37_state", None, 37, 12, 3, 2, True),    # several tiles per CTA, atomic d_s, runtime-C variant
     ("b1100", 2, 1100, 4, 3, 1, False),               # windows spanning tiles
+    ("saturated", 5, 40, 20, 3, 1, True),             # pre-activations to +-70 (capped exponentials), c to +-20
 ]
 
 
-def _inputs(n, b, t, lyr, c, state, seed):
+def _inputs(n, b, t, lyr, c, state, seed, saturate=False):
+    """``saturate``: the terms the kernels add with fp32 FMAs drive the gates into saturation -- inputs x3 and layer 0's
+    W_ih in +-3, biases i +10, f +20, g +-15 (one sign per unit), o uniform in +-50 -- so the pre-activations reach about
+    +-70 and c about +-T, while the tensor-core operands W_hh and W_ih of layers > 0 keep their usual +-0.25.  (With
+    those in +-2 as well, the two-plane kernel is 5.9e-5 off step-local and 1.1e-4 in the gradients, measured: three
+    bf16 passes keep ~16 bits of each product, so the error of a pre-activation grows with sum |W| |h|, here 8-fold,
+    while h stays within +-1.  The one-plane mode, whose reference rounds like the kernel, stayed within its bars.)"""
     gen = torch.Generator().manual_seed(seed)
-    xo = torch.randn(n, b, t, c, generator=gen)
+    xo = torch.randn(n, b, t, c, generator=gen) * (3.0 if saturate else 1.0)
     s = 0.2 + 0.8 * torch.rand(b, t, generator=gen)
     ws = []
     for l in range(lyr):
         in_l = c if l == 0 else HID
-        ws += [(torch.rand(4 * HID, in_l, generator=gen) - 0.5) * 0.5, (torch.rand(4 * HID, HID, generator=gen) - 0.5) * 0.5,
+        amp_ih = 6.0 if saturate and l == 0 else 0.5
+        ws += [(torch.rand(4 * HID, in_l, generator=gen) - 0.5) * amp_ih, (torch.rand(4 * HID, HID, generator=gen) - 0.5) * 0.5,
                (torch.rand(4 * HID, generator=gen) - 0.5) * 0.5, (torch.rand(4 * HID, generator=gen) - 0.5) * 0.5]
+        if saturate:
+            ws[-2] = torch.zeros(4 * HID)
+            ws[-2][:HID], ws[-2][HID:2 * HID] = 10.0, 20.0
+            ws[-2][2 * HID:3 * HID] = 15.0 * torch.sign(torch.randn(HID, generator=gen))
+            ws[-2][3 * HID:] = (torch.rand(HID, generator=gen) - 0.5) * 100.0
+            ws[-1] = torch.zeros(4 * HID)
     h0 = c0 = None
     if state:
         h0 = torch.randn(lyr, n * b, HID, generator=gen) * 0.3
@@ -118,16 +132,21 @@ def test_lstm16_kernels_match_the_fp64_plane_reference(case, planes):
     four gradients of every layer) of the tensor-core LSTM against the tape-forced fp64 reference.  Negative control:
     the reference in the other plane mode lands outside the forward bar.
 
-    Measured on an H100 (max over the seven cases): one plane -- step-local forward 3.5e-7 (excess over half a bf16
-    ulp for h), h_top / h_n / c_n 3.9e-7, gradients 6.0e-6, control 5.1e-4 .. 1.6e-3; two planes -- step-local forward
+    Measured on an H100 (max over the eight cases): one plane -- step-local forward 4.1e-7 (excess over half a bf16
+    ulp for h), h_top / h_n / c_n 3.9e-7, gradients 6.5e-6, control 5.1e-4 .. 1.6e-3; two planes -- step-local forward
     8.5e-6 (the hi + lo representation of h keeps ~17 bits), h_top / h_n / c_n 3.1e-6, gradients 1.4e-5, control
-    1.2e-3 .. 2.9e-3.  Before the layer-0 W_ih gradient took the lo plane of x*s, weight_ih_l0 was 8e-4 .. 2.2e-3 off
+    1.2e-3 .. 2.9e-3.  The saturated case: step-local forward 4.1e-7 / 4.9e-6, gradients 6.5e-6 / 1.1e-5 (one / two
+    planes).  Before the layer-0 W_ih gradient took the lo plane of x*s, weight_ih_l0 was 8e-4 .. 2.2e-3 off
     with one plane."""
     name, n, b, t, lyr, c, state = case
     if n is None:
         n = _wave_regions(b)
-    xo, s, h0, c0, ws, d_top = _inputs(n, b, t, lyr, c, state, seed=10 * CASES.index(case) + planes)
+    xo, s, h0, c0, ws, d_top = _inputs(n, b, t, lyr, c, state, seed=10 * CASES.index(case) + planes,
+                                       saturate=name == "saturated")
     h_top, hc_n, ktape, d_s, grads = _kernel(xo, s, h0, c0, ws, lyr, planes, d_top)
+    if name == "saturated":
+        assert all(bool(torch.isfinite(v).all()) for v in (h_top, ktape["c"], d_s, *grads))
+        assert float(ktape["c"].abs().max()) > 15.0, "the saturated case does not drive c far enough"
     hs, cs, layers, s64 = _reference(xo, s, h0, c0, ws, lyr, planes, ktape)
     errs = {"step-local forward": _step_local_error(ktape, hs, cs, planes),
             "h_top": O.max_rel_err(h_top.cpu().numpy(), hs[-1][-1].detach().cpu().numpy())}
