@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define STMGCN_ABI_VERSION 4
+#define STMGCN_ABI_VERSION 5
 
 /* error codes < 0 */
 #define STMGCN_ERR_ARG      (-1)   /* null pointer / bad enum */
@@ -122,41 +122,37 @@ int32_t stmgcn_gate_fwd(const float* pool, int64_t b, int32_t t, int64_t n_regio
 int32_t stmgcn_gate_bwd(const float* d_s, const float* z, const float* a1, const float* s, int64_t b,
                         int32_t t, const float* fcw, float* d_fcw, float* d_fcb, float* d_z, void* stream);
 
-/* ---- K3b (exact fp32, any H <= 128): shared-weight LSTM, one call per timestep (STMGCN.py:44, :47-50) ------------
- * The CUDA-core path for every shape the tensor-core kernels below do not cover (H != 64 or C > 4), and the on-device
- * reference the parity tests compare them with.  Weights are passed packed, H = hid, columns gate-interleaved
+/* ---- K3b (exact fp32, any H <= 128): shared-weight LSTM over the whole sequence (STMGCN.py:44, :47-50) ---------------
+ * The CUDA-core path for every shape the tensor-core kernels below do not cover (H != 64, C > 4 or T > 64), and the
+ * on-device reference the parity tests compare them with.  Weights are passed packed, H = hid, columns gate-interleaved
  * col = 4*unit + gate (gate order i,f,g,o):
- *   wx     : (C, 4H)      = W_ih_l0^T                      (layer-0 input weights)
- *   wp[l]  : (kd_l, 4H)   = W_hh_0^T (l = 0, kd_0 = H) or [W_ih_l^T ; W_hh_l^T] (l > 0, kd_l = 2H)
- *   bp[l]  : (4H)         = b_ih_l + b_hh_l
- *   wpt[l] : (4H, kd_l)   = wp[l]^T                        (backward data operand)
+ *   wx   : (C, 4H)      = W_ih_l0^T                      (layer-0 input weights)
+ *   wp   : flat, layer l's block wp_l (kd_l, 4H) = W_hh_0^T (l = 0, kd_0 = H) or [W_ih_l^T ; W_hh_l^T] (l > 0,
+ *          kd_l = 2H); the blocks lie back to back, so wp_l starts 4H*H*(l == 0 ? 0 : 2l - 1) floats in
+ *   wpt  : flat, layer l's block (4H, kd_l) = wp_l^T at the same offset (backward data operand)
+ *   bp   : (L, 4H)      = b_ih_l + b_hh_l
  * State / tape tensors, rows r = n*B + b, fp32 row-major:
  *   hs, cs: (L, T, R, H);  gates: (L, T, R, 4H) post-activation, gate-interleaved (NULL in inference);
  * xo: (R, T, C) node-major observations, s_gate: (B, T) context gate (the modulation xo * s is fused into the layer-0
  * input read, STMGCN.py:44).  h0/c0: (L, R, H) or NULL (zeros, STMGCN.py:53-57).
- * Step t computes layers 0..L-1.  Limits: H % 4 == 0, H <= 128, C <= 4, L <= 8. */
-int32_t stmgcn_lstm_step_fwd(int32_t t, int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid,
-                             int32_t c_in, int64_t b_inner, const float* xo, const float* s_gate,
-                             const float* wx, const float* const* wp, const float* const* bp,
-                             const float* h0, const float* c0, float* hs, float* cs, float* gates, void* stream);
-/* BPTT step t (call t = T-1 .. 0).  d_top: (R, H) gradient of hs[L-1][T-1] (read at t = T-1 only).
- * Workspaces: dh_rec, dc: (L, R, H); dx_work: (R, H).  No initialisation is needed: the call with t = T-1 treats the
- * incoming dh_rec / dc as zero without reading them (h_n / c_n carry no gradient, STMGCN.py:113).
- * gates[l][t] is overwritten IN PLACE with the pre-activation gradients dA (stmgcn_lstm_wgrad reads them).
- * Accumulates (+=; caller zeroes): d_s (B,T) = sum_{n,c} dxmod * xo (gate adjoint, STMGCN.py:44),
- * dwx (C,4H), dbp[l] (4H). */
-int32_t stmgcn_lstm_step_bwd(int32_t t, int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid,
-                             int32_t c_in, int64_t b_inner, const float* xo, const float* s_gate,
-                             const float* wx, const float* const* wpt, const float* c0, const float* cs,
-                             float* gates, const float* d_top, float* dh_rec, float* dc, float* dx_work,
-                             float* d_s, float* dwx, float* const* dbp, void* stream);
-/* weight gradients of one layer after all stmgcn_lstm_step_bwd calls:
- * dwp (kd_l, 4H) += [h_below_t | h_{t-1}]^T dA summed over all (t, r). */
-int32_t stmgcn_lstm_wgrad(int32_t layer, int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid,
-                          const float* h0, const float* hs, const float* gates_da, float* dwp, void* stream);
+ * Limits: H % 4 == 0, H <= 128, C <= 4, L <= 8. */
+int32_t stmgcn_lstm_fwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid, int32_t c_in, int64_t b_inner,
+                        const float* xo, const float* s_gate, const float* wx, const float* wp, const float* bp,
+                        const float* h0, const float* c0, float* hs, float* cs, float* gates, void* stream);
+/* BPTT over all timesteps, then the weight gradients.  d_top: (R, H) gradient of hs[L-1][T-1].
+ * Workspaces: dh_rec, dc: (L, R, H); dx_work: (R, H).  No initialisation is needed: the step t = T-1 treats the incoming
+ * dh_rec / dc as zero without reading them (h_n / c_n carry no gradient, STMGCN.py:113).
+ * gates is overwritten IN PLACE with the pre-activation gradients dA, so it serves one backward only.
+ * Accumulates (+=; caller zeroes): d_s (B,T) = sum_{n,c} dxmod * xo (gate adjoint, STMGCN.py:44), dwx (C,4H),
+ * dwp (laid out like wp) += [h_below_t | h_{t-1}]^T dA summed over all (t, r), dbp (L, 4H). */
+int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid, int32_t c_in, int64_t b_inner,
+                        const float* xo, const float* s_gate, const float* wx, const float* wpt, const float* h0,
+                        const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
+                        float* dh_rec, float* dc, float* dx_work, float* d_s, float* dwx, float* dwp, float* dbp,
+                        void* stream);
 
 /* ---- K3b on the tensor cores (H = 64, C <= 4): bf16-plane LSTM without a gate tape -----------------------------
- * Same arithmetic contract as stmgcn_lstm_step_fwd/_bwd/_wgrad (STMGCN.py:44, :47-50; nn.LSTM semantics, fp32 state and
+ * Same arithmetic contract as stmgcn_lstm_fwd/_bwd (STMGCN.py:44, :47-50; nn.LSTM semantics, fp32 state and
  * accumulation), different tape:
  *   hp : (L, T, P, R, 64) bf16 -- every hidden state as P planes; P = 2: hi = bf16(h), lo = bf16(h - hi) (3-pass
  *        "3xBF16" products, ~2^-18 operand error: fp32-grade, the 1e-4 parity bar holds with >10x margin);

@@ -54,9 +54,17 @@ struct TallCfg {
 
 // ----------------------------------------------------------------------------------------------------
 // forward: C tile [TM x TN] at rows [row0, row0+TM), columns [col0, col0+TN)
-// Epi::operator()(acc, row0, mg, MG, col0, tn) consumes the 8x8 register tile:
-//   acc[i][j] is row (row0 + mg + i*MG), column col0 + (j<4 ? 4*tn + j : TN/2 + 4*tn + j-4).
+// Epi::operator()(acc, tile, rows, nc) consumes the 8x8 register tile: acc[i][j] is row tile.row(i), column tile.col(j).
+// The columns of a thread are two float4 groups TN/2 apart, the two float4 each k step reads from the staged B row.
 // ----------------------------------------------------------------------------------------------------
+template <int TN>
+struct TallTile {
+    int64_t row0;
+    int mg, col0, tn;
+    __device__ __forceinline__ int64_t row(int i) const { return row0 + mg + (int64_t)i * TallCfg<TN>::MG; }
+    __device__ __forceinline__ int col(int j) const { return col0 + 4 * tn + (j & 3) + (j >> 2) * (TN / 2); }
+};
+
 template <int TN, bool VEC, class Epi>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 tall_gemm_kernel(ASegs a, int64_t rows, int kd, const float* __restrict__ bmat, int ldb, int nc, Epi epi) {
@@ -162,7 +170,7 @@ tall_gemm_kernel(ASegs a, int64_t rows, int kd, const float* __restrict__ bmat, 
         }
         __syncthreads();
     }
-    epi(acc, row0, mg, Cfg::MG, col0, tn, rows, nc);
+    epi(acc, TallTile<TN>{row0, mg, col0, tn}, rows, nc);
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -318,11 +326,27 @@ reduce_gemm_kernel(ASegs a, ReduceTime tm, int64_t rows, int kd, const float* __
 }
 
 // host-side launch helpers -----------------------------------------------------------------------------
-template <int TN, bool VEC, class Epi>
+// The VEC kernels stage A, B and D with 16-byte cp.async: every 4-float group must lie inside one segment and one row,
+// and start 16-byte aligned.  Loaders of both variants feed the same FMA order, so the choice never changes results.
+inline bool vec_ok(const ASegs& a, const float* b, int64_t ldb, int nc) {
+    if (a.segw % 4 || a.lda % 4 || ldb % 4 || nc % 4 || !aligned16(b)) return false;
+    for (int s = 0; s < a.nseg; ++s)
+        if (a.seg[s] && !aligned16(a.seg[s])) return false;
+    return true;
+}
+
+inline bool reduce_vec_ok(const ASegs& a, const ReduceTime& tm, const float* d, int64_t ldd, int nc) {
+    if (!vec_ok(a, d, ldd, nc) || tm.d_tstride % 4) return false;
+    for (int s = 0; s < a.nseg; ++s)
+        if (tm.a_tstride[s] % 4 || (tm.a_t0[s] && !aligned16(tm.a_t0[s]))) return false;
+    return true;
+}
+
+template <int TN, class Epi>
 inline int32_t launch_tall(const ASegs& a, int64_t rows, int kd, const float* bmat, int ldb, int nc,
                            const Epi& epi, cudaStream_t st, const char* what) {
     using Cfg = TallCfg<TN>;
-    auto kern = tall_gemm_kernel<TN, VEC, Epi>;
+    auto kern = vec_ok(a, bmat, ldb, nc) ? tall_gemm_kernel<TN, true, Epi> : tall_gemm_kernel<TN, false, Epi>;
     if (int32_t rc = ensure_dyn_smem((const void*)kern, Cfg::SMEM)) return rc;
     dim3 grid((unsigned)ceil_div(rows, Cfg::TM), (unsigned)ceil_div(nc, TN));
     kern<<<grid, kGemmThreads, Cfg::SMEM, st>>>(a, rows, kd, bmat, ldb, nc, epi);
@@ -330,11 +354,11 @@ inline int32_t launch_tall(const ASegs& a, int64_t rows, int kd, const float* bm
     return check_launch(what);
 }
 
-template <int TN, bool VEC>
+template <int TN>
 inline int32_t launch_reduce(const ASegs& a, const ReduceTime& tm, int64_t rows, int kd, const float* d,
                              int64_t ldd, int nc, float* gout, int ldg, cudaStream_t st, const char* what) {
     using Cfg = ReduceCfg<TN>;
-    auto kern = reduce_gemm_kernel<TN, VEC>;
+    auto kern = reduce_vec_ok(a, tm, d, ldd, nc) ? reduce_gemm_kernel<TN, true> : reduce_gemm_kernel<TN, false>;
     if (int32_t rc = ensure_dyn_smem((const void*)kern, Cfg::SMEM)) return rc;
     const int64_t total_chunks = ceil_div(rows, kKC) * tm.n_t;
     const int panels = (int)(ceil_div(kd, Cfg::TMK) * ceil_div(nc, TN));
@@ -345,13 +369,6 @@ inline int32_t launch_reduce(const ASegs& a, const ReduceTime& tm, int64_t rows,
     kern<<<grid, kGemmThreads, Cfg::SMEM, st>>>(a, tm, rows, kd, d, ldd, nc, gout, ldg);
     count_launch();
     return check_launch(what);
-}
-
-inline bool vec_ok(const ASegs& a, const float* b, int ldb, int nc) {
-    if (a.segw % 4 || a.lda % 4 || ldb % 4 || nc % 4 || !aligned16(b)) return false;
-    for (int s = 0; s < a.nseg; ++s)
-        if (a.seg[s] && !aligned16(a.seg[s])) return false;
-    return true;
 }
 
 }  // namespace stmgcn

@@ -30,17 +30,16 @@ struct ProjEpi {
     const float* bias;       // (q) or nullptr
     int act;
     float* out;              // (rows, q)
-    int half_cols;
 
-    __device__ __forceinline__ void operator()(float (&acc)[8][8], int64_t row0, int mg, int MG, int col0,
-                                               int tn, int64_t rows, int nc) const {
+    template <int TN>
+    __device__ __forceinline__ void operator()(float (&acc)[8][8], const TallTile<TN>& tile, int64_t rows, int nc) const {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            const int64_t r = row0 + mg + (int64_t)i * MG;
+            const int64_t r = tile.row(i);
             if (r >= rows) continue;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const int n = col0 + (j < 4 ? 4 * tn + j : half_cols + 4 * tn + (j - 4));
+                const int n = tile.col(j);
                 if (n >= nc) continue;
                 float v = acc[i][j] + (bias ? bias[n] : 0.f);
                 if (act == STMGCN_ACT_RELU) v = fmaxf(v, 0.f);
@@ -55,17 +54,16 @@ struct StoreSegEpi {
     float* u;
     int64_t stride_u;
     int p;
-    int half_cols;
 
-    __device__ __forceinline__ void operator()(float (&acc)[8][8], int64_t row0, int mg, int MG, int col0,
-                                               int tn, int64_t rows, int nc) const {
+    template <int TN>
+    __device__ __forceinline__ void operator()(float (&acc)[8][8], const TallTile<TN>& tile, int64_t rows, int nc) const {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            const int64_t r = row0 + mg + (int64_t)i * MG;
+            const int64_t r = tile.row(i);
             if (r >= rows) continue;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const int n = col0 + (j < 4 ? 4 * tn + j : half_cols + 4 * tn + (j - 4));
+                const int n = tile.col(j);
                 if (n >= nc) continue;
                 const int k = n / p;
                 u[(int64_t)k * stride_u + r * p + (n - k * p)] = acc[i][j];
@@ -156,22 +154,11 @@ small_wgrad_kernel(ASegs a, int64_t rows, int kd, const float* __restrict__ dz, 
 }
 
 template <class Epi>
-int32_t launch_tall_auto(const ASegs& a, int64_t rows, int kd, const float* b, int ldb, int nc, Epi epi,
+int32_t launch_tall_auto(const ASegs& a, int64_t rows, int kd, const float* b, int ldb, int nc, const Epi& epi,
                          cudaStream_t st, const char* what) {
-    const bool vec = vec_ok(a, b, ldb, nc);
-    if (nc <= 64) {
-        epi.half_cols = 32;
-        return vec ? launch_tall<64, true>(a, rows, kd, b, ldb, nc, epi, st, what)
-                   : launch_tall<64, false>(a, rows, kd, b, ldb, nc, epi, st, what);
-    }
-    if (nc <= 128) {
-        epi.half_cols = 64;
-        return vec ? launch_tall<128, true>(a, rows, kd, b, ldb, nc, epi, st, what)
-                   : launch_tall<128, false>(a, rows, kd, b, ldb, nc, epi, st, what);
-    }
-    epi.half_cols = 128;
-    return vec ? launch_tall<256, true>(a, rows, kd, b, ldb, nc, epi, st, what)
-               : launch_tall<256, false>(a, rows, kd, b, ldb, nc, epi, st, what);
+    if (nc <= 64) return launch_tall<64>(a, rows, kd, b, ldb, nc, epi, st, what);
+    if (nc <= 128) return launch_tall<128>(a, rows, kd, b, ldb, nc, epi, st, what);
+    return launch_tall<256>(a, rows, kd, b, ldb, nc, epi, st, what);
 }
 
 }  // namespace
@@ -189,11 +176,7 @@ int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     if (wimg && !pool && proj_tc_applicable(ks, p, q, s, out, nullptr) && stride_k % 4 == 0)   // wgmma path (proj_tc.cu)
         return launch_proj_fwd_tc(s, stride_k, ks, rows, wimg, bias, act, out, st);
     const ASegs a = stack_segs(s, stride_k, ks, p);
-    ProjEpi epi;
-    epi.bias = bias;
-    epi.act = act;
-    epi.out = out;
-    epi.half_cols = 0;
+    const ProjEpi epi{bias, act, out};
     if (int32_t rc = launch_tall_auto(a, rows, ks * p, w, q, q, epi, st, "proj_fwd")) return rc;
     if (pool) {
         STMGCN_REQUIRE(q == p, STMGCN_ERR_SHAPE, "proj_fwd: pooling needs q == p (got %d, %d)", q, p);
@@ -252,14 +235,8 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
         ReduceTime tm{};
         tm.n_t = 1;
         const int kd = ks * p;
-        bool vec = (p % 4 == 0) && (q % 4 == 0) && aligned16(s) && aligned16(dz_work) && (stride_k % 4 == 0);
-        int32_t rc;
-        if (q <= 64)
-            rc = vec ? launch_reduce<64, true>(a, tm, rows, kd, dz_work, q, q, dw, q, st, "proj_bwd dW")
-                     : launch_reduce<64, false>(a, tm, rows, kd, dz_work, q, q, dw, q, st, "proj_bwd dW");
-        else
-            rc = vec ? launch_reduce<256, true>(a, tm, rows, kd, dz_work, q, q, dw, q, st, "proj_bwd dW")
-                     : launch_reduce<256, false>(a, tm, rows, kd, dz_work, q, q, dw, q, st, "proj_bwd dW");
+        const int32_t rc = q <= 64 ? launch_reduce<64>(a, tm, rows, kd, dz_work, q, q, dw, q, st, "proj_bwd dW")
+                                   : launch_reduce<256>(a, tm, rows, kd, dz_work, q, q, dw, q, st, "proj_bwd dW");
         if (rc) return rc;
     }
     if (u) {    // U_k = dZ W_k^T : A = dZ (rows x q), B = W^T (q x ks*p)
@@ -268,11 +245,7 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
         a.segw = q;
         a.lda = q;
         a.seg[0] = dz_work;
-        StoreSegEpi epi;
-        epi.u = u;
-        epi.stride_u = stride_u;
-        epi.p = p;
-        epi.half_cols = 0;
+        const StoreSegEpi epi{u, stride_u, p};
         return launch_tall_auto(a, rows, q, wt, ks * p, ks * p, epi, st, "proj_bwd U");
     }
     return 0;

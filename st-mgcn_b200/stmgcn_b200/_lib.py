@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("STMGCN_LIB_PATH") or os.path.join(os.path.dirname(_HERE), "lib", "libstmgcn_b200.so")
 
 ACT_NONE, ACT_RELU = 0, 1
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 # (name, restype, argtypes) -- one row per symbol in include/stmgcn_b200.h
 _P = c_void_p
@@ -39,12 +39,10 @@ SIGNATURES = [
                                   c_float, c_int64, _P, _P, _P, _P, c_int64, _P, _P]),
     ("stmgcn_gate_fwd", c_int32, [_P, c_int64, c_int32, c_int64, _P, _P, _P, _P, _P, _P]),
     ("stmgcn_gate_bwd", c_int32, [_P, _P, _P, _P, c_int64, c_int32, _P, _P, _P, _P, _P]),
-    ("stmgcn_lstm_step_fwd", c_int32, [c_int32, c_int32, c_int32, c_int64, c_int32, c_int32, c_int64, _P, _P,
-                                       _P, POINTER(c_void_p), POINTER(c_void_p), _P, _P, _P, _P, _P, _P]),
-    ("stmgcn_lstm_step_bwd", c_int32, [c_int32, c_int32, c_int32, c_int64, c_int32, c_int32, c_int64, _P, _P,
-                                       _P, POINTER(c_void_p), _P, _P, _P, _P, _P, _P, _P, _P, _P,
-                                       POINTER(c_void_p), _P]),
-    ("stmgcn_lstm_wgrad", c_int32, [c_int32, c_int32, c_int32, c_int64, c_int32, _P, _P, _P, _P, _P]),
+    ("stmgcn_lstm_fwd", c_int32, [c_int32, c_int32, c_int64, c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P, _P,
+                                  _P, _P, _P, _P]),
+    ("stmgcn_lstm_bwd", c_int32, [c_int32, c_int32, c_int64, c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P, _P,
+                                  _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     ("stmgcn_lstm16_pack", c_int32, [_P, _P, _P, _P, c_int32, c_int32, _P, _P, _P, _P]),
     ("stmgcn_lstm16_layer_fwd", c_int32, [c_int32, c_int32, c_int32, c_int64, c_int32, c_int64, c_int32, _P, _P,
                                           _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -9,7 +9,7 @@ Functions (reference lines they replace):
   ChebGCN          GCN.py:24-43 on a sparse L~ (recurrence on features) -> out (N,B,q)
   TemporalPool     STMGCN.py:40-42: GCN over time-as-features + residual + sum over regions -> (B,T)
   ContextGate      STMGCN.py:42-43: /N, fc, relu, fc (same weights), sigmoid -> s (B,T)
-  SharedLSTM       STMGCN.py:44,47-50: modulate + 3-layer shared LSTM, one library call per timestep (lstm16.cu / lstm.cu)
+  SharedLSTM       STMGCN.py:44,47-50: modulate + 3-layer shared LSTM (lstm16.cu: one call per layer / lstm.cu: one call)
   FuseOut          STMGCN.py:116-118: sum over graphs + output FC -> (B,N,C)
 """
 from __future__ import annotations
@@ -366,7 +366,8 @@ def from_blocked(x: torch.Tensor, rows: int) -> torch.Tensor:
 
 
 def _pack_lstm(weights: Sequence[torch.Tensor], n_layers: int, hid: int):
-    """nn.LSTM parameters -> packed operands (see include/stmgcn_b200.h)."""
+    """nn.LSTM parameters -> packed operands (see include/stmgcn_b200.h): wx (C,4H); flat wp / wpt holding each layer's
+    (kd_l,4H) / (4H,kd_l) block after the blocks of the layers below (kd_0 = H, kd_l = 2H); bp (L,4H)."""
     w_ih0 = weights[0]
     c_in = w_ih0.shape[1]
     wx = w_ih0.reshape(4, hid, c_in).permute(2, 1, 0).reshape(c_in, 4 * hid).contiguous()
@@ -375,18 +376,18 @@ def _pack_lstm(weights: Sequence[torch.Tensor], n_layers: int, hid: int):
         w_ih, w_hh, b_ih, b_hh = weights[4 * l:4 * l + 4]
         cat = w_hh if l == 0 else torch.cat([w_ih, w_hh], dim=1)
         kd = cat.shape[1]
-        packed = cat.reshape(4, hid, kd).permute(2, 1, 0).reshape(kd, 4 * hid).contiguous()
-        wp.append(packed)
-        wpt.append(packed.t().contiguous())
-        bp.append((b_ih + b_hh).reshape(4, hid).t().reshape(4 * hid).contiguous())
-    return wx, wp, bp, wpt
+        packed = cat.reshape(4, hid, kd).permute(2, 1, 0).reshape(kd, 4 * hid)
+        wp.append(packed.reshape(-1))
+        wpt.append(packed.t().reshape(-1))
+        bp.append((b_ih + b_hh).reshape(4, hid).t().reshape(4 * hid))
+    return wx, torch.cat(wp), torch.stack(bp), torch.cat(wpt)
 
 
 def _unpack_lstm_grads(dwx, dwp, dbp, n_layers: int, hid: int, c_in: int):
     grads = []
-    for l in range(n_layers):
-        kd = dwp[l].shape[0]
-        full = dwp[l].reshape(kd, hid, 4).permute(2, 1, 0).reshape(4 * hid, kd)
+    kds = [hid] + [2 * hid] * (n_layers - 1)
+    for l, (kd, blk) in enumerate(zip(kds, dwp.split([kd * 4 * hid for kd in kds]))):
+        full = blk.reshape(kd, hid, 4).permute(2, 1, 0).reshape(4 * hid, kd)
         if l == 0:
             d_ih = dwx.reshape(c_in, hid, 4).permute(2, 1, 0).reshape(4 * hid, c_in).contiguous()
             d_hh = full.contiguous()
@@ -530,6 +531,46 @@ def _lstm16_backward(xo, s_gate, tape, n_layers, planes, d_top):
     return d_s, grads
 
 
+def _exact_forward(xo, s_gate, h0c, c0c, n_layers, hid, want_state, weights, keep_tape):
+    """Forward of the exact-fp32 path, one library call.  Returns (h_top (N,B,H), h_n, c_n, tape tuple or None)."""
+    n, b, t_len, c_in = xo.shape
+    rows = n * b
+    wx, wp, bp, wpt = _pack_lstm(weights, n_layers, hid)
+    hs = xo.new_empty((n_layers, t_len, rows, hid))
+    cs = xo.new_empty((n_layers, t_len, rows, hid))
+    gates = xo.new_empty((n_layers, t_len, rows, 4 * hid)) if keep_tape else None
+    _lib.check(L.stmgcn_lstm_fwd(t_len, n_layers, rows, hid, c_in, b, xo.data_ptr(), s_gate.data_ptr(), wx.data_ptr(),
+                                 wp.data_ptr(), bp.data_ptr(), _p(h0c), _p(c0c), hs.data_ptr(), cs.data_ptr(), _p(gates),
+                                 _stream()), "lstm_fwd")
+    h_top = hs[n_layers - 1, t_len - 1].view(n, b, hid)
+    if want_state:
+        h_n, c_n = hs[:, t_len - 1], cs[:, t_len - 1]
+    else:                       # ST_MGCN discards the final state (STMGCN.py:113)
+        h_n = c_n = hs.new_empty(0)
+    return h_top, h_n, c_n, ((h0c, c0c, hs, cs, gates, wx, wpt) if keep_tape else None)
+
+
+def _exact_backward(xo, s_gate, tape, n_layers, hid, d_top):
+    """BPTT of the exact-fp32 path, one library call; it overwrites the gate tape with dA.  Returns (d_s, grads)."""
+    h0, c0, hs, cs, gates, wx, wpt = tape
+    n, b, t_len, c_in = xo.shape
+    rows = n * b
+    d_top = _f32c(d_top).view(rows, hid)
+    # dh_rec / dc need no initialisation: the step at t = T-1 treats them as zero (stmgcn_lstm_bwd)
+    dh_rec = xo.new_empty((n_layers, rows, hid))
+    dc = xo.new_empty((n_layers, rows, hid))
+    dx_work = xo.new_empty((rows, hid))
+    d_s = xo.new_zeros((b, t_len))
+    dwx = torch.zeros_like(wx)
+    dwp = torch.zeros_like(wpt)
+    dbp = xo.new_zeros((n_layers, 4 * hid))
+    _lib.check(L.stmgcn_lstm_bwd(t_len, n_layers, rows, hid, c_in, b, xo.data_ptr(), s_gate.data_ptr(), wx.data_ptr(),
+                                 wpt.data_ptr(), _p(h0), _p(c0), cs.data_ptr(), hs.data_ptr(), gates.data_ptr(),
+                                 d_top.data_ptr(), dh_rec.data_ptr(), dc.data_ptr(), dx_work.data_ptr(), d_s.data_ptr(),
+                                 dwx.data_ptr(), dwp.data_ptr(), dbp.data_ptr(), _stream()), "lstm_bwd")
+    return d_s, _unpack_lstm_grads(dwx, dwp, dbp, n_layers, hid, c_in)
+
+
 class SharedLSTM(torch.autograd.Function):
     """h_top (N,B,H) of the shared multi-layer LSTM over rows r = n*B + b; input ``xo * s[b,t]``.
 
@@ -549,80 +590,38 @@ class SharedLSTM(torch.autograd.Function):
         _require_cuda(xo, s_gate, *weights)
         xo, s_gate = _f32c(xo), _f32c(s_gate)
         weights = [_f32c(w) for w in weights]
-        n, b, t_len, c_in = xo.shape
-        rows = n * b
-        dev = xo.device
+        c_in, t_len = xo.shape[3], xo.shape[2]
         h0c = _f32c(h0) if h0 is not None else None
         c0c = _f32c(c0) if c0 is not None else None
         need_grad = any(ctx.needs_input_grad)
-        ctx.dims = (n, b, t_len, c_in, n_layers, hid)
-        if hid == 64 and lstm_path() == "tc" and c_in <= 4 and t_len <= 64:
+        ctx.dims = (n_layers, hid)
+        ctx.planes16 = hid == 64 and lstm_path() == "tc" and c_in <= 4 and t_len <= 64
+        if ctx.planes16:
             planes = lstm_planes()
             h_top, h_n, c_n, tape = _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes, need_grad)
-            ctx.mark_non_differentiable(h_n, c_n)
-            ctx.planes16 = True
             if need_grad:
                 ctx.tape16, ctx.planes = tape, planes
                 ctx.save_for_backward(xo, s_gate)
-            return h_top, h_n, c_n
-        ctx.planes16 = False
-        wx, wp, bp, wpt = _pack_lstm(weights, n_layers, hid)
-        hs = torch.empty((n_layers, t_len, rows, hid), device=dev, dtype=torch.float32)
-        cs = torch.empty((n_layers, t_len, rows, hid), device=dev, dtype=torch.float32)
-        gates = torch.empty((n_layers, t_len, rows, 4 * hid), device=dev, dtype=torch.float32) if need_grad else None
-        wp_arr, bp_arr = _lib.ptr_array([w.data_ptr() for w in wp]), _lib.ptr_array([v.data_ptr() for v in bp])
-        st = _stream()
-        for t in range(t_len):
-            _lib.check(L.stmgcn_lstm_step_fwd(t, t_len, n_layers, rows, hid, c_in, b, xo.data_ptr(),
-                                              s_gate.data_ptr(), wx.data_ptr(), wp_arr, bp_arr, _p(h0c), _p(c0c),
-                                              hs.data_ptr(), cs.data_ptr(), _p(gates), st), "lstm_step_fwd")
-        if need_grad:
-            ctx.save_for_backward(xo, s_gate, h0c, c0c, hs, cs, gates, wx, *wpt)
-        h_top = hs[n_layers - 1, t_len - 1].view(n, b, hid)
-        if want_state:
-            h_n, c_n = hs[:, t_len - 1], cs[:, t_len - 1]
-        else:                       # ST_MGCN discards the final state (STMGCN.py:113)
-            h_n = c_n = hs.new_empty(0)
+        else:
+            h_top, h_n, c_n, tape = _exact_forward(xo, s_gate, h0c, c0c, n_layers, hid, want_state, weights, need_grad)
+            if need_grad:
+                ctx.save_for_backward(xo, s_gate, *tape)
         ctx.mark_non_differentiable(h_n, c_n)
         return h_top, h_n, c_n
 
     @staticmethod
     def backward(ctx, d_top, _dhn, _dcn):
-        n, b, t_len, c_in, n_layers, hid = ctx.dims
+        n_layers, hid = ctx.dims
         if ctx.planes16:
             xo, s_gate = ctx.saved_tensors
             d_s, w_grads = _lstm16_backward(xo, s_gate, ctx.tape16, n_layers, ctx.planes, d_top)
-            return (None, d_s, None, None, None, None, None, *w_grads)
-        if getattr(ctx, "tape_consumed", False):
-            raise RuntimeError("SharedLSTM (exact-fp32 kernels): the gate tape was overwritten in place by the first backward "
-                               "pass; a second backward over the same graph is not supported on this path")
-        ctx.tape_consumed = True
-        xo, s_gate, h0, c0, hs, cs, gates, wx, *wpt = ctx.saved_tensors
-        rows = n * b
-        dev = xo.device
-        d_top = _f32c(d_top).view(rows, hid)
-        # dh_rec / dc need no initialisation: the step at t = T-1 treats them as zero (stmgcn_lstm_step_bwd)
-        dh_rec = torch.empty((n_layers, rows, hid), device=dev, dtype=torch.float32)
-        dc = torch.empty((n_layers, rows, hid), device=dev, dtype=torch.float32)
-        dx_work = torch.empty((rows, hid), device=dev, dtype=torch.float32)
-        d_s = torch.zeros((b, t_len), device=dev, dtype=torch.float32)
-        dwx = torch.zeros_like(wx)
-        dbp = [torch.zeros(4 * hid, device=dev, dtype=torch.float32) for _ in range(n_layers)]
-        dwp = [torch.zeros((w.shape[1], 4 * hid), device=dev, dtype=torch.float32) for w in wpt]
-        wpt_arr = _lib.ptr_array([w.data_ptr() for w in wpt])
-        dbp_arr = _lib.ptr_array([v.data_ptr() for v in dbp])
-        st = _stream()
-        # NOTE: gates is overwritten in place with dA (the tape is consumed; see the guard above)
-        for t in range(t_len - 1, -1, -1):
-            _lib.check(L.stmgcn_lstm_step_bwd(t, t_len, n_layers, rows, hid, c_in, b, xo.data_ptr(),
-                                              s_gate.data_ptr(), wx.data_ptr(), wpt_arr, _p(c0), cs.data_ptr(),
-                                              gates.data_ptr(), d_top.data_ptr(), dh_rec.data_ptr(),
-                                              dc.data_ptr(), dx_work.data_ptr(), d_s.data_ptr(), dwx.data_ptr(),
-                                              dbp_arr, st), "lstm_step_bwd")
-        for l in range(n_layers):
-            _lib.check(L.stmgcn_lstm_wgrad(l, t_len, n_layers, rows, hid, _p(h0), hs.data_ptr(), gates.data_ptr(),
-                                           dwp[l].data_ptr(), st), "lstm_wgrad")
-        w_grads = _unpack_lstm_grads(dwx, dwp, dbp, n_layers, hid, c_in)
+        else:
+            if getattr(ctx, "tape_consumed", False):
+                raise RuntimeError("SharedLSTM (exact-fp32 kernels): the gate tape was overwritten in place by the first "
+                                   "backward pass; a second backward over the same graph is not supported on this path")
+            ctx.tape_consumed = True
+            xo, s_gate, *tape = ctx.saved_tensors
+            d_s, w_grads = _exact_backward(xo, s_gate, tape, n_layers, hid, d_top)
         return (None, d_s, None, None, None, None, None, *w_grads)
 
 

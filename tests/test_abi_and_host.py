@@ -39,7 +39,7 @@ def test_library_exports_every_declared_symbol():
 
 def test_c_abi_argument_errors_come_back_as_codes_with_a_message():
     """The C entry points validate their arguments before touching CUDA: a bad call returns a negative code and
-    stmgcn_last_error() explains it (no GPU needed).  Covers the entries added in ABI 3."""
+    stmgcn_last_error() explains it (no GPU needed)."""
     import ctypes
     from stmgcn_b200 import _lib
     lib = _lib.lib
@@ -47,6 +47,9 @@ def test_c_abi_argument_errors_come_back_as_codes_with_a_message():
     # time-fused LSTM backward: null workspaces
     rc = lib.stmgcn_lstm16_layer_bwd(0, 12, 3, 128, 1, 8, 2, *([null] * 18))
     assert rc < 0 and b"lstm16_layer_bwd" in lib.stmgcn_last_error()
+    # exact-fp32 LSTM backward over the whole sequence: null workspaces
+    rc = lib.stmgcn_lstm_bwd(12, 3, 128, 64, 1, 8, *([null] * 18))
+    assert rc < 0 and b"lstm_bwd: null pointer" in lib.stmgcn_last_error()
     # bf16 gather step: null graph; conversion: count not a multiple of 8
     rc = lib.stmgcn_cheb_spmm_step16(null, 0, 1.0, null, 0.0, null, 0.0, null, null, null, 64, null)
     assert rc < 0 and b"cheb_spmm_step16" in lib.stmgcn_last_error()
@@ -132,8 +135,9 @@ def test_lambda_max_options():
     assert_close(sp_.laplacian_dense().numpy(), got[1].numpy(), "sparse with lambda_max", 1e-3)
 
 
-def test_lstm_weight_packing_roundtrip():
-    """pack (nn.LSTM layout -> gate-interleaved K-major operands) and the gradient unpack are inverse views."""
+def test_lstm_flat_weight_packing_roundtrip():
+    """pack (nn.LSTM layout -> gate-interleaved K-major operands in flat per-layer blocks) and the gradient unpack are
+    inverse views."""
     from stmgcn_b200 import ops
     hid, c_in, lyr = 8, 2, 3
     gen = torch.Generator().manual_seed(0)
@@ -143,25 +147,35 @@ def test_lstm_weight_packing_roundtrip():
         ws += [torch.randn(4 * hid, in_l, generator=gen), torch.randn(4 * hid, hid, generator=gen),
                torch.randn(4 * hid, generator=gen), torch.randn(4 * hid, generator=gen)]
     wx, wp, bp, wpt = ops._pack_lstm(ws, lyr, hid)
+    assert wp.shape == wpt.shape == (4 * hid * hid * (2 * lyr - 1),) and bp.shape == (lyr, 4 * hid)
+
+    def block(flat, l, rows, cols):          # layer l's block of a flat wp / wpt (include/stmgcn_b200.h)
+        off = 4 * hid * hid * (0 if l == 0 else 2 * l - 1)
+        return flat[off:off + rows * cols].view(rows, cols)
+
+    wp_l = [block(wp, l, hid if l == 0 else 2 * hid, 4 * hid) for l in range(lyr)]
     # column 4*unit+gate of the packed operand is row gate*hid+unit of the nn.LSTM matrix
     for unit in (0, 3, 7):
         for gate in range(4):
             assert torch.equal(wx[:, 4 * unit + gate], ws[0][gate * hid + unit, :])
-            assert torch.equal(wp[0][:, 4 * unit + gate], ws[1][gate * hid + unit, :])
-            assert torch.equal(wp[1][:hid, 4 * unit + gate], ws[4][gate * hid + unit, :])
-            assert torch.equal(wp[1][hid:, 4 * unit + gate], ws[5][gate * hid + unit, :])
+            assert torch.equal(wp_l[0][:, 4 * unit + gate], ws[1][gate * hid + unit, :])
+            for l in (1, 2):
+                assert torch.equal(wp_l[l][:hid, 4 * unit + gate], ws[4 * l][gate * hid + unit, :])
+                assert torch.equal(wp_l[l][hid:, 4 * unit + gate], ws[4 * l + 1][gate * hid + unit, :])
             assert float(bp[2][4 * unit + gate]) == pytest.approx(float(ws[10][gate * hid + unit] + ws[11][gate * hid + unit]))
-    assert torch.equal(wpt[1], wp[1].t())
-    grads = ops._unpack_lstm_grads(wx, wp, [b.clone() for b in bp], lyr, hid, c_in)
+    for l in range(lyr):
+        assert torch.equal(block(wpt, l, 4 * hid, wp_l[l].shape[0]), wp_l[l].t())
+    grads = ops._unpack_lstm_grads(wx, wp, bp.clone(), lyr, hid, c_in)
     assert torch.equal(grads[0], ws[0]) and torch.equal(grads[1], ws[1])
     assert torch.equal(grads[4], ws[4]) and torch.equal(grads[5], ws[5])
+    assert torch.equal(grads[8], ws[8]) and torch.equal(grads[9], ws[9])
     assert torch.allclose(grads[2], ws[2] + ws[3])
 
 
 @pytest.mark.parametrize("rows", [128, 300, 1])
 def test_tile_blocked_layout_roundtrip_and_formula(rows):
     """to_blocked / from_blocked are inverse, pad to whole 128-row tiles, and place element (r, u) where the kernels'
-    ws_off() expects it: (((r/128)*16 + u/4)*128 + r%128)*4 + u%4  (include/stmgcn_b200.h, stmgcn_lstm16_step_fwd)."""
+    ws_off() expects it: (((r/128)*16 + u/4)*128 + r%128)*4 + u%4  (include/stmgcn_b200.h, stmgcn_lstm16_layer_fwd)."""
     from stmgcn_b200 import ops
     gen = torch.Generator().manual_seed(rows)
     x = torch.randn(2, rows, 64, generator=gen)

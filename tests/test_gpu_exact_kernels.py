@@ -213,6 +213,22 @@ def test_exact_lstm_second_backward_raises(monkeypatch):
         loss.backward()
 
 
+@pytest.mark.parametrize("lyr,t", [(3, 7), (1, 1)])
+def test_exact_lstm_launch_sequence(lyr, t, monkeypatch):
+    """The exact path's forward is one tall GEMM per (timestep, layer); its backward one pointwise kernel and one data
+    GEMM per (timestep, layer), then one weight-gradient reduce GEMM per layer."""
+    from stmgcn_b200 import _lib, ops
+    monkeypatch.setattr(ops, "_LSTM_PATH", "fma")
+    xo, s, _, _, ws, d_top = lstm_inputs(3, 4, t, lyr, 2, 36, False, seed=2)
+    ws_g = [w.to(DEV).requires_grad_(True) for w in ws]
+    n0 = _lib.launch_count()
+    h_top, _, _ = ops.SharedLSTM.apply(xo.to(DEV), s.to(DEV), None, None, lyr, 36, False, *ws_g)
+    n1 = _lib.launch_count()
+    (h_top.reshape(12, 36) * d_top.to(DEV)).sum().backward()
+    n2 = _lib.launch_count()
+    assert (n1 - n0, n2 - n1) == (lyr * t, 2 * lyr * t + lyr)
+
+
 # ======================================================================================================================
 # B. exact-fp32 projection and temporal pooling
 # ======================================================================================================================
