@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define STMGCN_ABI_VERSION 5
+#define STMGCN_ABI_VERSION 6
 
 /* error codes < 0 */
 #define STMGCN_ERR_ARG      (-1)   /* null pointer / bad enum */
@@ -159,46 +159,44 @@ int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
  *        P = 1: hi only, single-pass bf16 products (the arithmetic of the bf16-quoted BASELINE configs).
  *   cs : (L, T, ceil(R/128)*128, 64) fp32, tile-blocked (element (r,u) at (((r/128)*16 + u/4)*128 + r%128)*4 + u%4).
  * No gate tape: the backward recomputes the gates from hp (which it needs anyway for the weight gradients).
- * stmgcn_lstm16_pack turns one layer's nn.LSTM parameters (native layout: w_ih (256, in), w_hh (256, 64), b_ih, b_hh
- * (256), gate order i,f,g,o) into the resident operand image wimg (layer 0: 64 KB, layers > 0: 128 KB; tiles
- * [(segment, plane)] of [256 gate-interleaved columns][64 k] bf16, 128-byte swizzled), bias (256) = b_ih + b_hh
- * gate-interleaved (col = 4*unit + gate) and, for layer 0, wih_t (C, 256) = W_ih^T gate-interleaved. */
+ * Weights are passed as flat operand images:
+ *   wimg : layer l's resident image (tiles [(segment, plane)] of [256 gate-interleaved columns][64 k] bf16, 128-byte
+ *          swizzled; layer 0: 64 KB, layers > 0: 128 KB), back to back, so layer l starts 65536*(l == 0 ? 0 : 2l - 1)
+ *          bytes in;
+ *   bias : (L, 256) = b_ih_l + b_hh_l gate-interleaved (col = 4*unit + gate);
+ *   wih_t: (C, 256) = W_ih_l0^T gate-interleaved.
+ * h0p: (L, P, R, 64) bf16 planes of the initial hidden state and c0: (L, R_pad, 64) fp32 tile-blocked, or both NULL
+ * (zeros, STMGCN.py:53-57).  C <= 4, L <= 8.
+ * stmgcn_lstm16_pack turns layer `layer`'s nn.LSTM parameters (native layout: w_ih (256, in), w_hh (256, 64), b_ih,
+ * b_hh (256), gate order i,f,g,o) into that layer's slot of wimg and bias and, for layer 0, into wih_t. */
 int32_t stmgcn_lstm16_pack(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, int32_t layer,
                            int32_t c_in, void* wimg, float* bias, float* wih_t, void* stream);
-/* Forward of ONE layer through all timesteps 0 .. T-1 (call the layers bottom-up: layer l reads the hp planes of layer
- * l - 1).  A tile's rows never mix with other tiles', so each CTA walks its own tiles through time inside the layer's one
- * launch, keeping h_{t-1} in shared memory.  h0p: (L, P, R, 64) bf16 planes of the initial hidden state and c0:
- * (L, R_pad, 64) fp32 tile-blocked, or both NULL (zeros, STMGCN.py:53-57).  At t = T-1 the fp32 hidden state is also
- * written: into h_n[layer] (h_n: (L, R, 64)) when h_n != NULL, else for the top layer into h_top (R, 64) -- the (N,B,H)
- * operand of the spatial GCN (STMGCN.py:50, :114).  wimg / bias: this layer's operands from stmgcn_lstm16_pack.  C <= 4. */
-int32_t stmgcn_lstm16_layer_fwd(int32_t layer, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in,
-                                int64_t b_inner, int32_t planes, const float* xo, const float* s_gate,
-                                const void* wimg, const float* bias, const float* wih_t, const void* h0p,
-                                const float* c0, void* hp, float* cs, float* h_top, float* h_n, void* stream);
+/* Forward through all layers and timesteps: one launch per layer, bottom-up (layer l reads the hp planes of layer
+ * l - 1).  A tile's rows never mix with other tiles', so each CTA walks its own tiles through time inside a layer's
+ * launch, keeping h_{t-1} in shared memory.  At t = T-1 the fp32 hidden state is also written: into h_n (L, R, 64) when
+ * h_n != NULL, else for the top layer into h_top (R, 64) -- the (N,B,H) operand of the spatial GCN (STMGCN.py:50, :114). */
+int32_t stmgcn_lstm16_fwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner, int32_t planes,
+                          const float* xo, const float* s_gate, const void* wimg, const float* bias, const float* wih_t,
+                          const void* h0p, const float* c0, void* hp, float* cs, float* h_top, float* h_n,
+                          void* stream);
 
-/* grid (CTAs) the lstm16 kernels use for `rows` rows: the number of weight-gradient scratch slices per layer */
+/* grid (CTAs) the lstm16 kernels use for `rows` rows: the number of weight-gradient scratch slices */
 int32_t stmgcn_lstm16_grid(int64_t rows);
-/* BPTT of ONE layer through all timesteps T-1 .. 0 (call the layers top-down): recomputes the gates from hp, forms dA,
- * accumulates the weight and bias gradients and propagates [dx_below | dh_prev].  A tile's rows never mix with other
- * tiles', so each CTA walks its own tiles through time inside the layer's one launch.  T <= 64.
+/* BPTT through all layers and timesteps, T <= 64.  Per layer, top-down: one launch over T-1 .. 0 that recomputes the
+ * gates from hp, forms dA, accumulates the weight and bias gradients and propagates [dx_below | dh_prev]; then one
+ * launch that sums the layer's weight-gradient slices.  d_top: (R_pad, 64) tile-blocked gradient of the top layer's
+ * last hidden state.
  * Workspaces (tile-blocked, R_pad = ceil(R/128)*128 rows; none needs initialisation):
- *   dh_in : top layer: d_top (R_pad,64), the gradient of the top layer's last hidden state; other layers: the dx_out
- *           (T,R_pad,64) the layer above wrote;      dx_out: (T,R_pad,64), NULL for layer 0;
- *   dh_rec, dc: (R_pad,64) scratch of this layer;    dw_scratch: (stmgcn_lstm16_grid(rows), 128*256) floats;
+ *   dh_rec, dc: (R_pad, 64);   dx_work: (min(2, L-1), T, R_pad, 64), the dx one layer hands to the layer below (may be
+ *   NULL when L = 1);   dw_scratch: (stmgcn_lstm16_grid(rows), 128*256);   dbp: (L, 256);
  *   zero_tile: 16 KB of zeros (the h_prev operand at t = 0 without an initial state).
- * wimg / bias: this layer's operands from stmgcn_lstm16_pack.  Accumulates (+=; caller zeroes): d_s (B,T), dbp (256,
- * gate-interleaved). */
-int32_t stmgcn_lstm16_layer_bwd(int32_t layer, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in,
-                                int64_t b_inner, int32_t planes, const float* xo, const float* s_gate,
-                                const void* wimg, const float* bias, const float* wih_t, const void* h0p,
-                                const float* c0, const void* hp, const float* cs, const float* dh_in,
-                                float* dx_out, float* dh_rec, float* dc, float* d_s, float* dbp,
-                                float* dw_scratch, const void* zero_tile, void* stream);
-/* After stmgcn_lstm16_layer_bwd of layer `layer`: sum its scratch slices into nn.LSTM-native gradients
- * d_w_ih (256, in), d_w_hh (256, 64), d_b_ih = d_b_hh (256) (overwritten, not accumulated). */
-int32_t stmgcn_lstm16_wgrad_reduce(int32_t layer, int32_t c_in, int32_t n_slices, const float* slices,
-                                   const float* dbp, float* d_w_ih, float* d_w_hh, float* d_b_ih, float* d_b_hh,
-                                   void* stream);
+ * Accumulates (+=; caller zeroes) d_s (B,T) = sum_{n,c} dxmod * xo (gate adjoint, STMGCN.py:44).  Overwrites grads: one
+ * flat buffer in nn.LSTM parameter order, per layer d_w_ih (256, in_l) | d_w_hh (256, 64) | d_b_ih (256) | d_b_hh (256). */
+int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner, int32_t planes,
+                          const float* xo, const float* s_gate, const void* wimg, const float* bias, const float* wih_t,
+                          const void* h0p, const float* c0, const void* hp, const float* cs, const float* d_top,
+                          float* dh_rec, float* dc, float* dx_work, float* dw_scratch, float* dbp, const void* zero_tile,
+                          float* d_s, float* grads, void* stream);
 
 /* ---- fusion over graphs + output FC (STMGCN.py:116-118) ------------------------------------------
  * feat = sum_m g[m] (each (R, G) node-major); y[b, n, c] = feat[n*B+b, :] . fcw[c, :] + fcb[c]. */

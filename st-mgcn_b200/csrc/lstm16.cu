@@ -24,10 +24,6 @@
 using namespace stmgcn;
 using namespace stmgcn::tc;
 
-namespace stmgcn {
-bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t slices, int box_rows);
-}
-
 namespace {
 
 constexpr int kTileM = 128;
@@ -408,8 +404,8 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
 //         tiles already in shared memory), added into this CTA's own slice of a scratch buffer with vector reductions
 //   D_c : data gradient    [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T  (B: MN-major view of the resident weights;
 //         accumulated in registers over the four chunks, stored at the end of the item)
-// dA never leaves the SM; the gates are never stored.  stmgcn_lstm16_wgrad_reduce sums the slices once per layer and
-// writes nn.LSTM-native gradients.
+// dA never leaves the SM; the gates are never stored.  lstm16_wgrad_reduce_kernel sums the slices after each layer's
+// launch and writes nn.LSTM-native gradients.
 constexpr int kBWarpgroups = 2;
 constexpr int kBThreads = kBWarpgroups * 128 + 32;      // + producer warp
 constexpr int kBATiles = 4;                             // (seg0 | seg1) x (hi | lo); layer 0: seg 1 = the auxiliary [x*s] tile
@@ -831,7 +827,7 @@ static EncodeTiledFn16 encode_fn16() {
 }
 // (slices, rows, 64) bf16 plane tensor, box = 1 x box_rows x 64, 128-byte swizzle (rows past the end read as zeros;
 // stores drop them)
-bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t slices, int box_rows) {
+static bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t slices, int box_rows) {
     EncodeTiledFn16 fn = encode_fn16();
     if (fn == nullptr) return false;
     const cuuint64_t dims[3] = {(cuuint64_t)kHid, (cuuint64_t)rows, (cuuint64_t)slices};
@@ -842,47 +838,41 @@ bool make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t sl
               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-
-// The K segments of layer l at step t, in the order of the weight image's segments, and the cell state the step continues:
-// layers > 0 first read h of the layer below at step t; then h_prev: hp at t - 1, at t = 0 the initial state h0p if
-// there is one, else nothing (zeros, STMGCN.py:53-57).
-enum SegSrc { kSegHp = 0, kSegH0p = 1, kSegAbsent = 2 };     // = Bwd16Step::src
-struct StepSegs {
-    int nseg;                  // layers > 0: 2 (h_below, h_prev); layer 0: 1 (h_prev)
-    int src[2];                // SegSrc
-    int slice[2];              // the segment's hi-plane slice in its tensor (lo = + 1); 0 when absent
-    const float* c_prev;       // blocked or nullptr (zeros)
-};
-static StepSegs step_segs(int l, int t, int t_len, int planes, bool has_h0, const float* cs, const float* c0,
-                          int64_t cslice) {
-    StepSegs g{};
-    if (l > 0) {
-        g.src[g.nseg] = kSegHp;
-        g.slice[g.nseg] = ((l - 1) * t_len + t) * planes;
-        ++g.nseg;
-    }
-    if (t > 0) {
-        g.src[g.nseg] = kSegHp;
-        g.slice[g.nseg] = (l * t_len + t - 1) * planes;
-    } else if (has_h0) {
-        g.src[g.nseg] = kSegH0p;
-        g.slice[g.nseg] = l * planes;
-    } else {
-        g.src[g.nseg] = kSegAbsent;
-    }
-    ++g.nseg;
-    g.c_prev = t > 0 ? cs + (int64_t)(l * t_len + t - 1) * cslice : (c0 ? c0 + (int64_t)l * cslice : nullptr);
-    return g;
+// the maps of hp (L, T, P, R, 64) and, if given, h0p (L, P, R, 64)
+static int32_t make_plane_maps(const char* who, CUtensorMap* hp_map, CUtensorMap* h0_map, const void* hp, const void* h0p,
+                               int64_t rows, int n_layers, int t_len, int planes, int box_rows) {
+    STMGCN_REQUIRE(make_plane_map(hp_map, hp, rows, (int64_t)n_layers * t_len * planes, box_rows), STMGCN_ERR_STATE,
+                   "%s: cuTensorMapEncodeTiled failed (hp)", who);
+    if (h0p != nullptr)
+        STMGCN_REQUIRE(make_plane_map(h0_map, h0p, rows, (int64_t)n_layers * planes, box_rows), STMGCN_ERR_STATE,
+                       "%s: cuTensorMapEncodeTiled failed (h0p)", who);
+    return 0;
 }
 
-// kernel variant for (planes, cin): cin = 0 (not layer 0), 1 (layer 0, one input channel), kMaxC (layer 0, runtime count)
+static int32_t check_dims16(const char* who, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner,
+                            int32_t planes, const float* wih_t, const void* h0p, const float* c0) {
+    STMGCN_REQUIRE(planes == 1 || planes == 2, STMGCN_ERR_ARG, "%s: planes=%d", who, planes);
+    STMGCN_REQUIRE(n_layers >= 1 && n_layers <= 8 && t_len >= 1 && rows > 0 && c_in >= 1 && c_in <= kMaxC && b_inner > 0,
+                   STMGCN_ERR_SHAPE, "%s: L=%d T=%d rows=%lld C=%d", who, n_layers, t_len, (long long)rows, c_in);
+    STMGCN_REQUIRE(rows <= (1LL << 25), STMGCN_ERR_SHAPE, "%s: rows=%lld too large (32-bit element offsets)", who, (long long)rows);
+    STMGCN_REQUIRE((h0p == nullptr) == (c0 == nullptr), STMGCN_ERR_ARG, "%s: h0p and c0 go together", who);
+    STMGCN_REQUIRE(wih_t != nullptr, STMGCN_ERR_ARG, "%s: wih_t null", who);
+    return 0;
+}
+
+// start of layer l's image in the flat wimg: layer 0 has one K segment (64 KB), every other layer two (128 KB)
+static int64_t wimg_off(int l) { return (int64_t)2 * kWTileBytes * (l == 0 ? 0 : 2 * l - 1); }
+
+// kernel variant for (planes, layer): cin = 0 (not layer 0), 1 (layer 0, one input channel), kMaxC (layer 0, runtime count)
 using FwdFn = void (*)(const Fwd16Params);
 using BwdFn = void (*)(const Bwd16Params);
-static FwdFn fwd_kernel_for(int planes, int cin) {
+static FwdFn fwd_kernel_for(int planes, int l, int c_in) {
+    const int cin = l == 0 ? (c_in == 1 ? 1 : kMaxC) : 0;
     if (planes == 2) return cin == 0 ? lstm16_fwd_kernel<2, 0> : (cin == 1 ? lstm16_fwd_kernel<2, 1> : lstm16_fwd_kernel<2, kMaxC>);
     return cin == 0 ? lstm16_fwd_kernel<1, 0> : (cin == 1 ? lstm16_fwd_kernel<1, 1> : lstm16_fwd_kernel<1, kMaxC>);
 }
-static BwdFn bwd_kernel_for(int planes, int cin) {
+static BwdFn bwd_kernel_for(int planes, int l, int c_in) {
+    const int cin = l == 0 ? (c_in == 1 ? 1 : kMaxC) : 0;
     if (planes == 2) return cin == 0 ? lstm16_bwd_kernel<2, 0> : (cin == 1 ? lstm16_bwd_kernel<2, 1> : lstm16_bwd_kernel<2, kMaxC>);
     return cin == 0 ? lstm16_bwd_kernel<1, 0> : (cin == 1 ? lstm16_bwd_kernel<1, 1> : lstm16_bwd_kernel<1, kMaxC>);
 }
@@ -894,59 +884,51 @@ extern "C" int32_t stmgcn_lstm16_pack(const float* w_ih, const float* w_hh, cons
     STMGCN_REQUIRE(w_ih && w_hh && b_ih && b_hh && wimg && bias, STMGCN_ERR_ARG, "lstm16_pack: null pointer");
     STMGCN_REQUIRE(layer >= 0 && c_in >= 1 && c_in <= kMaxC, STMGCN_ERR_SHAPE, "lstm16_pack: layer=%d c_in=%d", layer, c_in);
     STMGCN_REQUIRE(layer > 0 || wih_t != nullptr, STMGCN_ERR_ARG, "lstm16_pack: layer 0 needs wih_t");
-    lstm16_pack_kernel<<<64, 256, 0, (cudaStream_t)stream>>>(w_ih, w_hh, b_ih, b_hh, layer, c_in, (uint8_t*)wimg, bias, wih_t);
+    lstm16_pack_kernel<<<64, 256, 0, (cudaStream_t)stream>>>(w_ih, w_hh, b_ih, b_hh, layer, c_in, (uint8_t*)wimg + wimg_off(layer),
+                                                              bias + (int64_t)layer * kGateCols, wih_t);
     count_launch();
     return check_launch("lstm16_pack");
 }
 
-extern "C" int32_t stmgcn_lstm16_layer_fwd(int32_t layer, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in,
-                                           int64_t b_inner, int32_t planes, const float* xo, const float* s_gate,
-                                           const void* wimg, const float* bias, const float* wih_t, const void* h0p,
-                                           const float* c0, void* hp, float* cs, float* h_top, float* h_n, void* stream) {
-    STMGCN_REQUIRE(xo && s_gate && wimg && bias && hp && cs, STMGCN_ERR_ARG, "lstm16_layer_fwd: null pointer");
-    STMGCN_REQUIRE(planes == 1 || planes == 2, STMGCN_ERR_ARG, "lstm16_layer_fwd: planes=%d", planes);
-    STMGCN_REQUIRE(layer >= 0 && layer < n_layers && n_layers <= 8 && t_len >= 1 && rows > 0 && c_in >= 1 && c_in <= kMaxC &&
-                       b_inner > 0,
-                   STMGCN_ERR_SHAPE, "lstm16_layer_fwd: layer=%d L=%d T=%d rows=%lld C=%d", layer, n_layers, t_len,
-                   (long long)rows, c_in);
-    STMGCN_REQUIRE(rows <= (1LL << 25), STMGCN_ERR_SHAPE, "lstm16_layer_fwd: rows=%lld too large (32-bit element offsets)", (long long)rows);
-    STMGCN_REQUIRE((h0p == nullptr) == (c0 == nullptr), STMGCN_ERR_ARG, "lstm16_layer_fwd: h0p and c0 go together");
-    STMGCN_REQUIRE(layer > 0 || wih_t != nullptr, STMGCN_ERR_ARG, "lstm16_layer_fwd: wih_t null");
-    STMGCN_REQUIRE(layer < n_layers - 1 || h_n != nullptr || h_top != nullptr, STMGCN_ERR_ARG, "lstm16_layer_fwd: h_top null");
+extern "C" int32_t stmgcn_lstm16_fwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner,
+                                     int32_t planes, const float* xo, const float* s_gate, const void* wimg,
+                                     const float* bias, const float* wih_t, const void* h0p, const float* c0, void* hp,
+                                     float* cs, float* h_top, float* h_n, void* stream) {
+    STMGCN_REQUIRE(xo && s_gate && wimg && bias && hp && cs, STMGCN_ERR_ARG, "lstm16_fwd: null pointer");
+    if (int32_t rc = check_dims16("lstm16_fwd", t_len, n_layers, rows, c_in, b_inner, planes, wih_t, h0p, c0)) return rc;
+    STMGCN_REQUIRE(h_n != nullptr || h_top != nullptr, STMGCN_ERR_ARG, "lstm16_fwd: h_top null");
     cudaStream_t st = (cudaStream_t)stream;
     const int n_tiles = (int)ceil_div(rows, kTileM);
     const int64_t cslice = (int64_t)n_tiles * kTileM * kHid;
-    const int l = layer;
-    const FwdFn fn = fwd_kernel_for(planes, l == 0 ? (c_in == 1 ? 1 : kMaxC) : 0);
-    if (int32_t rc = ensure_dyn_smem((const void*)fn, kFSmem)) return rc;
+    const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
     Fwd16Params p;
     memset(&p, 0, sizeof(p));
     // a warpgroup's 64 rows are one box: its h_below loads, h0 loads and tape stores
-    STMGCN_REQUIRE(make_plane_map(&p.hp_map, hp, rows, (int64_t)n_layers * t_len * planes, 64), STMGCN_ERR_STATE,
-                   "lstm16_layer_fwd: cuTensorMapEncodeTiled failed (hp)");
-    if (h0p != nullptr)
-        STMGCN_REQUIRE(make_plane_map(&p.h0_map, h0p, rows, (int64_t)n_layers * planes, 64), STMGCN_ERR_STATE,
-                       "lstm16_layer_fwd: cuTensorMapEncodeTiled failed (h0p)");
-    const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
-    p.wimg = (const uint8_t*)wimg;
-    p.bias = bias;
-    p.wih = (l == 0) ? wih_t : nullptr;
+    if (int32_t rc = make_plane_maps("lstm16_fwd", &p.hp_map, &p.h0_map, hp, h0p, rows, n_layers, t_len, planes, 64)) return rc;
     p.xo = xo;
     p.sg = s_gate;
-    p.layer = l;
     p.c_in = c_in;
     p.t_len = t_len;
     p.has_h0 = h0p != nullptr ? 1 : 0;
     p.b_inner = b_inner;
-    p.c0 = c0 != nullptr ? c0 + (int64_t)l * cslice : nullptr;
-    p.cs = cs + (int64_t)l * t_len * cslice;
-    if (h_n != nullptr) p.h_f32 = h_n + (int64_t)l * rows * kHid;
-    else if (l == n_layers - 1) p.h_f32 = h_top;
     p.rows = rows;
     p.n_tiles = n_tiles;
-    fn<<<grid, kFThreads, kFSmem, st>>>(p);
-    count_launch();
-    return check_launch("lstm16_layer_fwd");
+    // bottom-up: layer l reads the hp planes of layer l - 1
+    for (int l = 0; l < n_layers; ++l) {
+        const FwdFn fn = fwd_kernel_for(planes, l, c_in);
+        if (int32_t rc = ensure_dyn_smem((const void*)fn, kFSmem)) return rc;
+        p.wimg = (const uint8_t*)wimg + wimg_off(l);
+        p.bias = bias + (int64_t)l * kGateCols;
+        p.wih = l == 0 ? wih_t : nullptr;
+        p.layer = l;
+        p.c0 = c0 != nullptr ? c0 + (int64_t)l * cslice : nullptr;
+        p.cs = cs + (int64_t)l * t_len * cslice;
+        p.h_f32 = h_n != nullptr ? h_n + (int64_t)l * rows * kHid : (l == n_layers - 1 ? h_top : nullptr);
+        fn<<<grid, kFThreads, kFSmem, st>>>(p);
+        count_launch();
+        if (int32_t rc = check_launch("lstm16_fwd")) return rc;
+    }
+    return 0;
 }
 
 extern "C" int32_t stmgcn_lstm16_grid(int64_t rows) {
@@ -954,42 +936,27 @@ extern "C" int32_t stmgcn_lstm16_grid(int64_t rows) {
     return (int32_t)(n_tiles < sm_count() ? n_tiles : sm_count());
 }
 
-extern "C" int32_t stmgcn_lstm16_layer_bwd(int32_t layer, int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in,
-                                           int64_t b_inner, int32_t planes, const float* xo, const float* s_gate,
-                                           const void* wimg, const float* bias, const float* wih_t, const void* h0p,
-                                           const float* c0, const void* hp, const float* cs, const float* dh_in,
-                                           float* dx_out, float* dh_rec, float* dc, float* d_s, float* dbp,
-                                           float* dw_scratch, const void* zero_tile, void* stream) {
-    STMGCN_REQUIRE(xo && s_gate && wimg && bias && hp && cs && dh_in && dh_rec && dc && d_s && dbp && dw_scratch && zero_tile,
-                   STMGCN_ERR_ARG, "lstm16_layer_bwd: null pointer");
-    STMGCN_REQUIRE(planes == 1 || planes == 2, STMGCN_ERR_ARG, "lstm16_layer_bwd: planes=%d", planes);
-    STMGCN_REQUIRE(layer >= 0 && layer < n_layers && n_layers <= 8 && t_len >= 1 && t_len <= kBMaxSteps && rows > 0 && c_in >= 1 &&
-                       c_in <= kMaxC && b_inner > 0,
-                   STMGCN_ERR_SHAPE, "lstm16_layer_bwd: layer=%d L=%d T=%d (max %d) rows=%lld C=%d", layer, n_layers, t_len,
-                   kBMaxSteps, (long long)rows, c_in);
-    STMGCN_REQUIRE(rows <= (1LL << 25), STMGCN_ERR_SHAPE, "lstm16_layer_bwd: rows=%lld too large (32-bit element offsets)", (long long)rows);
-    STMGCN_REQUIRE((h0p == nullptr) == (c0 == nullptr), STMGCN_ERR_ARG, "lstm16_layer_bwd: h0p and c0 go together");
-    STMGCN_REQUIRE((layer == 0) == (dx_out == nullptr), STMGCN_ERR_ARG, "lstm16_layer_bwd: dx_out is for layers > 0 only");
-    STMGCN_REQUIRE(layer > 0 || wih_t != nullptr, STMGCN_ERR_ARG, "lstm16_layer_bwd: wih_t null");
+extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner,
+                                     int32_t planes, const float* xo, const float* s_gate, const void* wimg,
+                                     const float* bias, const float* wih_t, const void* h0p, const float* c0,
+                                     const void* hp, const float* cs, const float* d_top, float* dh_rec, float* dc,
+                                     float* dx_work, float* dw_scratch, float* dbp, const void* zero_tile, float* d_s,
+                                     float* grads, void* stream) {
+    STMGCN_REQUIRE(xo && s_gate && wimg && bias && hp && cs && d_top && dh_rec && dc && dw_scratch && dbp && zero_tile && d_s &&
+                       grads,
+                   STMGCN_ERR_ARG, "lstm16_bwd: null pointer");
+    if (int32_t rc = check_dims16("lstm16_bwd", t_len, n_layers, rows, c_in, b_inner, planes, wih_t, h0p, c0)) return rc;
+    STMGCN_REQUIRE(t_len <= kBMaxSteps, STMGCN_ERR_SHAPE, "lstm16_bwd: T=%d (max %d)", t_len, kBMaxSteps);
+    STMGCN_REQUIRE(n_layers == 1 || dx_work != nullptr, STMGCN_ERR_ARG, "lstm16_bwd: dx_work null with L=%d", n_layers);
     cudaStream_t st = (cudaStream_t)stream;
     const int n_tiles = (int)ceil_div(rows, kTileM);
     const int64_t cslice = (int64_t)n_tiles * kTileM * kHid;
-    const int l = layer;
-    const BwdFn fn = bwd_kernel_for(planes, l == 0 ? (c_in == 1 ? 1 : kMaxC) : 0);
-    if (int32_t rc = ensure_dyn_smem((const void*)fn, kBSmem)) return rc;
+    const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
     Bwd16Params p;
     memset(&p, 0, sizeof(p));
-    STMGCN_REQUIRE(make_plane_map(&p.maps[0], hp, rows, (int64_t)n_layers * t_len * planes, kTileM), STMGCN_ERR_STATE,
-                   "lstm16_layer_bwd: cuTensorMapEncodeTiled failed (hp)");
-    if (h0p != nullptr)
-        STMGCN_REQUIRE(make_plane_map(&p.maps[1], h0p, rows, (int64_t)n_layers * planes, kTileM), STMGCN_ERR_STATE,
-                       "lstm16_layer_bwd: cuTensorMapEncodeTiled failed (h0p)");
-    const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
-    const bool top = (l == n_layers - 1);
+    if (int32_t rc = make_plane_maps("lstm16_bwd", &p.maps[0], &p.maps[1], hp, h0p, rows, n_layers, t_len, planes, kTileM))
+        return rc;
     p.zero_tile = (const uint8_t*)zero_tile;
-    p.wimg = (const uint8_t*)wimg;
-    p.bias = bias;
-    p.wih = (l == 0) ? wih_t : nullptr;
     p.xo = xo;
     p.sg = s_gate;
     p.d_s = d_s;
@@ -998,42 +965,61 @@ extern "C" int32_t stmgcn_lstm16_layer_bwd(int32_t layer, int32_t t_len, int32_t
     p.b_inner = b_inner;
     p.dh_rec = dh_rec;
     p.dc = dc;
-    p.dbp = dbp;
     p.dw_slice = dw_scratch;
     p.rows = rows;
-    // every CTA adds into its own slice: start from zero
-    STMGCN_CUDA(cudaMemsetAsync(dw_scratch, 0, (size_t)grid * kTileM * kGateCols * sizeof(float), st));
     p.n_tiles = n_tiles;
-    // one launch covers all timesteps of the layer (t_len <= kBMaxSteps); the weight-gradient partials of every chunk are
+    // one launch covers all timesteps of a layer (t_len <= kBMaxSteps); the weight-gradient partials of every chunk are
     // added into fp32 memory, so the length of the run does not lengthen any tensor-core accumulation chain
     p.n_steps = t_len;
-    for (int si = 0; si < t_len; ++si) {
-        const int t = t_len - 1 - si;
-        Bwd16Step& sp = p.steps[si];
-        const StepSegs g = step_segs(l, t, t_len, planes, h0p != nullptr, cs, c0, cslice);
-        for (int s = 0; s < g.nseg; ++s) {                         // an absent h_prev segment reads the zero tile
-            sp.src[s] = (int8_t)g.src[s];
-            sp.slice[s] = g.slice[s];
+    STMGCN_CUDA(cudaMemsetAsync(dbp, 0, (size_t)n_layers * kGateCols * sizeof(float), st));
+    // top-down: layer l reads the dx that layer l + 1 wrote into one half of dx_work and writes its own into the other
+    const float* dh_in = d_top;
+    for (int l = n_layers - 1; l >= 0; --l) {
+        const BwdFn fn = bwd_kernel_for(planes, l, c_in);
+        if (int32_t rc = ensure_dyn_smem((const void*)fn, kBSmem)) return rc;
+        float* dx_out = l > 0 ? dx_work + (int64_t)((n_layers - 1 - l) % 2) * t_len * cslice : nullptr;
+        p.wimg = (const uint8_t*)wimg + wimg_off(l);
+        p.bias = bias + (int64_t)l * kGateCols;
+        p.wih = l == 0 ? wih_t : nullptr;
+        p.dbp = dbp + (int64_t)l * kGateCols;
+        for (int si = 0; si < t_len; ++si) {
+            const int t = t_len - 1 - si;
+            Bwd16Step& sp = p.steps[si];
+            sp = Bwd16Step{};
+            // the K segments in the order of the weight image's: layers > 0 first read h of the layer below at step t;
+            // then h_prev: hp at t - 1, at t = 0 the initial state h0p if there is one, else the zero tile (STMGCN.py:53-57)
+            const int s = l > 0 ? 1 : 0;
+            if (l > 0) sp.slice[0] = ((l - 1) * t_len + t) * planes;
+            if (t > 0) {
+                sp.slice[s] = (l * t_len + t - 1) * planes;
+            } else if (h0p != nullptr) {
+                sp.src[s] = 1;
+                sp.slice[s] = l * planes;
+            } else {
+                sp.src[s] = 2;
+            }
+            sp.t = t;
+            sp.first = (t == t_len - 1) ? 1 : 0;
+            sp.store_dh = (t > 0 || h0p != nullptr) ? 1 : 0;
+            sp.c_prev = t > 0 ? cs + (int64_t)(l * t_len + t - 1) * cslice : (c0 ? c0 + (int64_t)l * cslice : nullptr);
+            sp.dh_in = l == n_layers - 1 ? (t == t_len - 1 ? d_top : nullptr) : dh_in + (int64_t)t * cslice;
+            sp.dx_out = l > 0 ? dx_out + (int64_t)t * cslice : nullptr;
         }
-        sp.t = t;
-        sp.first = (t == t_len - 1) ? 1 : 0;
-        sp.store_dh = (t > 0 || h0p != nullptr) ? 1 : 0;
-        sp.c_prev = g.c_prev;
-        sp.dh_in = top ? (t == t_len - 1 ? dh_in : nullptr) : dh_in + (int64_t)t * cslice;
-        sp.dx_out = l > 0 ? dx_out + (int64_t)t * cslice : nullptr;
+        // every CTA adds into its own slice: start from zero
+        STMGCN_CUDA(cudaMemsetAsync(dw_scratch, 0, (size_t)grid * kTileM * kGateCols * sizeof(float), st));
+        fn<<<grid, kBThreads, kBSmem, st>>>(p);
+        count_launch();
+        if (int32_t rc = check_launch("lstm16_bwd")) return rc;
+        // the slices -> this layer's d_w_ih (256, in_l) | d_w_hh (256, 64) | d_b_ih | d_b_hh, before the next layer
+        // reuses dw_scratch
+        const int in_l = l == 0 ? c_in : kHid;
+        float* g = grads + (l == 0 ? 0 : (int64_t)kGateCols * (c_in + kHid + 2 + (l - 1) * (2 * kHid + 2)));
+        lstm16_wgrad_reduce_kernel<<<(kTileM * kGateCols) / 256, 256, 0, st>>>(dw_scratch, grid, l, c_in, p.dbp, g, g + kGateCols * in_l,
+                                                                               g + kGateCols * (in_l + kHid),
+                                                                               g + kGateCols * (in_l + kHid + 1));
+        count_launch();
+        if (int32_t rc = check_launch("lstm16_wgrad_reduce")) return rc;
+        dh_in = dx_out;
     }
-    fn<<<grid, kBThreads, kBSmem, st>>>(p);
-    count_launch();
-    return check_launch("lstm16_layer_bwd");
-}
-
-extern "C" int32_t stmgcn_lstm16_wgrad_reduce(int32_t layer, int32_t c_in, int32_t n_slices, const float* slices,
-                                              const float* dbp, float* d_w_ih, float* d_w_hh, float* d_b_ih,
-                                              float* d_b_hh, void* stream) {
-    STMGCN_REQUIRE(slices && dbp && d_w_ih && d_w_hh && d_b_ih && d_b_hh, STMGCN_ERR_ARG, "lstm16_wgrad_reduce: null pointer");
-    STMGCN_REQUIRE(layer >= 0 && n_slices >= 1 && c_in >= 1 && c_in <= kMaxC, STMGCN_ERR_SHAPE, "lstm16_wgrad_reduce: bad sizes");
-    lstm16_wgrad_reduce_kernel<<<(kTileM * kGateCols) / 256, 256, 0, (cudaStream_t)stream>>>(slices, n_slices, layer, c_in, dbp,
-                                                                                        d_w_ih, d_w_hh, d_b_ih, d_b_hh);
-    count_launch();
-    return check_launch("lstm16_wgrad_reduce");
+    return 0;
 }

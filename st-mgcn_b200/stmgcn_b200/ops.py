@@ -9,11 +9,12 @@ Functions (reference lines they replace):
   ChebGCN          GCN.py:24-43 on a sparse L~ (recurrence on features) -> out (N,B,q)
   TemporalPool     STMGCN.py:40-42: GCN over time-as-features + residual + sum over regions -> (B,T)
   ContextGate      STMGCN.py:42-43: /N, fc, relu, fc (same weights), sigmoid -> s (B,T)
-  SharedLSTM       STMGCN.py:44,47-50: modulate + 3-layer shared LSTM (lstm16.cu: one call per layer / lstm.cu: one call)
+  SharedLSTM       STMGCN.py:44,47-50: modulate + 3-layer shared LSTM (lstm16.cu / lstm.cu: one call each way)
   FuseOut          STMGCN.py:116-118: sum over graphs + output FC -> (B,N,C)
 """
 from __future__ import annotations
 
+import math
 import os
 from collections import OrderedDict
 from typing import List, Optional, Sequence
@@ -418,19 +419,19 @@ def set_lstm_planes(planes: int) -> None:
 
 
 def _lstm16_images(weights: Sequence[torch.Tensor], n_layers: int, c_in: int):
-    """Operand images of the shared LSTM's parameters for the bf16-plane kernels (stmgcn_lstm16_pack)."""
+    """Operand images of the shared LSTM's parameters for the bf16-plane kernels (stmgcn_lstm16_pack): the flat wimg,
+    bias (L, 256) and wih_t."""
 
     def pack():
         dev = weights[0].device
-        wimg = [torch.empty(65536 if l == 0 else 131072, dtype=torch.uint8, device=dev) for l in range(n_layers)]
-        bias = [torch.empty(256, dtype=torch.float32, device=dev) for _ in range(n_layers)]
+        wimg = torch.empty(65536 * (2 * n_layers - 1), dtype=torch.uint8, device=dev)
+        bias = torch.empty((n_layers, 256), dtype=torch.float32, device=dev)
         wih_t = torch.empty(c_in * 256, dtype=torch.float32, device=dev)
         st = _stream()
         for l in range(n_layers):
             w_ih, w_hh, b_ih, b_hh = weights[4 * l:4 * l + 4]
             _lib.check(L.stmgcn_lstm16_pack(w_ih.data_ptr(), w_hh.data_ptr(), b_ih.data_ptr(), b_hh.data_ptr(), l, c_in,
-                                            wimg[l].data_ptr(), bias[l].data_ptr(), wih_t.data_ptr() if l == 0 else None,
-                                            st), "lstm16_pack")
+                                            wimg.data_ptr(), bias.data_ptr(), wih_t.data_ptr(), st), "lstm16_pack")
         return dict(wimg=wimg, bias=bias, wih_t=wih_t)
 
     return _cached_images(weights, ("lstm16", c_in), pack)
@@ -445,34 +446,32 @@ def to_planes(x: torch.Tensor, planes: int) -> torch.Tensor:
     return torch.stack([hi, lo], dim=-3).contiguous()
 
 
+# the tensors of the bf16-plane path's tape, in the order SharedLSTM saves them
+_TAPE16 = ("hp", "cs", "h0p", "c0b", "wimg", "bias", "wih_t")
+
+
 def _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes, keep_tape):
-    """Forward of the bf16-plane path.  Returns (h_top (N,B,64), h_n, c_n, tape dict or None)."""
+    """Forward of the bf16-plane path, one library call.  Returns (h_top (N,B,64), h_n, c_n, tape dict or None): the
+    tape holds the _TAPE16 tensors and ``packed``, the image cache entry the backward waits for."""
     n, b, t_len, c_in = xo.shape
     rows = n * b
-    dev = xo.device
     rows_pad = ((rows + 127) // 128) * 128
     img = _lstm16_images(weights, n_layers, c_in)
-    hp = torch.empty((n_layers, t_len, planes, rows, 64), device=dev, dtype=torch.bfloat16)
-    cs = torch.empty((n_layers, t_len, rows_pad, 64), device=dev, dtype=torch.float32)
+    hp = torch.empty((n_layers, t_len, planes, rows, 64), device=xo.device, dtype=torch.bfloat16)
+    cs = xo.new_empty((n_layers, t_len, rows_pad, 64))
     h0p = to_planes(h0c, planes) if h0c is not None else None        # (L, P, R, 64)
     c0b = to_blocked(c0c) if c0c is not None else None
-    if want_state:
-        h_n = torch.empty((n_layers, rows, 64), device=dev, dtype=torch.float32)
-        h_top = h_n[n_layers - 1]
-    else:
-        h_n = None
-        h_top = torch.empty((rows, 64), device=dev, dtype=torch.float32)
-    st = _stream()
-    for l in range(n_layers):
-        _lib.check(L.stmgcn_lstm16_layer_fwd(l, t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(),
-                                             img["wimg"][l].data_ptr(), img["bias"][l].data_ptr(), img["wih_t"].data_ptr(),
-                                             _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(), h_top.data_ptr(), _p(h_n), st),
-                   "lstm16_layer_fwd")
+    h_n = xo.new_empty((n_layers, rows, 64)) if want_state else None
+    h_top = h_n[n_layers - 1] if want_state else xo.new_empty((rows, 64))
+    wimg, bias, wih_t = img["wimg"], img["bias"], img["wih_t"]
+    _lib.check(L.stmgcn_lstm16_fwd(t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(), wimg.data_ptr(),
+                                   bias.data_ptr(), wih_t.data_ptr(), _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(),
+                                   h_top.data_ptr(), _p(h_n), _stream()), "lstm16_fwd")
     if want_state:
         c_n = from_blocked(cs[:, t_len - 1], rows)
-    else:
-        h_n = c_n = torch.empty(0, device=dev, dtype=torch.float32)
-    tape = dict(hp=hp, cs=cs, h0p=h0p, c0b=c0b, img=img) if keep_tape else None
+    else:                       # ST_MGCN discards the final state (STMGCN.py:113)
+        h_n = c_n = xo.new_empty(0)
+    tape = dict(hp=hp, cs=cs, h0p=h0p, c0b=c0b, wimg=wimg, bias=bias, wih_t=wih_t, packed=img) if keep_tape else None
     return h_top.view(n, b, 64), h_n, c_n, tape
 
 
@@ -488,47 +487,29 @@ def _zero_tile(dev: torch.device) -> torch.Tensor:
 
 
 def _lstm16_backward(xo, s_gate, tape, n_layers, planes, d_top):
-    """BPTT of the bf16-plane path: ONE fused launch per layer over all timesteps (gate recompute + pointwise + data
-    gradient + weight gradient, stmgcn_lstm16_layer_bwd), layers top-down, then one reduction per layer.
-    Returns (d_s, [native nn.LSTM gradients])."""
+    """BPTT of the bf16-plane path, one library call (per layer one fused launch over all timesteps and one weight-gradient
+    reduction).  Returns (d_s, [native nn.LSTM gradients]): views of one flat buffer."""
+    _wait_packed(tape["packed"])
+    hp, cs, h0p, c0b, wimg, bias, wih_t = (tape[k] for k in _TAPE16)
     n, b, t_len, c_in = xo.shape
     rows = n * b
-    dev = xo.device
-    rows_pad = ((rows + 127) // 128) * 128
-    img = tape["img"]
-    _wait_packed(img)
-    d_top_b = to_blocked(_f32c(d_top).view(rows, 64))
-    dh_rec = torch.empty((rows_pad, 64), device=dev, dtype=torch.float32)
-    dc = torch.empty((rows_pad, 64), device=dev, dtype=torch.float32)
-    # dx of a layer for every timestep: written by layer l, read by layer l - 1 (two buffers ping-pong down the stack)
-    dx_bufs = [torch.empty((t_len, rows_pad, 64), device=dev, dtype=torch.float32) for _ in range(min(2, n_layers - 1))]
-    d_s = torch.zeros((b, t_len), device=dev, dtype=torch.float32)
-    dbp = torch.zeros((n_layers, 256), device=dev, dtype=torch.float32)
-    grid = int(L.stmgcn_lstm16_grid(rows))
-    scratch = torch.empty((n_layers, grid, 128 * 256), device=dev, dtype=torch.float32)
-    zero = _zero_tile(dev)
-    st = _stream()
-    dh_in = d_top_b
-    for l in range(n_layers - 1, -1, -1):
-        dx_out = dx_bufs[(n_layers - 1 - l) % 2] if l > 0 else None
-        _lib.check(L.stmgcn_lstm16_layer_bwd(l, t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(),
-                                             img["wimg"][l].data_ptr(), img["bias"][l].data_ptr(), img["wih_t"].data_ptr(),
-                                             _p(tape["h0p"]), _p(tape["c0b"]), tape["hp"].data_ptr(), tape["cs"].data_ptr(),
-                                             dh_in.data_ptr(), _p(dx_out), dh_rec.data_ptr(), dc.data_ptr(), d_s.data_ptr(),
-                                             dbp[l].data_ptr(), scratch[l].data_ptr(), zero.data_ptr(), st), "lstm16_layer_bwd")
-        dh_in = dx_out
-    grads = []
-    for l in range(n_layers):
-        in_l = c_in if l == 0 else 64
-        d_w_ih = torch.empty((256, in_l), device=dev, dtype=torch.float32)
-        d_w_hh = torch.empty((256, 64), device=dev, dtype=torch.float32)
-        d_b_ih = torch.empty(256, device=dev, dtype=torch.float32)
-        d_b_hh = torch.empty(256, device=dev, dtype=torch.float32)
-        _lib.check(L.stmgcn_lstm16_wgrad_reduce(l, c_in, grid, scratch[l].data_ptr(), dbp[l].data_ptr(), d_w_ih.data_ptr(),
-                                                d_w_hh.data_ptr(), d_b_ih.data_ptr(), d_b_hh.data_ptr(), st),
-                   "lstm16_wgrad_reduce")
-        grads += [d_w_ih, d_w_hh, d_b_ih, d_b_hh]
-    return d_s, grads
+    rows_pad = cs.shape[2]
+    d_top = to_blocked(_f32c(d_top).view(rows, 64))
+    # no workspace needs initialisation: stmgcn_lstm16_bwd zeroes dw_scratch and dbp itself
+    dh_rec = xo.new_empty((rows_pad, 64))
+    dc = xo.new_empty((rows_pad, 64))
+    dx_work = xo.new_empty((min(2, n_layers - 1), t_len, rows_pad, 64)) if n_layers > 1 else None
+    dw_scratch = xo.new_empty((int(L.stmgcn_lstm16_grid(rows)), 128 * 256))
+    dbp = xo.new_empty((n_layers, 256))
+    d_s = xo.new_zeros((b, t_len))
+    shapes = [s for l in range(n_layers) for s in ((256, c_in if l == 0 else 64), (256, 64), (256,), (256,))]
+    grads = xo.new_empty(sum(math.prod(s) for s in shapes))
+    _lib.check(L.stmgcn_lstm16_bwd(t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(), wimg.data_ptr(),
+                                   bias.data_ptr(), wih_t.data_ptr(), _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(),
+                                   d_top.data_ptr(), dh_rec.data_ptr(), dc.data_ptr(), _p(dx_work), dw_scratch.data_ptr(),
+                                   dbp.data_ptr(), _zero_tile(xo.device).data_ptr(), d_s.data_ptr(), grads.data_ptr(),
+                                   _stream()), "lstm16_bwd")
+    return d_s, [g.view(s) for g, s in zip(grads.split([math.prod(s) for s in shapes]), shapes)]
 
 
 def _exact_forward(xo, s_gate, h0c, c0c, n_layers, hid, want_state, weights, keep_tape):
@@ -597,30 +578,31 @@ class SharedLSTM(torch.autograd.Function):
         ctx.dims = (n_layers, hid)
         ctx.planes16 = hid == 64 and lstm_path() == "tc" and c_in <= 4 and t_len <= 64
         if ctx.planes16:
-            planes = lstm_planes()
-            h_top, h_n, c_n, tape = _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes, need_grad)
+            ctx.planes = lstm_planes()
+            h_top, h_n, c_n, tape = _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, ctx.planes,
+                                                    need_grad)
             if need_grad:
-                ctx.tape16, ctx.planes = tape, planes
-                ctx.save_for_backward(xo, s_gate)
+                ctx.packed = tape["packed"]
+                tape = [tape[k] for k in _TAPE16]
         else:
             h_top, h_n, c_n, tape = _exact_forward(xo, s_gate, h0c, c0c, n_layers, hid, want_state, weights, need_grad)
-            if need_grad:
-                ctx.save_for_backward(xo, s_gate, *tape)
+        if need_grad:
+            ctx.save_for_backward(xo, s_gate, *tape)
         ctx.mark_non_differentiable(h_n, c_n)
         return h_top, h_n, c_n
 
     @staticmethod
     def backward(ctx, d_top, _dhn, _dcn):
         n_layers, hid = ctx.dims
+        xo, s_gate, *tape = ctx.saved_tensors
         if ctx.planes16:
-            xo, s_gate = ctx.saved_tensors
-            d_s, w_grads = _lstm16_backward(xo, s_gate, ctx.tape16, n_layers, ctx.planes, d_top)
+            tape16 = dict(zip(_TAPE16, tape), packed=ctx.packed)
+            d_s, w_grads = _lstm16_backward(xo, s_gate, tape16, n_layers, ctx.planes, d_top)
         else:
             if getattr(ctx, "tape_consumed", False):
                 raise RuntimeError("SharedLSTM (exact-fp32 kernels): the gate tape was overwritten in place by the first "
                                    "backward pass; a second backward over the same graph is not supported on this path")
             ctx.tape_consumed = True
-            xo, s_gate, *tape = ctx.saved_tensors
             d_s, w_grads = _exact_backward(xo, s_gate, tape, n_layers, hid, d_top)
         return (None, d_s, None, None, None, None, None, *w_grads)
 

@@ -37,16 +37,18 @@ def test_library_exports_every_declared_symbol():
     assert _lib.lib.stmgcn_launch_count() >= 0
 
 
-def test_c_abi_argument_errors_come_back_as_codes_with_a_message():
+def test_c_abi_argument_errors_return_negative_codes_with_a_message():
     """The C entry points validate their arguments before touching CUDA: a bad call returns a negative code and
     stmgcn_last_error() explains it (no GPU needed)."""
     import ctypes
     from stmgcn_b200 import _lib
     lib = _lib.lib
     null = ctypes.c_void_p(0)
-    # time-fused LSTM backward: null workspaces
-    rc = lib.stmgcn_lstm16_layer_bwd(0, 12, 3, 128, 1, 8, 2, *([null] * 18))
-    assert rc < 0 and b"lstm16_layer_bwd" in lib.stmgcn_last_error()
+    # tensor-core LSTM over the whole stack: null operands / workspaces
+    rc = lib.stmgcn_lstm16_bwd(12, 3, 128, 1, 8, 2, *([null] * 19))
+    assert rc < 0 and b"lstm16_bwd: null pointer" in lib.stmgcn_last_error()
+    rc = lib.stmgcn_lstm16_fwd(12, 3, 128, 1, 8, 2, *([null] * 12))
+    assert rc < 0 and b"lstm16_fwd: null pointer" in lib.stmgcn_last_error()
     # exact-fp32 LSTM backward over the whole sequence: null workspaces
     rc = lib.stmgcn_lstm_bwd(12, 3, 128, 64, 1, 8, *([null] * 18))
     assert rc < 0 and b"lstm_bwd: null pointer" in lib.stmgcn_last_error()
@@ -175,7 +177,7 @@ def test_lstm_flat_weight_packing_roundtrip():
 @pytest.mark.parametrize("rows", [128, 300, 1])
 def test_tile_blocked_layout_roundtrip_and_formula(rows):
     """to_blocked / from_blocked are inverse, pad to whole 128-row tiles, and place element (r, u) where the kernels'
-    ws_off() expects it: (((r/128)*16 + u/4)*128 + r%128)*4 + u%4  (include/stmgcn_b200.h, stmgcn_lstm16_layer_fwd)."""
+    ws_off() expects it: (((r/128)*16 + u/4)*128 + r%128)*4 + u%4  (include/stmgcn_b200.h, the tensor-core LSTM)."""
     from stmgcn_b200 import ops
     gen = torch.Generator().manual_seed(rows)
     x = torch.randn(2, rows, 64, generator=gen)

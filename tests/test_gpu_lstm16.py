@@ -196,3 +196,42 @@ def test_shared_lstm_routing_at_the_step_limit(t_len, monkeypatch):
     print(f"SharedLSTM T={t_len} ({'tensor cores' if calls else 'FFMA'}): h_top {e_fwd:.2e}, worst gradient {max(gerrs):.2e}")
     assert e_fwd <= FWD_TOL, e_fwd
     assert max(gerrs) <= GRAD_TOL, gerrs
+
+
+@pytest.mark.parametrize("lyr,t", [(3, 12), (2, 5), (1, 1)])
+def test_lstm16_launch_sequence(lyr, t, monkeypatch):
+    """The tensor-core path's first forward packs each layer's weights and makes one launch per layer; with the images
+    cached a forward is one launch per layer; the backward is one fused launch and one weight-gradient reduction per
+    layer."""
+    from stmgcn_b200 import _lib, ops
+    monkeypatch.setattr(ops, "_LSTM_PATH", "tc")
+    xo, s, _, _, ws, d_top = _inputs(3, 40, t, lyr, 1, False, seed=3)
+    ws_g = [w.requires_grad_(True) for w in ws]
+    counts = []
+    for _ in range(2):
+        n0 = _lib.launch_count()
+        h_top, _, _ = ops.SharedLSTM.apply(xo, s, None, None, lyr, HID, False, *ws_g)
+        n1 = _lib.launch_count()
+        (h_top.reshape(-1, HID) * d_top).sum().backward()
+        counts.append((n1 - n0, _lib.launch_count() - n1))
+    assert counts == [(2 * lyr, 2 * lyr), (lyr, 2 * lyr)]
+
+
+def test_lstm16_second_backward_repeats_the_first(monkeypatch):
+    """The tensor-core backward leaves its tape intact: a second backward(retain_graph=True) over the same graph gives
+    the first one's gradients (within the gradient bar: the kernels sum them with atomics)."""
+    from stmgcn_b200 import ops
+    monkeypatch.setattr(ops, "_LSTM_PATH", "tc")
+    n, b, t, lyr, c = 5, 60, 7, 3, 2
+    xo, s, h0, c0, ws, d_top = _inputs(n, b, t, lyr, c, True, seed=4)
+    leaves = [s.clone().requires_grad_(True)] + [w.clone().requires_grad_(True) for w in ws]
+    h_top, _, _ = ops.SharedLSTM.apply(xo, leaves[0], h0, c0, lyr, HID, False, *leaves[1:])
+    loss = (h_top.reshape(n * b, HID) * d_top).sum()
+    grads = []
+    for _ in range(2):
+        for v in leaves:
+            v.grad = None
+        loss.backward(retain_graph=True)
+        grads.append([v.grad.clone() for v in leaves])
+    errs = [O.max_rel_err(a.cpu().numpy(), r.cpu().numpy()) for a, r in zip(grads[1], grads[0])]
+    assert max(errs) <= GRAD_TOL, errs
