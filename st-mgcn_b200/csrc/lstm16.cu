@@ -15,7 +15,8 @@
 //   2 warpgroups  : each walks its 64 rows of a tile through t = 0 .. T-1; per step 8 (P = 1) or 24 (P = 2) wgmma
 //                   m64n256k16 into registers: Ahi.Whi + Ahi.Wlo + Alo.Whi, then bias (+ layer 0: x*s . W_ih in exact
 //                   fp32) -> gates -> c, h -> h split into bf16 planes in shared memory, which is both the h_prev operand
-//                   of the next step and the source of a TMA tensor store of the tape.  Nothing of the gates leaves the SM.
+//                   of the next step and the source of a TMA tensor store of the tape; c stays in shared memory too
+//                   (and is stored to the cs tape).  Nothing of the gates leaves the SM.
 #include "tc16.cuh"
 #include <cuda.h>
 #include <stdlib.h>
@@ -39,6 +40,25 @@ constexpr int kATileBytes = kTile16Bytes;             // [128 rows][64 k] bf16 =
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, int c0, int c1, int c2, uint64_t* bar) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+
+// L2 policy for data a launch reads exactly once (the backward's A planes, c_prev, dh_in): evicted first, so that the
+// lines read again -- the recurrent dh_rec / dc, the weight-gradient slices -- keep their place in L2
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void tma_load_3d_hint(void* smem_dst, const void* tmap, int c0, int c1, int c2, uint64_t* bar,
+                                                 uint64_t pol) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
+                 " [%0], [%1, {%3, %4, %5}], [%2], %6;"
+                 :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(pol) : "memory");
+}
+__device__ __forceinline__ float ld_hint(const float* p, uint64_t pol) {
+    float v;
+    asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
+    return v;
 }
 
 // ---- LSTM cell with 8 MUFU operations instead of 10 ------------------------------------------------------------
@@ -118,7 +138,10 @@ __device__ __forceinline__ float4 gate_args(float4 v, float4 b, const float (&xs
 //            tensor store of hp[l, t].  At t = 0 the tiles are loaded from h0p, or the segment is absent (zeros).
 //   h_below: layers > 0: hp[l - 1, t], written by the previous launch, streamed by the producer into one stage per
 //            warpgroup; released as soon as the step's wgmma have completed, so the next load overlaps the epilogue.
-//   c      : the tile-blocked cs tape; c_{t-1} is read back by the thread that wrote it one step earlier (L2-hot).
+//   c      : never read back from global memory.  c_{t-1} of a cell is private to the thread that computes c_t, so each
+//            warpgroup keeps its rows' c in a private fp32 tile in shared memory (filled from c0, or zeros, at the start
+//            of a tile); c_t goes to it and, fire-and-forget, to the tile-blocked cs tape for the backward.  (Read back
+//            from the tape, every cell waited one L2 round trip: the load cannot pass the previous cell's tape store.)
 // Accumulator fragment (wgmma.cuh): thread holds columns 8j + 2(lane%4) + {0,1} of rows r0 and r0 + 8; with
 // gate-interleaved columns n = 4 unit + gate that is gates (i, f) (lane%4 even) or (g, o) (odd) of unit 2j + (lane%4)/2.
 // Partner lanes (lane ^ 1) swap one row's pair, after which the even lane owns the cell (r0, unit) and the odd lane the
@@ -127,6 +150,7 @@ constexpr int kFWarpgroups = 2;
 constexpr int kFThreads = kFWarpgroups * 128 + 32;     // + producer warp
 constexpr int kHTileBytes = 64 * 128;                  // one plane of a warpgroup's rows: [64 rows][64] bf16 = 8 KB
 constexpr int kFWgBytes = 4 * kHTileBytes;             // per warpgroup: h_prev hi | lo, h_below stage hi | lo
+constexpr int kFCBytes = 64 * kHid * 4;                // per warpgroup: fp32 c of its rows, [32 cells j][128 threads]
 
 struct F16Tail {
     float bias[kGateCols];
@@ -135,7 +159,8 @@ struct F16Tail {
     uint64_t h0_full[kFWarpgroups];    // h_prev tiles of warpgroup w loaded from h0p
     uint64_t w_full;
 };
-constexpr size_t kFSmem = 1024 + 4 * (size_t)kWTileBytes + kFWarpgroups * (size_t)kFWgBytes + sizeof(F16Tail);
+constexpr size_t kFSmem =
+    1024 + 4 * (size_t)kWTileBytes + kFWarpgroups * ((size_t)kFWgBytes + kFCBytes) + sizeof(F16Tail);
 static_assert(kFSmem <= 232448, "lstm16 forward kernel exceeds the 227 KB shared-memory limit");
 
 struct Fwd16Params {
@@ -185,7 +210,8 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* wsm = smem;                                           // resident weight tiles (seg*2 + plane)
     uint8_t* hsm = smem + 4 * (size_t)kWTileBytes;                 // per warpgroup: kFWgBytes
-    F16Tail* tail = (F16Tail*)(hsm + kFWarpgroups * (size_t)kFWgBytes);
+    uint8_t* csm = hsm + kFWarpgroups * (size_t)kFWgBytes;         // per warpgroup: kFCBytes
+    F16Tail* tail = (F16Tail*)(csm + kFWarpgroups * (size_t)kFCBytes);
     // layer 0 has one weight segment: the pre-scaled W_ih^T lives in the unused seg-1 weight slot
     float* wih_s = reinterpret_cast<float*>(wsm + 2 * (size_t)kWTileBytes);
     const int tid = threadIdx.x;
@@ -259,6 +285,8 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
     const uint32_t row_in_tile = 64u * (uint32_t)wg + row_in_wg;
     const uint32_t rows32 = (uint32_t)p.rows;
     uint8_t* h_sm = hsm + (size_t)wg * kFWgBytes;                  // h_prev: hi | lo
+    // c of this thread's 32 cells: element 128 j (thread-major: conflict free; only the owning thread touches it)
+    float* c_sm = reinterpret_cast<float*>(csm + (size_t)wg * kFCBytes) + (tid & 127);
     const uint32_t w_u = smem_u32(wsm), h_u = smem_u32(h_sm), b_u = h_u + 2u * kHTileBytes;
     const int64_t cslice = (int64_t)p.n_tiles * kTileM * kHid;
     float acc[128];
@@ -272,6 +300,11 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
         const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
         const bool valid = r < rows32;
         const uint32_t cbase = (uint32_t)tile * 8192u + row_in_tile * 4u;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+            const int unit = 2 * j + (q >> 1);
+            c_sm[128 * j] = (p.c0 != nullptr && valid) ? p.c0[cbase + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3)] : 0.f;
+        }
         if (p.has_h0) {
             if (issuer) {
                 bulk_wait_group_read0();                           // the previous tile's last store has read the tiles
@@ -324,7 +357,6 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
             }
             // ---- LSTM cell: 32 cells per thread, row row_in_tile, units 2j + q/2 ----
             float* c_out = p.cs + (int64_t)t * cslice;
-            const float* c_prev = t > 0 ? c_out - cslice : p.c0;
             float* h_f32 = t == p.t_len - 1 ? p.h_f32 : nullptr;
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
@@ -334,9 +366,9 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
                 const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
                 const float4 a = gate_args<CIN>(v, bv, xs, wih_s, col, p.c_in);
                 const uint32_t co = cbase + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
-                const float cp = (c_prev != nullptr && valid) ? c_prev[co] : 0.f;
                 float cn, hn;
-                lstm_cell_fwd8(a.x, a.y, a.z, a.w, cp, cn, hn);
+                lstm_cell_fwd8(a.x, a.y, a.z, a.w, c_sm[128 * j], cn, hn);
+                c_sm[128 * j] = cn;
                 if (valid) {
                     c_out[co] = cn;
                     if (h_f32 != nullptr) h_f32[r * (uint32_t)kHid + (uint32_t)unit] = hn;
@@ -419,7 +451,9 @@ static_assert(kBSmem <= 232448, "lstm16 backward kernel exceeds the 227 KB share
 
 // One launch = one LAYER, its timesteps from T-1 down (the tiles of a CTA are its own through time: rows never mix).
 // A step of a tile needs what the SAME CTA produced for that tile one step later (dh_rec, dc: global, in place), so nothing
-// but the launch order of the layers (top down) synchronises.
+// but the launch order of the layers (top down) synchronises.  Items are tile-major: a CTA walks one tile through all
+// T steps before the next, so dh_rec / dc are read back one item after they were written (64 KB per CTA, ~8.4 MB for
+// 132 CTAs, L2-resident) instead of after a whole step of every tile had gone through the 50 MB L2.
 constexpr int kBMaxSteps = 64;
 struct Bwd16Step {
     int32_t slice[2];          // plane slice of K segment s in its tensor map (hi plane; lo = + 1)
@@ -506,7 +540,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     fence_proxy_async_smem();
     __syncthreads();
     const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    const int n_items = my_tiles * p.n_steps;                      // work items (step, tile), step-major
+    const int n_items = my_tiles * p.n_steps;                      // work items (step, tile), tile-major
 
     if (warp == kProdWarp) {
         // ===================== producer =====================
@@ -517,8 +551,9 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 for (int pl = 0; pl < PLANES; ++pl)
                     bulk_g2s(w_sm + (size_t)(sg * 2 + pl) * kWTileBytes, p.wimg + (size_t)(sg * 2 + pl) * kWTileBytes, kWTileBytes,
                              &tail->w_full);
+            const uint64_t once = l2_evict_first();
             for (int w = 0; w < n_items; ++w) {
-                const int st = w / my_tiles, tile = (int)blockIdx.x + (w - st * my_tiles) * (int)gridDim.x;
+                const int ti = w / p.n_steps, st = w - ti * p.n_steps, tile = (int)blockIdx.x + ti * (int)gridDim.x;
                 const Bwd16Step& sp = p.steps[st];
                 mbar_wait_polite(&tail->a_empty, (uint32_t)(w & 1) ^ 1u);
                 mbar_arrive_expect_tx(&tail->a_full, (uint32_t)(kNseg * PLANES * kATileBytes));
@@ -526,7 +561,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                     for (int pl = 0; pl < PLANES; ++pl) {
                         uint8_t* dst = a_sm + (size_t)(sg * 2 + pl) * kATileBytes;
                         if (sp.src[sg] == 2) bulk_g2s(dst, p.zero_tile, kATileBytes, &tail->a_full);
-                        else tma_load_3d(dst, &p.maps[sp.src[sg]], 0, tile * kTileM, sp.slice[sg] + pl, &tail->a_full);
+                        else tma_load_3d_hint(dst, &p.maps[sp.src[sg]], 0, tile * kTileM, sp.slice[sg] + pl, &tail->a_full, once);
                     }
                 // the per-row inputs of this item -> L2 (a tile is one contiguous 32 KB run in every workspace)
                 const int64_t o = (int64_t)tile * kTileM * kHid;
@@ -548,19 +583,15 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     const uint32_t w_u = smem_u32(w_sm), a_u = smem_u32(a_sm), da_u = smem_u32(da_sm);
     const uint32_t a_rows = (uint32_t)wg * 64u * 128u;             // this warpgroup's rows inside a 128-row tile
     constexpr uint32_t kStepMN = 2048;                             // MN-major k16 step: 16 rows of 128 bytes
-    // layer 0: when b_inner divides the tile height, a thread's row belongs to the same window b in every tile: its share of
-    // d_s is summed in a register and added once per step
-    const bool ds_fixed = L0 && (kTileM % (uint32_t)p.b_inner) == 0u;
-    float ds_acc = 0.f;
     float* slice = p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols);
+    const uint64_t once = l2_evict_first();
     mbar_wait_raw(&tail->w_full, 0);
 
     for (int w = 0; w < n_items; ++w) {
-        const int st = w / my_tiles, tile = (int)blockIdx.x + (w - st * my_tiles) * (int)gridDim.x;
+        const int ti = w / p.n_steps, st = w - ti * p.n_steps, tile = (int)blockIdx.x + ti * (int)gridDim.x;
         const Bwd16Step& sp = p.steps[st];
         const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
         const bool valid = r < rows32;
-        const bool last_of_step = (w - st * my_tiles) == my_tiles - 1;
         float xs[kMaxC], xraw[kMaxC], dxs[kMaxC];
         if (L0) {
             const float sv = valid ? p.sg[(r % (uint32_t)p.b_inner) * (uint32_t)p.t_len + (uint32_t)sp.t] : 0.f;
@@ -609,12 +640,26 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 }
             }
             wg_commit();
+            // the cells' global inputs of this chunk, all issued while the recompute runs: each cell loading its own
+            // after the previous cell's dc store (which they may alias, as far as the compiler knows) waited one
+            // memory round trip per cell.  c_prev and dh_in are read once per launch: streaming loads (evict-first).
+            const uint32_t bo = (uint32_t)tile * 8192u + row_in_tile * 4u;
+            float cpv[8], dhv[8], dciv[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int unit = 16 * c + 2 * j + (q >> 1);
+                const uint32_t o = bo + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
+                cpv[j] = (valid && sp.c_prev) ? __ldcs(sp.c_prev + o) : 0.f;
+                dhv[j] = (valid && sp.dh_in) ? __ldcs(sp.dh_in + o) : 0.f;
+                const bool rec = valid && !sp.first;
+                if (rec) dhv[j] += p.dh_rec[o];
+                dciv[j] = rec ? p.dc[o] : 0.f;
+            }
             wg_wait<0>();
             wg_fence_regs(g);
             // ---- P_c: 8 cells per thread (row row_in_tile, units 16c + 2j + q/2) ----
             uint32_t dhi[8], dlo[8];
             float bs[32];                                          // dA of this thread's cells: bs[4j + gate]
-            const uint32_t bo = (uint32_t)tile * 8192u + row_in_tile * 4u;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const float4 v = frag_to_gates(g, j, odd);
@@ -625,15 +670,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                                                                bv.z * -2.8853900817779268f, bv.w * -1.4426950408889634f),
                                                 xs, wih_s, col, p.c_in);
                 const uint32_t o = bo + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
-                float cp = 0.f, dh = 0.f, dci = 0.f;
-                if (valid) {
-                    if (sp.c_prev) cp = sp.c_prev[o];
-                    if (sp.dh_in) dh = sp.dh_in[o];
-                    if (!sp.first) {
-                        dh += p.dh_rec[o];
-                        dci = p.dc[o];
-                    }
-                }
+                const float cp = cpv[j], dh = dhv[j], dci = dciv[j];
                 float gi, gf, gg, go, tc_;
                 lstm_cell_gates8(a.x, a.y, a.z, a.w, cp, gi, gf, gg, go, tc_);
                 // rows past the end: dh = dci = 0, so dA = 0
@@ -761,15 +798,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
 #pragma unroll
             for (int cc = 0; cc < kC; ++cc) contrib += dxs[cc] * xraw[cc];
             contrib += __shfl_xor_sync(0xffffffffu, contrib, 2);
-            if ((q >> 1) == 0 && valid) {
-                if (ds_fixed) ds_acc += contrib;
-                else atomicAdd(&p.d_s[(int64_t)(r % (uint32_t)p.b_inner) * p.t_len + sp.t], contrib);
-            }
-            if (ds_fixed && last_of_step) {
-                if ((q >> 1) == 0 && ds_acc != 0.f)
-                    atomicAdd(&p.d_s[(int64_t)(row_in_tile % (uint32_t)p.b_inner) * p.t_len + sp.t], ds_acc);
-                ds_acc = 0.f;
-            }
+            if ((q >> 1) == 0 && valid) atomicAdd(&p.d_s[(int64_t)(r % (uint32_t)p.b_inner) * p.t_len + sp.t], contrib);
         }
     }
     cons_sync(kCons);
