@@ -55,6 +55,10 @@ __device__ __forceinline__ void tma_load_3d_hint(void* smem_dst, const void* tma
                  " [%0], [%1, {%3, %4, %5}], [%2], %6;"
                  :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(pol) : "memory");
 }
+__device__ __forceinline__ void tma_prefetch_3d(const void* tmap, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
+                 :: "l"(tmap), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
 __device__ __forceinline__ float ld_hint(const float* p, uint64_t pol) {
     float v;
     asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
@@ -424,9 +428,11 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
 // backward: gate recompute + BPTT pointwise + data gradient + weight gradient in ONE kernel, time-fused per layer
 // (a launch = one layer x all its timesteps, see Bwd16Params; "item" below = one (step, tile) work item)
 // =====================================================================================================
-// CTA = two consumer warpgroups (warpgroup w: rows 64w .. 64w+63 of a tile) + one producer warp.  The layer's weight image
-// stays resident in shared memory; the producer streams the A planes ([h_below | h_prev], hi and lo) of each item with
-// TMA.  Per item the 256 gate columns are processed as four chunks of 64 (16 units x i,f,g,o):
+// CTA = two consumer warpgroups (warpgroup w: rows 64w .. 64w+63 of a tile) + one producer warpgroup, warp-specialised:
+// the producer drops to kBProdRegs registers so that the consumers can hold the accumulators of two chunks at once.
+// The layer's weight image stays resident in shared memory; one producer thread streams the A planes ([h_below |
+// h_prev], hi and lo) of each item with TMA and prefetches the next item's into L2.  Per item the 256 gate columns are
+// processed as four chunks of 64 (16 units x i,f,g,o):
 //   R_c : recompute  G_c[64 x 64] = [h_below | h_prev] . Wp[:, chunk]                      (registers, m64n64)
 //   P_c : gates -> c_t, tanh(c_t) -> BPTT pointwise -> dA_c (fp32) -> bf16 hi/lo planes in a 128-byte-swizzled
 //         shared-memory tile; dc in place
@@ -436,10 +442,18 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
 //         tiles already in shared memory), added into this CTA's own slice of a scratch buffer with vector reductions
 //   D_c : data gradient    [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T  (B: MN-major view of the resident weights;
 //         accumulated in registers over the four chunks, stored at the end of the item)
+// Schedule of a warpgroup (one dA tile shared by both warpgroups, so they stay in step at its two barriers per chunk):
+//   c = 0      : R_0; wait; P_0, B_0; barrier; dA_0 -> tile; barrier
+//   c = 1 .. 3 : R_c | W_{c-1} + D_{c-1} (two commit groups); wait for R_c only; P_c, B_c (dA_c kept in registers)
+//                while the tensor pipe runs W / D; wait; red.add W_{c-1}; barrier; dA_c -> tile; barrier
+//   item end   : W_3 | D_3; wait for W_3; A planes released to the producer; red.add W_3; wait for D_3; store
+// The wgmma operands and the accumulation order of every accumulator are those of the unpipelined schedule.
 // dA never leaves the SM; the gates are never stored.  lstm16_wgrad_reduce_kernel sums the slices after each layer's
 // launch and writes nn.LSTM-native gradients.
 constexpr int kBWarpgroups = 2;
-constexpr int kBThreads = kBWarpgroups * 128 + 32;      // + producer warp
+constexpr int kBThreads = kBWarpgroups * 128 + 128;     // + producer warpgroup (one thread of it issues the loads)
+// registers per thread after setmaxnreg: 256 * 240 + 128 * 24 = 64 512 of the SM's 65 536 (launched at 384 * 168)
+constexpr uint32_t kBConsRegs = 240, kBProdRegs = 24;
 constexpr int kBATiles = 4;                             // (seg0 | seg1) x (hi | lo); layer 0: seg 1 = the auxiliary [x*s] tile
 
 struct B16Tail {
@@ -487,11 +501,87 @@ struct Bwd16Params {
 static_assert(sizeof(Bwd16Params) <= 4096, "kernel parameter block exceeds 4 KB");
 
 __device__ __forceinline__ void cons_sync(int n_threads) { asm volatile("bar.sync 1, %0;" ::"r"(n_threads) : "memory"); }
+// a warpgroup's per-thread register budget (every warp of the warpgroup executes the same instruction)
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// R_c: g = [h_below | h_prev] . Wp[:, chunk c] of this warpgroup's 64 rows
+template <int PLANES, int NSEG>
+__device__ __forceinline__ void bwd_recompute_mma(float (&g)[32], uint32_t a_u, uint32_t a_rows, uint32_t w_u, int c) {
+#pragma unroll
+    for (int s = 0; s < NSEG; ++s) {
+        const uint64_t a_hi = desc16_k(a_u + (uint32_t)(s * 2) * kATileBytes + a_rows);
+        const uint64_t a_lo = desc16_k(a_u + (uint32_t)(s * 2 + 1) * kATileBytes + a_rows);
+        const uint64_t b_hi = desc16_k(w_u + (uint32_t)(s * 2) * kWTileBytes + (uint32_t)c * 8192u);
+        const uint64_t b_lo = desc16_k(w_u + (uint32_t)(s * 2 + 1) * kWTileBytes + (uint32_t)c * 8192u);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            wgmma_bf16_n64_t00(g, a_hi + 2 * kk, b_hi + 2 * kk, (s > 0 || kk > 0) ? 1u : 0u);
+            if (PLANES == 2) {
+                wgmma_bf16_n64_t00(g, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
+                wgmma_bf16_n64_t00(g, a_lo + 2 * kk, b_hi + 2 * kk, 1u);
+            }
+        }
+    }
+}
+
+constexpr uint32_t kStepMN = 2048;                             // MN-major k16 step: 16 rows of 128 bytes
+
+// W_c: wgr = A^T . dA_c, kd rows 64 wg .. 64 wg + 63 (wa_hi: this warpgroup's A tile, hi plane; its lo plane follows)
+template <int PLANES, bool L0>
+__device__ __forceinline__ void bwd_wgrad_mma(float (&wgr)[32], uint32_t wa_hi, uint32_t da_u) {
+    const uint32_t wa_lo = wa_hi + kATileBytes;
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+        const uint64_t ah = desc16_mn(wa_hi + ks * kStepMN, kATileBytes);
+        const uint64_t al = desc16_mn(wa_lo + ks * kStepMN, kATileBytes);
+        const uint64_t bh = desc16_mn(da_u + ks * kStepMN, kATileBytes);
+        const uint64_t bl = desc16_mn(da_u + kATileBytes + ks * kStepMN, kATileBytes);
+        // dA always has its lo plane; in the single-plane mode only the STORED operands are rounded to bf16.
+        // Layer 0's warpgroup 1 multiplies the auxiliary x*s tile, which is not stored: it keeps its lo plane in
+        // both modes, as the forward's fp32 FMAs do (warpgroup 0's lo slot is zero then, and adds nothing; both
+        // warpgroups issue the pass so that no wgmma sits on a warpgroup-dependent branch, which would make
+        // ptxas serialise every wgmma of the kernel)
+        wgmma_bf16_n64_t11(wgr, ah, bh, ks > 0 ? 1u : 0u);
+        wgmma_bf16_n64_t11(wgr, ah, bl, 1u);
+        if (PLANES == 2 || L0) wgmma_bf16_n64_t11(wgr, al, bh, 1u);
+    }
+}
+
+// D_c: [dx_below | dh_prev] += dA_c . Wp[:, chunk c]^T
+template <int PLANES, int NSEG>
+__device__ __forceinline__ void bwd_dgrad_mma(float (&dacc)[32 * NSEG], uint32_t da_u, uint32_t a_rows, uint32_t w_u, int c) {
+    const uint64_t ah = desc16_k(da_u + a_rows), al = desc16_k(da_u + kATileBytes + a_rows);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        const uint32_t wb = w_u + (uint32_t)c * 8192u + (uint32_t)kk * kStepMN;
+        const uint64_t bh = desc16_mn(wb, 2 * kWTileBytes), bl = desc16_mn(wb + kWTileBytes, 2 * kWTileBytes);
+        if constexpr (NSEG == 2) {
+            wgmma_bf16_n128_t01(dacc, ah + 2 * kk, bh, 1u);
+            if (PLANES == 2) wgmma_bf16_n128_t01(dacc, ah + 2 * kk, bl, 1u);
+            wgmma_bf16_n128_t01(dacc, al + 2 * kk, bh, 1u);
+        } else {
+            wgmma_bf16_n64_t01(dacc, ah + 2 * kk, bh, 1u);
+            if (PLANES == 2) wgmma_bf16_n64_t01(dacc, ah + 2 * kk, bl, 1u);
+            wgmma_bf16_n64_t01(dacc, al + 2 * kk, bh, 1u);
+        }
+    }
+}
+
+// weight-gradient fragment of chunk c -> this CTA's slice (row-major [kd][256]); rw0: the fragment's first row
+__device__ __forceinline__ void bwd_wgrad_red(float* slice, const float (&wgr)[32], uint32_t rw0, int q, int c) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const uint32_t n = (uint32_t)(64 * c + 8 * j + 2 * q);
+        red_add_f32x2(slice + (size_t)rw0 * kGateCols + n, wgr[4 * j], wgr[4 * j + 1]);
+        red_add_f32x2(slice + (size_t)(rw0 + 8) * kGateCols + n, wgr[4 * j + 2], wgr[4 * j + 3]);
+    }
+}
 
 // One reduce-scatter step between lanes l and l ^ mask over v[0 .. 2H): the lane with the mask bit set keeps the upper
 // half, the other the lower half, each adds its partner's copy of that half; the kept half moves to v[0 .. H).
-template <int H>
-__device__ __forceinline__ void col_sums_step(float (&v)[32], int mask, int lane) {
+template <int H, int N>
+__device__ __forceinline__ void col_sums_step(float (&v)[N], int mask, int lane) {
     const bool up = (lane & mask) != 0;
 #pragma unroll
     for (int i = 0; i < H; ++i) {
@@ -542,9 +632,10 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     const int n_items = my_tiles * p.n_steps;                      // work items (step, tile), tile-major
 
-    if (warp == kProdWarp) {
+    if (warp >= kProdWarp) {
         // ===================== producer =====================
-        const bool leader = elect_one_sync();
+        setmaxnreg_dec<kBProdRegs>();
+        const bool leader = warp == kProdWarp && elect_one_sync();
         if (leader && n_items > 0) {
             mbar_arrive_expect_tx(&tail->w_full, (uint32_t)(kNseg * PLANES * kWTileBytes));
             for (int sg = 0; sg < kNseg; ++sg)
@@ -568,12 +659,21 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 constexpr uint32_t kB = kTileM * kHid * 4;
                 if (sp.c_prev) prefetch_l2(sp.c_prev + o, kB);
                 if (sp.dh_in) prefetch_l2(sp.dh_in + o, kB);
+                // the next item's A planes -> L2, a whole item ahead of the load that waits for them
+                if (w + 1 < n_items) {
+                    const int ti1 = (w + 1) / p.n_steps, tile1 = (int)blockIdx.x + ti1 * (int)gridDim.x;
+                    const Bwd16Step& sp1 = p.steps[w + 1 - ti1 * p.n_steps];
+                    for (int sg = 0; sg < kNseg; ++sg)
+                        for (int pl = 0; pl < PLANES; ++pl)
+                            if (sp1.src[sg] != 2) tma_prefetch_3d(&p.maps[sp1.src[sg]], 0, tile1 * kTileM, sp1.slice[sg] + pl);
+                }
             }
         }
         return;
     }
 
     // ===================== consumers =====================
+    setmaxnreg_inc<kBConsRegs>();
     const int wg = tid >> 7;
     const int q = lane & 3;
     const bool odd = (q & 1) != 0;
@@ -582,7 +682,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     const uint32_t rows32 = (uint32_t)p.rows;
     const uint32_t w_u = smem_u32(w_sm), a_u = smem_u32(a_sm), da_u = smem_u32(da_sm);
     const uint32_t a_rows = (uint32_t)wg * 64u * 128u;             // this warpgroup's rows inside a 128-row tile
-    constexpr uint32_t kStepMN = 2048;                             // MN-major k16 step: 16 rows of 128 bytes
+    const uint32_t wa_u = a_u + (uint32_t)(wg * 2) * kATileBytes;  // W_c's A operand: this warpgroup's kd rows
     float* slice = p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols);
     const uint64_t once = l2_evict_first();
     mbar_wait_raw(&tail->w_full, 0);
@@ -617,34 +717,13 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         float dacc[32 * kNseg];                                    // [dx_below | dh_prev] (layer 0: [dh_prev])
 #pragma unroll
         for (int k = 0; k < 32 * kNseg; ++k) dacc[k] = 0.f;
-        for (int c = 0; c < 4; ++c) {
-            // ---- R_c ----
-            float g[32];
-#pragma unroll
-            for (int k = 0; k < 32; ++k) g[k] = 0.f;
-            wg_fence_regs(g);
-            wg_fence();
-#pragma unroll
-            for (int s = 0; s < kNseg; ++s) {
-                const uint64_t a_hi = desc16_k(a_u + (uint32_t)(s * 2) * kATileBytes + a_rows);
-                const uint64_t a_lo = desc16_k(a_u + (uint32_t)(s * 2 + 1) * kATileBytes + a_rows);
-                const uint64_t b_hi = desc16_k(w_u + (uint32_t)(s * 2) * kWTileBytes + (uint32_t)c * 8192u);
-                const uint64_t b_lo = desc16_k(w_u + (uint32_t)(s * 2 + 1) * kWTileBytes + (uint32_t)c * 8192u);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    wgmma_bf16_n64_t00(g, a_hi + 2 * kk, b_hi + 2 * kk, (s > 0 || kk > 0) ? 1u : 0u);
-                    if (PLANES == 2) {
-                        wgmma_bf16_n64_t00(g, a_hi + 2 * kk, b_lo + 2 * kk, 1u);
-                        wgmma_bf16_n64_t00(g, a_lo + 2 * kk, b_hi + 2 * kk, 1u);
-                    }
-                }
-            }
-            wg_commit();
-            // the cells' global inputs of this chunk, all issued while the recompute runs: each cell loading its own
-            // after the previous cell's dc store (which they may alias, as far as the compiler knows) waited one
-            // memory round trip per cell.  c_prev and dh_in are read once per launch: streaming loads (evict-first).
-            const uint32_t bo = (uint32_t)tile * 8192u + row_in_tile * 4u;
-            float cpv[8], dhv[8], dciv[8];
+        float wgr[32];                                             // W of the previous chunk, in flight during P_c
+        const uint32_t bo = (uint32_t)tile * 8192u + row_in_tile * 4u;
+        float cpv[8], dhv[8], dciv[8];
+        // the cells' global inputs of chunk c, all issued while the tensor pipe runs: each cell loading its own after
+        // the previous cell's dc store (which they may alias, as far as the compiler knows) waited one memory round
+        // trip per cell.  c_prev and dh_in are read once per launch: streaming loads (evict-first).
+        auto load_cells = [&](int c) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int unit = 16 * c + 2 * j + (q >> 1);
@@ -655,126 +734,126 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 if (rec) dhv[j] += p.dh_rec[o];
                 dciv[j] = rec ? p.dc[o] : 0.f;
             }
-            wg_wait<0>();
-            wg_fence_regs(g);
-            // ---- P_c: 8 cells per thread (row row_in_tile, units 16c + 2j + q/2) ----
-            uint32_t dhi[8], dlo[8];
-            float bs[32];                                          // dA of this thread's cells: bs[4j + gate]
+        };
+        uint32_t dpk[32];                                          // dA_c as bf16 planes: [4j, 4j+1] hi, [4j+2, 4j+3] lo
+        // ---- P_c: 8 cells per thread (row row_in_tile, units 16c + 2j + q/2) -> dpk, dc, db ----
+        auto cell_epilogue = [&](int c, const float (&g)[32]) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {                          // two halves of 4 cells: half the live fp32 dA
+                float bs[16];                                      // dA of this half's cells: bs[4 jj + gate]
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                    const int j = 4 * h + jj;
+                    const float4 v = frag_to_gates(g, j, odd);
+                    const int unit = 16 * c + 2 * j + (q >> 1);
+                    const int col = 4 * unit;
+                    const float4 bv = *reinterpret_cast<const float4*>(p.bias + col);     // scaled here (gate_scale)
+                    const float4 a = gate_args<CIN>(v, make_float4(bv.x * -1.4426950408889634f, bv.y * -1.4426950408889634f,
+                                                                   bv.z * -2.8853900817779268f, bv.w * -1.4426950408889634f),
+                                                    xs, wih_s, col, p.c_in);
+                    const uint32_t o = bo + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
+                    const float cp = cpv[j], dh = dhv[j], dci = dciv[j];
+                    float gi, gf, gg, go, tc_;
+                    lstm_cell_gates8(a.x, a.y, a.z, a.w, cp, gi, gf, gg, go, tc_);
+                    // rows past the end: dh = dci = 0, so dA = 0
+                    const float dcv = fmaf(dh * go, 1.f - tc_ * tc_, dci);
+                    const float da0 = dcv * gg * gi * (1.f - gi);
+                    const float da1 = dcv * cp * gf * (1.f - gf);
+                    const float da2 = dcv * gi * (1.f - gg * gg);
+                    const float da3 = dh * tc_ * go * (1.f - go);
+                    bs[4 * jj + 0] = da0; bs[4 * jj + 1] = da1; bs[4 * jj + 2] = da2; bs[4 * jj + 3] = da3;
+                    if (valid) p.dc[o] = dcv * gf;
+                    if (L0) {
+#pragma unroll
+                        for (int cc = 0; cc < kC; ++cc)
+                            if (CIN == 1 || cc < p.c_in) {
+                                // W_ih is stored pre-scaled: undo -log2(e) (and the g gate's extra factor 2)
+                                const float4 wv = *reinterpret_cast<const float4*>(&wih_s[cc * kGateCols + col]);
+                                dxs[cc] = fmaf(da0 * wv.x + da1 * wv.y + 0.5f * (da2 * wv.z) + da3 * wv.w, -0.6931471805599453f, dxs[cc]);
+                            }
+                    }
+                    split_bf16x2(da0, da1, dpk[4 * j], dpk[4 * j + 2]);
+                    split_bf16x2(da2, da3, dpk[4 * j + 1], dpk[4 * j + 3]);
+                }
+                // ---- B_c: db[chunk] += column sums of dA_c (rows past the end carry dA = 0) ----
+                // Lanes l ^ 1, ^ 4, ^ 8, ^ 16 hold the same units in other rows.  A reduce-scatter over those 16 lanes
+                // halves the list at each step; afterwards lane l holds the sum of bs[i0] for i0 = 8 b0 + 4 b2 + 2 b3 + b4
+                // (b = the bits of l), i.e. cell 4h + i0 / 4 (unit 16c + 2 (4h + i0 / 4) + q/2), gate i0 % 4.
+                col_sums_step<8>(bs, 1, lane);
+                col_sums_step<4>(bs, 4, lane);
+                col_sums_step<2>(bs, 8, lane);
+                col_sums_step<1>(bs, 16, lane);
+                const int i0 = 8 * (lane & 1) + 4 * ((lane >> 2) & 1) + 2 * ((lane >> 3) & 1) + ((lane >> 4) & 1);
+                atomicAdd(&tail->db[4 * (16 * c + 2 * (4 * h + (i0 >> 2)) + (q >> 1)) + (i0 & 3)], bs[0]);
+            }
+        };
+        // dpk -> the shared dA tile, once both warpgroups' W / D of the previous chunk have read it
+        auto store_da = [&]() {
+            cons_sync(kCons);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const float4 v = frag_to_gates(g, j, odd);
-                const int unit = 16 * c + 2 * j + (q >> 1);
-                const int col = 4 * unit;
-                const float4 bv = *reinterpret_cast<const float4*>(p.bias + col);     // scaled here (gate_scale)
-                const float4 a = gate_args<CIN>(v, make_float4(bv.x * -1.4426950408889634f, bv.y * -1.4426950408889634f,
-                                                               bv.z * -2.8853900817779268f, bv.w * -1.4426950408889634f),
-                                                xs, wih_s, col, p.c_in);
-                const uint32_t o = bo + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
-                const float cp = cpv[j], dh = dhv[j], dci = dciv[j];
-                float gi, gf, gg, go, tc_;
-                lstm_cell_gates8(a.x, a.y, a.z, a.w, cp, gi, gf, gg, go, tc_);
-                // rows past the end: dh = dci = 0, so dA = 0
-                const float dcv = fmaf(dh * go, 1.f - tc_ * tc_, dci);
-                const float da0 = dcv * gg * gi * (1.f - gi);
-                const float da1 = dcv * cp * gf * (1.f - gf);
-                const float da2 = dcv * gi * (1.f - gg * gg);
-                const float da3 = dh * tc_ * go * (1.f - go);
-                bs[4 * j + 0] = da0; bs[4 * j + 1] = da1; bs[4 * j + 2] = da2; bs[4 * j + 3] = da3;
-                if (valid) p.dc[o] = dcv * gf;
-                if (L0) {
-#pragma unroll
-                    for (int cc = 0; cc < kC; ++cc)
-                        if (CIN == 1 || cc < p.c_in) {
-                            // W_ih is stored pre-scaled: undo -log2(e) (and the g gate's extra factor 2)
-                            const float4 wv = *reinterpret_cast<const float4*>(&wih_s[cc * kGateCols + col]);
-                            dxs[cc] = fmaf(da0 * wv.x + da1 * wv.y + 0.5f * (da2 * wv.z) + da3 * wv.w, -0.6931471805599453f, dxs[cc]);
-                        }
-                }
-                split_bf16x2(da0, da1, dhi[j], dlo[j]);
-                uint32_t h2, l2;
-                split_bf16x2(da2, da3, h2, l2);
                 const uint32_t off = row_in_tile * 128u + ((((uint32_t)j) ^ (row_in_tile & 7u)) << 4) + (uint32_t)(q >> 1) * 8u;
-                if (j == 0) cons_sync(kCons);                      // W / D of the previous chunk have read the dA tile
-                *reinterpret_cast<uint2*>(da_sm + off) = make_uint2(dhi[j], h2);
-                *reinterpret_cast<uint2*>(da_sm + kATileBytes + off) = make_uint2(dlo[j], l2);
-            }
-            // ---- B_c: db[chunk] += column sums of dA_c (rows past the end carry dA = 0) ----
-            // Lanes l ^ 1, ^ 4, ^ 8, ^ 16 hold the same units in other rows.  A reduce-scatter over those 16 lanes halves
-            // the list at each step; afterwards lane l holds the sums of bs[i0], bs[i0 + 1] for
-            // i0 = 16 b0 + 8 b2 + 4 b3 + 2 b4 (b = the bits of l), i.e. unit 2 (i0 / 4) + q/2 of the chunk, gates i0 % 4 + {0, 1}.
-            col_sums_step<16>(bs, 1, lane);
-            col_sums_step<8>(bs, 4, lane);
-            col_sums_step<4>(bs, 8, lane);
-            col_sums_step<2>(bs, 16, lane);
-            {
-                const int i0 = 16 * (lane & 1) + 8 * ((lane >> 2) & 1) + 4 * ((lane >> 3) & 1) + 2 * ((lane >> 4) & 1);
-                const int col = 64 * c + 4 * (2 * (i0 >> 2) + (q >> 1)) + (i0 & 3);
-                atomicAdd(&tail->db[col], bs[0]);
-                atomicAdd(&tail->db[col + 1], bs[1]);
+                *reinterpret_cast<uint2*>(da_sm + off) = make_uint2(dpk[4 * j], dpk[4 * j + 1]);
+                *reinterpret_cast<uint2*>(da_sm + kATileBytes + off) = make_uint2(dpk[4 * j + 2], dpk[4 * j + 3]);
             }
             fence_proxy_async_smem();
             cons_sync(kCons);                                      // the dA tile (both row halves) is complete
-            // ---- W_c: dWp[kd rows 64 wg .., chunk] = A^T . dA_c ----
-            float wgr[32];
-#pragma unroll
-            for (int k = 0; k < 32; ++k) wgr[k] = 0.f;
+        };
+        // ---- chunk 0: R_0 alone ----
+        {
+            float g[32];                                           // (the first wgmma of R overwrites: scale-d 0)
+            wg_fence_regs(g);
+            wg_fence();
+            bwd_recompute_mma<PLANES, kNseg>(g, a_u, a_rows, w_u, 0);
+            wg_commit();
+            load_cells(0);
+            wg_wait<0>();
+            wg_fence_regs(g);
+            cell_epilogue(0, g);
+            store_da();
+        }
+        // ---- chunks 1..3, software-pipelined: R_c and W_{c-1} + D_{c-1} are committed as two groups; waiting for the
+        // first retires R_c only, so P_c runs on the CUDA cores while the tensor pipe still works on chunk c - 1.  The dA
+        // tile holds dA_{c-1} until W / D of both warpgroups have read it, so dA_c waits in registers (dpk) until then.
+        // (The loop is not unrolled, and no wgmma is behind a branch: either makes ptxas serialise the wgmma.)
+#pragma unroll 1
+        for (int c = 1; c < 4; ++c) {
+            float g[32];
+            wg_fence_regs(g);
             wg_fence_regs(wgr);
             wg_fence_regs(dacc);
             wg_fence();
-            {
-                const uint32_t wa_hi = a_u + (uint32_t)(wg * 2) * kATileBytes, wa_lo = wa_hi + kATileBytes;
-#pragma unroll
-                for (int ks = 0; ks < 8; ++ks) {
-                    const uint64_t ah = desc16_mn(wa_hi + ks * kStepMN, kATileBytes);
-                    const uint64_t al = desc16_mn(wa_lo + ks * kStepMN, kATileBytes);
-                    const uint64_t bh = desc16_mn(da_u + ks * kStepMN, kATileBytes);
-                    const uint64_t bl = desc16_mn(da_u + kATileBytes + ks * kStepMN, kATileBytes);
-                    // dA always has its lo plane; in the single-plane mode only the STORED operands are rounded to bf16.
-                    // Layer 0's warpgroup 1 multiplies the auxiliary x*s tile, which is not stored: it keeps its lo plane in
-                    // both modes, as the forward's fp32 FMAs do (warpgroup 0's lo slot is zero then, and adds nothing; both
-                    // warpgroups issue the pass so that no wgmma sits on a warpgroup-dependent branch, which would make
-                    // ptxas serialise every wgmma of the kernel)
-                    wgmma_bf16_n64_t11(wgr, ah, bh, ks > 0 ? 1u : 0u);
-                    wgmma_bf16_n64_t11(wgr, ah, bl, 1u);
-                    if (PLANES == 2 || L0) wgmma_bf16_n64_t11(wgr, al, bh, 1u);
-                }
-            }
-            // ---- D_c: [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T ----
-            {
-                const uint64_t ah = desc16_k(da_u + a_rows), al = desc16_k(da_u + kATileBytes + a_rows);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    const uint32_t wb = w_u + (uint32_t)c * 8192u + (uint32_t)kk * kStepMN;
-                    const uint64_t bh = desc16_mn(wb, 2 * kWTileBytes), bl = desc16_mn(wb + kWTileBytes, 2 * kWTileBytes);
-                    if constexpr (kNseg == 2) {
-                        wgmma_bf16_n128_t01(dacc, ah + 2 * kk, bh, 1u);
-                        if (PLANES == 2) wgmma_bf16_n128_t01(dacc, ah + 2 * kk, bl, 1u);
-                        wgmma_bf16_n128_t01(dacc, al + 2 * kk, bh, 1u);
-                    } else {
-                        wgmma_bf16_n64_t01(dacc, ah + 2 * kk, bh, 1u);
-                        if (PLANES == 2) wgmma_bf16_n64_t01(dacc, ah + 2 * kk, bl, 1u);
-                        wgmma_bf16_n64_t01(dacc, al + 2 * kk, bh, 1u);
-                    }
-                }
-            }
+            bwd_recompute_mma<PLANES, kNseg>(g, a_u, a_rows, w_u, c);
             wg_commit();
+            bwd_wgrad_mma<PLANES, L0>(wgr, wa_u, da_u);
+            bwd_dgrad_mma<PLANES, kNseg>(dacc, da_u, a_rows, w_u, c - 1);
+            wg_commit();
+            load_cells(c);
+            wg_wait<1>();
+            wg_fence_regs(g);
+            cell_epilogue(c, g);
             wg_wait<0>();
             wg_fence_regs(wgr);
             wg_fence_regs(dacc);
-            // weight-gradient fragment -> this CTA's slice (row-major [kd][256])
-            {
-                const uint32_t m0 = rw0;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const uint32_t n = (uint32_t)(64 * c + 8 * j + 2 * q);
-                    red_add_f32x2(slice + (size_t)m0 * kGateCols + n, wgr[4 * j], wgr[4 * j + 1]);
-                    red_add_f32x2(slice + (size_t)(m0 + 8) * kGateCols + n, wgr[4 * j + 2], wgr[4 * j + 3]);
-                }
-            }
+            bwd_wgrad_red(slice, wgr, rw0, q, c - 1);
+            store_da();
         }
+        // ---- chunk 3's gradients: W_3 alone first, so that the A planes go back to the producer before D_3 is done ----
+        wg_fence_regs(wgr);
+        wg_fence_regs(dacc);
+        wg_fence();
+        bwd_wgrad_mma<PLANES, L0>(wgr, wa_u, da_u);
+        wg_commit();
+        bwd_dgrad_mma<PLANES, kNseg>(dacc, da_u, a_rows, w_u, 3);
+        wg_commit();
+        wg_wait<1>();
+        wg_fence_regs(wgr);
         // the A planes of this item have been read by every MMA: one arrival per warpgroup
         asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
         if ((tid & 127) == 0) mbar_arrive(&tail->a_empty);
+        bwd_wgrad_red(slice, wgr, rw0, q, 3);
+        wg_wait<0>();
+        wg_fence_regs(dacc);
         // ---- [dx_below | dh_prev] fragment -> tile-blocked workspaces ----
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
