@@ -33,7 +33,16 @@ int32_t ensure_dyn_smem(const void* kernel, size_t bytes);   // per-(kernel, dev
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// ---- persistent schedule: `work` tiles dealt round-robin over at most one CTA per SM; this CTA's count and i-th tile --
+static inline int persistent_grid(int64_t work) { return (int)(work < sm_count() ? work : sm_count()); }
+__device__ __forceinline__ int cta_tiles(int n_tiles) { return (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x; }
+__device__ __forceinline__ int cta_tile(int i) { return (int)blockIdx.x + i * (int)gridDim.x; }
+
 // ---- device helpers ---------------------------------------------------------------------------------
+// exponent factors of the activations, e^-v = 2^(kNegLog2e v) and e^-2v = 2^(kNeg2Log2e v), and ln 2, which undoes them
+constexpr float kNegLog2e = -1.4426950408889634f;
+constexpr float kNeg2Log2e = -2.8853900817779268f;
+constexpr float kLn2 = 0.6931471805599453f;
 // sigmoid / tanh on the MUFU pipe: ex2.approx + rcp.approx (~2 ulp each); absolute error < 1e-6, far inside
 // the 1e-4 parity budget, and 2 MUFU + 3 FP32 ops per value instead of an IEEE division sequence.
 // Written with the .ftz MUFU forms directly: __expf / __fdividef wrap the same instructions in denormal-range fix-ups
@@ -49,10 +58,8 @@ __device__ __forceinline__ float rcp_ftz_(float x) {
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-__device__ __forceinline__ float sigmoidf_(float v) { return rcp_ftz_(1.0f + ex2_ftz_(-1.4426950408889634f * v)); }
-__device__ __forceinline__ float tanhf_(float v) {
-    return fmaf(2.0f, rcp_ftz_(1.0f + ex2_ftz_(-2.8853900817779268f * v)), -1.0f);
-}
+__device__ __forceinline__ float sigmoidf_(float v) { return rcp_ftz_(1.0f + ex2_ftz_(kNegLog2e * v)); }
+__device__ __forceinline__ float tanhf_(float v) { return fmaf(2.0f, rcp_ftz_(1.0f + ex2_ftz_(kNeg2Log2e * v)), -1.0f); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

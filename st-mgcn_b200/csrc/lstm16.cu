@@ -34,36 +34,12 @@ constexpr int kMaxC = 4;
 constexpr int kWTileBytes = kGateCols * 128;          // [256 gate cols][64 k] bf16 = 32 KB
 constexpr int kATileBytes = kTile16Bytes;             // [128 rows][64 k] bf16 = 16 KB
 
-// element (row r, unit u) of a tile-blocked (rows_pad x 64) fp32 workspace lives at
-//   (((r >> 7) * 16 + (unit >> 2)) * 128 + (r & 127)) * 4 + (unit & 3)        (host side: ops.to_blocked / from_blocked)
-
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, int c0, int c1, int c2, uint64_t* bar) {
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-                 :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+// Tile-blocked (rows_pad x 64) fp32 workspaces (cs, c0, dh, dc, dx): [tile][unit / 4][128 rows][4 units], a tile one 32 KB
+// run.  Offset of (row of tile, unit), and the size of a (layer, step) slice.  Host side: ops.to_blocked / from_blocked.
+__host__ __device__ __forceinline__ uint32_t blocked_off(uint32_t tile, uint32_t row, uint32_t unit) {
+    return tile * 8192u + (unit >> 2) * 512u + row * 4u + (unit & 3u);
 }
-
-// L2 policy for data a launch reads exactly once (the backward's A planes, c_prev, dh_in): evicted first, so that the
-// lines read again -- the recurrent dh_rec / dc, the weight-gradient slices -- keep their place in L2
-__device__ __forceinline__ uint64_t l2_evict_first() {
-    uint64_t pol;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    return pol;
-}
-__device__ __forceinline__ void tma_load_3d_hint(void* smem_dst, const void* tmap, int c0, int c1, int c2, uint64_t* bar,
-                                                 uint64_t pol) {
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
-                 " [%0], [%1, {%3, %4, %5}], [%2], %6;"
-                 :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_3d(const void* tmap, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
-                 :: "l"(tmap), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ float ld_hint(const float* p, uint64_t pol) {
-    float v;
-    asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
-    return v;
-}
+__host__ __device__ __forceinline__ int64_t blocked_slice(int n_tiles) { return (int64_t)n_tiles * kTileM * kHid; }
 
 // ---- LSTM cell with 8 MUFU operations instead of 10 ------------------------------------------------------------
 // sigmoid(v) = 1 / (1 + e^-v), tanh(v) = (1 - e^-2v) / (1 + e^-2v).  Five exponentials per cell are unavoidable (i, f, g, o,
@@ -72,16 +48,16 @@ __device__ __forceinline__ float ld_hint(const float* p, uint64_t pol) {
 // product of two (1 + e^30) terms stays far below the fp32 overflow threshold.  The cell epilogue is MUFU-bound
 // (16 MUFU results per clock and SM), so this is 20 % off its critical resource.
 // (one-sided: only a large NEGATIVE argument makes e^-v large; for large positive v the exponential underflows to 0, which is exact)
-// The kernels keep bias and W_ih PRE-SCALED by the exponent factor of their gate (kGateScale: -log2(e) for i, f, o and
-// -2 log2(e) for g), so "accumulator + bias, times -log2(e)" is ONE fma per gate: arg = fma(acc, scale, bias_scaled).
-__device__ __forceinline__ float gate_scale(int col) { return (col & 3) == 2 ? -2.8853900817779268f : -1.4426950408889634f; }
+// The kernels keep bias and W_ih PRE-SCALED by the exponent factor of their gate (gate_scale: kNegLog2e for i, f, o and
+// kNeg2Log2e for g), so "accumulator + bias, times -log2(e)" is ONE fma per gate: arg = fma(acc, scale, bias_scaled).
+__device__ __forceinline__ float gate_scale(int col) { return (col & 3) == 2 ? kNeg2Log2e : kNegLog2e; }
 __device__ __forceinline__ float exp_arg_(float a) { return ex2_ftz_(fminf(a, 43.28f)); }      // e^(-v) or e^(-2v), <= e^30
 // forward: exponent arguments of (i, f, g, o) and c_{t-1} -> c_t, h_t
 __device__ __forceinline__ void lstm_cell_fwd8(float ai, float af, float ag, float ao, float cp, float& c, float& h) {
     const float ei = exp_arg_(ai), ef = exp_arg_(af), eg = exp_arg_(ag), eo = exp_arg_(ao);
     const float ig = (1.f - eg) * rcp_ftz_((1.f + ei) * (1.f + eg));          // sigmoid(pi) * tanh(pg)
     c = fmaf(rcp_ftz_(1.f + ef), cp, ig);
-    const float ec = exp_arg_(-2.8853900817779268f * c);
+    const float ec = exp_arg_(kNeg2Log2e * c);
     h = (1.f - ec) * rcp_ftz_((1.f + eo) * (1.f + ec));                      // sigmoid(po) * tanh(c)
 }
 // backward recompute: all four gate activations, c_t and tanh(c_t)
@@ -95,7 +71,7 @@ __device__ __forceinline__ void lstm_cell_gates8(float ai, float af, float ag, f
     gg = (1.f - eg) * (r1 * ei);
     gf = r2 * eo;
     go = r2 * ef;
-    const float ec = exp_arg_(-2.8853900817779268f * fmaf(gf, cp, gi * gg));
+    const float ec = exp_arg_(kNeg2Log2e * fmaf(gf, cp, gi * gg));
     tc = (1.f - ec) * rcp_ftz_(1.f + ec);
 }
 
@@ -115,8 +91,8 @@ __device__ __forceinline__ float4 frag_to_gates(const float (&d)[R], int j, bool
 template <int CIN>
 __device__ __forceinline__ float4 gate_args(float4 v, float4 b, const float (&xs)[kMaxC], const float* wih, int col, int c_in) {
     constexpr int kC = (CIN == 1) ? 1 : kMaxC;
-    float4 a = make_float4(fmaf(v.x, -1.4426950408889634f, b.x), fmaf(v.y, -1.4426950408889634f, b.y),
-                           fmaf(v.z, -2.8853900817779268f, b.z), fmaf(v.w, -1.4426950408889634f, b.w));
+    float4 a = make_float4(fmaf(v.x, kNegLog2e, b.x), fmaf(v.y, kNegLog2e, b.y), fmaf(v.z, kNeg2Log2e, b.z),
+                           fmaf(v.w, kNegLog2e, b.w));
     if (CIN > 0) {
 #pragma unroll
         for (int c = 0; c < kC; ++c)
@@ -127,6 +103,15 @@ __device__ __forceinline__ float4 gate_args(float4 v, float4 b, const float (&xs
             }
     }
     return a;
+}
+
+// producer: the layer's resident weight image p.wimg (tiles seg * 2 + plane of kWTileBytes) -> shared memory, on bar
+template <int NSEG, int PLANES, class Params>
+__device__ __forceinline__ void load_weights(uint8_t* w_sm, const Params& p, uint64_t* bar) {
+    mbar_arrive_expect_tx(bar, (uint32_t)(NSEG * PLANES * kWTileBytes));
+    for (int s = 0; s < NSEG; ++s)
+        for (int pl = 0; pl < PLANES; ++pl)
+            bulk_g2s(w_sm + (size_t)(s * 2 + pl) * kWTileBytes, p.wimg + (size_t)(s * 2 + pl) * kWTileBytes, kWTileBytes, bar);
 }
 
 // =====================================================================================================
@@ -152,6 +137,7 @@ __device__ __forceinline__ float4 gate_args(float4 v, float4 b, const float (&xs
 // cell (r0 + 8, unit).
 constexpr int kFWarpgroups = 2;
 constexpr int kFThreads = kFWarpgroups * 128 + 32;     // + producer warp
+constexpr uint32_t kFBarWg = 1;                        // named barrier kFBarWg + w: warpgroup w (128 threads)
 constexpr int kHTileBytes = 64 * 128;                  // one plane of a warpgroup's rows: [64 rows][64] bf16 = 8 KB
 constexpr int kFWgBytes = 4 * kHTileBytes;             // per warpgroup: h_prev hi | lo, h_below stage hi | lo
 constexpr int kFCBytes = 64 * kHid * 4;                // per warpgroup: fp32 c of its rows, [32 cells j][128 threads]
@@ -201,8 +187,6 @@ __device__ __forceinline__ void fwd_segment_mma(float (&acc)[128], uint32_t a_u,
     }
 }
 
-__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
-
 // CIN: 0 = not layer 0; 1 = layer 0 with one input channel (the reference's input_dim, compile-time: no predicated-off
 // W_ih FMAs / loads in the cell loop); kMaxC = layer 0 with a runtime channel count <= kMaxC
 template <int PLANES, int CIN>
@@ -211,7 +195,7 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
     constexpr int kC = (CIN == 1) ? 1 : kMaxC;
     constexpr int kNseg = L0 ? 1 : 2;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
     uint8_t* wsm = smem;                                           // resident weight tiles (seg*2 + plane)
     uint8_t* hsm = smem + 4 * (size_t)kWTileBytes;                 // per warpgroup: kFWgBytes
     uint8_t* csm = hsm + kFWarpgroups * (size_t)kFWgBytes;         // per warpgroup: kFCBytes
@@ -236,17 +220,13 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
     if (L0)
         for (int i = tid; i < p.c_in * kGateCols; i += kFThreads) wih_s[i] = p.wih[i] * gate_scale(i);
     __syncthreads();
-    const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    const int my_tiles = cta_tiles(p.n_tiles);
 
     if (warp == kProdWarp) {
         // ===================== producer: resident weights once, then h_below of every (tile, step) =====================
         const bool leader = elect_one_sync();
         if (leader && my_tiles > 0) {
-            mbar_arrive_expect_tx(&tail->w_full, (uint32_t)(kNseg * PLANES * kWTileBytes));
-            for (int s = 0; s < kNseg; ++s)
-                for (int pl = 0; pl < PLANES; ++pl)
-                    bulk_g2s(wsm + (size_t)(s * 2 + pl) * kWTileBytes, p.wimg + (size_t)(s * 2 + pl) * kWTileBytes, kWTileBytes,
-                             &tail->w_full);
+            load_weights<kNseg, PLANES>(wsm, p, &tail->w_full);
             if (!L0) {
                 // the warpgroups drift apart: serve whichever has released its stage instead of alternating
                 const int n_loads = my_tiles * p.t_len;
@@ -259,7 +239,7 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
                         const int n = done[w];
                         if (n < n_loads && mbar_try_wait(&tail->empty[w], (uint32_t)(n & 1) ^ 1u)) {
                             const int i = n / p.t_len, t = n - i * p.t_len;
-                            const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * kTileM + 64 * w;
+                            const int row0 = cta_tile(i) * kTileM + 64 * w;
                             uint8_t* stage = hsm + (size_t)w * kFWgBytes + 2 * (size_t)kHTileBytes;
                             mbar_arrive_expect_tx(&tail->full[w], (uint32_t)(PLANES * kHTileBytes));
                             for (int pl = 0; pl < PLANES; ++pl)
@@ -292,22 +272,22 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
     // c of this thread's 32 cells: element 128 j (thread-major: conflict free; only the owning thread touches it)
     float* c_sm = reinterpret_cast<float*>(csm + (size_t)wg * kFCBytes) + (tid & 127);
     const uint32_t w_u = smem_u32(wsm), h_u = smem_u32(h_sm), b_u = h_u + 2u * kHTileBytes;
-    const int64_t cslice = (int64_t)p.n_tiles * kTileM * kHid;
+    const int64_t cslice = blocked_slice(p.n_tiles);
     float acc[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     mbar_wait_raw(&tail->w_full, 0);
     uint32_t n_below = 0;                                          // h_below stages consumed
     for (int i = 0; i < my_tiles; ++i) {
-        const int tile = (int)blockIdx.x + i * (int)gridDim.x;
+        const int tile = cta_tile(i);
         const int row0 = tile * kTileM + 64 * wg;                  // first row of this warpgroup
         const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
         const bool valid = r < rows32;
-        const uint32_t cbase = (uint32_t)tile * 8192u + row_in_tile * 4u;
+        const uint32_t cbase = blocked_off(tile, row_in_tile, 0);    // this thread's row; unit u is + blocked_off(0, 0, u)
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
             const int unit = 2 * j + (q >> 1);
-            c_sm[128 * j] = (p.c0 != nullptr && valid) ? p.c0[cbase + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3)] : 0.f;
+            c_sm[128 * j] = (p.c0 != nullptr && valid) ? p.c0[cbase + blocked_off(0, 0, unit)] : 0.f;
         }
         if (p.has_h0) {
             if (issuer) {
@@ -354,7 +334,7 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
             // every warp's wgmma have read the operands, and the store of h_{t-1} has read the h_prev tiles: the stage
             // goes back to the producer, and the tiles may be overwritten
             if (issuer) bulk_wait_group_read0();
-            wg_sync(wg);
+            bar_sync(kFBarWg + wg, 128);
             if (!L0) {
                 if (issuer) mbar_arrive(&tail->empty[wg]);
                 ++n_below;
@@ -369,7 +349,7 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
                 const int col = 4 * unit;
                 const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
                 const float4 a = gate_args<CIN>(v, bv, xs, wih_s, col, p.c_in);
-                const uint32_t co = cbase + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
+                const uint32_t co = cbase + blocked_off(0, 0, unit);
                 float cn, hn;
                 lstm_cell_fwd8(a.x, a.y, a.z, a.w, c_sm[128 * j], cn, hn);
                 c_sm[128 * j] = cn;
@@ -378,14 +358,14 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
                     if (h_f32 != nullptr) h_f32[r * (uint32_t)kHid + (uint32_t)unit] = hn;
                 }
                 // rows past the end are computed too (a row's gates depend on that row alone) and dropped by the store
-                const uint32_t off = sw128_off16(row_in_wg, (uint32_t)unit);
+                const uint32_t off = sw128<2>(row_in_wg, (uint32_t)unit);
                 const __nv_bfloat16 hb = __float2bfloat16_rn(hn);
                 *reinterpret_cast<__nv_bfloat16*>(h_sm + off) = hb;
                 if (PLANES == 2) *reinterpret_cast<__nv_bfloat16*>(h_sm + kHTileBytes + off) = __float2bfloat16_rn(hn - __bfloat162float(hb));
             }
             // h_t -> the async proxy (the store below, the next step's wgmma)
             fence_proxy_async_smem();
-            wg_sync(wg);
+            bar_sync(kFBarWg + wg, 128);
             if (issuer) {
                 for (int pl = 0; pl < PLANES; ++pl)
                     tma_store_3d(&p.hp_map, h_sm + (size_t)pl * kHTileBytes, 0, row0, (p.layer * p.t_len + t) * PLANES + pl);
@@ -411,7 +391,7 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
         const float v = src[(int64_t)nat * kHid + k];
         const __nv_bfloat16 h = __float2bfloat16_rn(v);
         const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
-        const uint32_t off = sw128_off16((uint32_t)n, (uint32_t)k);
+        const uint32_t off = sw128<2>((uint32_t)n, (uint32_t)k);
         *reinterpret_cast<__nv_bfloat16*>(wimg + (size_t)(s * 2) * kWTileBytes + off) = h;
         *reinterpret_cast<__nv_bfloat16*>(wimg + (size_t)(s * 2 + 1) * kWTileBytes + off) = l;
     }
@@ -452,6 +432,9 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
 // launch and writes nn.LSTM-native gradients.
 constexpr int kBWarpgroups = 2;
 constexpr int kBThreads = kBWarpgroups * 128 + 128;     // + producer warpgroup (one thread of it issues the loads)
+constexpr int kBCons = kBWarpgroups * 128;              // consumer threads
+constexpr uint32_t kBBarCons = 1;                       // named barrier of the consumer warpgroups (kBCons threads)
+constexpr uint32_t kBBarWg = 2;                         // named barrier kBBarWg + w: consumer warpgroup w (128 threads)
 // registers per thread after setmaxnreg: 256 * 240 + 128 * 24 = 64 512 of the SM's 65 536 (launched at 384 * 168)
 constexpr uint32_t kBConsRegs = 240, kBProdRegs = 24;
 constexpr int kBATiles = 4;                             // (seg0 | seg1) x (hi | lo); layer 0: seg 1 = the auxiliary [x*s] tile
@@ -499,11 +482,6 @@ struct Bwd16Params {
     Bwd16Step steps[kBMaxSteps];   // in execution order: steps[0] is t = T-1
 };
 static_assert(sizeof(Bwd16Params) <= 4096, "kernel parameter block exceeds 4 KB");
-
-__device__ __forceinline__ void cons_sync(int n_threads) { asm volatile("bar.sync 1, %0;" ::"r"(n_threads) : "memory"); }
-// a warpgroup's per-thread register budget (every warp of the warpgroup executes the same instruction)
-template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // R_c: g = [h_below | h_prev] . Wp[:, chunk c] of this warpgroup's 64 rows
 template <int PLANES, int NSEG>
@@ -597,7 +575,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     constexpr int kC = (CIN == 1) ? 1 : kMaxC;
     constexpr int kNseg = L0 ? 1 : 2;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
     uint8_t* w_sm = smem;                                          // resident weights: tiles (seg*2 + plane) of 32 KB
     uint8_t* a_sm = w_sm + 4 * (size_t)kWTileBytes;                // A planes: tiles (seg*2 + plane) of 16 KB
     uint8_t* da_sm = a_sm + kBATiles * (size_t)kATileBytes;        // dA chunk: hi tile | lo tile
@@ -608,7 +586,6 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     const int warp = tid >> 5;
     const int lane = tid & 31;
     constexpr int kProdWarp = kBWarpgroups * 4;
-    constexpr int kCons = kBWarpgroups * 128;
 
     if (tid == 0) {
         mbar_init(&tail->a_full, 1);
@@ -629,7 +606,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     }
     fence_proxy_async_smem();
     __syncthreads();
-    const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    const int my_tiles = cta_tiles(p.n_tiles);
     const int n_items = my_tiles * p.n_steps;                      // work items (step, tile), tile-major
 
     if (warp >= kProdWarp) {
@@ -637,14 +614,10 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         setmaxnreg_dec<kBProdRegs>();
         const bool leader = warp == kProdWarp && elect_one_sync();
         if (leader && n_items > 0) {
-            mbar_arrive_expect_tx(&tail->w_full, (uint32_t)(kNseg * PLANES * kWTileBytes));
-            for (int sg = 0; sg < kNseg; ++sg)
-                for (int pl = 0; pl < PLANES; ++pl)
-                    bulk_g2s(w_sm + (size_t)(sg * 2 + pl) * kWTileBytes, p.wimg + (size_t)(sg * 2 + pl) * kWTileBytes, kWTileBytes,
-                             &tail->w_full);
-            const uint64_t once = l2_evict_first();
+            load_weights<kNseg, PLANES>(w_sm, p, &tail->w_full);
+            const uint64_t once = l2_evict_first();          // the A planes; dh_rec / dc and the slices keep their L2 place
             for (int w = 0; w < n_items; ++w) {
-                const int ti = w / p.n_steps, st = w - ti * p.n_steps, tile = (int)blockIdx.x + ti * (int)gridDim.x;
+                const int ti = w / p.n_steps, st = w - ti * p.n_steps, tile = cta_tile(ti);
                 const Bwd16Step& sp = p.steps[st];
                 mbar_wait_polite(&tail->a_empty, (uint32_t)(w & 1) ^ 1u);
                 mbar_arrive_expect_tx(&tail->a_full, (uint32_t)(kNseg * PLANES * kATileBytes));
@@ -661,7 +634,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 if (sp.dh_in) prefetch_l2(sp.dh_in + o, kB);
                 // the next item's A planes -> L2, a whole item ahead of the load that waits for them
                 if (w + 1 < n_items) {
-                    const int ti1 = (w + 1) / p.n_steps, tile1 = (int)blockIdx.x + ti1 * (int)gridDim.x;
+                    const int ti1 = (w + 1) / p.n_steps, tile1 = cta_tile(ti1);
                     const Bwd16Step& sp1 = p.steps[w + 1 - ti1 * p.n_steps];
                     for (int sg = 0; sg < kNseg; ++sg)
                         for (int pl = 0; pl < PLANES; ++pl)
@@ -684,11 +657,10 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     const uint32_t a_rows = (uint32_t)wg * 64u * 128u;             // this warpgroup's rows inside a 128-row tile
     const uint32_t wa_u = a_u + (uint32_t)(wg * 2) * kATileBytes;  // W_c's A operand: this warpgroup's kd rows
     float* slice = p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols);
-    const uint64_t once = l2_evict_first();
     mbar_wait_raw(&tail->w_full, 0);
 
     for (int w = 0; w < n_items; ++w) {
-        const int ti = w / p.n_steps, st = w - ti * p.n_steps, tile = (int)blockIdx.x + ti * (int)gridDim.x;
+        const int ti = w / p.n_steps, st = w - ti * p.n_steps, tile = cta_tile(ti);
         const Bwd16Step& sp = p.steps[st];
         const uint32_t r = (uint32_t)tile * kTileM + row_in_tile;
         const bool valid = r < rows32;
@@ -703,13 +675,13 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             }
         }
         // the previous item's stores (dh_rec, dc of other threads' cells) and its reads of the shared tiles are complete
-        cons_sync(kCons);
+        bar_sync(kBBarCons, kBCons);
         if (L0 && (q >> 1) == 0) {
             // auxiliary weight-gradient operand (seg-1 slots): row = this thread's row, columns 0..C-1 = x*s (hi / lo split)
             uint32_t hi[2], lo[2];
             split_bf16x2(xs[0], xs[1], hi[0], lo[0]);
             split_bf16x2(xs[2], xs[3], hi[1], lo[1]);
-            const uint32_t off = row_in_tile * 128u + ((0u ^ (row_in_tile & 7u)) << 4);
+            const uint32_t off = sw128<2>(row_in_tile, 0);
             *reinterpret_cast<uint2*>(a_sm + 2 * (size_t)kATileBytes + off) = make_uint2(hi[0], hi[1]);
             *reinterpret_cast<uint2*>(a_sm + 3 * (size_t)kATileBytes + off) = make_uint2(lo[0], lo[1]);
         }
@@ -718,7 +690,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
 #pragma unroll
         for (int k = 0; k < 32 * kNseg; ++k) dacc[k] = 0.f;
         float wgr[32];                                             // W of the previous chunk, in flight during P_c
-        const uint32_t bo = (uint32_t)tile * 8192u + row_in_tile * 4u;
+        const uint32_t bo = blocked_off(tile, row_in_tile, 0);     // this thread's row; unit u is + blocked_off(0, 0, u)
         float cpv[8], dhv[8], dciv[8];
         // the cells' global inputs of chunk c, all issued while the tensor pipe runs: each cell loading its own after
         // the previous cell's dc store (which they may alias, as far as the compiler knows) waited one memory round
@@ -727,7 +699,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int unit = 16 * c + 2 * j + (q >> 1);
-                const uint32_t o = bo + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
+                const uint32_t o = bo + blocked_off(0, 0, unit);
                 cpv[j] = (valid && sp.c_prev) ? __ldcs(sp.c_prev + o) : 0.f;
                 dhv[j] = (valid && sp.dh_in) ? __ldcs(sp.dh_in + o) : 0.f;
                 const bool rec = valid && !sp.first;
@@ -748,10 +720,10 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                     const int unit = 16 * c + 2 * j + (q >> 1);
                     const int col = 4 * unit;
                     const float4 bv = *reinterpret_cast<const float4*>(p.bias + col);     // scaled here (gate_scale)
-                    const float4 a = gate_args<CIN>(v, make_float4(bv.x * -1.4426950408889634f, bv.y * -1.4426950408889634f,
-                                                                   bv.z * -2.8853900817779268f, bv.w * -1.4426950408889634f),
+                    const float4 a = gate_args<CIN>(v, make_float4(bv.x * kNegLog2e, bv.y * kNegLog2e, bv.z * kNeg2Log2e,
+                                                                   bv.w * kNegLog2e),
                                                     xs, wih_s, col, p.c_in);
-                    const uint32_t o = bo + (uint32_t)(unit >> 2) * 512u + (uint32_t)(unit & 3);
+                    const uint32_t o = bo + blocked_off(0, 0, unit);
                     const float cp = cpv[j], dh = dhv[j], dci = dciv[j];
                     float gi, gf, gg, go, tc_;
                     lstm_cell_gates8(a.x, a.y, a.z, a.w, cp, gi, gf, gg, go, tc_);
@@ -767,9 +739,9 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
 #pragma unroll
                         for (int cc = 0; cc < kC; ++cc)
                             if (CIN == 1 || cc < p.c_in) {
-                                // W_ih is stored pre-scaled: undo -log2(e) (and the g gate's extra factor 2)
+                                // W_ih is stored pre-scaled: undo kNegLog2e (and the g gate's extra factor 2)
                                 const float4 wv = *reinterpret_cast<const float4*>(&wih_s[cc * kGateCols + col]);
-                                dxs[cc] = fmaf(da0 * wv.x + da1 * wv.y + 0.5f * (da2 * wv.z) + da3 * wv.w, -0.6931471805599453f, dxs[cc]);
+                                dxs[cc] = fmaf(da0 * wv.x + da1 * wv.y + 0.5f * (da2 * wv.z) + da3 * wv.w, -kLn2, dxs[cc]);
                             }
                     }
                     split_bf16x2(da0, da1, dpk[4 * j], dpk[4 * j + 2]);
@@ -789,15 +761,15 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         };
         // dpk -> the shared dA tile, once both warpgroups' W / D of the previous chunk have read it
         auto store_da = [&]() {
-            cons_sync(kCons);
+            bar_sync(kBBarCons, kBCons);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const uint32_t off = row_in_tile * 128u + ((((uint32_t)j) ^ (row_in_tile & 7u)) << 4) + (uint32_t)(q >> 1) * 8u;
+                const uint32_t off = sw128<2>(row_in_tile, 4 * (2 * j + (q >> 1)));   // gates of unit 16c + 2j + q/2
                 *reinterpret_cast<uint2*>(da_sm + off) = make_uint2(dpk[4 * j], dpk[4 * j + 1]);
                 *reinterpret_cast<uint2*>(da_sm + kATileBytes + off) = make_uint2(dpk[4 * j + 2], dpk[4 * j + 3]);
             }
             fence_proxy_async_smem();
-            cons_sync(kCons);                                      // the dA tile (both row halves) is complete
+            bar_sync(kBBarCons, kBCons);                           // the dA tile (both row halves) is complete
         };
         // ---- chunk 0: R_0 alone ----
         {
@@ -849,7 +821,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         wg_wait<1>();
         wg_fence_regs(wgr);
         // the A planes of this item have been read by every MMA: one arrival per warpgroup
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+        bar_sync(kBBarWg + wg, 128);
         if ((tid & 127) == 0) mbar_arrive(&tail->a_empty);
         bwd_wgrad_red(slice, wgr, rw0, q, 3);
         wg_wait<0>();
@@ -867,6 +839,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 float* base = is_dx ? sp.dx_out : p.dh_rec;
                 if (base == nullptr || !(is_dx || sp.store_dh)) continue;
                 const int unit = col & 63;
+                // = blocked_off(tile, rr, unit), added to the pointer term by term (one 32-bit sum compiles differently)
                 *reinterpret_cast<float2*>(base + (uint32_t)tile * 8192u + (uint32_t)(unit >> 2) * 512u + rr * 4u + (uint32_t)(unit & 3)) =
                     make_float2(dacc[4 * j + 2 * h], dacc[4 * j + 2 * h + 1]);
             }
@@ -880,8 +853,8 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             if ((q >> 1) == 0 && valid) atomicAdd(&p.d_s[(int64_t)(r % (uint32_t)p.b_inner) * p.t_len + sp.t], contrib);
         }
     }
-    cons_sync(kCons);
-    for (int i = tid; i < kGateCols; i += kCons)
+    bar_sync(kBBarCons, kBCons);
+    for (int i = tid; i < kGateCols; i += kBCons)
         if (n_items > 0) atomicAdd(&p.dbp[i], tail->db[i]);
 }
 
@@ -971,18 +944,13 @@ static int32_t check_dims16(const char* who, int32_t t_len, int32_t n_layers, in
 // start of layer l's image in the flat wimg: layer 0 has one K segment (64 KB), every other layer two (128 KB)
 static int64_t wimg_off(int l) { return (int64_t)2 * kWTileBytes * (l == 0 ? 0 : 2 * l - 1); }
 
-// kernel variant for (planes, layer): cin = 0 (not layer 0), 1 (layer 0, one input channel), kMaxC (layer 0, runtime count)
-using FwdFn = void (*)(const Fwd16Params);
-using BwdFn = void (*)(const Bwd16Params);
-static FwdFn fwd_kernel_for(int planes, int l, int c_in) {
+// kernel(Int<PLANES>, Int<CIN>) for (planes, layer): CIN = 0 (not layer 0), 1 (layer 0, one input channel), else kMaxC
+template <int N> struct Int { static constexpr int value = N; };
+template <class Kernel>
+static auto kernel_for(Kernel kernel, int planes, int l, int c_in) {
     const int cin = l == 0 ? (c_in == 1 ? 1 : kMaxC) : 0;
-    if (planes == 2) return cin == 0 ? lstm16_fwd_kernel<2, 0> : (cin == 1 ? lstm16_fwd_kernel<2, 1> : lstm16_fwd_kernel<2, kMaxC>);
-    return cin == 0 ? lstm16_fwd_kernel<1, 0> : (cin == 1 ? lstm16_fwd_kernel<1, 1> : lstm16_fwd_kernel<1, kMaxC>);
-}
-static BwdFn bwd_kernel_for(int planes, int l, int c_in) {
-    const int cin = l == 0 ? (c_in == 1 ? 1 : kMaxC) : 0;
-    if (planes == 2) return cin == 0 ? lstm16_bwd_kernel<2, 0> : (cin == 1 ? lstm16_bwd_kernel<2, 1> : lstm16_bwd_kernel<2, kMaxC>);
-    return cin == 0 ? lstm16_bwd_kernel<1, 0> : (cin == 1 ? lstm16_bwd_kernel<1, 1> : lstm16_bwd_kernel<1, kMaxC>);
+    if (planes == 2) return cin == 1 ? kernel(Int<2>{}, Int<1>{}) : (cin == kMaxC ? kernel(Int<2>{}, Int<kMaxC>{}) : kernel(Int<2>{}, Int<0>{}));
+    return cin == 1 ? kernel(Int<1>{}, Int<1>{}) : (cin == kMaxC ? kernel(Int<1>{}, Int<kMaxC>{}) : kernel(Int<1>{}, Int<0>{}));
 }
 
 }  // namespace stmgcn
@@ -1007,8 +975,8 @@ extern "C" int32_t stmgcn_lstm16_fwd(int32_t t_len, int32_t n_layers, int64_t ro
     STMGCN_REQUIRE(h_n != nullptr || h_top != nullptr, STMGCN_ERR_ARG, "lstm16_fwd: h_top null");
     cudaStream_t st = (cudaStream_t)stream;
     const int n_tiles = (int)ceil_div(rows, kTileM);
-    const int64_t cslice = (int64_t)n_tiles * kTileM * kHid;
-    const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
+    const int64_t cslice = blocked_slice(n_tiles);
+    const int grid = persistent_grid(n_tiles);
     Fwd16Params p;
     memset(&p, 0, sizeof(p));
     // a warpgroup's 64 rows are one box: its h_below loads, h0 loads and tape stores
@@ -1023,7 +991,7 @@ extern "C" int32_t stmgcn_lstm16_fwd(int32_t t_len, int32_t n_layers, int64_t ro
     p.n_tiles = n_tiles;
     // bottom-up: layer l reads the hp planes of layer l - 1
     for (int l = 0; l < n_layers; ++l) {
-        const FwdFn fn = fwd_kernel_for(planes, l, c_in);
+        const auto fn = kernel_for([](auto P, auto C) { return lstm16_fwd_kernel<P.value, C.value>; }, planes, l, c_in);
         if (int32_t rc = ensure_dyn_smem((const void*)fn, kFSmem)) return rc;
         p.wimg = (const uint8_t*)wimg + wimg_off(l);
         p.bias = bias + (int64_t)l * kGateCols;
@@ -1039,10 +1007,7 @@ extern "C" int32_t stmgcn_lstm16_fwd(int32_t t_len, int32_t n_layers, int64_t ro
     return 0;
 }
 
-extern "C" int32_t stmgcn_lstm16_grid(int64_t rows) {
-    const int64_t n_tiles = ceil_div(rows, kTileM);
-    return (int32_t)(n_tiles < sm_count() ? n_tiles : sm_count());
-}
+extern "C" int32_t stmgcn_lstm16_grid(int64_t rows) { return persistent_grid(ceil_div(rows, kTileM)); }
 
 extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner,
                                      int32_t planes, const float* xo, const float* s_gate, const void* wimg,
@@ -1058,8 +1023,8 @@ extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t ro
     STMGCN_REQUIRE(n_layers == 1 || dx_work != nullptr, STMGCN_ERR_ARG, "lstm16_bwd: dx_work null with L=%d", n_layers);
     cudaStream_t st = (cudaStream_t)stream;
     const int n_tiles = (int)ceil_div(rows, kTileM);
-    const int64_t cslice = (int64_t)n_tiles * kTileM * kHid;
-    const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
+    const int64_t cslice = blocked_slice(n_tiles);
+    const int grid = persistent_grid(n_tiles);
     Bwd16Params p;
     memset(&p, 0, sizeof(p));
     if (int32_t rc = make_plane_maps("lstm16_bwd", &p.maps[0], &p.maps[1], hp, h0p, rows, n_layers, t_len, planes, kTileM))
@@ -1083,7 +1048,7 @@ extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t ro
     // top-down: layer l reads the dx that layer l + 1 wrote into one half of dx_work and writes its own into the other
     const float* dh_in = d_top;
     for (int l = n_layers - 1; l >= 0; --l) {
-        const BwdFn fn = bwd_kernel_for(planes, l, c_in);
+        const auto fn = kernel_for([](auto P, auto C) { return lstm16_bwd_kernel<P.value, C.value>; }, planes, l, c_in);
         if (int32_t rc = ensure_dyn_smem((const void*)fn, kBSmem)) return rc;
         float* dx_out = l > 0 ? dx_work + (int64_t)((n_layers - 1 - l) % 2) * t_len * cslice : nullptr;
         p.wimg = (const uint8_t*)wimg + wimg_off(l);

@@ -38,7 +38,7 @@ __device__ __forceinline__ void split_store_t(uint8_t* hi_tile, uint8_t* lo_tile
     const float vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-        const uint32_t off = sw128_offset((uint32_t)(mn + j), (uint32_t)k);
+        const uint32_t off = sw128<4>((uint32_t)(mn + j), (uint32_t)k);
         const float hi = tf32_hi(vv[j]);
         *reinterpret_cast<float*>(hi_tile + off) = hi;
         *reinterpret_cast<float*>(lo_tile + off) = tf32_lo(vv[j], hi);
@@ -57,7 +57,7 @@ __global__ void pack_image_kernel(const float* __restrict__ src, int n_rows, int
         const float hi = tf32_hi(v);
         const float lo = tf32_lo(v, hi);
         const int kb = k / kKB, kk = k % kKB;
-        const uint32_t off = sw128_offset((uint32_t)n, (uint32_t)kk) / 4;
+        const uint32_t off = sw128<4>((uint32_t)n, (uint32_t)kk) / 4;
         float* base = img + (size_t)kb * (2 * tile_floats);
         base[off] = hi;
         base[tile_floats + off] = lo;
@@ -117,7 +117,7 @@ template <int N, bool DZ>
 __global__ void __launch_bounds__(kPThreads, 1) proj_rows_tc_kernel(const __grid_constant__ PParams p) {
     using Cfg = PCfg<N>;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* st = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // keeps the __shared__ address space
+    uint8_t* st = smem_raw + smem_pad1024(smem_raw);
     PTail* tail = (PTail*)(st + (size_t)Cfg::kStageBytes);
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
@@ -190,6 +190,7 @@ __global__ void __launch_bounds__(kPThreads, 1) proj_rows_tc_kernel(const __grid
 #pragma unroll
             for (int i = 0; i < kPer; ++i) {
                 const int row = rsub + 32 * i;
+                // sw128<16>(row, c) without its final & 7, which would keep the swizzle from being hoisted out of i
                 split_store(st, (uint32_t)row * 128u + (uint32_t)((c ^ (row & 7)) << 4), v[i]);
             }
 #pragma unroll
@@ -247,7 +248,7 @@ __global__ void __launch_bounds__(kPThreads, 1) proj_rows_tc_kernel(const __grid
 // dW[kd x 64] += sum over rows r of [S_k | S_{k+1}][r, :]^T . dZ[r, :]   (kd = 128; kd = 64: S_k alone)
 // M = kd index (warpgroup w owns kd rows 64w .. 64w+63), N = 64, K = rows, 32 rows per k-block.  Both operands are
 // row-major in HBM (K is the slow dimension) and tf32 wgmma reads K-major operands only, so the loaders transpose on
-// their way to shared memory: element (row r, m) lands at sw128_offset(m, r) of a [m][32 k] tile.  The accumulators live
+// their way to shared memory: element (row r, m) lands at sw128<4>(m, r) of a [m][32 k] tile.  The accumulators live
 // for the whole launch and are flushed with atomics once.
 // =====================================================================================================
 constexpr int kWgBBytes = 64 * kKB * 4;                            // dZ: [64][32 k] K-major
@@ -265,7 +266,7 @@ struct WgParams {
 
 __global__ void __launch_bounds__(kPThreads, 1) proj_wgrad_tc_kernel(const __grid_constant__ WgParams p) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* st = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // keeps the __shared__ address space
+    uint8_t* st = smem_raw + smem_pad1024(smem_raw);
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const int lane = tid & 31;
@@ -337,8 +338,6 @@ __global__ void __launch_bounds__(kPThreads, 1) proj_wgrad_tc_kernel(const __gri
     }
 }
 
-int grid_for(int64_t work) { return (int)(work < sm_count() ? work : sm_count()); }
-
 int32_t launch_pack_image(const float* src, int n_rows, int k_cols, int64_t rs, int64_t cs, float* img, int tile_rows,
                           cudaStream_t st) {
     pack_image_kernel<<<(n_rows * k_cols + 255) / 256, 256, 0, st>>>(src, n_rows, k_cols, rs, cs, img, tile_rows);
@@ -365,7 +364,7 @@ int32_t launch_rows_bwd(const float* d_out, const float* out_act, int act, int64
     p.stride_u = stride_u;
     p.rows = rows;
     p.n_tiles = (int)ceil_div(rows, kTileM);
-    kern<<<grid_for(p.n_tiles), kPThreads, psmem<256>(), st>>>(p);
+    kern<<<persistent_grid(p.n_tiles), kPThreads, psmem<256>(), st>>>(p);
     count_launch();
     return check_launch("proj_bwd_tc");
 }
@@ -380,7 +379,7 @@ int32_t launch_wgrad(const float* s, int64_t stride_k, int kd, const float* dz, 
     p.kd = kd;
     p.rows = rows;
     p.n_chunks = ceil_div(rows, kKB);
-    proj_wgrad_tc_kernel<<<grid_for(p.n_chunks), kPThreads, kWgSmem, st>>>(p);
+    proj_wgrad_tc_kernel<<<persistent_grid(p.n_chunks), kPThreads, kWgSmem, st>>>(p);
     count_launch();
     return check_launch("proj_wgrad_tc");
 }
@@ -407,7 +406,7 @@ int32_t launch_proj_fwd_tc(const float* s, int64_t stride_k, int ks, int64_t row
     p.out = out;
     p.rows = rows;
     p.n_tiles = (int)ceil_div(rows, kTileM);
-    kern<<<grid_for(p.n_tiles), kPThreads, psmem<64>(), st>>>(p);
+    kern<<<persistent_grid(p.n_tiles), kPThreads, psmem<64>(), st>>>(p);
     count_launch();
     return check_launch("proj_fwd_tc");
 }

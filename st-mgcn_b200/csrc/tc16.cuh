@@ -8,13 +8,12 @@
 // number they replace.  A single pass over the hi planes is the bf16 arithmetic mode of the bf16-quoted configurations
 // (BASELINE.json configs[1], [3], [4]).
 //
-// One tile layout for everything: a [rows][64 bf16] tile, 128 bytes per row, 8-row groups of 1024 bytes, 16-byte
-// chunk index XORed with (row & 7) -- the TMA SWIZZLE_128B pattern.  Read with a K-major descriptor it is an operand
-// whose K runs along the 64 columns (M/N = rows); read with an MN-major descriptor (canonical layout ((64,n),(8,k)),
-// tc_common.cuh) it is the TRANSPOSED operand: M/N runs along the 64 columns (one 64-element atom; further atoms LBO
-// bytes apart), K along the rows (8-row atoms, SBO = 1024 bytes apart).  So the same shared-memory image of
-// [h_below | h_prev] feeds the gate GEMM (K-major A) and the weight-gradient GEMM (MN-major A), and one image of dA
-// feeds the data-gradient GEMM (K-major A) and the weight-gradient GEMM (MN-major B).
+// One tile layout for everything: a [rows][64 bf16] tile with the 128-byte swizzle (sw128, tc_common.cuh).  Read with a
+// K-major descriptor it is an operand whose K runs along the 64 columns (M/N = rows); read with an MN-major descriptor
+// (canonical layout ((64,n),(8,k)), tc_common.cuh) it is the TRANSPOSED operand: M/N runs along the 64 columns (one
+// 64-element atom; further atoms LBO bytes apart), K along the rows (8-row atoms, SBO = 1024 bytes apart).  So the same
+// shared-memory image of [h_below | h_prev] feeds the gate GEMM (K-major A) and the weight-gradient GEMM (MN-major A),
+// and one image of dA feeds the data-gradient GEMM (K-major A) and the weight-gradient GEMM (MN-major B).
 #pragma once
 #include "tc_common.cuh"
 #include "wgmma.cuh"
@@ -24,11 +23,6 @@ namespace stmgcn {
 namespace tc {
 
 constexpr int kTile16Bytes = 128 * 128;               // [128 rows][64 bf16] = 16 KB
-
-// byte offset of element (row, col) in a [rows][64 bf16] 128B-swizzled tile
-__host__ __device__ __forceinline__ uint32_t sw128_off16(uint32_t row, uint32_t col) {
-    return row * 128u + ((((col >> 3) ^ (row & 7u)) & 7u) << 4) + ((col & 7u) << 1);
-}
 
 // K-major 128B-swizzled tile: rows of 128 B, 8-row groups 1024 B apart; one k16 MMA consumes 32 bytes of the row:
 // advance the start address by 32 B (+2 in the encoded field) per k-step.

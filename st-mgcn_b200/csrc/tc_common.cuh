@@ -1,5 +1,5 @@
-// Hopper (sm_90a) primitives used by the tensor-core kernels: mbarrier, 1-D bulk async copy, TMA tensor stores, wgmma
-// shared-memory matrix descriptors (the instructions themselves: wgmma.cuh).
+// Hopper (sm_90a) primitives used by the tensor-core kernels: barriers, register budgets, bulk and TMA tensor copies, L2
+// policies, the 128-byte swizzle and wgmma shared-memory matrix descriptors (the instructions themselves: wgmma.cuh).
 //
 // Precision scheme "3xTF32": every fp32 operand v is split into hi = v with the low 13 mantissa bits cleared
 // (exactly representable in tf32, so the tensor core's own fp32->tf32 conversion cannot change it) and
@@ -13,6 +13,17 @@ namespace stmgcn {
 namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// bytes from the dynamic shared memory to its first 1024-byte boundary, where swizzled tiles may start (launches request
+// 1024 bytes more than they use); kernels offset the __shared__ array itself by it, which keeps its address space
+__device__ __forceinline__ uint32_t smem_pad1024(const void* smem_raw) { return (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u; }
+
+// named barrier `id` (0 is __syncthreads') over n_threads threads, a multiple of 32
+__device__ __forceinline__ void bar_sync(uint32_t id, uint32_t n_threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
+}
+// a warpgroup's per-thread register budget (every warp of the warpgroup executes the same instruction)
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ---- tf32 split ---------------------------------------------------------------------------------------
 __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
@@ -81,8 +92,22 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                  : "memory");
 }
 
-// ---- TMA tensor store shared -> global through a CUtensorMap (rows past the tensor's end are dropped); completion is
-// tracked per issuing thread in bulk async-groups ---------------------------------------------------------------------
+// ---- TMA tensor copies through a CUtensorMap: a load completes on an mbarrier; a store drops the rows past the tensor's
+// end, and its completion is tracked per issuing thread in bulk async-groups ------------------------------------------
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, int c0, int c1, int c2, uint64_t* bar) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+                 :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void tma_load_3d_hint(void* smem_dst, const void* tmap, int c0, int c1, int c2, uint64_t* bar,
+                                                 uint64_t pol) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
+                 " [%0], [%1, {%3, %4, %5}], [%2], %6;"
+                 :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void tma_prefetch_3d(const void* tmap, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
+                 :: "l"(tmap), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
 __device__ __forceinline__ void tma_store_3d(const void* tmap, const void* smem_src, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
                  :: "l"(tmap), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
@@ -105,6 +130,12 @@ __device__ __forceinline__ void red_add_f32x2(float* dst, float a, float b) {
 // L2 prefetch of a contiguous global range (no registers, no shared memory)
 __device__ __forceinline__ void prefetch_l2(const void* gmem, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem), "r"(bytes) : "memory");
+}
+// L2 policy for data a launch reads exactly once: evicted first, so that the lines read again keep their place in L2
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
 }
 
 // ---- wgmma shared-memory matrix descriptors (sm_90: start >> 4 [0,14), LBO >> 4 [16,30), SBO >> 4 [32,46),
@@ -131,9 +162,12 @@ __device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t smem_addr, uint3
     return d;
 }
 
-// byte offset of element (row, k) inside a [rows][32 fp32] K-major tile with the 128-byte swizzle
-__host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t k) {
-    return row * 128u + ((((k >> 2) ^ (row & 7u)) & 7u) << 4) + ((k & 3u) << 2);
+// ---- 128-byte swizzle (TMA SWIZZLE_128B): 128-byte rows, 8-row groups of 1024 bytes, a byte's 16-byte chunk index XORed
+// with (row & 7).  Byte offset of element e of a row of BYTES-byte elements (sw128<1>: byte e; <2>: bf16; <4>: fp32):
+template <uint32_t BYTES>
+__host__ __device__ __forceinline__ uint32_t sw128(uint32_t row, uint32_t e) {
+    constexpr uint32_t kPerChunk = 16u / BYTES;
+    return row * 128u + ((((e / kPerChunk) ^ (row & 7u)) & 7u) << 4) + ((e % kPerChunk) * BYTES);
 }
 
 }  // namespace tc
