@@ -12,10 +12,9 @@
  *     the CUDA stream as void* (a cudaStream_t; NULL = legacy default stream).
  *   - every entry returns int32_t: 0 ok, >0 a cudaError_t, <0 an argument / shape / alignment error.
  *     stmgcn_last_error() returns a thread-local message for the last non-zero return.
- *   - the library never allocates per call and never frees caller memory; all tensors and workspaces are
- *     caller-owned device buffers.  Only graph handles own device memory (immutable after creation).
- *   - entries enqueue on the given stream and return; no device synchronisation inside (graph creation
- *     excepted: it must read back the non-zero count).
+ *   - the library never allocates, never frees and owns no memory; all tensors and workspaces are
+ *     caller-owned device buffers.
+ *   - entries enqueue on the given stream and return; no device synchronisation inside.
  *   - all feature tensors are fp32, "node-major": rows r = n * B + b (region n outer, window b inner),
  *     features contiguous.  (N, B, p) row-major == (N, B*p) row-major == (N*B, p) row-major.
  */
@@ -28,19 +27,17 @@
 extern "C" {
 #endif
 
-#define STMGCN_ABI_VERSION 6
+#define STMGCN_ABI_VERSION 7
 
 /* error codes < 0 */
 #define STMGCN_ERR_ARG      (-1)   /* null pointer / bad enum */
 #define STMGCN_ERR_SHAPE    (-2)   /* size out of the supported range */
 #define STMGCN_ERR_ALIGN    (-3)   /* pointer or leading dimension not aligned as required */
-#define STMGCN_ERR_STATE    (-4)   /* handle does not carry what the call needs (e.g. no transpose) */
+#define STMGCN_ERR_STATE    (-4)   /* the call could not set up what it needs (e.g. a TMA descriptor) */
 
 /* activation of the projection epilogue (GCN.py:42; the reference passes nn.ReLU or None) */
 #define STMGCN_ACT_NONE 0
 #define STMGCN_ACT_RELU 1
-
-typedef struct stmgcn_graph stmgcn_graph_t;    /* opaque: CSR (+ CSR of the transpose) on one device */
 
 int32_t     stmgcn_abi_version(void);
 const char* stmgcn_last_error(void);
@@ -49,40 +46,25 @@ int32_t     stmgcn_sm_count(void);
 /* how many kernels this library has launched in this process (bench.py "gpu_launches") */
 int64_t     stmgcn_launch_count(void);
 
-/* ---- graph handles: the constant operand GCN.forward receives as A[k] (GCN.py:24-36) ------------- */
-/* From one dense N x N support (row-major, leading dimension ld floats) already on the device: exact
- * zeros are dropped, everything else kept verbatim (so supports[1] of Adj_Preprocessor.process,
- * GCN.py:57-97, becomes the sparse rescaled Laplacian).  build_transpose != 0 also builds CSR of A^T
- * (needed by the backward, SURVEY.md section 8(a)). */
-int32_t stmgcn_graph_from_dense(stmgcn_graph_t** out, const float* dense, int64_t n, int64_t ld,
-                                int32_t build_transpose, void* stream);
-/* From device CSR arrays (copied into the handle). rowptr has n+1 int32 entries. */
-int32_t stmgcn_graph_from_csr(stmgcn_graph_t** out, int64_t n, int64_t nnz, const int32_t* rowptr,
-                              const int32_t* colidx, const float* vals, int32_t build_transpose,
-                              void* stream);
-int32_t stmgcn_graph_destroy(stmgcn_graph_t* g);
-int64_t stmgcn_graph_n(const stmgcn_graph_t* g);
-int64_t stmgcn_graph_nnz(const stmgcn_graph_t* g);
-/* copy the CSR (transpose != 0: of A^T) out to caller device buffers (tests / introspection) */
-int32_t stmgcn_graph_export(const stmgcn_graph_t* g, int32_t transpose, int32_t* rowptr, int32_t* colidx,
-                            float* vals, void* stream);
-
 /* ---- K1: one Chebyshev recurrence step on the features --------------------------------------------
- * Y = alpha * op(A) X + beta * Z + gamma * U,   op(A) = A or A^T,  X/Z/U/Y: (N, f_total) fp32 row-major.
+ * Y = alpha * op(A) X + beta * Z + gamma * U,   X/Z/U/Y: (N, f_total) fp32 row-major.
+ * op(A) is the N x N sparse support GCN.forward receives as A[k] (GCN.py:24-36), given as the caller's device CSR:
+ * rowptr (n+1 int32, non-decreasing from 0), colidx (int32 column indices) and vals (fp32), nnz = rowptr[n] entries.
+ * colidx and vals may be NULL only when the matrix has no entries.  Passing the CSR of A^T makes op(A) = A^T.
  * Z and U may be NULL (their terms vanish).  Forward step k (replaces the dense einsum GCN.py:35 and the
- * matrix recurrence GCN.py:134): alpha=2 (1 for k=1), beta=-1, Z=T_{k-2}X.  Backward (adjoint Clenshaw):
- * transpose=1, U = U_k.  Y must not alias X. */
-int32_t stmgcn_cheb_spmm_step(const stmgcn_graph_t* g, int32_t transpose, float alpha, const float* x,
-                              float beta, const float* z, float gamma, const float* u, float* y,
+ * matrix recurrence GCN.py:134): op(A) = L~, alpha=2 (1 for k=1), beta=-1, Z=T_{k-2}X.  Backward (adjoint Clenshaw,
+ * SURVEY.md section 8(a)): op(A) = L~^T, U = U_k.  Y must not alias X. */
+int32_t stmgcn_cheb_spmm_step(int64_t n, const int32_t* rowptr, const int32_t* colidx, const float* vals, float alpha,
+                              const float* x, float beta, const float* z, float gamma, const float* u, float* y,
                               int64_t f_total, void* stream);
 
 /* The same step with the GATHERED operand read from a bf16 copy (the bf16-arithmetic mode of the bf16-quoted
  * configurations: the kernel's time is its gather volume): x16 (N, f_total) bf16; z, u, y stay fp32; y16 (nullable) receives
  * the bf16 copy of y for the next step.  f_total must be a multiple of 8.  stmgcn_to_bf16 makes the first copy
  * (count elements, a multiple of 8). */
-int32_t stmgcn_cheb_spmm_step16(const stmgcn_graph_t* g, int32_t transpose, float alpha, const void* x16,
-                                float beta, const float* z, float gamma, const float* u, float* y, void* y16,
-                                int64_t f_total, void* stream);
+int32_t stmgcn_cheb_spmm_step16(int64_t n, const int32_t* rowptr, const int32_t* colidx, const float* vals,
+                                float alpha, const void* x16, float beta, const float* z, float gamma, const float* u,
+                                float* y, void* y16, int64_t f_total, void* stream);
 int32_t stmgcn_to_bf16(const float* x, void* y16, int64_t count, void* stream);
 
 /* ---- layout: obs (B,T,N,C) -> node-major (STMGCN.py:36,39 sum over C + permute; :47 row order) ----

@@ -10,10 +10,6 @@
 #include "common.cuh"
 #include <stdlib.h>
 
-namespace stmgcn {
-void graph_view(const stmgcn_graph* g, bool transpose, int64_t* n, int64_t* nnz, const int32_t** rowptr,
-                const int32_t** colidx, const float** vals, bool* ok);
-}
 using namespace stmgcn;
 
 namespace {
@@ -196,42 +192,32 @@ extern "C" int32_t stmgcn_to_bf16(const float* x, void* y16, int64_t count, void
     return check_launch("to_bf16");
 }
 
-extern "C" int32_t stmgcn_cheb_spmm_step16(const stmgcn_graph_t* g, int32_t transpose, float alpha, const void* x16,
-                                           float beta, const float* z, float gamma, const float* u, float* y,
-                                           void* y16, int64_t f_total, void* stream) {
-    STMGCN_REQUIRE(g && x16 && y, STMGCN_ERR_ARG, "cheb_spmm_step16: null pointer");
+extern "C" int32_t stmgcn_cheb_spmm_step16(int64_t n, const int32_t* rowptr, const int32_t* colidx, const float* vals,
+                                           float alpha, const void* x16, float beta, const float* z, float gamma,
+                                           const float* u, float* y, void* y16, int64_t f_total, void* stream) {
+    STMGCN_REQUIRE(rowptr && x16 && y, STMGCN_ERR_ARG, "cheb_spmm_step16: null pointer");
+    STMGCN_REQUIRE(n > 0, STMGCN_ERR_SHAPE, "cheb_spmm_step16: n=%lld", (long long)n);
     STMGCN_REQUIRE(x16 != y16, STMGCN_ERR_ARG, "cheb_spmm_step16: y16 must not alias x16");
     STMGCN_REQUIRE(f_total > 0 && f_total % 8 == 0 && aligned16(x16) && aligned16(y) && (!y16 || aligned16(y16)) &&
                        (!z || aligned16(z)) && (!u || aligned16(u)),
                    STMGCN_ERR_SHAPE, "cheb_spmm_step16: f_total=%lld must be a multiple of 8, pointers 16-byte aligned",
                    (long long)f_total);
-    int64_t n, nnz;
-    const int32_t *rp, *ci;
-    const float* va;
-    bool ok;
-    graph_view(g, transpose != 0, &n, &nnz, &rp, &ci, &va, &ok);
-    STMGCN_REQUIRE(ok, STMGCN_ERR_STATE, "cheb_spmm_step16: transpose requested but handle has none");
     const int64_t col_tiles = ceil_div(f_total, 32 * 8);
     STMGCN_REQUIRE(col_tiles <= 65535, STMGCN_ERR_SHAPE, "cheb_spmm_step16: f_total=%lld too wide", (long long)f_total);
     dim3 grid((unsigned)ceil_div(n, kRowsPerCta), (unsigned)col_tiles);
-    spmm_row_gather16_kernel<<<grid, kWarpsPerCta * 32, 0, (cudaStream_t)stream>>>(n, rp, ci, va, alpha, (const uint16_t*)x16, beta, z,
-                                                                                gamma, u, y, (uint16_t*)y16, f_total);
+    spmm_row_gather16_kernel<<<grid, kWarpsPerCta * 32, 0, (cudaStream_t)stream>>>(n, rowptr, colidx, vals, alpha, (const uint16_t*)x16,
+                                                                                beta, z, gamma, u, y, (uint16_t*)y16, f_total);
     count_launch();
     return check_launch("cheb_spmm_step16");
 }
 
-extern "C" int32_t stmgcn_cheb_spmm_step(const stmgcn_graph_t* g, int32_t transpose, float alpha,
-                                         const float* x, float beta, const float* z, float gamma,
+extern "C" int32_t stmgcn_cheb_spmm_step(int64_t n, const int32_t* rowptr, const int32_t* colidx, const float* vals,
+                                         float alpha, const float* x, float beta, const float* z, float gamma,
                                          const float* u, float* y, int64_t f_total, void* stream) {
-    STMGCN_REQUIRE(g && x && y, STMGCN_ERR_ARG, "cheb_spmm_step: null pointer");
+    STMGCN_REQUIRE(rowptr && x && y, STMGCN_ERR_ARG, "cheb_spmm_step: null pointer");
+    STMGCN_REQUIRE(n > 0, STMGCN_ERR_SHAPE, "cheb_spmm_step: n=%lld", (long long)n);
     STMGCN_REQUIRE(x != y, STMGCN_ERR_ARG, "cheb_spmm_step: y must not alias x");
     STMGCN_REQUIRE(f_total > 0, STMGCN_ERR_SHAPE, "cheb_spmm_step: f_total=%lld", (long long)f_total);
-    int64_t n, nnz;
-    const int32_t *rp, *ci;
-    const float* va;
-    bool ok;
-    graph_view(g, transpose != 0, &n, &nnz, &rp, &ci, &va, &ok);
-    STMGCN_REQUIRE(ok, STMGCN_ERR_STATE, "cheb_spmm_step: transpose requested but handle has none");
     cudaStream_t st = (cudaStream_t)stream;
     const bool vec4 = (f_total % 4 == 0) && aligned16(x) && aligned16(y) && (!z || aligned16(z)) &&
                       (!u || aligned16(u));
@@ -240,9 +226,9 @@ extern "C" int32_t stmgcn_cheb_spmm_step(const stmgcn_graph_t* g, int32_t transp
     STMGCN_REQUIRE(col_tiles <= 65535, STMGCN_ERR_SHAPE, "cheb_spmm_step: f_total=%lld too wide", (long long)f_total);
     dim3 grid((unsigned)ceil_div(n, kRowsPerCta), (unsigned)col_tiles);
     if (vec4)
-        spmm_row_gather_kernel<4><<<grid, kWarpsPerCta * 32, 0, st>>>(n, rp, ci, va, alpha, x, beta, z, gamma, u, y, f_total);
+        spmm_row_gather_kernel<4><<<grid, kWarpsPerCta * 32, 0, st>>>(n, rowptr, colidx, vals, alpha, x, beta, z, gamma, u, y, f_total);
     else
-        spmm_row_gather_kernel<1><<<grid, kWarpsPerCta * 32, 0, st>>>(n, rp, ci, va, alpha, x, beta, z, gamma, u, y, f_total);
+        spmm_row_gather_kernel<1><<<grid, kWarpsPerCta * 32, 0, st>>>(n, rowptr, colidx, vals, alpha, x, beta, z, gamma, u, y, f_total);
     count_launch();
     return check_launch("cheb_spmm_step");
 }

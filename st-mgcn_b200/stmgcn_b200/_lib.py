@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("STMGCN_LIB_PATH") or os.path.join(os.path.dirname(_HERE), "lib", "libstmgcn_b200.so")
 
 ACT_NONE, ACT_RELU = 0, 1
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 # (name, restype, argtypes) -- one row per symbol in include/stmgcn_b200.h
 _P = c_void_p
@@ -22,14 +22,9 @@ SIGNATURES = [
     ("stmgcn_last_error", c_char_p, []),
     ("stmgcn_sm_count", c_int32, []),
     ("stmgcn_launch_count", c_int64, []),
-    ("stmgcn_graph_from_dense", c_int32, [POINTER(c_void_p), _P, c_int64, c_int64, c_int32, _P]),
-    ("stmgcn_graph_from_csr", c_int32, [POINTER(c_void_p), c_int64, c_int64, _P, _P, _P, c_int32, _P]),
-    ("stmgcn_graph_destroy", c_int32, [_P]),
-    ("stmgcn_graph_n", c_int64, [_P]),
-    ("stmgcn_graph_nnz", c_int64, [_P]),
-    ("stmgcn_graph_export", c_int32, [_P, c_int32, _P, _P, _P, _P]),
-    ("stmgcn_cheb_spmm_step", c_int32, [_P, c_int32, c_float, _P, c_float, _P, c_float, _P, _P, c_int64, _P]),
-    ("stmgcn_cheb_spmm_step16", c_int32, [_P, c_int32, c_float, _P, c_float, _P, c_float, _P, _P, _P, c_int64, _P]),
+    ("stmgcn_cheb_spmm_step", c_int32, [c_int64, _P, _P, _P, c_float, _P, c_float, _P, c_float, _P, _P, c_int64, _P]),
+    ("stmgcn_cheb_spmm_step16", c_int32, [c_int64, _P, _P, _P, c_float, _P, c_float, _P, c_float, _P, _P, _P, c_int64,
+                                          _P]),
     ("stmgcn_to_bf16", c_int32, [_P, _P, c_int64, _P]),
     ("stmgcn_obs_to_node_major", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),
     ("stmgcn_proj_fwd", c_int32, [_P, c_int64, c_int32, c_int64, c_int32, _P, _P, c_int32, c_int32, _P, _P,

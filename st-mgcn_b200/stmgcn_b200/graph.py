@@ -16,66 +16,52 @@ materialises ``N x N`` matrices (SURVEY.md section 8(f)-1).
 """
 from __future__ import annotations
 
-import ctypes
 from collections import OrderedDict
 from typing import List, Optional
 
 import torch
 
-from . import _lib
 
-
-def _stream() -> int:
-    return torch.cuda.current_stream().cuda_stream
+def csr_from_coo(n: int, rows: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor):
+    """int32 CSR ``(rowptr, colidx, vals)`` of the ``n x n`` matrix whose entries ``(rows, cols, vals)`` are sorted
+    row-major (by row, then column)."""
+    nnz = rows.numel()
+    if not 0 < n < 2 ** 30 or nnz >= 2 ** 31:
+        raise ValueError(f"CSR: n={n} must be in [1, 2^30) and nnz={nnz} below 2^31 (int32 indices)")
+    rowptr = torch.zeros(n + 1, dtype=torch.int32, device=rows.device)
+    rowptr[1:] = torch.cumsum(torch.bincount(rows, minlength=n), 0)
+    return rowptr, cols.to(torch.int32), vals.to(torch.float32).contiguous()
 
 
 class GraphHandle:
-    """Owns one ``stmgcn_graph_t`` (CSR + CSR^T of one support matrix on one device)."""
+    """CSR and CSR^T of one ``n x n`` support matrix: int32 ``rowptr`` / ``colidx`` and fp32 ``vals`` tensors."""
 
-    def __init__(self, ptr: int, device: torch.device):
-        self.ptr = ctypes.c_void_p(ptr)
-        self.device = device
-        self.n = int(_lib.lib.stmgcn_graph_n(self.ptr))
-        self.nnz = int(_lib.lib.stmgcn_graph_nnz(self.ptr))
+    def __init__(self, n: int, rows: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor):
+        """From the matrix's entries, sorted row-major; ``rows`` and ``cols`` are int64."""
+        self.n, self.nnz, self.device = n, rows.numel(), rows.device
+        # CSR^T: the entries in column-major order (stable: repeated (row, col) entries keep their order)
+        order = torch.argsort(cols * n + rows, stable=True)
+        self._csr = (csr_from_coo(n, rows, cols, vals), csr_from_coo(n, cols[order], rows[order], vals[order]))
 
     @classmethod
     def from_dense(cls, mat: torch.Tensor) -> "GraphHandle":
-        assert mat.is_cuda and mat.dtype == torch.float32 and mat.dim() == 2 and mat.shape[0] == mat.shape[1]
-        assert mat.stride(1) == 1
-        out = ctypes.c_void_p()
-        with torch.cuda.device(mat.device):
-            _lib.check(_lib.lib.stmgcn_graph_from_dense(ctypes.byref(out), mat.data_ptr(), mat.shape[0],
-                                                        mat.stride(0), 1, _stream()), "graph_from_dense")
-        return cls(out.value, mat.device)
+        """Exact zeros (-0.0 included) are dropped, every other entry (NaN included) is kept verbatim: supports[1] of
+        ``Adj_Preprocessor.process`` (``GCN.py:57-97``) becomes the sparse rescaled Laplacian."""
+        assert mat.dtype == torch.float32 and mat.dim() == 2 and mat.shape[0] == mat.shape[1]
+        rows, cols = (mat != 0).nonzero(as_tuple=True)           # row-major order
+        return cls(mat.shape[0], rows, cols, mat[rows, cols])
 
     @classmethod
     def from_csr(cls, n: int, rowptr: torch.Tensor, colidx: torch.Tensor, vals: torch.Tensor) -> "GraphHandle":
-        assert rowptr.is_cuda and rowptr.dtype == torch.int32 and colidx.dtype == torch.int32
+        assert rowptr.dtype == torch.int32 and colidx.dtype == torch.int32
         assert vals.dtype == torch.float32 and rowptr.numel() == n + 1
-        rowptr, colidx, vals = rowptr.contiguous(), colidx.contiguous(), vals.contiguous()
-        out = ctypes.c_void_p()
-        with torch.cuda.device(rowptr.device):
-            _lib.check(_lib.lib.stmgcn_graph_from_csr(ctypes.byref(out), n, colidx.numel(), rowptr.data_ptr(),
-                                                      colidx.data_ptr(), vals.data_ptr(), 1, _stream()),
-                       "graph_from_csr")
-        return cls(out.value, rowptr.device)
+        rows = torch.repeat_interleave(torch.arange(n, device=rowptr.device), (rowptr[1:] - rowptr[:-1]).long(),
+                                       output_size=colidx.numel())
+        return cls(n, rows, colidx.long(), vals)
 
     def export(self, transpose: bool = False):
-        rowptr = torch.empty(self.n + 1, dtype=torch.int32, device=self.device)
-        colidx = torch.empty(max(self.nnz, 1), dtype=torch.int32, device=self.device)
-        vals = torch.empty(max(self.nnz, 1), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib.stmgcn_graph_export(self.ptr, int(transpose), rowptr.data_ptr(),
-                                                    colidx.data_ptr(), vals.data_ptr(), _stream()), "graph_export")
-        return rowptr, colidx[:self.nnz], vals[:self.nnz]
-
-    def __del__(self):
-        try:
-            if self.ptr:
-                _lib.lib.stmgcn_graph_destroy(self.ptr)
-                self.ptr = None
-        except Exception:
-            pass
+        """``(rowptr, colidx, vals)`` of the matrix, or with ``transpose`` of its transpose."""
+        return self._csr[int(transpose)]
 
 
 class SupportSet:
@@ -134,8 +120,6 @@ def supports_from_dense(a: torch.Tensor) -> SupportSet:
     af = a.detach()
     if af.dtype != torch.float32:
         af = af.float()
-    if af.stride(2) != 1:
-        af = af.contiguous()
     ks, n, _ = af.shape
     with torch.cuda.device(a.device):
         if _is_chebyshev_stack(af):

@@ -197,6 +197,11 @@ class ST_MGCN(nn.Module):
                     feats.append(self.gcn_list[m].forward_node_major(ssets[m], h_top))
                 xo.record_stream(streams[m])
                 xt.record_stream(streams[m])
+                # the CSR tensors belong to the stream that built them: once freed (their support set dropped from the
+                # cache), their memory must not be reused while this branch's kernels may still read it
+                for g in ssets[m].graphs:
+                    for t in g.export(False) + g.export(True):
+                        t.record_stream(streams[m])
             for m in range(self.M):
                 main.wait_stream(streams[m])
                 feats[m].record_stream(main)

@@ -1,7 +1,7 @@
 """``torch.autograd.Function`` wrappers around the C ABI -- host plumbing only.
 
 Every tensor the kernels touch is allocated here through torch's caching allocator on the current stream
-(the library never allocates per call, SURVEY.md section 8(b) "ownership").  All feature tensors are fp32
+(the library never allocates, SURVEY.md section 8(b) "ownership").  All feature tensors are fp32
 "node-major": ``(N, B, p)`` contiguous, rows ``r = n*B + b``.
 
 Functions (reference lines they replace):
@@ -67,19 +67,22 @@ def _require_cuda(*ts):
 # --------------------------------------------------------------------------------------------------
 def spmm_step(g, transpose: bool, alpha: float, x: torch.Tensor, beta: float, z: Optional[torch.Tensor],
               gamma: float, u: Optional[torch.Tensor], y: torch.Tensor) -> None:
-    """``y = alpha * op(A) x + beta * z + gamma * u`` on ``(N, F)`` views."""
+    """``y = alpha * op(A) x + beta * z + gamma * u`` on ``(N, F)`` views; op(A) = A, or A^T with ``transpose``."""
     n = g.n
     f_total = x.numel() // n
-    _lib.check(L.stmgcn_cheb_spmm_step(g.ptr, int(transpose), alpha, x.data_ptr(), beta, _p(z), gamma, _p(u),
-                                       y.data_ptr(), f_total, _stream()), "cheb_spmm_step")
+    rowptr, colidx, vals = g.export(transpose)
+    _lib.check(L.stmgcn_cheb_spmm_step(n, rowptr.data_ptr(), colidx.data_ptr(), vals.data_ptr(), alpha, x.data_ptr(),
+                                       beta, _p(z), gamma, _p(u), y.data_ptr(), f_total, _stream()), "cheb_spmm_step")
 
 
 def spmm_step16(g, transpose: bool, alpha: float, x16: torch.Tensor, beta: float, z: Optional[torch.Tensor],
                 gamma: float, u: Optional[torch.Tensor], y: torch.Tensor, y16: Optional[torch.Tensor]) -> None:
     """:func:`spmm_step` with the gathered operand read from its bf16 copy ``x16``; writes the bf16 copy of ``y`` to ``y16``."""
     f_total = y.numel() // g.n
-    _lib.check(L.stmgcn_cheb_spmm_step16(g.ptr, int(transpose), alpha, x16.data_ptr(), beta, _p(z), gamma, _p(u),
-                                         y.data_ptr(), _p(y16), f_total, _stream()), "cheb_spmm_step16")
+    rowptr, colidx, vals = g.export(transpose)
+    _lib.check(L.stmgcn_cheb_spmm_step16(g.n, rowptr.data_ptr(), colidx.data_ptr(), vals.data_ptr(), alpha,
+                                         x16.data_ptr(), beta, _p(z), gamma, _p(u), y.data_ptr(), _p(y16), f_total,
+                                         _stream()), "cheb_spmm_step16")
 
 
 def to_bf16(x: torch.Tensor) -> torch.Tensor:

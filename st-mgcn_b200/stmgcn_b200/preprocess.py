@@ -16,7 +16,7 @@ from typing import Union
 
 import torch
 
-from .graph import ChebSupports
+from .graph import ChebSupports, csr_from_coo
 
 
 class Adj_Preprocessor(object):
@@ -113,10 +113,7 @@ class Adj_Preprocessor(object):
         lt = torch.sparse_coo_tensor(torch.stack([idx_r, idx_c]), vals, (n, n)).coalesce()
         keep = lt.values() != 0
         r, c, v = lt.indices()[0][keep], lt.indices()[1][keep], lt.values()[keep]
-        counts = torch.bincount(r, minlength=n)
-        rowptr = torch.zeros(n + 1, dtype=torch.int64, device=v.device)
-        rowptr[1:] = torch.cumsum(counts, 0)
-        return ChebSupports(n, self.K + 1, rowptr.to(torch.int32), c.to(torch.int32), v)
+        return ChebSupports(n, self.K + 1, *csr_from_coo(n, r, c, v))
 
     @staticmethod
     def _lambda_sparse(n, row, col, a_norm) -> float:

@@ -37,9 +37,10 @@ def test_library_exports_every_declared_symbol():
     assert _lib.lib.stmgcn_launch_count() >= 0
 
 
-def test_c_abi_argument_errors_return_negative_codes_with_a_message():
+def test_c_abi_argument_errors_including_the_spmm_csr_return_negative_codes_with_a_message():
     """The C entry points validate their arguments before touching CUDA: a bad call returns a negative code and
-    stmgcn_last_error() explains it (no GPU needed)."""
+    stmgcn_last_error() explains it (no GPU needed).  The Chebyshev steps take the support as a CSR (rowptr, colidx,
+    vals) and reject a null rowptr and n <= 0."""
     import ctypes
     from stmgcn_b200 import _lib
     lib = _lib.lib
@@ -52,12 +53,63 @@ def test_c_abi_argument_errors_return_negative_codes_with_a_message():
     # exact-fp32 LSTM backward over the whole sequence: null workspaces
     rc = lib.stmgcn_lstm_bwd(12, 3, 128, 64, 1, 8, *([null] * 18))
     assert rc < 0 and b"lstm_bwd: null pointer" in lib.stmgcn_last_error()
-    # bf16 gather step: null graph; conversion: count not a multiple of 8
-    rc = lib.stmgcn_cheb_spmm_step16(null, 0, 1.0, null, 0.0, null, 0.0, null, null, null, 64, null)
-    assert rc < 0 and b"cheb_spmm_step16" in lib.stmgcn_last_error()
-    buf = (ctypes.c_float * 16)()
-    rc = lib.stmgcn_to_bf16(ctypes.addressof(buf), ctypes.addressof(buf), 12, null)
+    # Chebyshev steps (fp32 and bf16 gather): null rowptr, then n <= 0 with every pointer set
+    rc = lib.stmgcn_cheb_spmm_step16(4, null, null, null, 1.0, null, 0.0, null, 0.0, null, null, null, 64, null)
+    assert rc < 0 and b"cheb_spmm_step16: null pointer" in lib.stmgcn_last_error()
+    rc = lib.stmgcn_cheb_spmm_step(4, null, null, null, 1.0, null, 0.0, null, 0.0, null, null, 64, null)
+    assert rc < 0 and b"cheb_spmm_step: null pointer" in lib.stmgcn_last_error()
+    buf, out = (ctypes.c_float * 16)(), (ctypes.c_float * 16)()
+    p, q = ctypes.addressof(buf), ctypes.addressof(out)
+    rc = lib.stmgcn_cheb_spmm_step16(0, p, p, p, 1.0, p, 0.0, None, 0.0, None, q, None, 64, null)
+    assert rc < 0 and b"cheb_spmm_step16: n=0" in lib.stmgcn_last_error()
+    rc = lib.stmgcn_cheb_spmm_step(0, p, p, p, 1.0, p, 0.0, None, 0.0, None, q, 64, null)
+    assert rc < 0 and b"cheb_spmm_step: n=0" in lib.stmgcn_last_error()
+    # conversion: count not a multiple of 8
+    rc = lib.stmgcn_to_bf16(p, p, 12, null)
     assert rc < 0 and b"multiple of 8" in lib.stmgcn_last_error()
+
+
+def _csr_case(n, kind):
+    rng = np.random.default_rng(n)
+    if kind == "zero":
+        return np.zeros((n, n), np.float32)
+    if n == 1:
+        return np.full((1, 1), {"one": 0.7, "nan": np.nan, "neg_zero": -0.0}[kind], np.float32)
+    a = (rng.random((n, n)) < 0.1) * rng.standard_normal((n, n))
+    idx = rng.permutation(n)
+    k = max(1, n // 10)
+    a[idx[:k], :] = 0.0                                      # empty rows
+    a[:, idx[k:2 * k]] = 0.0                                 # empty columns
+    a[idx[2 * k:3 * k], :] = a[:, idx[2 * k:3 * k]] = 0.0     # isolated indices
+    a[idx[3 * k], idx[4 * k]] = -0.0                         # an explicit -0.0 ...
+    a[idx[4 * k], idx[3 * k]] = np.nan                       # ... and a NaN
+    return a.astype(np.float32)
+
+
+@pytest.mark.parametrize("n,kind", [(1, "one"), (1, "nan"), (1, "neg_zero"), (1, "zero"), (33, "isolated"),
+                                    (33, "zero"), (300, "isolated")])
+def test_graph_csr_equals_scipy(n, kind):
+    """GraphHandle.from_dense / from_csr build the CSR and CSR^T with torch, on any device: equal to scipy's CSR of A
+    and of A^T exactly, with empty rows and columns, no entries at all, n = 1, -0.0 entries (dropped, as exact zeros)
+    and NaN entries (kept)."""
+    import scipy.sparse as sp
+    from stmgcn_b200.graph import GraphHandle
+    a = _csr_case(n, kind)
+    ref, ref_t = sp.csr_matrix(a), sp.csr_matrix(a.T)
+    if kind == "isolated":
+        assert (np.diff(ref.indptr) == 0).any() and (np.diff(ref_t.indptr) == 0).any()
+        assert (np.signbit(a) & (a == 0)).any() and np.isnan(ref.data).sum() == 1
+    handles = {"dense": GraphHandle.from_dense(torch.from_numpy(a)),
+               "csr": GraphHandle.from_csr(n, torch.from_numpy(ref.indptr), torch.from_numpy(ref.indices),
+                                           torch.from_numpy(ref.data))}
+    for src, g in handles.items():
+        assert g.n == n and g.nnz == ref.nnz, src
+        for transpose, want in ((False, ref), (True, ref_t)):
+            rp, ci, va = g.export(transpose)
+            assert rp.dtype == ci.dtype == torch.int32 and va.dtype == torch.float32, (src, transpose)
+            assert np.array_equal(rp.numpy(), want.indptr), (src, transpose)
+            assert np.array_equal(ci.numpy(), want.indices), (src, transpose)
+            assert np.array_equal(va.numpy(), want.data, equal_nan=True), (src, transpose)
 
 
 def test_no_cpu_fallback_is_loud():

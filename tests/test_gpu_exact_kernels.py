@@ -5,7 +5,7 @@ dispatch variant and edge the kernels branch on:
 * B. the exact-fp32 projection (proj.cu: tall GEMM, dz_kernel, small_wgrad_kernel, reduce GEMM, pool_kernel) through
   ``ops._proj_fwd`` / ``ops._proj_bwd`` without a weight image, and ``ops.TemporalPool``;
 * C. small.cu: ``ops.ContextGate``, ``ops.FuseOut``, ``ops.obs_to_node_major``;
-* D. graph.cu construction and the SpMM step on graphs with empty rows, empty columns and no entries at all, and one
+* D. CSR construction on the device and the SpMM step on graphs with empty rows, empty columns and no entries at all, and one
   model with an isolated region against the fp64 sparse oracle.
 
 Bars: 2e-5 on forward values, 5e-5 on gradients (max-norm relative, ``O.max_rel_err``), the bars of the tensor-core
