@@ -12,6 +12,7 @@
  *     the CUDA stream as void* (a cudaStream_t; NULL = legacy default stream).
  *   - every entry returns int32_t: 0 ok, >0 a cudaError_t, <0 an argument / shape / alignment error.
  *     stmgcn_last_error() returns a thread-local message for the last non-zero return.
+ *   - a negative return means nothing was enqueued: the call checks all its arguments before its first launch.
  *   - the library never allocates, never frees and owns no memory; all tensors and workspaces are
  *     caller-owned device buffers.
  *   - entries enqueue on the given stream and return; no device synchronisation inside.
@@ -140,6 +141,8 @@ int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
  *        "3xBF16" products, ~2^-18 operand error: fp32-grade, the 1e-4 parity bar holds with >10x margin);
  *        P = 1: hi only, single-pass bf16 products (the arithmetic of the bf16-quoted BASELINE configs).
  *   cs : (L, T, ceil(R/128)*128, 64) fp32, tile-blocked (element (r,u) at (((r/128)*16 + u/4)*128 + r%128)*4 + u%4).
+ *        Of every tile-blocked tensor only the first R rows mean anything; the padding rows of the tile-blocked inputs
+ *        c0 and d_top are never read.
  * No gate tape: the backward recomputes the gates from hp (which it needs anyway for the weight gradients).
  * Weights are passed as flat operand images:
  *   wimg : layer l's resident image (tiles [(segment, plane)] of [256 gate-interleaved columns][64 k] bf16, 128-byte

@@ -172,6 +172,8 @@ int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     STMGCN_REQUIRE(ks >= 1 && ks <= kMaxSegs, STMGCN_ERR_SHAPE, "proj_fwd: %d supports (max %d)", ks, kMaxSegs);
     STMGCN_REQUIRE(rows > 0 && p > 0 && q > 0, STMGCN_ERR_SHAPE, "proj_fwd: bad shape");
     STMGCN_REQUIRE(act == STMGCN_ACT_NONE || act == STMGCN_ACT_RELU, STMGCN_ERR_ARG, "proj_fwd: act=%d", act);
+    STMGCN_REQUIRE(!pool || q == p, STMGCN_ERR_SHAPE, "proj_fwd: pooling needs q == p (got %d, %d)", q, p);
+    STMGCN_REQUIRE(!pool || (b_inner > 0 && rows % b_inner == 0), STMGCN_ERR_SHAPE, "proj_fwd: rows %% b_inner != 0");
     cudaStream_t st = (cudaStream_t)stream;
     if (wimg && !pool && proj_tc_applicable(ks, p, q, s, out, nullptr) && stride_k % 4 == 0)   // wgmma path (proj_tc.cu)
         return launch_proj_fwd_tc(s, stride_k, ks, rows, wimg, bias, act, out, st);
@@ -179,8 +181,6 @@ int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     const ProjEpi epi{bias, act, out};
     if (int32_t rc = launch_tall_auto(a, rows, ks * p, w, q, q, epi, st, "proj_fwd")) return rc;
     if (pool) {
-        STMGCN_REQUIRE(q == p, STMGCN_ERR_SHAPE, "proj_fwd: pooling needs q == p (got %d, %d)", q, p);
-        STMGCN_REQUIRE(b_inner > 0 && rows % b_inner == 0, STMGCN_ERR_SHAPE, "proj_fwd: rows %% b_inner != 0");
         const int64_t cols = b_inner * q, n_regions = rows / b_inner;
         int64_t gy = (int64_t)sm_count() * 8 / ceil_div(cols, 256);
         if (gy < 1) gy = 1;

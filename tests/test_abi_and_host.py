@@ -67,6 +67,12 @@ def test_c_abi_argument_errors_including_the_spmm_csr_return_negative_codes_with
     # conversion: count not a multiple of 8
     rc = lib.stmgcn_to_bf16(p, p, 12, null)
     assert rc < 0 and b"multiple of 8" in lib.stmgcn_last_error()
+    # projection with gate pooling: q != p, and rows not a multiple of b_inner (rejected before the GEMM is launched)
+    pool = (ctypes.c_float * 16)()
+    rc = lib.stmgcn_proj_fwd(p, 4, 1, 4, 2, p, None, 3, 0, q, ctypes.addressof(pool), 2, None, null)
+    assert rc == -2 and b"pooling needs q == p" in lib.stmgcn_last_error()
+    rc = lib.stmgcn_proj_fwd(p, 4, 1, 4, 2, p, None, 2, 0, q, ctypes.addressof(pool), 3, None, null)
+    assert rc == -2 and b"rows % b_inner != 0" in lib.stmgcn_last_error()
 
 
 def _csr_case(n, kind):
