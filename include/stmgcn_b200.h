@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define STMGCN_ABI_VERSION 7
+#define STMGCN_ABI_VERSION 8
 
 /* error codes < 0 */
 #define STMGCN_ERR_ARG      (-1)   /* null pointer / bad enum */
@@ -72,6 +72,10 @@ int32_t stmgcn_to_bf16(const float* x, void* y16, int64_t count, void* stream);
  * xo: (N,B,T,C) copy of obs;  xt: (N,B,T) = sum_c obs.  xo may be NULL when C == 1 (xt is then xo). */
 int32_t stmgcn_obs_to_node_major(const float* obs, float* xo, float* xt, int64_t b, int64_t t,
                                  int64_t n, int64_t c, void* stream);
+/* Its adjoint (the gradient w.r.t. obs): d_obs[b,t,n,c] = d_xo[n,b,t,c] + d_xt[n,b,t], d_obs (B,T,N,C) overwritten.
+ * d_xo (N,B,T,C) and d_xt (N,B,T) may each be NULL (that term vanishes). */
+int32_t stmgcn_obs_grad(const float* d_xo, const float* d_xt, float* d_obs, int64_t b, int64_t t, int64_t n, int64_t c,
+                        void* stream);
 
 /* ---- K2: stacked-K projection (GCN.py:37-42) --------------------------------------------------------
  * out[r,:] = act( sum_k S_k[r,:] W[k*p:(k+1)*p, :] + bias ),  r in [0, rows), S_k = s + k*stride_k
@@ -124,7 +128,7 @@ int32_t stmgcn_lstm_fwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
                         const float* h0, const float* c0, float* hs, float* cs, float* gates, void* stream);
 /* BPTT over all timesteps, then the weight gradients.  d_top: (R, H) gradient of hs[L-1][T-1].
  * Workspaces: dh_rec, dc: (L, R, H); dx_work: (R, H).  No initialisation is needed: the step t = T-1 treats the incoming
- * dh_rec / dc as zero without reading them (h_n / c_n carry no gradient, STMGCN.py:113).
+ * dh_rec / dc as zero without reading them (ST_MGCN discards h_n / c_n, STMGCN.py:113); stmgcn_lstm_bwd_ex seeds them.
  * gates is overwritten IN PLACE with the pre-activation gradients dA, so it serves one backward only.
  * Accumulates (+=; caller zeroes): d_s (B,T) = sum_{n,c} dxmod * xo (gate adjoint, STMGCN.py:44), dwx (C,4H),
  * dwp (laid out like wp) += [h_below_t | h_{t-1}]^T dA summed over all (t, r), dbp (L, 4H). */
@@ -133,6 +137,17 @@ int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
                         const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
                         float* dh_rec, float* dc, float* dx_work, float* d_s, float* dwx, float* dwp, float* dbp,
                         void* stream);
+/* stmgcn_lstm_bwd with the gradients at the model's inputs and recurrent state (nn.LSTM semantics).  All (L, R, H)
+ * row-major, each NULL when unused:
+ *   dh_n, dc_n: incoming gradients of the final state h_n = hs[:, T-1] / c_n = cs[:, T-1] (dh_n[L-1] adds to d_top);
+ *   dh0, dc0  : overwritten with the gradients of h0 / c0 (of the zero initial state when h0 / c0 are NULL).
+ * d_xo: (R, T, C) overwritten with the gradient of xo (d xo = dxmod * s[b, t]), or NULL.
+ * With every extra NULL this is stmgcn_lstm_bwd, launch for launch. */
+int32_t stmgcn_lstm_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid, int32_t c_in, int64_t b_inner,
+                           const float* xo, const float* s_gate, const float* wx, const float* wpt, const float* h0,
+                           const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
+                           float* dh_rec, float* dc, float* dx_work, float* d_s, float* dwx, float* dwp, float* dbp,
+                           const float* dh_n, const float* dc_n, float* dh0, float* dc0, float* d_xo, void* stream);
 
 /* ---- K3b on the tensor cores (H = 64, C <= 4): bf16-plane LSTM without a gate tape -----------------------------
  * Same arithmetic contract as stmgcn_lstm_fwd/_bwd (STMGCN.py:44, :47-50; nn.LSTM semantics, fp32 state and
@@ -182,6 +197,20 @@ int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t
                           const void* h0p, const float* c0, const void* hp, const float* cs, const float* d_top,
                           float* dh_rec, float* dc, float* dx_work, float* dw_scratch, float* dbp, const void* zero_tile,
                           float* d_s, float* grads, void* stream);
+/* stmgcn_lstm16_bwd with the gradients at the model's inputs and recurrent state.  dh_n, dc_n, dh0, dc0: (L, R_pad, 64)
+ * fp32 tile-blocked like c0, each NULL when unused; the padding rows of dh_n / dc_n are never used, those of dh0 / dc0
+ * are unspecified.
+ *   dh_n, dc_n: incoming gradients of the final state (dh_n[L-1] adds to d_top), copied into dh_rec / dc before each
+ *               layer's launch (the other one zeroed when only one is given);
+ *   dh0, dc0  : overwritten with the gradients of the initial state (of the zero state when h0p / c0 are NULL);
+ *   d_xo      : (R, T, C) overwritten with the gradient of xo, or NULL.
+ * With every extra NULL this is stmgcn_lstm16_bwd, launch for launch. */
+int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner, int32_t planes,
+                             const float* xo, const float* s_gate, const void* wimg, const float* bias, const float* wih_t,
+                             const void* h0p, const float* c0, const void* hp, const float* cs, const float* d_top,
+                             float* dh_rec, float* dc, float* dx_work, float* dw_scratch, float* dbp, const void* zero_tile,
+                             float* d_s, float* grads, const float* dh_n, const float* dc_n, float* dh0, float* dc0,
+                             float* d_xo, void* stream);
 
 /* ---- fusion over graphs + output FC (STMGCN.py:116-118) ------------------------------------------
  * feat = sum_m g[m] (each (R, G) node-major); y[b, n, c] = feat[n*B+b, :] . fcw[c, :] + fcb[c]. */

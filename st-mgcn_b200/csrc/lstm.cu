@@ -121,8 +121,9 @@ lstm_bwd_pointwise_kernel(int64_t rows, int hid, float* __restrict__ gates, cons
                           // layer-0 extras (wx == nullptr otherwise)
                           const float* __restrict__ wx, float* __restrict__ dwx, const float* __restrict__ xo,
                           const float* __restrict__ sg, float* __restrict__ d_s, int c_in, int t, int t_len,
-                          int64_t b_inner) {
-    const bool first = (t == t_len - 1);     // the incoming dh_rec / dc are zero by definition at the last time step
+                          int64_t b_inner, float* __restrict__ d_xo, int seeded) {
+    // the incoming dh_rec / dc are zero at the last time step unless the caller seeded them with dh_n / dc_n
+    const bool first = (t == t_len - 1) && !seeded;
     extern __shared__ float sm[];            // [4H] dbias | [C*4H] dwx | [b_inner] ds (if it fits)
     const int h4 = 4 * hid;
     float* s_db = sm;
@@ -149,8 +150,9 @@ lstm_bwd_pointwise_kernel(int64_t rows, int hid, float* __restrict__ gates, cons
          r += (int64_t)gridDim.x * (blockDim.x >> 5)) {
         float xs[kMaxC];
         float dxs[kMaxC];
+        float sv = 0.f;
         if (wx != nullptr) {
-            const float sv = sg[(r % b_inner) * t_len + t];
+            sv = sg[(r % b_inner) * t_len + t];
 #pragma unroll
             for (int c = 0; c < kMaxC; ++c) {
                 xs[c] = (c < c_in) ? xo[(r * t_len + t) * c_in + c] * sv : 0.f;
@@ -198,6 +200,7 @@ lstm_bwd_pointwise_kernel(int64_t rows, int hid, float* __restrict__ gates, cons
                 if (c < c_in) {
                     const float dx = warp_sum(dxs[c]);
                     contrib = fmaf(dx, xo[(r * t_len + t) * c_in + c], contrib);
+                    if (d_xo != nullptr && lane == 0) d_xo[(r * t_len + t) * c_in + c] = dx * sv;   // input gradient
                 }
             }
             if (lane == 0) {
@@ -303,17 +306,26 @@ int32_t stmgcn_lstm_fwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
     return 0;
 }
 
-int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid, int32_t c_in, int64_t b_inner,
-                        const float* xo, const float* s_gate, const float* wx, const float* wpt, const float* h0,
-                        const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
-                        float* dh_rec, float* dc, float* dx_work, float* d_s, float* dwx, float* dwp, float* dbp,
-                        void* stream) {
+int32_t stmgcn_lstm_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid, int32_t c_in, int64_t b_inner,
+                           const float* xo, const float* s_gate, const float* wx, const float* wpt, const float* h0,
+                           const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
+                           float* dh_rec, float* dc, float* dx_work, float* d_s, float* dwx, float* dwp, float* dbp,
+                           const float* dh_n, const float* dc_n, float* dh0, float* dc0, float* d_xo, void* stream) {
     STMGCN_REQUIRE(xo && s_gate && wx && wpt && cs && hs && gates && dh_rec && dc && dx_work && d_s && dwx && dwp && dbp,
                    STMGCN_ERR_ARG, "lstm_bwd: null pointer");
     if (int32_t rc = check_dims("lstm_bwd", t_len, n_layers, rows, hid, c_in, b_inner)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t rh = rows * hid;
     const int h4 = 4 * hid;
+    const size_t state_bytes = (size_t)n_layers * rh * sizeof(float);
+    const int seeded = (dh_n != nullptr || dc_n != nullptr) ? 1 : 0;
+    if (seeded) {
+        // the gradients of h_n / c_n are what the step at T-1 reads as the incoming dh_rec / dc
+        if (dh_n != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dh_rec, dh_n, state_bytes, cudaMemcpyDeviceToDevice, st));
+        else STMGCN_CUDA(cudaMemsetAsync(dh_rec, 0, state_bytes, st));
+        if (dc_n != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dc, dc_n, state_bytes, cudaMemcpyDeviceToDevice, st));
+        else STMGCN_CUDA(cudaMemsetAsync(dc, 0, state_bytes, st));
+    }
     const int grid_pw = (int)((ceil_div(rows, 8) < (int64_t)sm_count() * 4) ? ceil_div(rows, 8) : (int64_t)sm_count() * 4);
     for (int t = t_len - 1; t >= 0; --t) {
         for (int l = n_layers - 1; l >= 0; --l) {
@@ -326,7 +338,8 @@ int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
             if (l0 && b_inner <= 2048) smem += (size_t)b_inner * sizeof(float);
             lstm_bwd_pointwise_kernel<<<grid_pw, 256, smem, st>>>(
                 rows, hid, g_lt, c_t, c_prev, dh_in, dh_rec + (int64_t)l * rh, dc + (int64_t)l * rh, dbp + (int64_t)l * h4,
-                l0 ? wx : nullptr, l0 ? dwx : nullptr, xo, s_gate, d_s, c_in, t, t_len, b_inner);
+                l0 ? wx : nullptr, l0 ? dwx : nullptr, xo, s_gate, d_s, c_in, t, t_len, b_inner, l0 ? d_xo : nullptr,
+                seeded);
             count_launch();
             if (int32_t rc = check_launch("lstm_bwd_pointwise")) return rc;
             // data gradients: [dx_below | dh_rec] = dA . wpt_l      (dA: rows x 4H, wpt_l: 4H x kd_l)
@@ -348,6 +361,9 @@ int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
             if (rc) return rc;
         }
     }
+    // after the step at t = 0, dh_rec / dc hold the gradients of h0 / c0 (also of a zero initial state)
+    if (dh0 != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dh0, dh_rec, state_bytes, cudaMemcpyDeviceToDevice, st));
+    if (dc0 != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dc0, dc, state_bytes, cudaMemcpyDeviceToDevice, st));
     // weight gradients: dwp_l (kd_l, 4H) += [h_below_t | h_{t-1}]^T dA summed over all (t, r)
     for (int l = 0; l < n_layers; ++l) {
         ASegs a{};
@@ -375,6 +391,15 @@ int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
             return rc;
     }
     return 0;
+}
+
+int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid, int32_t c_in, int64_t b_inner,
+                        const float* xo, const float* s_gate, const float* wx, const float* wpt, const float* h0,
+                        const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
+                        float* dh_rec, float* dc, float* dx_work, float* d_s, float* dwx, float* dwp, float* dbp,
+                        void* stream) {
+    return stmgcn_lstm_bwd_ex(t_len, n_layers, rows, hid, c_in, b_inner, xo, s_gate, wx, wpt, h0, c0, cs, hs, gates, d_top,
+                              dh_rec, dc, dx_work, d_s, dwx, dwp, dbp, nullptr, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 }  // extern "C"

@@ -455,8 +455,8 @@ constexpr int kBMaxSteps = 64;
 struct Bwd16Step {
     int32_t slice[2];          // plane slice of K segment s in its tensor map (hi plane; lo = + 1)
     int8_t src[2];             // 0: maps[0] (hp), 1: maps[1] (h0p), 2: zeros (h_prev at t = 0 without an initial state)
-    int8_t first;              // t == T-1: incoming dh_rec / dc are zero and not read
-    int8_t store_dh;           // write dh_prev (t > 0 or an initial state exists)
+    int8_t first;              // t == T-1 without seeds: incoming dh_rec / dc are zero and not read
+    int8_t store_dh;           // write dh_prev (t > 0, an initial state exists, or its gradient is wanted)
     int32_t t;
     const float* c_prev;       // blocked or nullptr (zeros)
     const float* dh_in;        // blocked or nullptr: gradient from the layer above at this step (top layer: d_top at T-1)
@@ -471,6 +471,7 @@ struct Bwd16Params {
     const float* xo;           // (rows, T, C)
     const float* sg;           // (B, T)
     float* d_s;                // (B, T) +=   (layer 0)
+    float* d_xo;               // (rows, T, C) overwritten, or nullptr   (layer 0)
     int c_in, t_len, n_steps;
     int64_t b_inner;
     float* dh_rec;             // blocked, in (unless first) / out, in place through the steps
@@ -851,6 +852,16 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             for (int cc = 0; cc < kC; ++cc) contrib += dxs[cc] * xraw[cc];
             contrib += __shfl_xor_sync(0xffffffffu, contrib, 2);
             if ((q >> 1) == 0 && valid) atomicAdd(&p.d_s[(int64_t)(r % (uint32_t)p.b_inner) * p.t_len + sp.t], contrib);
+            if (p.d_xo != nullptr) {
+                // input gradient: d xo[r, t, c] = dxmod[r, c] * s[b, t]; the lane pair (q, q ^ 2) holds the row's two halves
+                float* dst = p.d_xo + ((int64_t)r * p.t_len + sp.t) * p.c_in;
+                const float sv = valid ? p.sg[(r % (uint32_t)p.b_inner) * (uint32_t)p.t_len + (uint32_t)sp.t] : 0.f;
+#pragma unroll
+                for (int cc = 0; cc < kC; ++cc) {
+                    const float dx = dxs[cc] + __shfl_xor_sync(0xffffffffu, dxs[cc], 2);
+                    if ((q >> 1) == 0 && valid && (CIN == 1 || cc < p.c_in)) dst[cc] = dx * sv;
+                }
+            }
         }
     }
     bar_sync(kBBarCons, kBCons);
@@ -1009,12 +1020,13 @@ extern "C" int32_t stmgcn_lstm16_fwd(int32_t t_len, int32_t n_layers, int64_t ro
 
 extern "C" int32_t stmgcn_lstm16_grid(int64_t rows) { return persistent_grid(ceil_div(rows, kTileM)); }
 
-extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner,
-                                     int32_t planes, const float* xo, const float* s_gate, const void* wimg,
-                                     const float* bias, const float* wih_t, const void* h0p, const float* c0,
-                                     const void* hp, const float* cs, const float* d_top, float* dh_rec, float* dc,
-                                     float* dx_work, float* dw_scratch, float* dbp, const void* zero_tile, float* d_s,
-                                     float* grads, void* stream) {
+extern "C" int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner,
+                                        int32_t planes, const float* xo, const float* s_gate, const void* wimg,
+                                        const float* bias, const float* wih_t, const void* h0p, const float* c0,
+                                        const void* hp, const float* cs, const float* d_top, float* dh_rec, float* dc,
+                                        float* dx_work, float* dw_scratch, float* dbp, const void* zero_tile, float* d_s,
+                                        float* grads, const float* dh_n, const float* dc_n, float* dh0, float* dc0,
+                                        float* d_xo, void* stream) {
     STMGCN_REQUIRE(xo && s_gate && wimg && bias && hp && cs && d_top && dh_rec && dc && dw_scratch && dbp && zero_tile && d_s &&
                        grads,
                    STMGCN_ERR_ARG, "lstm16_bwd: null pointer");
@@ -1036,6 +1048,8 @@ extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t ro
     p.c_in = c_in;
     p.t_len = t_len;
     p.b_inner = b_inner;
+    const bool seeded = dh_n != nullptr || dc_n != nullptr;
+    const size_t slice_bytes = (size_t)blocked_slice(n_tiles) * sizeof(float);
     p.dh_rec = dh_rec;
     p.dc = dc;
     p.dw_slice = dw_scratch;
@@ -1055,6 +1069,14 @@ extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t ro
         p.bias = bias + (int64_t)l * kGateCols;
         p.wih = l == 0 ? wih_t : nullptr;
         p.dbp = dbp + (int64_t)l * kGateCols;
+        p.d_xo = l == 0 ? d_xo : nullptr;
+        if (seeded) {
+            // the gradients of h_n[l] / c_n[l] are what the step at T-1 reads as the incoming dh_rec / dc
+            if (dh_n != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dh_rec, dh_n + (int64_t)l * cslice, slice_bytes, cudaMemcpyDeviceToDevice, st));
+            else STMGCN_CUDA(cudaMemsetAsync(dh_rec, 0, slice_bytes, st));
+            if (dc_n != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dc, dc_n + (int64_t)l * cslice, slice_bytes, cudaMemcpyDeviceToDevice, st));
+            else STMGCN_CUDA(cudaMemsetAsync(dc, 0, slice_bytes, st));
+        }
         for (int si = 0; si < t_len; ++si) {
             const int t = t_len - 1 - si;
             Bwd16Step& sp = p.steps[si];
@@ -1072,8 +1094,9 @@ extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t ro
                 sp.src[s] = 2;
             }
             sp.t = t;
-            sp.first = (t == t_len - 1) ? 1 : 0;
-            sp.store_dh = (t > 0 || h0p != nullptr) ? 1 : 0;
+            sp.first = (t == t_len - 1 && !seeded) ? 1 : 0;
+            // the gradient at a zero initial state is well defined: dh0 wants it stored too
+            sp.store_dh = (t > 0 || h0p != nullptr || dh0 != nullptr) ? 1 : 0;
             sp.c_prev = t > 0 ? cs + (int64_t)(l * t_len + t - 1) * cslice : (c0 ? c0 + (int64_t)l * cslice : nullptr);
             sp.dh_in = l == n_layers - 1 ? (t == t_len - 1 ? d_top : nullptr) : dh_in + (int64_t)t * cslice;
             sp.dx_out = l > 0 ? dx_out + (int64_t)t * cslice : nullptr;
@@ -1083,6 +1106,9 @@ extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t ro
         fn<<<grid, kBThreads, kBSmem, st>>>(p);
         count_launch();
         if (int32_t rc = check_launch("lstm16_bwd")) return rc;
+        // after the step at t = 0, dh_rec / dc hold the gradients of h0[l] / c0[l]: out before the next layer reuses them
+        if (dh0 != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dh0 + (int64_t)l * cslice, dh_rec, slice_bytes, cudaMemcpyDeviceToDevice, st));
+        if (dc0 != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dc0 + (int64_t)l * cslice, dc, slice_bytes, cudaMemcpyDeviceToDevice, st));
         // the slices -> this layer's d_w_ih (256, in_l) | d_w_hh (256, 64) | d_b_ih | d_b_hh, before the next layer
         // reuses dw_scratch
         const int in_l = l == 0 ? c_in : kHid;
@@ -1095,4 +1121,15 @@ extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t ro
         dh_in = dx_out;
     }
     return 0;
+}
+
+extern "C" int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner,
+                                     int32_t planes, const float* xo, const float* s_gate, const void* wimg,
+                                     const float* bias, const float* wih_t, const void* h0p, const float* c0,
+                                     const void* hp, const float* cs, const float* d_top, float* dh_rec, float* dc,
+                                     float* dx_work, float* dw_scratch, float* dbp, const void* zero_tile, float* d_s,
+                                     float* grads, void* stream) {
+    return stmgcn_lstm16_bwd_ex(t_len, n_layers, rows, c_in, b_inner, planes, xo, s_gate, wimg, bias, wih_t, h0p, c0, hp, cs,
+                                d_top, dh_rec, dc, dx_work, dw_scratch, dbp, zero_tile, d_s, grads, nullptr, nullptr, nullptr,
+                                nullptr, nullptr, stream);
 }

@@ -29,6 +29,21 @@ __global__ void obs_to_node_major_kernel(const float* __restrict__ obs, float* _
     }
 }
 
+// adjoint of obs_to_node_major: d_obs[b,t,n,c] = d_xo[n,b,t,c] + d_xt[n,b,t]   (either input may be NULL)
+__global__ void obs_grad_kernel(const float* __restrict__ d_xo, const float* __restrict__ d_xt, float* __restrict__ d_obs,
+                                int64_t b_sz, int64_t t_len, int64_t n, int64_t c_in) {
+    // one thread per (b, t, n); consecutive threads walk n (coalesced writes, strided reads)
+    const int64_t total = b_sz * t_len * n;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+         i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t nn = i % n;
+        const int64_t bt = i / n;                           // = b * t_len + t
+        const int64_t j = nn * b_sz * t_len + bt;           // (n, b, t) node-major
+        const float g = d_xt != nullptr ? d_xt[j] : 0.f;
+        for (int64_t c = 0; c < c_in; ++c) d_obs[i * c_in + c] = (d_xo != nullptr ? d_xo[j * c_in + c] : 0.f) + g;
+    }
+}
+
 // ---- context gate ----------------------------------------------------------------------------------
 // one CTA per window b; T threads-worth of work looped over blockDim
 __global__ void gate_fwd_kernel(const float* __restrict__ pool, int t_len, float inv_n,
@@ -170,6 +185,18 @@ int32_t stmgcn_obs_to_node_major(const float* obs, float* xo, float* xt, int64_t
         obs, xo, xt, b, t, n, c);
     count_launch();
     return check_launch("obs_to_node_major");
+}
+
+int32_t stmgcn_obs_grad(const float* d_xo, const float* d_xt, float* d_obs, int64_t b, int64_t t, int64_t n, int64_t c,
+                        void* stream) {
+    STMGCN_REQUIRE(d_obs, STMGCN_ERR_ARG, "obs_grad: null pointer");
+    STMGCN_REQUIRE(b > 0 && t > 0 && n > 0 && c > 0, STMGCN_ERR_SHAPE, "obs_grad: bad shape");
+    const int64_t total = n * b * t;
+    const int64_t blocks = ceil_div(total, 256);
+    const int64_t cap = (int64_t)sm_count() * 16;
+    obs_grad_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(d_xo, d_xt, d_obs, b, t, n, c);
+    count_launch();
+    return check_launch("obs_grad");
 }
 
 int32_t stmgcn_gate_fwd(const float* pool, int64_t b, int32_t t, int64_t n_regions, const float* fcw,

@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("STMGCN_LIB_PATH") or os.path.join(os.path.dirname(_HERE), "lib", "libstmgcn_b200.so")
 
 ACT_NONE, ACT_RELU = 0, 1
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 # (name, restype, argtypes) -- one row per symbol in include/stmgcn_b200.h
 _P = c_void_p
@@ -27,6 +27,7 @@ SIGNATURES = [
                                           _P]),
     ("stmgcn_to_bf16", c_int32, [_P, _P, c_int64, _P]),
     ("stmgcn_obs_to_node_major", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),
+    ("stmgcn_obs_grad", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),
     ("stmgcn_proj_fwd", c_int32, [_P, c_int64, c_int32, c_int64, c_int32, _P, _P, c_int32, c_int32, _P, _P,
                                   c_int64, _P, _P]),
     ("stmgcn_proj_pack_tc", c_int32, [_P, c_int32, _P, _P, _P]),
@@ -38,12 +39,16 @@ SIGNATURES = [
                                   _P, _P, _P, _P]),
     ("stmgcn_lstm_bwd", c_int32, [c_int32, c_int32, c_int64, c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    ("stmgcn_lstm_bwd_ex", c_int32, [c_int32, c_int32, c_int64, c_int32, c_int32, c_int64, _P, _P, _P, _P, _P, _P, _P,
+                                     _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     ("stmgcn_lstm16_pack", c_int32, [_P, _P, _P, _P, c_int32, c_int32, _P, _P, _P, _P]),
     ("stmgcn_lstm16_fwd", c_int32, [c_int32, c_int32, c_int64, c_int32, c_int64, c_int32, _P, _P, _P, _P, _P, _P, _P,
                                     _P, _P, _P, _P, _P]),
     ("stmgcn_lstm16_grid", c_int32, [c_int64]),
     ("stmgcn_lstm16_bwd", c_int32, [c_int32, c_int32, c_int64, c_int32, c_int64, c_int32, _P, _P, _P, _P, _P, _P, _P,
                                     _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    ("stmgcn_lstm16_bwd_ex", c_int32, [c_int32, c_int32, c_int64, c_int32, c_int64, c_int32, _P, _P, _P, _P, _P, _P,
+                                       _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     ("stmgcn_fuse_out_fwd", c_int32, [POINTER(c_void_p), c_int32, c_int64, c_int64, c_int32, c_int32, _P, _P,
                                       _P, _P, _P]),
     ("stmgcn_fuse_out_bwd", c_int32, [_P, _P, c_int64, c_int64, c_int32, c_int32, _P, _P, _P, _P, _P]),

@@ -5,7 +5,7 @@ Every tensor the kernels touch is allocated here through torch's caching allocat
 "node-major": ``(N, B, p)`` contiguous, rows ``r = n*B + b``.
 
 Functions (reference lines they replace):
-  ObsToNodeMajor   STMGCN.py:36,39 (sum over C, permute) and :47 (row order of the shared LSTM)
+  ObsToNodeMajor   STMGCN.py:36,39 (sum over C, permute) and :47 (row order of the shared LSTM); only when obs requires grad
   ChebGCN          GCN.py:24-43 on a sparse L~ (recurrence on features) -> out (N,B,q)
   TemporalPool     STMGCN.py:40-42: GCN over time-as-features + residual + sum over regions -> (B,T)
   ContextGate      STMGCN.py:42-43: /N, fc, relu, fc (same weights), sigmoid -> s (B,T)
@@ -245,17 +245,49 @@ def _proj_bwd(s: torch.Tensor, w: torch.Tensor, act: int, out: torch.Tensor, d_o
 # autograd Functions
 # --------------------------------------------------------------------------------------------------
 def obs_to_node_major(obs: torch.Tensor):
-    """obs (B,T,N,C) -> xo (N,B,T,C), xt (N,B,T).  Observations are data: no gradient flows back."""
+    """obs (B,T,N,C) -> xo (N,B,T,C), xt (N,B,T).  With ``obs.requires_grad`` both carry gradients back to obs."""
     _require_cuda(obs)
     if obs.requires_grad:
-        raise NotImplementedError("stmgcn_b200 treats obs_seq as data; gradients w.r.t. obs_seq are not provided")
-    obs = _f32c(obs.detach())
+        xt_or_both = ObsToNodeMajor.apply(obs)
+        if obs.shape[3] > 1:
+            return xt_or_both
+        # C == 1: xo is a view of xt outside the Function, so autograd folds both gradients into d_xt
+        xt = xt_or_both
+        return xt.unsqueeze(3), xt
+    return _obs_to_node_major(_f32c(obs.detach()))
+
+
+def _obs_to_node_major(obs: torch.Tensor):
     b, t, n, c = obs.shape
     xt = torch.empty((n, b, t), device=obs.device, dtype=torch.float32)
     xo = torch.empty((n, b, t, c), device=obs.device, dtype=torch.float32) if c > 1 else None
     _lib.check(L.stmgcn_obs_to_node_major(obs.data_ptr(), _p(xo), xt.data_ptr(), b, t, n, c, _stream()),
                "obs_to_node_major")
     return (xo if xo is not None else xt.view(n, b, t, 1)), xt
+
+
+class ObsToNodeMajor(torch.autograd.Function):
+    """:func:`obs_to_node_major` for an obs that requires grad: returns (xo, xt), or xt alone when C == 1.
+    Backward: d_obs[b,t,n,c] = d_xo[n,b,t,c] + d_xt[n,b,t] (stmgcn_obs_grad)."""
+
+    @staticmethod
+    def forward(ctx, obs):
+        ctx.set_materialize_grads(False)
+        ctx.shape, ctx.dtype = tuple(obs.shape), obs.dtype
+        xo, xt = _obs_to_node_major(_f32c(obs.detach()))
+        return (xo, xt) if obs.shape[3] > 1 else xt
+
+    @staticmethod
+    def backward(ctx, *grads):
+        d_xo, d_xt = grads if len(grads) == 2 else (None, grads[0])
+        if d_xo is None and d_xt is None:
+            return None
+        b, t, n, c = ctx.shape
+        d_obs = torch.empty((b, t, n, c), device=(d_xt if d_xt is not None else d_xo).device, dtype=torch.float32)
+        d_xo = _f32c(d_xo) if d_xo is not None else None
+        d_xt = _f32c(d_xt) if d_xt is not None else None
+        _lib.check(L.stmgcn_obs_grad(_p(d_xo), _p(d_xt), d_obs.data_ptr(), b, t, n, c, _stream()), "obs_grad")
+        return d_obs.to(ctx.dtype)
 
 
 class ChebGCN(torch.autograd.Function):
@@ -290,8 +322,7 @@ class ChebGCN(torch.autograd.Function):
 
 
 class TemporalPool(torch.autograd.Function):
-    """pool (B,T) = sum_n ( x + act(GCN_T(x)) )[n,b,:]  (STMGCN.py:40-42 before the division by N).
-    x is data (no gradient)."""
+    """pool (B,T) = sum_n ( x + act(GCN_T(x)) )[n,b,:]  (STMGCN.py:40-42 before the division by N)."""
 
     @staticmethod
     def forward(ctx, x, w, bias, sset: SupportSet, act: int):
@@ -310,7 +341,7 @@ class TemporalPool(torch.autograd.Function):
             # generic supports (localpool, hand-made stacks): s[0] = A_0 x is NOT the residual of STMGCN.py:41
             out = _proj_fwd(s, w, bias_c, act, None, b)
             pool = (x + out).sum(dim=0)
-        ctx.act, ctx.has_bias = act, bias is not None
+        ctx.act, ctx.has_bias, ctx.sset = act, bias is not None, sset
         if any(ctx.needs_input_grad):
             ctx.save_for_backward(s, w, out)
         return pool
@@ -319,8 +350,13 @@ class TemporalPool(torch.autograd.Function):
     def backward(ctx, d_pool):
         s, w, out = ctx.saved_tensors
         d_pool = _f32c(d_pool)
-        dw, db, _ = _proj_bwd(s, w, ctx.act, out, None, d_pool, 1.0, s.shape[2], ctx.has_bias, False)
-        return None, dw, db, None, None
+        need_dx = ctx.needs_input_grad[0]
+        dw, db, u = _proj_bwd(s, w, ctx.act, out, None, d_pool, 1.0, s.shape[2], ctx.has_bias, need_dx)
+        dx = None
+        if need_dx:
+            # the GCN's dX (adjoint Clenshaw / sum_k A_k^T U_k) plus the residual's: d_pool broadcast over regions
+            dx = adjoint_stack_(ctx.sset, u) + d_pool.unsqueeze(0)
+        return dx, dw, db, None, None
 
 
 class ContextGate(torch.autograd.Function):
@@ -492,6 +528,13 @@ def _zero_tile(dev: torch.device) -> torch.Tensor:
 def _lstm16_backward(xo, s_gate, tape, n_layers, planes, d_top):
     """BPTT of the bf16-plane path, one library call (per layer one fused launch over all timesteps and one weight-gradient
     reduction).  Returns (d_s, [native nn.LSTM gradients]): views of one flat buffer."""
+    return _lstm16_backward_ex(xo, s_gate, tape, n_layers, planes, d_top)[:2]
+
+
+def _lstm16_backward_ex(xo, s_gate, tape, n_layers, planes, d_top, dh_n=None, dc_n=None, want=(False, False, False)):
+    """:func:`_lstm16_backward` with the gradients at the inputs and the recurrent state: returns (d_s, grads, (d_xo, dh0,
+    dc0)).  dh_n / dc_n (L, R, 64) or None seed the final state's gradients; ``want`` = which of d_xo, dh0, dc0 to compute
+    (None otherwise).  Without any of them the plain entry point runs."""
     _wait_packed(tape["packed"])
     hp, cs, h0p, c0b, wimg, bias, wih_t = (tape[k] for k in _TAPE16)
     n, b, t_len, c_in = xo.shape
@@ -507,12 +550,24 @@ def _lstm16_backward(xo, s_gate, tape, n_layers, planes, d_top):
     d_s = xo.new_zeros((b, t_len))
     shapes = [s for l in range(n_layers) for s in ((256, c_in if l == 0 else 64), (256, 64), (256,), (256,))]
     grads = xo.new_empty(sum(math.prod(s) for s in shapes))
-    _lib.check(L.stmgcn_lstm16_bwd(t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(), wimg.data_ptr(),
-                                   bias.data_ptr(), wih_t.data_ptr(), _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(),
-                                   d_top.data_ptr(), dh_rec.data_ptr(), dc.data_ptr(), _p(dx_work), dw_scratch.data_ptr(),
-                                   dbp.data_ptr(), _zero_tile(xo.device).data_ptr(), d_s.data_ptr(), grads.data_ptr(),
-                                   _stream()), "lstm16_bwd")
-    return d_s, [g.view(s) for g, s in zip(grads.split([math.prod(s) for s in shapes]), shapes)]
+    args = (t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(), wimg.data_ptr(), bias.data_ptr(),
+            wih_t.data_ptr(), _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(), d_top.data_ptr(), dh_rec.data_ptr(),
+            dc.data_ptr(), _p(dx_work), dw_scratch.data_ptr(), dbp.data_ptr(), _zero_tile(xo.device).data_ptr(),
+            d_s.data_ptr(), grads.data_ptr())
+    w_grads = [g.view(s) for g, s in zip(grads.split([math.prod(s) for s in shapes]), shapes)]
+    if dh_n is None and dc_n is None and not any(want):
+        _lib.check(L.stmgcn_lstm16_bwd(*args, _stream()), "lstm16_bwd")
+        return d_s, w_grads, (None, None, None)
+    # the state gradients are tile-blocked (L, R_pad, 64) at the C ABI
+    dh_nb = to_blocked(_f32c(dh_n)) if dh_n is not None else None
+    dc_nb = to_blocked(_f32c(dc_n)) if dc_n is not None else None
+    d_xo = xo.new_empty(xo.shape) if want[0] else None
+    dh0b = xo.new_empty((n_layers, rows_pad, 64)) if want[1] else None
+    dc0b = xo.new_empty((n_layers, rows_pad, 64)) if want[2] else None
+    _lib.check(L.stmgcn_lstm16_bwd_ex(*args, _p(dh_nb), _p(dc_nb), _p(dh0b), _p(dc0b), _p(d_xo), _stream()), "lstm16_bwd_ex")
+    dh0 = from_blocked(dh0b, rows) if dh0b is not None else None
+    dc0 = from_blocked(dc0b, rows) if dc0b is not None else None
+    return d_s, w_grads, (d_xo, dh0, dc0)
 
 
 def _exact_forward(xo, s_gate, h0c, c0c, n_layers, hid, want_state, weights, keep_tape):
@@ -536,6 +591,11 @@ def _exact_forward(xo, s_gate, h0c, c0c, n_layers, hid, want_state, weights, kee
 
 def _exact_backward(xo, s_gate, tape, n_layers, hid, d_top):
     """BPTT of the exact-fp32 path, one library call; it overwrites the gate tape with dA.  Returns (d_s, grads)."""
+    return _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top)[:2]
+
+
+def _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top, dh_n=None, dc_n=None, want=(False, False, False)):
+    """:func:`_exact_backward` with the extras of :func:`_lstm16_backward_ex`: returns (d_s, grads, (d_xo, dh0, dc0))."""
     h0, c0, hs, cs, gates, wx, wpt = tape
     n, b, t_len, c_in = xo.shape
     rows = n * b
@@ -548,11 +608,20 @@ def _exact_backward(xo, s_gate, tape, n_layers, hid, d_top):
     dwx = torch.zeros_like(wx)
     dwp = torch.zeros_like(wpt)
     dbp = xo.new_zeros((n_layers, 4 * hid))
-    _lib.check(L.stmgcn_lstm_bwd(t_len, n_layers, rows, hid, c_in, b, xo.data_ptr(), s_gate.data_ptr(), wx.data_ptr(),
-                                 wpt.data_ptr(), _p(h0), _p(c0), cs.data_ptr(), hs.data_ptr(), gates.data_ptr(),
-                                 d_top.data_ptr(), dh_rec.data_ptr(), dc.data_ptr(), dx_work.data_ptr(), d_s.data_ptr(),
-                                 dwx.data_ptr(), dwp.data_ptr(), dbp.data_ptr(), _stream()), "lstm_bwd")
-    return d_s, _unpack_lstm_grads(dwx, dwp, dbp, n_layers, hid, c_in)
+    args = (t_len, n_layers, rows, hid, c_in, b, xo.data_ptr(), s_gate.data_ptr(), wx.data_ptr(), wpt.data_ptr(), _p(h0),
+            _p(c0), cs.data_ptr(), hs.data_ptr(), gates.data_ptr(), d_top.data_ptr(), dh_rec.data_ptr(), dc.data_ptr(),
+            dx_work.data_ptr(), d_s.data_ptr(), dwx.data_ptr(), dwp.data_ptr(), dbp.data_ptr())
+    extras = (None, None, None)
+    if dh_n is None and dc_n is None and not any(want):
+        _lib.check(L.stmgcn_lstm_bwd(*args, _stream()), "lstm_bwd")
+    else:
+        dh_n = _f32c(dh_n) if dh_n is not None else None
+        dc_n = _f32c(dc_n) if dc_n is not None else None
+        extras = tuple(xo.new_empty(shape) if w else None
+                       for w, shape in zip(want, (xo.shape, (n_layers, rows, hid), (n_layers, rows, hid))))
+        _lib.check(L.stmgcn_lstm_bwd_ex(*args, _p(dh_n), _p(dc_n), _p(extras[1]), _p(extras[2]), _p(extras[0]),
+                                        _stream()), "lstm_bwd_ex")
+    return d_s, _unpack_lstm_grads(dwx, dwp, dbp, n_layers, hid, c_in), extras
 
 
 class SharedLSTM(torch.autograd.Function):
@@ -560,7 +629,8 @@ class SharedLSTM(torch.autograd.Function):
 
     forward(xo (N,B,T,C), s (B,T), h0|None, c0|None (L,R,H), n_layers, hid, want_state, *lstm_weights) where
     lstm_weights = [w_ih_l0, w_hh_l0, b_ih_l0, b_hh_l0, w_ih_l1, ...] (nn.LSTM names/shapes).
-    Returns (h_top, h_n (L,R,H), c_n (L,R,H)); the last two are not differentiable.
+    Returns (h_top, h_n (L,R,H), c_n (L,R,H)), three distinct tensors; h_n / c_n are differentiable with ``want_state``
+    (empty and not differentiable without).  Gradients flow to xo, s, h0, c0 and the weights.
 
     Two kernel families (include/stmgcn_b200.h):
     * H = 64, C <= 4, T <= 64 (the reference's configuration, Main.py:62) and ``lstm_path() == "tc"``: the tensor-core bf16-plane
@@ -591,23 +661,34 @@ class SharedLSTM(torch.autograd.Function):
             h_top, h_n, c_n, tape = _exact_forward(xo, s_gate, h0c, c0c, n_layers, hid, want_state, weights, need_grad)
         if need_grad:
             ctx.save_for_backward(xo, s_gate, *tape)
-        ctx.mark_non_differentiable(h_n, c_n)
+        ctx.set_materialize_grads(False)
+        if want_state:
+            # three distinct outputs: h_top is a view of h_n (tensor cores) or both are views of the tape (exact path)
+            h_top = h_top.clone()
+            if not ctx.planes16:
+                h_n, c_n = h_n.clone(), c_n.clone()
+        else:
+            ctx.mark_non_differentiable(h_n, c_n)
         return h_top, h_n, c_n
 
     @staticmethod
-    def backward(ctx, d_top, _dhn, _dcn):
+    def backward(ctx, d_top, dh_n, dc_n):
         n_layers, hid = ctx.dims
         xo, s_gate, *tape = ctx.saved_tensors
+        if d_top is None:
+            d_top = xo.new_zeros((xo.shape[0], xo.shape[1], hid))
+        want = (ctx.needs_input_grad[0], ctx.needs_input_grad[2], ctx.needs_input_grad[3])
         if ctx.planes16:
             tape16 = dict(zip(_TAPE16, tape), packed=ctx.packed)
-            d_s, w_grads = _lstm16_backward(xo, s_gate, tape16, n_layers, ctx.planes, d_top)
+            d_s, w_grads, extras = _lstm16_backward_ex(xo, s_gate, tape16, n_layers, ctx.planes, d_top, dh_n, dc_n, want)
         else:
             if getattr(ctx, "tape_consumed", False):
                 raise RuntimeError("SharedLSTM (exact-fp32 kernels): the gate tape was overwritten in place by the first "
                                    "backward pass; a second backward over the same graph is not supported on this path")
             ctx.tape_consumed = True
-            d_s, w_grads = _exact_backward(xo, s_gate, tape, n_layers, hid, d_top)
-        return (None, d_s, None, None, None, None, None, *w_grads)
+            d_s, w_grads, extras = _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top, dh_n, dc_n, want)
+        d_xo, dh0, dc0 = extras
+        return (d_xo, d_s, dh0, dc0, None, None, None, *w_grads)
 
 
 class FuseOut(torch.autograd.Function):
