@@ -416,16 +416,18 @@ __global__ void lstm16_pack_kernel(const float* __restrict__ w_ih, const float* 
 //   R_c : recompute  G_c[64 x 64] = [h_below | h_prev] . Wp[:, chunk]                      (registers, m64n64)
 //   P_c : gates -> c_t, tanh(c_t) -> BPTT pointwise -> dA_c (fp32) -> bf16 hi/lo planes in a 128-byte-swizzled
 //         shared-memory tile; dc in place
-//   B_c : bias gradient    db[chunk] += column sums of the fp32 dA_c: a reduce-scatter over the 16 lanes of a warp that
-//         hold the same units, then one shared-memory add per warp and column
+//   B_c : bias gradient    db[chunk] += column sums of dA_c = hi + lo, read back from the shared tile by two producer
+//         warps (kBDbWarps) while the consumers go on with the next chunk; fp32 sums in their registers for the
+//         whole launch, one global atomic per column and warp at the end
 //   W_c : weight gradient  dWp[kd, chunk] = A^T . dA_c, warpgroup w: kd rows 64w .. (both operands: MN-major views of
 //         tiles already in shared memory), added into this CTA's own slice of a scratch buffer with vector reductions
 //   D_c : data gradient    [dx_below | dh_prev] += dA_c . Wp[:, chunk]^T  (B: MN-major view of the resident weights;
 //         accumulated in registers over the four chunks, stored at the end of the item)
-// Schedule of a warpgroup (one dA tile shared by both warpgroups, so they stay in step at its two barriers per chunk):
-//   c = 0      : R_0; wait; P_0, B_0; barrier; dA_0 -> tile; barrier
-//   c = 1 .. 3 : R_c | W_{c-1} + D_{c-1} (two commit groups); wait for R_c only; P_c, B_c (dA_c kept in registers)
-//                while the tensor pipe runs W / D; wait; red.add W_{c-1}; barrier; dA_c -> tile; barrier
+// Schedule of a warpgroup (one dA tile shared by both warpgroups and the B_c warps, so they stay in step at its two
+// barriers per chunk):
+//   c = 0      : R_0; wait; P_0; barrier; dA_0 -> tile; barrier                                   (then B_0)
+//   c = 1 .. 3 : R_c | W_{c-1} + D_{c-1} (two commit groups); wait for R_c only; P_c (dA_c kept in registers)
+//                while the tensor pipe runs W / D; wait; red.add W_{c-1}; barrier; dA_c -> tile; barrier (then B_c)
 //   item end   : W_3 | D_3; wait for W_3; A planes released to the producer; red.add W_3; wait for D_3; store
 // The wgmma operands and the accumulation order of every accumulator are those of the unpipelined schedule.
 // dA never leaves the SM; the gates are never stored.  lstm16_wgrad_reduce_kernel sums the slices after each layer's
@@ -435,12 +437,15 @@ constexpr int kBThreads = kBWarpgroups * 128 + 128;     // + producer warpgroup 
 constexpr int kBCons = kBWarpgroups * 128;              // consumer threads
 constexpr uint32_t kBBarCons = 1;                       // named barrier of the consumer warpgroups (kBCons threads)
 constexpr uint32_t kBBarWg = 2;                         // named barrier kBBarWg + w: consumer warpgroup w (128 threads)
+constexpr int kBDbWarps = 2;                            // producer warps 1 .. kBDbWarps: the bias gradient (B_c)
+constexpr uint32_t kBBarDa = 4;                         // named barrier of the dA tile: consumers + the B_c warps
+constexpr uint32_t kBDaThreads = kBCons + 32 * kBDbWarps;
 // registers per thread after setmaxnreg: 256 * 240 + 128 * 24 = 64 512 of the SM's 65 536 (launched at 384 * 168)
 constexpr uint32_t kBConsRegs = 240, kBProdRegs = 24;
 constexpr int kBATiles = 4;                             // (seg0 | seg1) x (hi | lo); layer 0: seg 1 = the auxiliary [x*s] tile
 
 struct B16Tail {
-    float db[kGateCols];
+    float bias[kGateCols];             // gate-interleaved bias, pre-scaled (gate_scale) as the forward's
     uint64_t a_full, a_empty, w_full;
 };
 constexpr size_t kBSmem = 1024 + 4 * (size_t)kWTileBytes + kBATiles * (size_t)kATileBytes + 2 * (size_t)kATileBytes + sizeof(B16Tail);
@@ -557,19 +562,6 @@ __device__ __forceinline__ void bwd_wgrad_red(float* slice, const float (&wgr)[3
     }
 }
 
-// One reduce-scatter step between lanes l and l ^ mask over v[0 .. 2H): the lane with the mask bit set keeps the upper
-// half, the other the lower half, each adds its partner's copy of that half; the kept half moves to v[0 .. H).
-template <int H, int N>
-__device__ __forceinline__ void col_sums_step(float (&v)[N], int mask, int lane) {
-    const bool up = (lane & mask) != 0;
-#pragma unroll
-    for (int i = 0; i < H; ++i) {
-        const float send = up ? v[i] : v[i + H];
-        const float keep = up ? v[i + H] : v[i];
-        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, mask);
-    }
-}
-
 template <int PLANES, int CIN>                                  // CIN: see lstm16_fwd_kernel
 __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_constant__ Bwd16Params p) {
     constexpr bool L0 = CIN > 0;
@@ -594,7 +586,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         mbar_init(&tail->w_full, 1);
         fence_barrier_init();
     }
-    for (int i = tid; i < kGateCols; i += kBThreads) tail->db[i] = 0.f;
+    for (int i = tid; i < kGateCols; i += kBThreads) tail->bias[i] = p.bias[i] * gate_scale(i);
     if (L0) {
         for (int i = tid; i < p.c_in * kGateCols; i += kBThreads) wih_s[i] = p.wih[i] * gate_scale(i);
         // auxiliary tiles (seg-1 slots): zero once; columns 0..C-1 are rewritten per item.  One plane: the h_prev lo slot is
@@ -641,6 +633,38 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                         for (int pl = 0; pl < PLANES; ++pl)
                             if (sp1.src[sg] != 2) tma_prefetch_3d(&p.maps[sp1.src[sg]], 0, tile1 * kTileM, sp1.slice[sg] + pl);
                 }
+            }
+        } else if (warp > kProdWarp && warp <= kProdWarp + kBDbWarps && n_items > 0) {
+            // ---- B_c: bias gradient, column sums of every dA_c tile (hi + lo; rows past the end carry dA = 0) ----
+            // Warp kProdWarp + 1 + h sums rows 64h .. 64h + 63, lane l the columns 2l, 2l + 1 of each chunk: a warp reads one
+            // 128-byte tile row per load, conflict free.  The tile is read between store_da's second barrier (complete)
+            // and the first of the next store_da (free to be overwritten), which the consumers reach a whole chunk later.
+            // All of it fits the producer's kBProdRegs registers: 8 sums for the launch, 8 loaded words in flight.
+            // (rows: this warp's first row, a multiple of 8, so a row's swizzle phase is its index in the warp's half & 7)
+            const uint8_t* rows = da_sm + (size_t)(warp - kProdWarp - 1) * 64u * 128u;
+            float db[4][2] = {};
+            for (int w = 0; w < n_items; ++w) {
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    bar_sync(kBBarDa, kBDaThreads);                // store_da: the tile is free
+                    bar_sync(kBBarDa, kBDaThreads);                // store_da: dA_c is complete
+#pragma unroll 1
+                    for (uint32_t r4 = 0; r4 < 64u; r4 += 4u) {
+#pragma unroll
+                        for (uint32_t k = 0; k < 4; ++k) {
+                            const uint32_t off = sw128<2>(r4 + k, 2u * (uint32_t)lane);
+                            const uint32_t hi = *reinterpret_cast<const uint32_t*>(rows + off);
+                            const uint32_t lo = *reinterpret_cast<const uint32_t*>(rows + kATileBytes + off);
+                            db[c][0] += bf16_lo_as_f32(hi) + bf16_lo_as_f32(lo);
+                            db[c][1] += bf16_hi_as_f32(hi) + bf16_hi_as_f32(lo);
+                        }
+                    }
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                atomicAdd(&p.dbp[64 * c + 2 * lane], db[c][0]);
+                atomicAdd(&p.dbp[64 * c + 2 * lane + 1], db[c][1]);
             }
         }
         return;
@@ -695,74 +719,60 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         float cpv[8], dhv[8], dciv[8];
         // the cells' global inputs of chunk c, all issued while the tensor pipe runs: each cell loading its own after
         // the previous cell's dc store (which they may alias, as far as the compiler knows) waited one memory round
-        // trip per cell.  c_prev and dh_in are read once per launch: streaming loads (evict-first).
+        // trip per cell.  dh_in and dh_rec are added once all loads are issued, so that no load waits on an add.
+        // c_prev and dh_in are read once per launch: streaming loads (evict-first).
         auto load_cells = [&](int c) {
+            float dhr[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int unit = 16 * c + 2 * j + (q >> 1);
                 const uint32_t o = bo + blocked_off(0, 0, unit);
+                const bool rec = valid && !sp.first;
                 cpv[j] = (valid && sp.c_prev) ? __ldcs(sp.c_prev + o) : 0.f;
                 dhv[j] = (valid && sp.dh_in) ? __ldcs(sp.dh_in + o) : 0.f;
-                const bool rec = valid && !sp.first;
-                if (rec) dhv[j] += p.dh_rec[o];
+                dhr[j] = rec ? p.dh_rec[o] : 0.f;
                 dciv[j] = rec ? p.dc[o] : 0.f;
             }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) dhv[j] += dhr[j];
         };
         uint32_t dpk[32];                                          // dA_c as bf16 planes: [4j, 4j+1] hi, [4j+2, 4j+3] lo
-        // ---- P_c: 8 cells per thread (row row_in_tile, units 16c + 2j + q/2) -> dpk, dc, db ----
+        // ---- P_c: 8 cells per thread (row row_in_tile, units 16c + 2j + q/2) -> dpk, dc ----
         auto cell_epilogue = [&](int c, const float (&g)[32]) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {                          // two halves of 4 cells: half the live fp32 dA
-                float bs[16];                                      // dA of this half's cells: bs[4 jj + gate]
+            for (int j = 0; j < 8; ++j) {
+                const float4 v = frag_to_gates(g, j, odd);
+                const int unit = 16 * c + 2 * j + (q >> 1);
+                const int col = 4 * unit;
+                const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
+                const float4 a = gate_args<CIN>(v, bv, xs, wih_s, col, p.c_in);
+                const uint32_t o = bo + blocked_off(0, 0, unit);
+                const float cp = cpv[j], dh = dhv[j], dci = dciv[j];
+                float gi, gf, gg, go, tc_;
+                lstm_cell_gates8(a.x, a.y, a.z, a.w, cp, gi, gf, gg, go, tc_);
+                // rows past the end: dh = dci = 0, so dA = 0
+                const float dcv = fmaf(dh * go, 1.f - tc_ * tc_, dci);
+                const float da0 = dcv * gg * gi * (1.f - gi);
+                const float da1 = dcv * cp * gf * (1.f - gf);
+                const float da2 = dcv * gi * (1.f - gg * gg);
+                const float da3 = dh * tc_ * go * (1.f - go);
+                if (valid) p.dc[o] = dcv * gf;
+                if (L0) {
 #pragma unroll
-                for (int jj = 0; jj < 4; ++jj) {
-                    const int j = 4 * h + jj;
-                    const float4 v = frag_to_gates(g, j, odd);
-                    const int unit = 16 * c + 2 * j + (q >> 1);
-                    const int col = 4 * unit;
-                    const float4 bv = *reinterpret_cast<const float4*>(p.bias + col);     // scaled here (gate_scale)
-                    const float4 a = gate_args<CIN>(v, make_float4(bv.x * kNegLog2e, bv.y * kNegLog2e, bv.z * kNeg2Log2e,
-                                                                   bv.w * kNegLog2e),
-                                                    xs, wih_s, col, p.c_in);
-                    const uint32_t o = bo + blocked_off(0, 0, unit);
-                    const float cp = cpv[j], dh = dhv[j], dci = dciv[j];
-                    float gi, gf, gg, go, tc_;
-                    lstm_cell_gates8(a.x, a.y, a.z, a.w, cp, gi, gf, gg, go, tc_);
-                    // rows past the end: dh = dci = 0, so dA = 0
-                    const float dcv = fmaf(dh * go, 1.f - tc_ * tc_, dci);
-                    const float da0 = dcv * gg * gi * (1.f - gi);
-                    const float da1 = dcv * cp * gf * (1.f - gf);
-                    const float da2 = dcv * gi * (1.f - gg * gg);
-                    const float da3 = dh * tc_ * go * (1.f - go);
-                    bs[4 * jj + 0] = da0; bs[4 * jj + 1] = da1; bs[4 * jj + 2] = da2; bs[4 * jj + 3] = da3;
-                    if (valid) p.dc[o] = dcv * gf;
-                    if (L0) {
-#pragma unroll
-                        for (int cc = 0; cc < kC; ++cc)
-                            if (CIN == 1 || cc < p.c_in) {
-                                // W_ih is stored pre-scaled: undo kNegLog2e (and the g gate's extra factor 2)
-                                const float4 wv = *reinterpret_cast<const float4*>(&wih_s[cc * kGateCols + col]);
-                                dxs[cc] = fmaf(da0 * wv.x + da1 * wv.y + 0.5f * (da2 * wv.z) + da3 * wv.w, -kLn2, dxs[cc]);
-                            }
-                    }
-                    split_bf16x2(da0, da1, dpk[4 * j], dpk[4 * j + 2]);
-                    split_bf16x2(da2, da3, dpk[4 * j + 1], dpk[4 * j + 3]);
+                    for (int cc = 0; cc < kC; ++cc)
+                        if (CIN == 1 || cc < p.c_in) {
+                            // W_ih is stored pre-scaled: undo kNegLog2e (and the g gate's extra factor 2)
+                            const float4 wv = *reinterpret_cast<const float4*>(&wih_s[cc * kGateCols + col]);
+                            dxs[cc] = fmaf(da0 * wv.x + da1 * wv.y + 0.5f * (da2 * wv.z) + da3 * wv.w, -kLn2, dxs[cc]);
+                        }
                 }
-                // ---- B_c: db[chunk] += column sums of dA_c (rows past the end carry dA = 0) ----
-                // Lanes l ^ 1, ^ 4, ^ 8, ^ 16 hold the same units in other rows.  A reduce-scatter over those 16 lanes
-                // halves the list at each step; afterwards lane l holds the sum of bs[i0] for i0 = 8 b0 + 4 b2 + 2 b3 + b4
-                // (b = the bits of l), i.e. cell 4h + i0 / 4 (unit 16c + 2 (4h + i0 / 4) + q/2), gate i0 % 4.
-                col_sums_step<8>(bs, 1, lane);
-                col_sums_step<4>(bs, 4, lane);
-                col_sums_step<2>(bs, 8, lane);
-                col_sums_step<1>(bs, 16, lane);
-                const int i0 = 8 * (lane & 1) + 4 * ((lane >> 2) & 1) + 2 * ((lane >> 3) & 1) + ((lane >> 4) & 1);
-                atomicAdd(&tail->db[4 * (16 * c + 2 * (4 * h + (i0 >> 2)) + (q >> 1)) + (i0 & 3)], bs[0]);
+                split_bf16x2(da0, da1, dpk[4 * j], dpk[4 * j + 2]);
+                split_bf16x2(da2, da3, dpk[4 * j + 1], dpk[4 * j + 3]);
             }
         };
-        // dpk -> the shared dA tile, once both warpgroups' W / D of the previous chunk have read it
+        // dpk -> the shared dA tile, once both warpgroups' W / D and the B warps of the previous chunk have read it
         auto store_da = [&]() {
-            bar_sync(kBBarCons, kBCons);
+            bar_sync(kBBarDa, kBDaThreads);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const uint32_t off = sw128<2>(row_in_tile, 4 * (2 * j + (q >> 1)));   // gates of unit 16c + 2j + q/2
@@ -770,7 +780,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 *reinterpret_cast<uint2*>(da_sm + kATileBytes + off) = make_uint2(dpk[4 * j + 2], dpk[4 * j + 3]);
             }
             fence_proxy_async_smem();
-            bar_sync(kBBarCons, kBCons);                           // the dA tile (both row halves) is complete
+            bar_sync(kBBarDa, kBDaThreads);                        // the dA tile (both row halves) is complete
         };
         // ---- chunk 0: R_0 alone ----
         {
@@ -791,15 +801,20 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         // (The loop is not unrolled, and no wgmma is behind a branch: either makes ptxas serialise the wgmma.)
 #pragma unroll 1
         for (int c = 1; c < 4; ++c) {
+            // the operand addresses, opaque to the compiler once per chunk: the wgmma descriptors derived from them are
+            // then rebuilt in the uniform datapath at each issue instead of being hoisted out of the loop, where their
+            // 64-bit values outlived P_c and were spilled to local memory
+            uint32_t a_c = a_u, w_c = w_u, wa_c = wa_u, da_c = da_u;
+            asm volatile("" : "+r"(a_c), "+r"(w_c), "+r"(wa_c), "+r"(da_c));
             float g[32];
             wg_fence_regs(g);
             wg_fence_regs(wgr);
             wg_fence_regs(dacc);
             wg_fence();
-            bwd_recompute_mma<PLANES, kNseg>(g, a_u, a_rows, w_u, c);
+            bwd_recompute_mma<PLANES, kNseg>(g, a_c, a_rows, w_c, c);
             wg_commit();
-            bwd_wgrad_mma<PLANES, L0>(wgr, wa_u, da_u);
-            bwd_dgrad_mma<PLANES, kNseg>(dacc, da_u, a_rows, w_u, c - 1);
+            bwd_wgrad_mma<PLANES, L0>(wgr, wa_c, da_c);
+            bwd_dgrad_mma<PLANES, kNseg>(dacc, da_c, a_rows, w_c, c - 1);
             wg_commit();
             load_cells(c);
             wg_wait<1>();
@@ -864,9 +879,6 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             }
         }
     }
-    bar_sync(kBBarCons, kBCons);
-    for (int i = tid; i < kGateCols; i += kBCons)
-        if (n_items > 0) atomicAdd(&p.dbp[i], tail->db[i]);
 }
 
 // Sum the per-CTA weight-gradient slices of one layer and write nn.LSTM-native gradients:
