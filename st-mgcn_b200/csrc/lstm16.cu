@@ -141,6 +141,7 @@ constexpr uint32_t kFBarWg = 1;                        // named barrier kFBarWg 
 constexpr int kHTileBytes = 64 * 128;                  // one plane of a warpgroup's rows: [64 rows][64] bf16 = 8 KB
 constexpr int kFWgBytes = 4 * kHTileBytes;             // per warpgroup: h_prev hi | lo, h_below stage hi | lo
 constexpr int kFCBytes = 64 * kHid * 4;                // per warpgroup: fp32 c of its rows, [32 cells j][128 threads]
+constexpr int kFCellBatch = 8;                         // cells per batch of the cell epilogue (of a thread's 32)
 
 struct F16Tail {
     float bias[kGateCols];
@@ -217,8 +218,10 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
         fence_barrier_init();
     }
     for (int i = tid; i < kGateCols; i += kFThreads) tail->bias[i] = p.bias[i] * gate_scale(i);
+    // rows c_in .. kC-1 of W_ih^T are zeros, so that the cells add all kC channels without a predicate per channel
+    // (x * s of those channels is zero too; the extra fma(0, 0, a) turns at most a -0 into +0, and ex2 of either is 1)
     if (L0)
-        for (int i = tid; i < p.c_in * kGateCols; i += kFThreads) wih_s[i] = p.wih[i] * gate_scale(i);
+        for (int i = tid; i < kC * kGateCols; i += kFThreads) wih_s[i] = i < p.c_in * kGateCols ? p.wih[i] * gate_scale(i) : 0.f;
     __syncthreads();
     const int my_tiles = cta_tiles(p.n_tiles);
 
@@ -340,28 +343,45 @@ __global__ void __launch_bounds__(kFThreads, 1) lstm16_fwd_kernel(const __grid_c
                 ++n_below;
             }
             // ---- LSTM cell: 32 cells per thread, row row_in_tile, units 2j + q/2 ----
-            float* c_out = p.cs + (int64_t)t * cslice;
-            float* h_f32 = t == p.t_len - 1 ? p.h_f32 : nullptr;
+            // In batches of kFCellBatch independent cells: the batch's shuffles, then its shared-memory loads, then the
+            // cells' arithmetic, then its stores.  A cell's loads cannot pass an earlier cell's stores (they may alias,
+            // as far as the compiler knows), so cells written one after another run their MUFU chains strictly in
+            // sequence, with nothing to hide the latency.  The stores are predicated: a branch around a cell's stores
+            // is a scheduling barrier as well.
+            // c_row / h_row: this thread's row of the cs slice and of h_f32; cell j sits at a constant offset from it
+            float* c_row = p.cs + (int64_t)t * cslice + cbase + blocked_off(0, 0, q >> 1);
+            const bool store_h = valid && t == p.t_len - 1 && p.h_f32 != nullptr;    // h_f32 only at t = T-1
+            float* h_row = p.h_f32 + (store_h ? r * (uint32_t)kHid + (uint32_t)(q >> 1) : 0u);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                const float4 v = frag_to_gates(acc, j, odd);
-                const int unit = 2 * j + (q >> 1);
-                const int col = 4 * unit;
-                const float4 bv = *reinterpret_cast<const float4*>(&tail->bias[col]);      // pre-scaled (gate_scale)
-                const float4 a = gate_args<CIN>(v, bv, xs, wih_s, col, p.c_in);
-                const uint32_t co = cbase + blocked_off(0, 0, unit);
-                float cn, hn;
-                lstm_cell_fwd8(a.x, a.y, a.z, a.w, c_sm[128 * j], cn, hn);
-                c_sm[128 * j] = cn;
-                if (valid) {
-                    c_out[co] = cn;
-                    if (h_f32 != nullptr) h_f32[r * (uint32_t)kHid + (uint32_t)unit] = hn;
+            for (int j0 = 0; j0 < 32; j0 += kFCellBatch) {
+                float4 v[kFCellBatch], bv[kFCellBatch];
+                float cp[kFCellBatch], cn[kFCellBatch], hn[kFCellBatch];
+#pragma unroll
+                for (int k = 0; k < kFCellBatch; ++k) v[k] = frag_to_gates(acc, j0 + k, odd);
+#pragma unroll
+                for (int k = 0; k < kFCellBatch; ++k) {
+                    const int col = 4 * (2 * (j0 + k) + (q >> 1));
+                    bv[k] = *reinterpret_cast<const float4*>(&tail->bias[col]);         // pre-scaled (gate_scale)
+                    cp[k] = c_sm[128 * (j0 + k)];
                 }
-                // rows past the end are computed too (a row's gates depend on that row alone) and dropped by the store
-                const uint32_t off = sw128<2>(row_in_wg, (uint32_t)unit);
-                const __nv_bfloat16 hb = __float2bfloat16_rn(hn);
-                *reinterpret_cast<__nv_bfloat16*>(h_sm + off) = hb;
-                if (PLANES == 2) *reinterpret_cast<__nv_bfloat16*>(h_sm + kHTileBytes + off) = __float2bfloat16_rn(hn - __bfloat162float(hb));
+#pragma unroll
+                for (int k = 0; k < kFCellBatch; ++k) {
+                    const int col = 4 * (2 * (j0 + k) + (q >> 1));
+                    const float4 a = gate_args<CIN>(v[k], bv[k], xs, wih_s, col, kC);
+                    lstm_cell_fwd8(a.x, a.y, a.z, a.w, cp[k], cn[k], hn[k]);
+                }
+#pragma unroll
+                for (int k = 0; k < kFCellBatch; ++k) {
+                    const int unit = 2 * (j0 + k) + (q >> 1);
+                    c_sm[128 * (j0 + k)] = cn[k];
+                    if (valid) c_row[blocked_off(0, 0, 2 * (j0 + k))] = cn[k];
+                    if (store_h) h_row[2 * (j0 + k)] = hn[k];
+                    // rows past the end are computed too (a row's gates depend on that row alone) and dropped by the store
+                    const uint32_t off = sw128<2>(row_in_wg, (uint32_t)unit);
+                    const __nv_bfloat16 hb = __float2bfloat16_rn(hn[k]);
+                    *reinterpret_cast<__nv_bfloat16*>(h_sm + off) = hb;
+                    if (PLANES == 2) *reinterpret_cast<__nv_bfloat16*>(h_sm + kHTileBytes + off) = __float2bfloat16_rn(hn[k] - __bfloat162float(hb));
+                }
             }
             // h_t -> the async proxy (the store below, the next step's wgmma)
             fence_proxy_async_smem();
