@@ -44,13 +44,14 @@ CASES = [
 ]
 
 
-def _inputs(n, b, t, lyr, c, state, seed, saturate=False):
+def _inputs(n, b, t, lyr, c, state, seed, saturate=False, device=DEV):
     """``saturate``: the terms the kernels add with fp32 FMAs drive the gates into saturation -- inputs x3 and layer 0's
     W_ih in +-3, biases i +10, f +20, g +-15 (one sign per unit), o uniform in +-50 -- so the pre-activations reach about
     +-70 and c about +-T, while the tensor-core operands W_hh and W_ih of layers > 0 keep their usual +-0.25.  (With
     those in +-2 as well, the two-plane kernel is 5.9e-5 off step-local and 1.1e-4 in the gradients, measured: three
     bf16 passes keep ~16 bits of each product, so the error of a pre-activation grows with sum |W| |h|, here 8-fold,
-    while h stays within +-1.  The one-plane mode, whose reference rounds like the kernel, stayed within its bars.)"""
+    while h stays within +-1.  The one-plane mode, whose reference rounds like the kernel, stayed within its bars.)
+    The draws are made on the CPU; ``device`` is where the tensors land."""
     gen = torch.Generator().manual_seed(seed)
     xo = torch.randn(n, b, t, c, generator=gen) * (3.0 if saturate else 1.0)
     s = 0.2 + 0.8 * torch.rand(b, t, generator=gen)
@@ -71,7 +72,7 @@ def _inputs(n, b, t, lyr, c, state, seed, saturate=False):
         h0 = torch.randn(lyr, n * b, HID, generator=gen) * 0.3
         c0 = torch.randn(lyr, n * b, HID, generator=gen) * 0.5
     d_top = torch.randn(n * b, HID, generator=gen)
-    dev = lambda v: None if v is None else v.to(DEV).contiguous()      # noqa: E731
+    dev = lambda v: None if v is None else v.to(device).contiguous()      # noqa: E731
     return dev(xo), dev(s), dev(h0), dev(c0), [dev(w) for w in ws], dev(d_top)
 
 
