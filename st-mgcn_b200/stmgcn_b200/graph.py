@@ -6,16 +6,19 @@ features (``GCN.py:34-36``).  Here the stack is inspected ONCE per tensor (cache
 
 * if it is a Chebyshev stack -- ``A[0] = I`` and ``A[k] = 2 A[1] A[k-1] - A[k-2]`` (``GCN.py:125-135``),
   checked with a random probe -- only ``L~ = A[1]`` is kept, as CSR + CSR^T on the device, and the forward
-  runs the recurrence on the features (``SupportSet.mode == "cheb"``);
+  runs the recurrence on the features (``SupportSet.mode == "cheb"``, one chain);
 * otherwise (``localpool``, hand-made supports) every slice is sparsified on its own and applied
   directly (``mode == "generic"``) -- same kernels, same results as the reference's einsum.
 
-``ChebSupports`` is the sparse-native handle ``GCN.Adj_Preprocessor.process_sparse`` returns: it quacks
-like the reference's tensor where ``Main.py`` touches it (``.to(device)``, ``len``, ``.shape``) but never
-materialises ``N x N`` matrices (SURVEY.md section 8(f)-1).
+``SparseSupports`` is the sparse-native handle ``GCN.Adj_Preprocessor.process_sparse`` returns (``ChebSupports``
+for ``chebyshev``): it quacks like the reference's tensor where ``Main.py`` touches it (``.to(device)``, ``len``,
+``.shape``) but never materialises ``N x N`` polynomials (SURVEY.md section 8(f)-1).  Its ``"cheb"`` stacks are one or
+more recurrence chains that share ``T_0 = I``: one for ``chebyshev`` (``L~``), two for ``random_walk_diffusion``
+(``P_f^T`` and ``P_b^T``, DCRNN's dual random-walk diffusion).
 """
 from __future__ import annotations
 
+import copy
 from collections import OrderedDict
 from typing import List, Optional
 
@@ -65,11 +68,27 @@ class GraphHandle:
 
 
 class SupportSet:
-    """What the kernels need to know about one ``(Ks, N, N)`` support stack."""
+    """What the kernels need to know about one ``(Ks, N, N)`` support stack.
+
+    ``"cheb"``: ``graphs`` are the recurrence matrices ``X_c`` of chains that share ``T_0 = I``; chain ``c`` owns the
+    segments ``1 + cK .. (c+1)K``, ``T_k(X_c)`` with ``K = (Ks - 1) / len(graphs)`` (no graph when ``Ks == 1``).
+    ``"generic"``: ``graphs[k]`` is ``A_k``.
+    """
 
     def __init__(self, mode: str, n: int, ks: int, graphs: List[GraphHandle], device: torch.device):
         assert mode in ("cheb", "generic")
+        assert len(graphs) == ks if mode == "generic" else (ks - 1) % max(len(graphs), 1) == 0 and (ks == 1) == (not graphs)
         self.mode, self.n, self.ks, self.graphs, self.device = mode, n, ks, graphs, device
+
+    @property
+    def order(self) -> int:
+        """``K`` of each chain (``"cheb"`` only)."""
+        return (self.ks - 1) // len(self.graphs) if self.graphs else 0
+
+    def chain_segments(self, c: int) -> List[int]:
+        """Stack indices of chain ``c``'s terms ``T_0 .. T_K`` (``T_0 = I`` is segment 0 for every chain)."""
+        k = self.order
+        return [0] + list(range(1 + c * k, 1 + (c + 1) * k))
 
     @property
     def nnz(self) -> int:
@@ -105,7 +124,7 @@ _CACHE_MAX = 32
 
 def supports_from_dense(a: torch.Tensor) -> SupportSet:
     """Cached conversion of a dense support stack (keyed on tensor identity + in-place version)."""
-    if isinstance(a, ChebSupports):
+    if isinstance(a, SparseSupports):
         return a.support_set()
     if not isinstance(a, torch.Tensor) or a.dim() != 3 or a.shape[1] != a.shape[2]:
         raise ValueError(f"supports must be a (K, N, N) tensor, got {type(a)} {getattr(a, 'shape', None)}")
@@ -137,16 +156,20 @@ def clear_cache() -> None:
     _CACHE.clear()
 
 
-class ChebSupports:
-    """Sparse-native Chebyshev supports: ``L~`` as CSR plus the number of supports ``Ks``.
+class SparseSupports:
+    """Sparse-native ``(Ks, N, N)`` support stack: the matrices of a :class:`SupportSet` as CSR, nothing ``N x N``.
 
-    Stands in for the dense ``(Ks, N, N)`` tensor of the reference where its callers touch it:
-    ``.to(device)`` (``Main.py:54``), ``len()`` / ``.shape[0]`` (``GCN.py:31``).
+    ``mode == "cheb"``: ``mats`` are the recurrence matrices of the chains (see :class:`SupportSet`);
+    ``mode == "generic"``: ``mats[k]`` is ``A_k``.  Each matrix is an int32 ``rowptr`` / ``colidx``, fp32 ``vals`` triple.
+
+    Stands in for the dense tensor of the reference where its callers touch it: ``.to(device)`` (``Main.py:54``),
+    ``len()`` / ``.shape[0]`` (``GCN.py:31``), ``.device``, ``.is_cuda``.
     """
 
-    def __init__(self, n: int, ks: int, rowptr: torch.Tensor, colidx: torch.Tensor, vals: torch.Tensor):
-        self.n, self.ks = int(n), int(ks)
-        self.rowptr, self.colidx, self.vals = rowptr.to(torch.int32), colidx.to(torch.int32), vals.float()
+    def __init__(self, mode: str, n: int, ks: int, mats):
+        assert mode in ("cheb", "generic") and len(mats) >= 1
+        self.mode, self.n, self.ks = mode, int(n), int(ks)
+        self.mats = [(rp.to(torch.int32), ci.to(torch.int32), v.float()) for rp, ci, v in mats]
         self._sset: Optional[SupportSet] = None
 
     @property
@@ -155,20 +178,23 @@ class ChebSupports:
 
     @property
     def device(self):
-        return self.rowptr.device
+        return self.mats[0][0].device
 
     @property
     def is_cuda(self):
-        return self.rowptr.is_cuda
+        return self.mats[0][0].is_cuda
 
     def __len__(self):
         return self.ks
 
     def to(self, device, *_, **__):
         device = torch.device(device)
-        if device == self.rowptr.device:
+        if device == self.device:
             return self
-        return ChebSupports(self.n, self.ks, self.rowptr.to(device), self.colidx.to(device), self.vals.to(device))
+        moved = copy.copy(self)
+        moved.mats = [tuple(t.to(device) for t in m) for m in self.mats]
+        moved._sset = None
+        return moved
 
     def cuda(self, device=None):
         return self.to(torch.device("cuda", torch.cuda.current_device() if device is None else device))
@@ -176,12 +202,36 @@ class ChebSupports:
     def support_set(self) -> SupportSet:
         if self._sset is None:
             if not self.is_cuda:
-                raise RuntimeError("ChebSupports must be moved to a CUDA device before use (.to(device))")
-            graphs = [GraphHandle.from_csr(self.n, self.rowptr, self.colidx, self.vals)] if self.ks > 1 else []
-            self._sset = SupportSet("cheb", self.n, self.ks, graphs, self.rowptr.device)
+                raise RuntimeError(f"{type(self).__name__} must be moved to a CUDA device before use (.to(device))")
+            mats = self.mats if self.mode == "generic" or self.ks > 1 else []
+            graphs = [GraphHandle.from_csr(self.n, *m) for m in mats]
+            self._sset = SupportSet(self.mode, self.n, self.ks, graphs, self.device)
         return self._sset
+
+    def matrices_dense(self) -> List[torch.Tensor]:
+        """The stored matrices as dense ``(N, N)`` tensors (tests / small graphs only)."""
+        return [torch.sparse_csr_tensor(rp.long(), ci.long(), v, size=(self.n, self.n)).to_dense()
+                for rp, ci, v in self.mats]
+
+
+class ChebSupports(SparseSupports):
+    """Sparse-native Chebyshev supports: ``L~`` as CSR plus the number of supports ``Ks`` (one chain)."""
+
+    def __init__(self, n: int, ks: int, rowptr: torch.Tensor, colidx: torch.Tensor, vals: torch.Tensor):
+        super().__init__("cheb", n, ks, [(rowptr, colidx, vals)])
+
+    @property
+    def rowptr(self):
+        return self.mats[0][0]
+
+    @property
+    def colidx(self):
+        return self.mats[0][1]
+
+    @property
+    def vals(self):
+        return self.mats[0][2]
 
     def laplacian_dense(self) -> torch.Tensor:
         """Dense ``L~`` (tests / small graphs only)."""
-        crow = self.rowptr.long()
-        return torch.sparse_csr_tensor(crow, self.colidx.long(), self.vals, size=(self.n, self.n)).to_dense()
+        return self.matrices_dense()[0]

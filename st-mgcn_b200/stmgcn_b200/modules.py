@@ -62,7 +62,7 @@ class GCN(nn.Module):
         return self.activation(out) if code is None else out
 
     def forward(self, A, x: torch.Tensor):
-        """``A``: (K, N, N) supports (dense tensor as in the reference, or ``ChebSupports``);
+        """``A``: (K, N, N) supports (dense tensor as in the reference, or a ``SparseSupports`` handle);
         ``x``: (batch, N, input_dim) -> (batch, N, hidden_dim).  Reference ``GCN.py:24-43``."""
         assert self.K == A.shape[0]
         sset = supports_from_dense(A)

@@ -92,31 +92,36 @@ def to_bf16(x: torch.Tensor) -> torch.Tensor:
 
 
 def _gather16(sset: SupportSet, x: torch.Tensor) -> bool:
-    """bf16 gather copies: only in the single-plane (bf16 arithmetic) mode, for the recurrence over one graph."""
+    """bf16 gather copies: only in the single-plane (bf16 arithmetic) mode, for the recurrence chains of a "cheb" stack."""
     return lstm_planes() == 1 and sset.mode == "cheb" and (x.numel() // sset.graphs[0].n) % 8 == 0 and x.numel() % 8 == 0
 
 
 def cheb_stack_(sset: SupportSet, s: torch.Tensor, gather16: bool = False) -> None:
-    """Fill ``s[1:]`` from ``s[0]``;  s: (Ks, N, B, p).  ``gather16``: allow bf16 gather copies (bf16-arithmetic mode only)."""
-    ks = sset.ks
-    if sset.mode == "cheb":
-        if ks > 1:
-            g = sset.graphs[0]
-            if gather16 and _gather16(sset, s[0]):
-                # bf16 mode: every step gathers from the bf16 copy of the previous term (half the gather volume)
-                src = to_bf16(s[0])
-                nxt = torch.empty_like(src) if ks > 2 else None
-                for k in range(1, ks):
-                    out16 = nxt if k < ks - 1 else None
-                    spmm_step16(g, False, 1.0 if k == 1 else 2.0, src, 0.0 if k == 1 else -1.0, None if k == 1 else s[k - 2],
-                                0.0, None, s[k], out16)
-                    src, nxt = out16, src
-                return
-            spmm_step(g, False, 1.0, s[0], 0.0, None, 0.0, None, s[1])
-            for k in range(2, ks):
-                spmm_step(g, False, 2.0, s[k - 1], -1.0, s[k - 2], 0.0, None, s[k])
-    else:
+    """Fill ``s[1:]`` from ``s[0]``;  s: (Ks, N, B, p).  ``gather16``: allow bf16 gather copies (bf16-arithmetic mode only).
+
+    One recurrence per chain of the support set (SupportSet), each over its own segments of ``s``."""
+    if sset.mode != "cheb":
         raise AssertionError("generic supports are stacked by cheb_stack_generic")
+    for c, g in enumerate(sset.graphs):
+        _cheb_chain_(g, [s[i] for i in sset.chain_segments(c)], gather16 and _gather16(sset, s[0]))
+
+
+def _cheb_chain_(g, t: List[torch.Tensor], gather16: bool) -> None:
+    """``t[k] = T_k(X) t[0]`` for k >= 1, X the matrix of ``g``: T_1 = X t_0, T_k = 2 X T_{k-1} - T_{k-2}."""
+    ks = len(t)
+    if gather16:
+        # bf16 mode: every step gathers from the bf16 copy of the previous term (half the gather volume)
+        src = to_bf16(t[0])
+        nxt = torch.empty_like(src) if ks > 2 else None
+        for k in range(1, ks):
+            out16 = nxt if k < ks - 1 else None
+            spmm_step16(g, False, 1.0 if k == 1 else 2.0, src, 0.0 if k == 1 else -1.0, None if k == 1 else t[k - 2],
+                        0.0, None, t[k], out16)
+            src, nxt = out16, src
+        return
+    spmm_step(g, False, 1.0, t[0], 0.0, None, 0.0, None, t[1])
+    for k in range(2, ks):
+        spmm_step(g, False, 2.0, t[k - 1], -1.0, t[k - 2], 0.0, None, t[k])
 
 
 def cheb_stack_generic(sset: SupportSet, x: torch.Tensor) -> torch.Tensor:
@@ -139,31 +144,34 @@ def build_stack(sset: SupportSet, x: torch.Tensor, gather16: bool = False) -> to
 def adjoint_stack_(sset: SupportSet, u: torch.Tensor) -> torch.Tensor:
     """Given U_k = dZ W_k^T stacked in ``u`` (Ks, N, B, p) return dX (N, B, p); ``u`` is clobbered.
 
-    cheb: adjoint Clenshaw with L~^T (SURVEY.md section 8(a)); generic: sum_k A_k^T U_k.
+    cheb: one adjoint Clenshaw per chain with X_c^T (SURVEY.md section 8(a)), each adding its part into U_0 (T_0 = I is
+    shared); generic: sum_k A_k^T U_k.
     """
-    ks = sset.ks
     if sset.mode == "cheb":
-        if ks == 1:
-            return u[0]
-        g = sset.graphs[0]
-        k_ord = ks - 1
-        # b_K = U_K (in place).  b_k = U_k + 2 L^T b_{k+1} - b_{k+2}  written over U_k.
-        # (always fp32 gathers here, also in the bf16-arithmetic mode: rounding b_{k+1} to bf16 before every gather puts
-        # ~1.5e-2 into dX on the golden case -- the Clenshaw sum cancels -- and pushed one LSTM weight gradient to 2.2e-2,
-        # past the 2e-2 bar of that mode; measured.  The forward stack keeps its bf16 gather copies.)
-        for k in range(k_ord - 1, 0, -1):
-            z = u[k + 2] if k + 2 <= k_ord else None
-            spmm_step(g, True, 2.0, u[k + 1], -1.0 if z is not None else 0.0, z, 1.0, u[k], u[k])
-        z = u[2] if k_ord >= 2 else None
-        spmm_step(g, True, 1.0, u[1], -1.0 if z is not None else 0.0, z, 1.0, u[0], u[0])
+        for c, g in enumerate(sset.graphs):
+            _adjoint_chain_(g, [u[i] for i in sset.chain_segments(c)])
         return u[0]
     out = torch.empty_like(u[0])
     acc = None
-    for k in range(ks):
+    for k in range(sset.ks):
         tgt = out if (k % 2 == 0) else torch.empty_like(out)
         spmm_step(sset.graphs[k], True, 1.0, u[k], 0.0, None, 1.0 if acc is not None else 0.0, acc, tgt)
         acc = tgt
     return acc
+
+
+def _adjoint_chain_(g, u: List[torch.Tensor]) -> None:
+    """Adjoint of :func:`_cheb_chain_`: ``u[0] += sum_{k>=1} T_k(X)^T u[k]``; ``u[1:]`` is clobbered."""
+    k_ord = len(u) - 1
+    # b_K = U_K (in place).  b_k = U_k + 2 X^T b_{k+1} - b_{k+2}  written over U_k.
+    # (always fp32 gathers here, also in the bf16-arithmetic mode: rounding b_{k+1} to bf16 before every gather puts
+    # ~1.5e-2 into dX on the golden case -- the Clenshaw sum cancels -- and pushed one LSTM weight gradient to 2.2e-2,
+    # past the 2e-2 bar of that mode; measured.  The forward stack keeps its bf16 gather copies.)
+    for k in range(k_ord - 1, 0, -1):
+        z = u[k + 2] if k + 2 <= k_ord else None
+        spmm_step(g, True, 2.0, u[k + 1], -1.0 if z is not None else 0.0, z, 1.0, u[k], u[k])
+    z = u[2] if k_ord >= 2 else None
+    spmm_step(g, True, 1.0, u[1], -1.0 if z is not None else 0.0, z, 1.0, u[0], u[0])
 
 
 _IMAGE_CACHE: "OrderedDict" = OrderedDict()

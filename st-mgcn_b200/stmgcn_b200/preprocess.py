@@ -2,9 +2,10 @@
 sparse-native path of SURVEY.md section 8(f)-1.
 
 ``process(adj)`` returns the same dense ``(K+1, N, N)`` stack the reference returns (so ``Main.py:49-55``
-runs unchanged); ``process_sparse(adj)`` returns a :class:`~stmgcn_b200.graph.ChebSupports` holding only
-the rescaled Laplacian as CSR -- no ``N x N`` polynomial is ever built (the reference needs K dense
-``N^3`` products and 19 GB of supports at 16384 regions).
+runs unchanged); ``process_sparse(adj)`` returns a :class:`~stmgcn_b200.graph.SparseSupports` holding only
+the matrices the kernels multiply by, as CSR (for ``chebyshev`` the rescaled Laplacian, for
+``random_walk_diffusion`` the forward and backward transition matrices) -- no ``N x N`` polynomial is ever built
+(the reference needs K dense ``N^3`` products and 19 GB of supports at 16384 regions).
 
 ``lambda_max``: the reference calls ``torch.eig`` (``GCN.py:117``), which no longer exists in torch >= 1.13;
 its bare ``except`` then uses 2 (``GCN.py:119-121``).  ``lambda_max="reference"`` (default) reproduces that
@@ -16,7 +17,7 @@ from typing import Union
 
 import torch
 
-from .graph import ChebSupports, csr_from_coo
+from .graph import ChebSupports, SparseSupports, csr_from_coo
 
 
 class Adj_Preprocessor(object):
@@ -82,20 +83,47 @@ class Adj_Preprocessor(object):
             kernels = self._polynomials(self.random_walk_normalize(adj).T)
         return torch.stack(kernels, dim=0)
 
-    def process_sparse(self, adj: torch.Tensor) -> ChebSupports:
-        """Chebyshev supports without dense polynomials: only ``L~`` is formed, as CSR.
+    def process_sparse(self, adj: torch.Tensor) -> SparseSupports:
+        """The supports of :meth:`process` without dense polynomials or dense ``N x N`` products: only the matrices the
+        kernels multiply into the features are formed, as CSR.
+
+        * ``chebyshev``: ``L~`` (a :class:`ChebSupports`, ``K+1`` supports, one recurrence chain);
+        * ``random_walk_diffusion``: ``P_f^T`` and ``P_b^T``, ``P_f = D_out^-1 A``, ``P_b = D_in^-1 A^T`` (a zero
+          degree gives ``d_inv = 0``, ``GCN.py:100-104``): the ``2K+1`` bidirectional supports
+          ``[I, T_1(P_f^T) .. T_K(P_f^T), T_1(P_b^T) .. T_K(P_b^T)]`` of the reference's commented-out block
+          (``GCN.py:82-90``), two recurrence chains sharing ``T_0 = I``.  ``A`` may be directed.  At most
+          8 supports (``K <= 3``): the projection kernels take up to 8;
+        * ``localpool``: ``I + D^-1/2 A D^-1/2`` as one generic support.
 
         ``adj`` may be dense ``(N,N)`` or a sparse COO/CSR tensor.  The result is accepted wherever the
         dense stack is (``GCN.forward``, ``ST_MGCN.forward``'s ``sta_adj_list``)."""
-        if self.kernel_type != "chebyshev":
-            raise ValueError("process_sparse is defined for kernel_type='chebyshev' only")
         coo = adj.to_sparse_coo().coalesce() if adj.layout != torch.sparse_coo else adj.coalesce()
         n = coo.shape[0]
         row, col = coo.indices()
         val = coo.values().to(torch.float32)
-        deg = torch.zeros(n, dtype=torch.float32, device=val.device).index_add_(0, row, val)
+        dev = val.device
+        if self.kernel_type == "random_walk_diffusion":
+            ks = 2 * self.K + 1
+            if ks > 8:
+                raise ValueError(f"process_sparse: random_walk_diffusion with K={self.K} needs {ks} supports; the "
+                                 f"projection kernels take at most 8 supports (K <= 3)")
+
+            def inv(deg):
+                d = deg.pow(-1)
+                return torch.where(torch.isinf(d), torch.zeros_like(d), d)
+            d_out = inv(torch.zeros(n, dtype=torch.float32, device=dev).index_add_(0, row, val))
+            d_in = inv(torch.zeros(n, dtype=torch.float32, device=dev).index_add_(0, col, val))
+            # P_f^T[j, i] = A[i, j] / out_deg(i);  P_b^T[i, j] = A[i, j] / in_deg(j)
+            mats = [_csr(n, col, row, val * d_out[row]), _csr(n, row, col, val * d_in[col])]
+            return SparseSupports("cheb", n, ks, mats)
+        deg = torch.zeros(n, dtype=torch.float32, device=dev).index_add_(0, row, val)
         d = deg.pow(-0.5)
         a_norm = d[row] * val * d[col]
+        ar = torch.arange(n, device=dev)
+        if self.kernel_type == "localpool":
+            ones = torch.ones(n, dtype=torch.float32, device=dev)
+            return SparseSupports("generic", n, 1, [_csr(n, torch.cat([row, ar]), torch.cat([col, ar]),
+                                                         torch.cat([a_norm, ones]))])
         if self.lambda_max == "reference":
             lam = 2.0
         elif isinstance(self.lambda_max, (int, float)):
@@ -107,13 +135,9 @@ class Adj_Preprocessor(object):
         diag_val = scale - 1.0
         idx_r, idx_c, vals = row, col, -scale * a_norm
         if diag_val != 0.0:
-            ar = torch.arange(n, device=val.device)
             idx_r, idx_c = torch.cat([idx_r, ar]), torch.cat([idx_c, ar])
-            vals = torch.cat([vals, torch.full((n,), diag_val, dtype=torch.float32, device=val.device)])
-        lt = torch.sparse_coo_tensor(torch.stack([idx_r, idx_c]), vals, (n, n)).coalesce()
-        keep = lt.values() != 0
-        r, c, v = lt.indices()[0][keep], lt.indices()[1][keep], lt.values()[keep]
-        return ChebSupports(n, self.K + 1, *csr_from_coo(n, r, c, v))
+            vals = torch.cat([vals, torch.full((n,), diag_val, dtype=torch.float32, device=dev)])
+        return ChebSupports(n, self.K + 1, *_csr(n, idx_r, idx_c, vals))
 
     @staticmethod
     def _lambda_sparse(n, row, col, a_norm) -> float:
@@ -126,3 +150,10 @@ class Adj_Preprocessor(object):
                 break
             lam, v = nrm / max(float(v.norm()), 1e-30), w / nrm
         return lam
+
+
+def _csr(n: int, rows: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor):
+    """CSR of the ``n x n`` matrix with entries ``(rows, cols, vals)`` in any order (repeats summed, exact zeros dropped)."""
+    m = torch.sparse_coo_tensor(torch.stack([rows, cols]), vals, (n, n)).coalesce()
+    keep = m.values() != 0
+    return csr_from_coo(n, m.indices()[0][keep], m.indices()[1][keep], m.values()[keep])

@@ -67,6 +67,19 @@ def make_adjacency(n: int, m: int, density: float) -> torch.Tensor:
     return a.to(torch.float32)
 
 
+def make_directed_adjacency(n: int, m: int, density: float) -> torch.Tensor:
+    """Dense 0/1 float32 DIRECTED adjacency of graph ``m`` (the ``random_walk_diffusion`` workloads), CPU:
+    ``g = torch.Generator().manual_seed(2000 + m)``; arcs ``rand(N, N) < density``, no self-loops, and a one-way ring
+    ``i -> (i + 1) mod N``, so every region has an out-arc and an in-arc (the Chebyshev normalisation of the same graph,
+    by row sums, stays finite too)."""
+    g = torch.Generator().manual_seed(2000 + m)
+    a = torch.rand(n, n, generator=g) < density
+    idx = torch.arange(n)
+    a[idx, (idx + 1) % n] = True
+    a.fill_diagonal_(False)
+    return a.to(torch.float32)
+
+
 def make_adjacency_list(w: Workload) -> List[torch.Tensor]:
     return [make_adjacency(w.n_regions, m, w.density) for m in range(w.n_graphs)]
 
