@@ -16,7 +16,6 @@ from __future__ import annotations
 
 import math
 import os
-from collections import OrderedDict
 from typing import List, Optional, Sequence
 
 import torch
@@ -174,53 +173,15 @@ def _adjoint_chain_(g, u: List[torch.Tensor]) -> None:
     spmm_step(g, True, 1.0, u[1], -1.0 if z is not None else 0.0, z, 1.0, u[0], u[0])
 
 
-_IMAGE_CACHE: "OrderedDict" = OrderedDict()
-_IMAGE_CACHE_MAX = 48
-
-
-def _cached_images(params: Sequence[torch.Tensor], extra: tuple, pack) -> dict:
-    """Tensor-core operand images of ``params``, as the dict ``pack()`` returns, cached on (storage, in-place version) of
-    every parameter plus ``extra``: re-packed only after an optimizer step changed them.  During CUDA-graph capture the
-    cache is bypassed so the pack kernels become part of the graph (replays see updated weights)."""
-    capturing = torch.cuda.is_current_stream_capturing()
-    key = tuple((w.data_ptr(), w._version) for w in params) + extra + (str(params[0].device),)
-    if not capturing:
-        hit = _IMAGE_CACHE.get(key)
-        if hit is not None:
-            _IMAGE_CACHE.move_to_end(key)
-            _wait_packed(hit)
-            return hit
-    entry = pack()
-    entry["keep"] = list(params)        # keeps the storages alive: a recycled data_ptr can never alias the key
-    if not capturing:
-        entry["event"] = torch.cuda.Event()
-        entry["event"].record()
-        _IMAGE_CACHE[key] = entry
-        while len(_IMAGE_CACHE) > _IMAGE_CACHE_MAX:
-            _IMAGE_CACHE.popitem(last=False)
-    return entry
-
-
-def _wait_packed(entry: dict) -> None:
-    """The current stream waits for the pack kernels of a cached entry (an entry packed during capture has no event)."""
-    if "event" in entry:
-        torch.cuda.current_stream().wait_event(entry["event"])
-
-
 def _proj_images(w: torch.Tensor, ks: int, p: int, need_bwd: bool):
     """Tensor-core operand images (forward, backward or None) of the projection weights (p = q = 64, ks <= 8), or
-    (None, None) when the tensor-core path does not apply."""
+    (None, None) when the tensor-core path does not apply.  Packed from ``w`` as it is now, on every call."""
     if lstm_path() != "tc" or p != 64 or w.shape[1] != 64 or ks > 8:
         return None, None
-
-    def pack():
-        img_f = torch.empty(ks * 64 * 64 * 2, device=w.device, dtype=torch.float32)
-        img_b = torch.zeros((2 if ks > 4 else 1) * 2 * 2 * 256 * 32, device=w.device, dtype=torch.float32) if need_bwd else None
-        _lib.check(L.stmgcn_proj_pack_tc(w.data_ptr(), ks, img_f.data_ptr(), _p(img_b), _stream()), "proj_pack_tc")
-        return dict(fwd=img_f, bwd=img_b)
-
-    img = _cached_images([w], ("proj", ks, need_bwd), pack)
-    return img["fwd"], img["bwd"]
+    img_f = torch.empty(ks * 64 * 64 * 2, device=w.device, dtype=torch.float32)
+    img_b = torch.zeros((2 if ks > 4 else 1) * 2 * 2 * 256 * 32, device=w.device, dtype=torch.float32) if need_bwd else None
+    _lib.check(L.stmgcn_proj_pack_tc(w.data_ptr(), ks, img_f.data_ptr(), _p(img_b), _stream()), "proj_pack_tc")
+    return img_f, img_b
 
 
 def _proj_fwd(s: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], act: int, pool: Optional[torch.Tensor],
@@ -447,7 +408,7 @@ def _unpack_lstm_grads(dwx, dwp, dbp, n_layers: int, hid: int, c_in: int):
 
 
 # --------------------------------------------------------------------------------------------------
-# bf16-plane LSTM path (H = 64): resident weight images cached per parameter version
+# bf16-plane LSTM path (H = 64): weight images packed on every forward
 # --------------------------------------------------------------------------------------------------
 _PLANES = int(os.environ.get("STMGCN_LSTM_PLANES", "2"))     # 2: 3xBF16 (fp32-grade); 1: single-pass bf16 arithmetic
 
@@ -467,21 +428,17 @@ def set_lstm_planes(planes: int) -> None:
 
 def _lstm16_images(weights: Sequence[torch.Tensor], n_layers: int, c_in: int):
     """Operand images of the shared LSTM's parameters for the bf16-plane kernels (stmgcn_lstm16_pack): the flat wimg,
-    bias (L, 256) and wih_t."""
-
-    def pack():
-        dev = weights[0].device
-        wimg = torch.empty(65536 * (2 * n_layers - 1), dtype=torch.uint8, device=dev)
-        bias = torch.empty((n_layers, 256), dtype=torch.float32, device=dev)
-        wih_t = torch.empty(c_in * 256, dtype=torch.float32, device=dev)
-        st = _stream()
-        for l in range(n_layers):
-            w_ih, w_hh, b_ih, b_hh = weights[4 * l:4 * l + 4]
-            _lib.check(L.stmgcn_lstm16_pack(w_ih.data_ptr(), w_hh.data_ptr(), b_ih.data_ptr(), b_hh.data_ptr(), l, c_in,
-                                            wimg.data_ptr(), bias.data_ptr(), wih_t.data_ptr(), st), "lstm16_pack")
-        return dict(wimg=wimg, bias=bias, wih_t=wih_t)
-
-    return _cached_images(weights, ("lstm16", c_in), pack)
+    bias (L, 256) and wih_t, packed from the weights as they are now, on every call."""
+    dev = weights[0].device
+    wimg = torch.empty(65536 * (2 * n_layers - 1), dtype=torch.uint8, device=dev)
+    bias = torch.empty((n_layers, 256), dtype=torch.float32, device=dev)
+    wih_t = torch.empty(c_in * 256, dtype=torch.float32, device=dev)
+    st = _stream()
+    for l in range(n_layers):
+        w_ih, w_hh, b_ih, b_hh = weights[4 * l:4 * l + 4]
+        _lib.check(L.stmgcn_lstm16_pack(w_ih.data_ptr(), w_hh.data_ptr(), b_ih.data_ptr(), b_hh.data_ptr(), l, c_in,
+                                        wimg.data_ptr(), bias.data_ptr(), wih_t.data_ptr(), st), "lstm16_pack")
+    return wimg, bias, wih_t
 
 
 def to_planes(x: torch.Tensor, planes: int) -> torch.Tensor:
@@ -498,19 +455,18 @@ _TAPE16 = ("hp", "cs", "h0p", "c0b", "wimg", "bias", "wih_t")
 
 
 def _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes, keep_tape):
-    """Forward of the bf16-plane path, one library call.  Returns (h_top (N,B,64), h_n, c_n, tape dict or None): the
-    tape holds the _TAPE16 tensors and ``packed``, the image cache entry the backward waits for."""
+    """Forward of the bf16-plane path, one library call after the weight packs.  Returns (h_top (N,B,64), h_n, c_n, tape
+    dict or None): the tape holds the _TAPE16 tensors, the weight images among them."""
     n, b, t_len, c_in = xo.shape
     rows = n * b
     rows_pad = ((rows + 127) // 128) * 128
-    img = _lstm16_images(weights, n_layers, c_in)
+    wimg, bias, wih_t = _lstm16_images(weights, n_layers, c_in)
     hp = torch.empty((n_layers, t_len, planes, rows, 64), device=xo.device, dtype=torch.bfloat16)
     cs = xo.new_empty((n_layers, t_len, rows_pad, 64))
     h0p = to_planes(h0c, planes) if h0c is not None else None        # (L, P, R, 64)
     c0b = to_blocked(c0c) if c0c is not None else None
     h_n = xo.new_empty((n_layers, rows, 64)) if want_state else None
     h_top = h_n[n_layers - 1] if want_state else xo.new_empty((rows, 64))
-    wimg, bias, wih_t = img["wimg"], img["bias"], img["wih_t"]
     _lib.check(L.stmgcn_lstm16_fwd(t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(), wimg.data_ptr(),
                                    bias.data_ptr(), wih_t.data_ptr(), _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(),
                                    h_top.data_ptr(), _p(h_n), _stream()), "lstm16_fwd")
@@ -518,7 +474,7 @@ def _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes,
         c_n = from_blocked(cs[:, t_len - 1], rows)
     else:                       # ST_MGCN discards the final state (STMGCN.py:113)
         h_n = c_n = xo.new_empty(0)
-    tape = dict(hp=hp, cs=cs, h0p=h0p, c0b=c0b, wimg=wimg, bias=bias, wih_t=wih_t, packed=img) if keep_tape else None
+    tape = dict(hp=hp, cs=cs, h0p=h0p, c0b=c0b, wimg=wimg, bias=bias, wih_t=wih_t) if keep_tape else None
     return h_top.view(n, b, 64), h_n, c_n, tape
 
 
@@ -543,7 +499,6 @@ def _lstm16_backward_ex(xo, s_gate, tape, n_layers, planes, d_top, dh_n=None, dc
     """:func:`_lstm16_backward` with the gradients at the inputs and the recurrent state: returns (d_s, grads, (d_xo, dh0,
     dc0)).  dh_n / dc_n (L, R, 64) or None seed the final state's gradients; ``want`` = which of d_xo, dh0, dc0 to compute
     (None otherwise).  Without any of them the plain entry point runs."""
-    _wait_packed(tape["packed"])
     hp, cs, h0p, c0b, wimg, bias, wih_t = (tape[k] for k in _TAPE16)
     n, b, t_len, c_in = xo.shape
     rows = n * b
@@ -663,7 +618,6 @@ class SharedLSTM(torch.autograd.Function):
             h_top, h_n, c_n, tape = _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, ctx.planes,
                                                     need_grad)
             if need_grad:
-                ctx.packed = tape["packed"]
                 tape = [tape[k] for k in _TAPE16]
         else:
             h_top, h_n, c_n, tape = _exact_forward(xo, s_gate, h0c, c0c, n_layers, hid, want_state, weights, need_grad)
@@ -687,7 +641,7 @@ class SharedLSTM(torch.autograd.Function):
             d_top = xo.new_zeros((xo.shape[0], xo.shape[1], hid))
         want = (ctx.needs_input_grad[0], ctx.needs_input_grad[2], ctx.needs_input_grad[3])
         if ctx.planes16:
-            tape16 = dict(zip(_TAPE16, tape), packed=ctx.packed)
+            tape16 = dict(zip(_TAPE16, tape))
             d_s, w_grads, extras = _lstm16_backward_ex(xo, s_gate, tape16, n_layers, ctx.planes, d_top, dh_n, dc_n, want)
         else:
             if getattr(ctx, "tape_consumed", False):

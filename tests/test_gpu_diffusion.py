@@ -298,13 +298,15 @@ def test_negative_controls_fail(control, monkeypatch):
         assert errs["out"] <= TOL            # only the backward is broken
 
 
-# launches of libstmgcn_b200 kernels by one Chebyshev step (3 graphs, K=3, forward + MSE + backward, the weight images
-# already packed), counted on an H100 with the build before the support stacks were parametrised by chain
-CHEB_LAUNCHES = {"planes2": 87, "planes1": 90, "fma": 393}
+# launches of libstmgcn_b200 kernels by one Chebyshev step (3 graphs, K=3, forward + MSE + backward), counted on an H100.
+# The tensor-core columns include the weight packs every forward makes, 5 per graph branch (one per LSTM layer, the
+# spatial projection's forward and backward images); the exact path packs nothing and keeps the count of the build
+# before the support stacks were parametrised by chain
+CHEB_LAUNCHES = {"planes2": 102, "planes1": 105, "fma": 393}
 
 
 @pytest.mark.parametrize("mode", sorted(CHEB_LAUNCHES))
-def test_chebyshev_step_launches_as_many_kernels_as_before(mode):
+def test_chebyshev_step_launch_count_includes_the_weight_packs(mode):
     import GCN
     from stmgcn_b200 import _lib, ops, synth
     from helpers import build_model
