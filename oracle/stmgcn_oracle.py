@@ -20,6 +20,10 @@ Two independent restatements of the reference algorithm (all citations into the 
   out.  It is validated against the dense restatement (and through it against the reference) in
   ``tests/test_oracle.py`` and is the oracle at sizes where dense supports are infeasible.
 
+``BF16ModeReference`` (torch autograd, fp64) is the sparse model once more, in the bf16-arithmetic mode: it rounds where
+the kernels of that mode round and can be forced with the kernels' own values at every rounding point.  With rounding
+off it is pinned to ``SparseOracle`` in ``tests/test_oracle.py``.
+
 Parity pin: the reference has no tests, golden vectors or fixtures of its own (SURVEY.md section 4) --
 "parity unpinned" by the reference's own tests.  The pin used here is the reference code itself,
 imported from a reference checkout (``oracle/make_golden.py`` ->
@@ -27,6 +31,7 @@ imported from a reference checkout (``oracle/make_golden.py`` ->
 """
 from __future__ import annotations
 
+import warnings
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -517,6 +522,193 @@ class SparseOracle:
         loss = float(np.mean(diff * diff))
         grads = self.backward(2.0 * diff / diff.size)
         return out, loss, grads
+
+
+# --------------------------------------------------------------------------------------------------
+# the bf16-arithmetic mode (STMGCN_LSTM_PLANES=1), torch fp64 autograd, optionally forced with the kernels' values
+# --------------------------------------------------------------------------------------------------
+class CsrMatmul(torch.autograd.Function):
+    """``L @ X`` for a sparse CSR ``L`` held together with its transpose: the backward is ``L^T @ G`` (torch's own sparse
+    autograd is not involved)."""
+
+    @staticmethod
+    def forward(ctx, x, lap, lap_t):
+        ctx.lap_t = lap_t
+        return lap @ x
+
+    @staticmethod
+    def backward(ctx, g):
+        return ctx.lap_t @ g, None, None
+
+
+def torch_csr_pair(mat, device="cpu", dtype=torch.float64):
+    """``(L, L^T)`` as torch sparse CSR tensors from a scipy matrix, for :class:`CsrMatmul`."""
+    def conv(m):
+        m = m.tocsr()
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")           # "sparse CSR support is in beta"
+            return torch.sparse_csr_tensor(torch.from_numpy(m.indptr).long(), torch.from_numpy(m.indices).long(),
+                                           torch.from_numpy(m.data).to(dtype), size=m.shape).to(device)
+    return conv(mat), conv(mat.T)
+
+
+class BF16ModeReference:
+    """``ST_MGCN`` / ``CG_LSTM`` in the bf16-arithmetic mode (``ops.set_lstm_planes(1)``), as a torch autograd model in
+    fp64 (or any dtype) on any device.
+
+    The mode rounds at two places, and so does this model (``rounding=True``):
+
+    * the shared LSTM keeps one bf16 hidden-state plane: :func:`lstm_planes_reference` with ``planes=1``;
+    * the spatial GCN's Chebyshev recurrence gathers from bf16 copies, per chain of the support set (one chain ``L~`` for
+      ``chebyshev``, two for ``random_walk_diffusion``, segments as ``SupportSet.chain_segments``):
+      ``S_1 = X bf16(S_0)``, ``S_k = 2 X bf16(S_{k-1}) - S_{k-2}`` with ``S_{k-2}`` in full precision.
+
+    The rounding is straight-through (:func:`round_bf16`), so the autograd backward is the exact adjoint the kernels run
+    (fp32 gathers in the adjoint Clenshaw).  The temporal GCN, the context gate, the projections, the fusion and the
+    output FC are not rounded.  ``rounding=False``: two planes and no bf16 gathers, i.e. the model of
+    :class:`SparseOracle` (fp32-grade mode).
+
+    ``chains[m]``: the recurrence matrices of graph ``m`` (scipy); ``n_supports = 1 + len(chains[m]) * K``.
+    ``relu``: ReLU after both GCNs (else no activation); ``relu_masks`` as for :class:`SparseOracle` (boolean
+    ``(N, B, q)`` arrays or tensors, order temporal 0, spatial 0, temporal 1, ...): ``out = z * mask``.
+
+    ``tapes`` (optional, per graph): the kernels' values at every rounding point, in this model's dtype, rows
+    ``r = n*B + b`` of the windows this model is given -- ``h``, ``c`` (L, T, R, H) and ``h0`` (L, R, H) as
+    :func:`lstm_planes_reference` takes them, and ``s`` (Ks, N, B, H): the spatial stack, ``s[0]`` the fp32 h_top.
+    Every operand of the spatial recurrence, and every stack term the projection reads, then takes the tape's value with
+    the gradient routed through this model's own value (``tape + (computed - computed.detach())``), so each layer-step
+    and each ``S_k`` is one step from the kernels' own inputs and the gradients are the kernels' backward.
+    """
+
+    def __init__(self, params: Dict[str, torch.Tensor], chains, n_supports: int, relu: bool = True,
+                 rounding: bool = True, relu_masks=None, device="cpu", dtype=torch.float64):
+        self.dev, self.dt = torch.device(device), dtype
+        self.p = {k: torch.as_tensor(v).to(self.dev, dtype) for k, v in params.items()}
+        self.chains = [[torch_csr_pair(c, self.dev, dtype) for c in ch] for ch in chains]
+        self.ks, self.relu, self.rounding = n_supports, relu, rounding
+        self.masks = None if relu_masks is None else [torch.as_tensor(mk).to(self.dev, dtype) for mk in relu_masks]
+        self.m = len(chains)
+        self.n_layers = _count_lstm_layers(self.p, "rnn_list.0.lstm.")
+        assert all(ch and (n_supports - 1) % len(ch) == 0 for ch in self.chains) or n_supports == 1
+
+    def leaves(self) -> Dict[str, torch.Tensor]:
+        """Fresh autograd leaves of the parameters (pass them to the methods below)."""
+        return {k: v.detach().clone().requires_grad_(True) for k, v in self.p.items()}
+
+    def _rnd(self, v):
+        return round_bf16(v) if self.rounding else v
+
+    def _stack(self, m, x, spatial: bool, tape_s=None):
+        """x (N, B, p) -> (terms the projection reads, terms as computed): (Ks, N, B*p) each; ``spatial``: the recurrence
+        gathers from bf16 copies (rounding on) and is forced with ``tape_s``."""
+        n = x.shape[0]
+        flat = x.reshape(n, -1)
+        rnd = self._rnd if spatial else (lambda v: v)
+
+        def forced(k, computed):
+            if tape_s is None:
+                return computed
+            return tape_s[k].reshape(n, -1) + (computed - computed.detach())
+        used, comp = [forced(0, flat)] + [None] * (self.ks - 1), [flat] + [None] * (self.ks - 1)
+        chains = self.chains[m] if self.ks > 1 else []
+        k_ord = (self.ks - 1) // max(len(chains), 1)
+        for c, (lap, lap_t) in enumerate(chains):
+            seg = [0] + list(range(1 + c * k_ord, 1 + (c + 1) * k_ord))
+            for j in range(1, len(seg)):
+                y = CsrMatmul.apply(rnd(used[seg[j - 1]]), lap, lap_t)
+                if j > 1:
+                    y = 2.0 * y - used[seg[j - 2]]
+                comp[seg[j]], used[seg[j]] = y, forced(seg[j], y)
+        return used, comp
+
+    def _gcn(self, m, x, w, b, mask_i, spatial, tape_s=None):
+        """act(sum_k S_k W_k + b) on node-major x (N, B, p) -> (out (N, B, q), computed stack terms)."""
+        n, bsz, p = x.shape
+        used, comp = self._stack(m, x, spatial, tape_s)
+        z = sum(used[k].reshape(n, bsz, p) @ w[k * p:(k + 1) * p] for k in range(self.ks))
+        if b is not None:
+            z = z + b
+        if self.relu:
+            z = z * self.masks[mask_i] if self.masks is not None else torch.relu(z)
+        return z, comp
+
+    def cg_lstm_node_major(self, p, m, xo, tape=None, h0=None, c0=None):
+        """Graph ``m``'s ``CG_LSTM`` on node-major xo (N, B, T, C) -> (h_top (N, B, H), h_n, c_n (L, R, H), (hs, cs)):
+        ``hs`` / ``cs`` the computed states of every layer-step (see :func:`lstm_planes_reference`)."""
+        pre = f"rnn_list.{m}."
+        n, bsz, t_len, c_in = xo.shape
+        xt = xo.sum(-1)
+        gt, _ = self._gcn(m, xt, p[pre + "gconv_temporal_feats.W"], p.get(pre + "gconv_temporal_feats.b"), 2 * m,
+                          False)
+        z = (xt + gt).sum(0) / n
+        fw, fb = p[pre + "fc.weight"], p[pre + "fc.bias"]
+        s = torch.sigmoid(torch.relu(z @ fw.t() + fb) @ fw.t() + fb)
+        rows = (xo * s[None, :, :, None]).reshape(n * bsz, t_len, c_in)
+        layers = _lstm_layers(p, pre + "lstm.", self.n_layers)
+        lstm_tape = None if tape is None else {k: tape[k] for k in ("h", "c", "h0") if k in tape}
+        _, (h_n, c_n), (hs, cs) = lstm_planes_reference(rows, layers, 1 if self.rounding else 2, h0, c0, lstm_tape)
+        return hs[-1][-1].reshape(n, bsz, -1), h_n, c_n, (hs, cs)
+
+    def cg_lstm(self, p, obs, hidden=None, tape=None, m=0):
+        """``CG_LSTM.forward`` on graph ``m``: obs (B, T, N, C), ``hidden`` = (h0, c0) (L, B*N, H) with the module's rows
+        ``b*N + n``, or None -> (out (B, N, H), (h_n, c_n)) in the module's layout.  ``tape`` rows are ``n*B + b``."""
+        bsz, _, n, _ = obs.shape
+        h0 = c0 = None
+        if hidden is not None:
+            lyr, _, hid = hidden[0].shape
+            h0, c0 = (v.reshape(lyr, bsz, n, hid).permute(0, 2, 1, 3).reshape(lyr, n * bsz, hid) for v in hidden)
+        h_top, h_n, c_n, _ = self.cg_lstm_node_major(p, m, obs.permute(2, 0, 1, 3), tape, h0, c0)
+        to_module = lambda v: v.reshape(v.shape[0], n, bsz, -1).permute(0, 2, 1, 3).reshape(v.shape[0], bsz * n, -1)  # noqa: E731
+        return h_top.permute(1, 0, 2), (to_module(h_n), to_module(c_n))
+
+    def branch(self, p, m, xo, tape=None):
+        """Graph ``m``'s branch of ``ST_MGCN`` on node-major xo -> dict: ``out`` (N, B, G) and the computed values of
+        every rounding point -- ``hs`` / ``cs`` (per layer, per step) and ``stack`` (spatial S_k, (N, B*H) each)."""
+        h_top, _, _, (hs, cs) = self.cg_lstm_node_major(p, m, xo, tape)
+        g, stack = self._gcn(m, h_top, p[f"gcn_list.{m}.W"], p.get(f"gcn_list.{m}.b"), 2 * m + 1, True,
+                             None if tape is None else tape["s"])
+        return dict(out=g, hs=hs, cs=cs, stack=stack)
+
+    def forward(self, p, obs, tapes=None):
+        """``ST_MGCN.forward``: obs (B, T, N, C) -> y (B, N, C), all branches in one autograd graph."""
+        xo = obs.permute(2, 0, 1, 3)
+        fused = sum(self.branch(p, m, xo, None if tapes is None else tapes[m])["out"] for m in range(self.m))
+        return (fused @ p["fc.weight"].t() + p["fc.bias"]).permute(1, 0, 2)
+
+    def loss_and_grads(self, obs, y, tapes=None, want_obs: bool = False, on_branch=None):
+        """MSE(mean) loss and the gradient of every parameter (and of obs with ``want_obs``), one graph branch in memory
+        at a time: the branches' outputs first (no autograd), then the fusion's gradient, then each branch's backward.
+        ``on_branch(m, branch dict)`` (optional) sees each branch's forward values.  Returns (out, loss, grads)."""
+        obs = torch.as_tensor(obs).to(self.dev, self.dt)
+        y = torch.as_tensor(y).to(self.dev, self.dt)
+        p = self.leaves()
+        xo = obs.permute(2, 0, 1, 3)
+        with torch.no_grad():
+            outs = []
+            for m in range(self.m):
+                br = self.branch(p, m, xo, None if tapes is None else tapes[m])
+                if on_branch is not None:
+                    on_branch(m, br)
+                outs.append(br["out"])
+                del br
+        gs = [o.requires_grad_(True) for o in outs]
+        out = (sum(gs) @ p["fc.weight"].t() + p["fc.bias"]).permute(1, 0, 2)
+        loss = torch.mean((out - y) ** 2)
+        top = torch.autograd.grad(loss, gs + [p["fc.weight"], p["fc.bias"]])
+        grads = {"fc.weight": top[-2], "fc.bias": top[-1]}
+        d_obs = torch.zeros_like(obs) if want_obs else None
+        for m in range(self.m):
+            ob = obs.detach().clone().requires_grad_(want_obs)
+            g = self.branch(p, m, ob.permute(2, 0, 1, 3), None if tapes is None else tapes[m])["out"]
+            keys = [k for k in p if k.startswith((f"rnn_list.{m}.", f"gcn_list.{m}."))]
+            res = torch.autograd.grad(g, [p[k] for k in keys] + ([ob] if want_obs else []), grad_outputs=top[m])
+            grads.update(zip(keys, res))
+            if want_obs:
+                d_obs += res[-1]
+            del g, res
+        if want_obs:
+            grads["obs"] = d_obs
+        return out.detach(), loss.detach(), grads
 
 
 def laplacian_csr_from_supports(supports: torch.Tensor):

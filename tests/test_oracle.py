@@ -272,3 +272,136 @@ def test_sparse_oracle_relu_masks():
     o3, _, g3 = O.SparseOracle(params, laps, k + 1, relu=False, relu_masks=flipped).loss_and_grads(x, y)
     o4, _, g4 = O.SparseOracle(params, laps, k + 1, relu=False).loss_and_grads(x, y)
     assert np.array_equal(o3, o4) and all(np.array_equal(g3[key], g4[key]) for key in g3)
+
+
+def _bf16_case(seed, kind="chebyshev", n=17, m=2, k=3, t=5, b=3, c=2, hid=8, lyr=2, g=6):
+    """A small random model for BF16ModeReference: (params (torch), chains per graph (scipy), n_supports, x, y)."""
+    import diffusion_oracle as D
+    from stmgcn_b200 import synth
+    gen = torch.Generator().manual_seed(seed)
+    if kind == "chebyshev":
+        adjs = [synth.make_adjacency(n, i, 0.3) * (0.2 + torch.rand(n, n, generator=gen)) for i in range(m)]
+        chains = [[O.laplacian_csr_from_supports(O.chebyshev_supports_dense(a.double(), k, lambda_max=1.6))] for a in adjs]
+        ks = k + 1
+    else:
+        adjs = [synth.make_directed_adjacency(n, i, 0.3) for i in range(m)]
+        chains = [D.diffusion_chains_csr(a.double()) for a in adjs]
+        ks = 2 * k + 1
+    params = O.init_params(m, t, c, hid, lyr, g, ks, seed=seed)
+    x, y = torch.randn(b, t, n, c, generator=gen), torch.randn(b, n, c, generator=gen)
+    return params, chains, ks, x, y
+
+
+def test_csr_matmul_backward_is_the_transpose_product():
+    a = sp.random(9, 9, 0.3, format="csr", random_state=0)
+    lap, lap_t = O.torch_csr_pair(a)
+    x = torch.randn(9, 4, dtype=torch.float64, requires_grad=True)
+    g = torch.randn(9, 4, dtype=torch.float64)
+    y = O.CsrMatmul.apply(x, lap, lap_t)
+    (dx,) = torch.autograd.grad(y, x, g)
+    dense = torch.from_numpy(a.toarray())
+    assert torch.allclose(y, dense @ x, rtol=0, atol=1e-14)
+    assert torch.allclose(dx, dense.t() @ g, rtol=0, atol=1e-14)
+
+
+@pytest.mark.parametrize("relu", [True, False])
+def test_bf16_mode_reference_without_rounding_is_the_sparse_oracle(relu):
+    """Rounding off, no tapes: the fp64 torch model is the recurrence-on-features model of SparseOracle -- output, loss,
+    every parameter gradient (one branch at a time through loss_and_grads) and the all-branches forward, to fp64
+    rounding."""
+    for seed, shape in enumerate([dict(), dict(n=23, m=3, k=2, t=4, b=2, c=1, lyr=3), dict(k=1, lyr=1, t=1)]):
+        params, chains, ks, x, y = _bf16_case(seed, **shape)
+        ref = O.BF16ModeReference(params, [ch for ch in chains], ks, relu=relu, rounding=False)
+        out, loss, grads = ref.loss_and_grads(x, y, want_obs=True)
+        orc = O.SparseOracle({k_: v.numpy() for k_, v in params.items()}, [ch[0] for ch in chains], ks, relu=relu)
+        o2, l2, g2 = orc.loss_and_grads(x.numpy(), y.numpy())
+        assert_close(out.numpy(), o2, "forward", 1e-12)
+        assert abs(float(loss) - l2) <= 1e-12 * abs(l2)
+        assert set(grads) == set(g2) | {"obs"}
+        for key in g2:
+            assert_close(grads[key].numpy(), g2[key], f"grad {key}", 1e-12)
+        with torch.no_grad():
+            assert_close(ref.forward(ref.leaves(), x.double()).numpy(), o2, "all-branch forward", 1e-12)
+        # d obs against autograd through the dense restatement
+        xd = x.double().requires_grad_(True)
+        sups = []
+        for ch in chains:
+            lap = torch.from_numpy(ch[0].toarray())
+            polys = [torch.eye(lap.shape[0], dtype=lap.dtype), lap]
+            while len(polys) < ks:
+                polys.append(2.0 * lap @ polys[-1] - polys[-2])
+            sups.append(torch.stack(polys[:ks]))
+        p64 = {k_: v.double() for k_, v in params.items()}
+        (d_obs,) = torch.autograd.grad(torch.mean((O.dense_st_mgcn(p64, xd, sups, relu) - y.double()) ** 2), [xd])
+        assert_close(grads["obs"].numpy(), d_obs.numpy(), "d obs", 1e-10)
+
+
+def test_bf16_mode_reference_without_rounding_is_the_chain_oracle():
+    """random_walk_diffusion (two chains per graph), rounding off: diffusion_oracle.ChainOracle, to fp64 rounding."""
+    import diffusion_oracle as D
+    params, chains, ks, x, y = _bf16_case(4, kind="random_walk_diffusion", k=2)
+    out, loss, grads = O.BF16ModeReference(params, chains, ks, rounding=False).loss_and_grads(x, y)
+    orc = D.ChainOracle({k_: v.numpy() for k_, v in params.items()}, chains, ks)
+    o2, l2, g2 = orc.loss_and_grads(x.numpy(), y.numpy())
+    assert_close(out.numpy(), o2, "forward", 1e-12)
+    for key in g2:
+        assert_close(grads[key].numpy(), g2[key], f"grad {key}", 1e-12)
+
+
+def _own_tapes(ref, x):
+    """The tapes of ``ref``'s own free-running forward, in the layout BF16ModeReference takes."""
+    tapes = {}
+
+    def keep(m, br):
+        n, b = x.shape[2], x.shape[0]
+        tapes[m] = dict(h=torch.stack([torch.stack(v) for v in br["hs"]]), c=torch.stack([torch.stack(v) for v in br["cs"]]),
+                        s=torch.stack(br["stack"]).reshape(ref.ks, n, b, -1))
+    ref.loss_and_grads(x, torch.zeros(x.shape[0], x.shape[2], x.shape[3]), on_branch=keep)
+    return [tapes[m] for m in range(ref.m)]
+
+
+@pytest.mark.parametrize("kind", ["chebyshev", "random_walk_diffusion"])
+def test_bf16_mode_reference_forced_with_its_own_values_changes_nothing(kind):
+    """Rounding on: forced with the tapes of its own free-running forward, the model reproduces its free-running output
+    and gradients to fp64 rounding -- forcing replaces values only, and here the values agree.  And rounding on vs off
+    differ at the bf16 level, above the 1e-4 bar in the output and tenfold in the gradients: the model really rounds."""
+    params, chains, ks, x, y = _bf16_case(7, kind=kind, hid=16, b=4)
+    ref = O.BF16ModeReference(params, chains, ks, relu=True)
+    out, loss, grads = ref.loss_and_grads(x, y, want_obs=True)
+    out_f, loss_f, grads_f = ref.loss_and_grads(x, y, tapes=_own_tapes(ref, x), want_obs=True)
+    assert_close(out_f.numpy(), out.numpy(), "forced forward", 1e-12)
+    assert abs(float(loss_f) - float(loss)) <= 1e-12 * abs(float(loss))
+    for key in grads:
+        assert_close(grads_f[key].numpy(), grads[key].numpy(), f"forced grad {key}", 1e-12)
+    out_o, _, grads_o = O.BF16ModeReference(params, chains, ks, relu=True, rounding=False).loss_and_grads(x, y)
+    assert 3 * TOL < O.max_rel_err(out.numpy(), out_o.numpy()) < 2e-2
+    assert max(O.max_rel_err(grads[k_].numpy(), grads_o[k_].numpy()) for k_ in grads_o) > 1e-3
+
+
+def test_bf16_mode_reference_rounds_the_spatial_gathers_only():
+    """With the tapes of a free-running forward, each spatial term S_k is one step from the tape: 2 X bf16(S_{k-1}) -
+    S_{k-2}.  Moving one tape term by far less than a bf16 ulp moves the next term through S_{k-2} (full precision) but
+    not through the rounded gather; the temporal GCN does not round at all."""
+    params, chains, ks, x, y = _bf16_case(8, k=3, hid=16, b=2, m=1)
+    ref = O.BF16ModeReference(params, chains, ks)
+    tapes = _own_tapes(ref, x)
+    p = ref.leaves()
+    xo = x.double().permute(2, 0, 1, 3)
+    lap = torch.from_numpy(chains[0][0].toarray())
+    with torch.no_grad():
+        s = tapes[0]["s"].reshape(ks, 17, -1)
+        bf = lambda v: v.float().to(torch.bfloat16).double()          # noqa: E731
+        stack = ref.branch(p, 0, xo, tapes[0])["stack"]
+        assert torch.allclose(stack[1], lap @ bf(s[0]), rtol=0, atol=1e-13)
+        for k in range(2, ks):
+            assert torch.allclose(stack[k], 2.0 * lap @ bf(s[k - 1]) - s[k - 2], rtol=0, atol=1e-13)
+        # a change of 1e-12 relative: invisible through bf16(S_1) in S_2, visible through S_1 in S_3
+        pert = dict(tapes[0])
+        pert["s"] = tapes[0]["s"].clone()
+        pert["s"][1] *= 1.0 + 1e-12
+        stack2 = ref.branch(p, 0, xo, pert)["stack"]
+        assert torch.equal(stack2[2], stack[2]) and not torch.equal(stack2[3], stack[3])
+        # the temporal GCN's stack: full precision (the same as without rounding)
+        _, comp = ref._stack(0, xo.sum(-1), False)
+        _, comp_o = O.BF16ModeReference(params, chains, ks, rounding=False)._stack(0, xo.sum(-1), False)
+        assert all(torch.equal(a, b) for a, b in zip(comp, comp_o))
