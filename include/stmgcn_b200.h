@@ -18,6 +18,16 @@
  *   - entries enqueue on the given stream and return; no device synchronisation inside.
  *   - all feature tensors are fp32, "node-major": rows r = n * B + b (region n outer, window b inner),
  *     features contiguous.  (N, B, p) row-major == (N, B*p) row-major == (N*B, p) row-major.
+ *   - non-finite values propagate as torch's IEEE arithmetic does: a NaN or +-Inf in data, weights or supports reaches
+ *     every result that depends on it and no other.  ReLU is torch's (relu(NaN) = NaN; its backward masks with
+ *     out <= 0, so it passes the gradient at NaN), and the tensor-core LSTM's capped exponential keeps a NaN argument.
+ *     Three deviations from a dense torch restatement, by design:
+ *       spmm_stored_entries_only -- the SpMM multiplies stored entries only, so a NaN in X reaches the rows with a
+ *         stored entry in its column, not every row (a dense product forms 0 * NaN);
+ *       inf_through_split_operands -- the 3xTF32 / 3xBF16 operand splits form lo = Inf - Inf = NaN, so an Inf operand
+ *         of a tensor-core product gives NaN where torch gives +-Inf (relu(-Inf) = 0 becomes NaN): still non-finite;
+ *       products_skipped_with_a_zero_initial_state -- without h0 the tensor-core LSTM skips W_hh . 0 at t = 0, so a
+ *         NaN W_hh leaves step 0 finite (the exact-fp32 LSTM forms the product, as torch does).
  */
 #ifndef STMGCN_B200_H_
 #define STMGCN_B200_H_

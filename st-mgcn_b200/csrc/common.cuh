@@ -61,6 +61,14 @@ __device__ __forceinline__ float rcp_ftz_(float x) {
 __device__ __forceinline__ float sigmoidf_(float v) { return rcp_ftz_(1.0f + ex2_ftz_(kNegLog2e * v)); }
 __device__ __forceinline__ float tanhf_(float v) { return fmaf(2.0f, rcp_ftz_(1.0f + ex2_ftz_(kNeg2Log2e * v)), -1.0f); }
 
+// ReLU as torch defines it: NaN stays NaN (fmaxf(NaN, 0) would be 0).  max.NaN is one FMNMX.NAN, as cheap as fmaxf.
+// Its backward masks with out <= 0, which passes the gradient at a NaN output, as torch's does.
+__device__ __forceinline__ float relu_(float v) {
+    float y;
+    asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(y) : "f"(v));
+    return y;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -51,7 +51,12 @@ __host__ __device__ __forceinline__ int64_t blocked_slice(int n_tiles) { return 
 // The kernels keep bias and W_ih PRE-SCALED by the exponent factor of their gate (gate_scale: kNegLog2e for i, f, o and
 // kNeg2Log2e for g), so "accumulator + bias, times -log2(e)" is ONE fma per gate: arg = fma(acc, scale, bias_scaled).
 __device__ __forceinline__ float gate_scale(int col) { return (col & 3) == 2 ? kNeg2Log2e : kNegLog2e; }
-__device__ __forceinline__ float exp_arg_(float a) { return ex2_ftz_(fminf(a, 43.28f)); }      // e^(-v) or e^(-2v), <= e^30
+// min.NaN keeps a NaN argument (fminf(NaN, c) would return the cap, a saturated gate), so a NaN gate stays NaN.
+__device__ __forceinline__ float exp_arg_(float a) {                                          // e^(-v) or e^(-2v), <= e^30
+    float m;
+    asm("min.NaN.f32 %0, %1, %2;" : "=f"(m) : "f"(a), "f"(43.28f));
+    return ex2_ftz_(m);
+}
 // forward: exponent arguments of (i, f, g, o) and c_{t-1} -> c_t, h_t
 __device__ __forceinline__ void lstm_cell_fwd8(float ai, float af, float ag, float ao, float cp, float& c, float& h) {
     const float ei = exp_arg_(ai), ef = exp_arg_(af), eg = exp_arg_(ag), eo = exp_arg_(ao);

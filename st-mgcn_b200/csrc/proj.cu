@@ -1,6 +1,6 @@
 // K2 (exact-fp32 CUDA-core path): the stacked-K projection of the Chebyshev GCN, reference GCN.py:37-42.
 //   forward : out = act( sum_k (T_k X) W_k + b )  -- reads T_0X..T_KX as K+1 A-segments (no torch.cat copy)
-//   backward: dZ = dOut (.) [out>0];  db = sum dZ;  dW_k = (T_k X)^T dZ;  U_k = dZ W_k^T  (SURVEY.md 8(a))
+//   backward: dZ = dOut (.) [!(out <= 0)] (torch's ReLU mask: NaN passes);  db = sum dZ;  dW_k = (T_k X)^T dZ;  U_k = dZ W_k^T  (SURVEY.md 8(a))
 #include "gemm_tall.cuh"
 
 using namespace stmgcn;
@@ -42,7 +42,7 @@ struct ProjEpi {
                 const int n = tile.col(j);
                 if (n >= nc) continue;
                 float v = acc[i][j] + (bias ? bias[n] : 0.f);
-                if (act == STMGCN_ACT_RELU) v = fmaxf(v, 0.f);
+                if (act == STMGCN_ACT_RELU) v = relu_(v);
                 out[r * nc + n] = v;
             }
         }
@@ -98,7 +98,7 @@ dz_kernel(const float* __restrict__ out, const float* __restrict__ d_out, const 
         const int64_t r = e / q;
         const int j = (int)(e - r * q);
         float v = d_out ? d_out[e] : d_bcast[(r % b_inner) * q + j] * scale;
-        if (act == STMGCN_ACT_RELU && !(out[e] > 0.f)) v = 0.f;
+        if (act == STMGCN_ACT_RELU && out[e] <= 0.f) v = 0.f;
         dz[e] = v;
         if (v != 0.f) atomicAdd(&s_db[j], v);
     }

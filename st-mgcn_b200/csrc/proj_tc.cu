@@ -3,7 +3,7 @@
 //             -- the A operand is read segment by segment straight from the Chebyshev stack the SpMM steps wrote
 //             (no torch.cat), split to tf32 hi/lo on its way to shared memory, accumulated in registers by wgmma
 //             (3xTF32, tc_common.cuh)
-//   backward: dZ = dOut (.) [out > 0] is formed in the loader (and written out for the weight-gradient kernel, with
+//   backward: dZ = dOut (.) [!(out <= 0)] is formed in the loader (and written out for the weight-gradient kernel, with
 //             the bias gradient as a by-product);  U[128 x Ks*64] = dZ[128 x 64] . W^T  -> U_k segments;
 //             dW[kd x 64] += [T_kX | T_{k+1}X]^T . dZ per pair of supports (proj_wgrad_tc_kernel)
 // CTA = two warpgroups, one 128-row tile at a time (persistent over tiles); warpgroup w owns rows 64w .. 64w+63 of the
@@ -80,7 +80,7 @@ constexpr size_t psmem() { return 1024 + (size_t)PCfg<N>::kStageBytes + sizeof(P
 struct PParams {
     const float* seg[kMaxSeg];   // forward: A segments (rows x 64)
     int nkb;                     // k-blocks (2 per 64-wide segment)
-    // backward (dz mode): A = d_out (.) [out > 0]
+    // backward (dz mode): A = d_out (.) [!(out <= 0)]
     const float* d_out;          // (rows, 64) or nullptr
     const float* out_act;        // (rows, 64) forward output (mask source)
     int act;
@@ -152,10 +152,10 @@ __global__ void __launch_bounds__(kPThreads, 1) proj_rows_tc_kernel(const __grid
                         d = *reinterpret_cast<const float4*>(p.d_out + r * 64 + koff);
                         if (p.act == STMGCN_ACT_RELU) {
                             const float4 m = *reinterpret_cast<const float4*>(p.out_act + r * 64 + koff);
-                            if (!(m.x > 0.f)) d.x = 0.f;
-                            if (!(m.y > 0.f)) d.y = 0.f;
-                            if (!(m.z > 0.f)) d.z = 0.f;
-                            if (!(m.w > 0.f)) d.w = 0.f;
+                            if (m.x <= 0.f) d.x = 0.f;
+                            if (m.y <= 0.f) d.y = 0.f;
+                            if (m.z <= 0.f) d.z = 0.f;
+                            if (m.w <= 0.f) d.w = 0.f;
                         }
                     }
                     v[i] = d;
@@ -224,7 +224,7 @@ __global__ void __launch_bounds__(kPThreads, 1) proj_rows_tc_kernel(const __grid
                 if (N == 64) {
                     o.x += tail->bias[col];
                     o.y += tail->bias[col + 1];
-                    if (p.act == STMGCN_ACT_RELU) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                    if (p.act == STMGCN_ACT_RELU) { o.x = relu_(o.x); o.y = relu_(o.y); }
                     *reinterpret_cast<float2*>(p.out + r * 64 + col) = o;
                 } else {
                     if ((col >> 6) >= p.ks_out) continue;      // U_k, k = col / 64

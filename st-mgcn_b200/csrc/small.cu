@@ -63,7 +63,7 @@ __global__ void gate_fwd_kernel(const float* __restrict__ pool, int t_len, float
         float acc = fcb[j];
         for (int i = 0; i < t_len; ++i) acc = fmaf(fcw[j * t_len + i], zs[i], acc);
         a1[b * t_len + j] = acc;
-        rs[j] = fmaxf(acc, 0.f);
+        rs[j] = relu_(acc);
     }
     __syncthreads();
     for (int j = threadIdx.x; j < t_len; j += blockDim.x) {
@@ -86,14 +86,14 @@ __global__ void gate_bwd_kernel(const float* __restrict__ d_s, const float* __re
     for (int j = threadIdx.x; j < t_len; j += blockDim.x) {
         const float sv = s[b * t_len + j];
         da2[j] = d_s[b * t_len + j] * sv * (1.f - sv);
-        r1[j] = fmaxf(a1[b * t_len + j], 0.f);
+        r1[j] = relu_(a1[b * t_len + j]);
         zs[j] = z[b * t_len + j];
     }
     __syncthreads();
     for (int i = threadIdx.x; i < t_len; i += blockDim.x) {
         float acc = 0.f;                                     // d r1[i] = sum_j da2[j] fcw[j,i]
         for (int j = 0; j < t_len; ++j) acc = fmaf(da2[j], fcw[j * t_len + i], acc);
-        da1[i] = (a1[b * t_len + i] > 0.f) ? acc : 0.f;
+        da1[i] = (a1[b * t_len + i] <= 0.f) ? 0.f : acc;
     }
     __syncthreads();
     for (int i = threadIdx.x; i < t_len; i += blockDim.x) {
