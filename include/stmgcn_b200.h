@@ -104,7 +104,9 @@ int32_t stmgcn_proj_pack_tc(const float* w, int32_t ks, float* img_fwd, float* i
  * tensor (d_out) or, when d_out_bcast != NULL, the broadcast dOut[r,:] = d_out_bcast[(r % b_inner), :] *
  * bcast_scale (the mean-pool adjoint dz/N, STMGCN.py:42).  dz_work: (rows, q) workspace receiving dZ.
  * Accumulates (+=) dw (ks*p, q) and dbias (q, may be NULL) -- caller zeroes them -- and, if u != NULL,
- * writes U_k = dZ W_k^T into u + k*stride_u (rows x p); wt is then W^T, (q, ks*p) row-major. */
+ * writes U_k = dZ W_k^T into u + k*stride_u (rows x p); wt is then W^T, (q, ks*p) row-major.
+ * dw may be NULL (a frozen W): no dW launch on either path (neither proj_wgrad_tc_kernel nor the FFMA dW); dz_work and u
+ * are written as before.  dw, dbias and u all NULL is STMGCN_ERR_ARG. */
 int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t rows, int32_t p,
                         const float* wt, int32_t q, int32_t act, const float* out, const float* d_out,
                         const float* d_out_bcast, float bcast_scale, int64_t b_inner, float* dz_work,
@@ -115,7 +117,8 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
  * z = pool / n_regions; a1 = z fcw^T + fcb; s = sigmoid(relu(a1) fcw^T + fcb).  All (B, T); fcw (T,T). */
 int32_t stmgcn_gate_fwd(const float* pool, int64_t b, int32_t t, int64_t n_regions, const float* fcw,
                         const float* fcb, float* z, float* a1, float* s, void* stream);
-/* d_s -> d_fcw (+=), d_fcb (+=), d_z (B,T) */
+/* d_s -> d_fcw (+=), d_fcb (+=), d_z (B,T).  d_fcw and d_fcb may be NULL together (a frozen fc): d_z only.  One of
+ * them NULL without the other is STMGCN_ERR_ARG. */
 int32_t stmgcn_gate_bwd(const float* d_s, const float* z, const float* a1, const float* s, int64_t b,
                         int32_t t, const float* fcw, float* d_fcw, float* d_fcb, float* d_z, void* stream);
 
@@ -141,7 +144,9 @@ int32_t stmgcn_lstm_fwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
  * dh_rec / dc as zero without reading them (ST_MGCN discards h_n / c_n, STMGCN.py:113); stmgcn_lstm_bwd_ex seeds them.
  * gates is overwritten IN PLACE with the pre-activation gradients dA, so it serves one backward only.
  * Accumulates (+=; caller zeroes): d_s (B,T) = sum_{n,c} dxmod * xo (gate adjoint, STMGCN.py:44), dwx (C,4H),
- * dwp (laid out like wp) += [h_below_t | h_{t-1}]^T dA summed over all (t, r), dbp (L, 4H). */
+ * dwp (laid out like wp) += [h_below_t | h_{t-1}]^T dA summed over all (t, r), dbp (L, 4H).
+ * dwx, dwp and dbp may be NULL together (frozen LSTM weights): the per-layer reduce GEMMs and the bias / dwx sums are
+ * skipped, everything else is as with them.  A mix of NULL and non-NULL is STMGCN_ERR_ARG. */
 int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid, int32_t c_in, int64_t b_inner,
                         const float* xo, const float* s_gate, const float* wx, const float* wpt, const float* h0,
                         const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
@@ -152,7 +157,7 @@ int32_t stmgcn_lstm_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t h
  *   dh_n, dc_n: incoming gradients of the final state h_n = hs[:, T-1] / c_n = cs[:, T-1] (dh_n[L-1] adds to d_top);
  *   dh0, dc0  : overwritten with the gradients of h0 / c0 (of the zero initial state when h0 / c0 are NULL).
  * d_xo: (R, T, C) overwritten with the gradient of xo (d xo = dxmod * s[b, t]), or NULL.
- * With every extra NULL this is stmgcn_lstm_bwd, launch for launch. */
+ * With every extra NULL this is stmgcn_lstm_bwd, launch for launch; dwx, dwp, dbp may be NULL together as there. */
 int32_t stmgcn_lstm_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_t hid, int32_t c_in, int64_t b_inner,
                            const float* xo, const float* s_gate, const float* wx, const float* wpt, const float* h0,
                            const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
@@ -201,7 +206,10 @@ int32_t stmgcn_lstm16_grid(int64_t rows);
  *   NULL when L = 1);   dw_scratch: (stmgcn_lstm16_grid(rows), 128*256);   dbp: (L, 256);
  *   zero_tile: 16 KB of zeros (the h_prev operand at t = 0 without an initial state).
  * Accumulates (+=; caller zeroes) d_s (B,T) = sum_{n,c} dxmod * xo (gate adjoint, STMGCN.py:44).  Overwrites grads: one
- * flat buffer in nn.LSTM parameter order, per layer d_w_ih (256, in_l) | d_w_hh (256, 64) | d_b_ih (256) | d_b_hh (256). */
+ * flat buffer in nn.LSTM parameter order, per layer d_w_ih (256, in_l) | d_w_hh (256, 64) | d_b_ih (256) | d_b_hh (256).
+ * grads may be NULL (frozen LSTM weights), and dw_scratch and dbp with it: no weight or bias gradients for any layer --
+ * each layer's launch runs the kernel variant without the weight-gradient stage and the slice-sum launch is skipped.
+ * Every other output is bit-identical to the call with grads. */
 int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner, int32_t planes,
                           const float* xo, const float* s_gate, const void* wimg, const float* bias, const float* wih_t,
                           const void* h0p, const float* c0, const void* hp, const float* cs, const float* d_top,
@@ -214,7 +222,7 @@ int32_t stmgcn_lstm16_bwd(int32_t t_len, int32_t n_layers, int64_t rows, int32_t
  *               layer's launch (the other one zeroed when only one is given);
  *   dh0, dc0  : overwritten with the gradients of the initial state (of the zero state when h0p / c0 are NULL);
  *   d_xo      : (R, T, C) overwritten with the gradient of xo, or NULL.
- * With every extra NULL this is stmgcn_lstm16_bwd, launch for launch. */
+ * With every extra NULL this is stmgcn_lstm16_bwd, launch for launch; grads (with dw_scratch, dbp) may be NULL as there. */
 int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_t c_in, int64_t b_inner, int32_t planes,
                              const float* xo, const float* s_gate, const void* wimg, const float* bias, const float* wih_t,
                              const void* h0p, const float* c0, const void* hp, const float* cs, const float* d_top,
@@ -227,7 +235,8 @@ int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int3
 int32_t stmgcn_fuse_out_fwd(const float* const* g, int32_t m, int64_t n, int64_t b, int32_t gdim,
                             int32_t c, const float* fcw, const float* fcb, float* feat, float* y,
                             void* stream);
-/* d_y (B,N,C) -> d_feat (R,G), d_fcw (C,G) +=, d_fcb (C) += */
+/* d_y (B,N,C) -> d_feat (R,G), d_fcw (C,G) +=, d_fcb (C) +=.  d_fcw and d_fcb may be NULL together (a frozen output fc):
+ * d_feat only.  One of them NULL without the other is STMGCN_ERR_ARG. */
 int32_t stmgcn_fuse_out_bwd(const float* d_y, const float* feat, int64_t n, int64_t b, int32_t gdim,
                             int32_t c, const float* fcw, float* d_feat, float* d_fcw, float* d_fcb,
                             void* stream);

@@ -117,7 +117,7 @@ __global__ void __launch_bounds__(256)
 lstm_bwd_pointwise_kernel(int64_t rows, int hid, float* __restrict__ gates, const float* __restrict__ c_t,
                           const float* __restrict__ c_prev, const float* __restrict__ dh_in,
                           const float* __restrict__ dh_rec, float* __restrict__ dc,
-                          float* __restrict__ dbp,            // (4H) +=
+                          float* __restrict__ dbp,            // (4H) +=, or nullptr: no bias / dwx gradients
                           // layer-0 extras (wx == nullptr otherwise)
                           const float* __restrict__ wx, float* __restrict__ dwx, const float* __restrict__ xo,
                           const float* __restrict__ sg, float* __restrict__ d_s, int c_in, int t, int t_len,
@@ -211,10 +211,11 @@ lstm_bwd_pointwise_kernel(int64_t rows, int hid, float* __restrict__ gates, cons
         }
     }
     // CTA reduction of the bias / wx gradients through shared memory, then one global atomic per entry
+    const bool wgrad = dbp != nullptr;
 #pragma unroll
     for (int u = 0; u < kMaxUnitsPerLane; ++u) {
         const int unit = lane + 32 * u;
-        if (u >= ul || unit >= hid) continue;
+        if (!wgrad || u >= ul || unit >= hid) continue;
         atomicAdd(&s_db[4 * unit + 0], acc_b[u].x);
         atomicAdd(&s_db[4 * unit + 1], acc_b[u].y);
         atomicAdd(&s_db[4 * unit + 2], acc_b[u].z);
@@ -232,9 +233,9 @@ lstm_bwd_pointwise_kernel(int64_t rows, int hid, float* __restrict__ gates, cons
         }
     }
     __syncthreads();
-    for (int e = threadIdx.x; e < h4; e += blockDim.x) atomicAdd(&dbp[e], s_db[e]);
+    if (wgrad) for (int e = threadIdx.x; e < h4; e += blockDim.x) atomicAdd(&dbp[e], s_db[e]);
     if (wx != nullptr) {
-        for (int e = threadIdx.x; e < c_in * h4; e += blockDim.x) atomicAdd(&dwx[e], s_dwx[e]);
+        if (wgrad) for (int e = threadIdx.x; e < c_in * h4; e += blockDim.x) atomicAdd(&dwx[e], s_dwx[e]);
         if (ds_in_smem)
             for (int e = threadIdx.x; e < b_inner; e += blockDim.x) atomicAdd(&d_s[(int64_t)e * t_len + t], s_ds[e]);
     }
@@ -311,8 +312,12 @@ int32_t stmgcn_lstm_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_
                            const float* c0, const float* cs, const float* hs, float* gates, const float* d_top,
                            float* dh_rec, float* dc, float* dx_work, float* d_s, float* dwx, float* dwp, float* dbp,
                            const float* dh_n, const float* dc_n, float* dh0, float* dc0, float* d_xo, void* stream) {
-    STMGCN_REQUIRE(xo && s_gate && wx && wpt && cs && hs && gates && dh_rec && dc && dx_work && d_s && dwx && dwp && dbp,
-                   STMGCN_ERR_ARG, "lstm_bwd: null pointer");
+    STMGCN_REQUIRE(xo && s_gate && wx && wpt && cs && hs && gates && dh_rec && dc && dx_work && d_s, STMGCN_ERR_ARG,
+                   "lstm_bwd: null pointer");
+    // dwx, dwp and dbp all NULL: no weight or bias gradients (no reduce GEMMs, no bias sums)
+    const bool wgrad = dwx != nullptr;
+    STMGCN_REQUIRE((dwp != nullptr) == wgrad && (dbp != nullptr) == wgrad, STMGCN_ERR_ARG,
+                   "lstm_bwd: dwx, dwp and dbp go together");
     if (int32_t rc = check_dims("lstm_bwd", t_len, n_layers, rows, hid, c_in, b_inner)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t rh = rows * hid;
@@ -337,9 +342,9 @@ int32_t stmgcn_lstm_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_
             size_t smem = (size_t)h4 * (1 + (l0 ? c_in : 0)) * sizeof(float);
             if (l0 && b_inner <= 2048) smem += (size_t)b_inner * sizeof(float);
             lstm_bwd_pointwise_kernel<<<grid_pw, 256, smem, st>>>(
-                rows, hid, g_lt, c_t, c_prev, dh_in, dh_rec + (int64_t)l * rh, dc + (int64_t)l * rh, dbp + (int64_t)l * h4,
-                l0 ? wx : nullptr, l0 ? dwx : nullptr, xo, s_gate, d_s, c_in, t, t_len, b_inner, l0 ? d_xo : nullptr,
-                seeded);
+                rows, hid, g_lt, c_t, c_prev, dh_in, dh_rec + (int64_t)l * rh, dc + (int64_t)l * rh,
+                wgrad ? dbp + (int64_t)l * h4 : nullptr, l0 ? wx : nullptr, l0 ? dwx : nullptr, xo, s_gate, d_s, c_in, t,
+                t_len, b_inner, l0 ? d_xo : nullptr, seeded);
             count_launch();
             if (int32_t rc = check_launch("lstm_bwd_pointwise")) return rc;
             // data gradients: [dx_below | dh_rec] = dA . wpt_l      (dA: rows x 4H, wpt_l: 4H x kd_l)
@@ -365,7 +370,7 @@ int32_t stmgcn_lstm_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int32_
     if (dh0 != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dh0, dh_rec, state_bytes, cudaMemcpyDeviceToDevice, st));
     if (dc0 != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dc0, dc, state_bytes, cudaMemcpyDeviceToDevice, st));
     // weight gradients: dwp_l (kd_l, 4H) += [h_below_t | h_{t-1}]^T dA summed over all (t, r)
-    for (int l = 0; l < n_layers; ++l) {
+    for (int l = 0; l < n_layers && wgrad; ++l) {
         ASegs a{};
         ReduceTime tm{};
         a.segw = hid;

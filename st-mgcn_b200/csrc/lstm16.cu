@@ -587,9 +587,15 @@ __device__ __forceinline__ void bwd_wgrad_red(float* slice, const float (&wgr)[3
     }
 }
 
-template <int PLANES, int CIN>                                  // CIN: see lstm16_fwd_kernel
+// CIN: see lstm16_fwd_kernel.  WGRAD = false: the variant for a caller that wants no weight gradients -- the schedule
+// above with the W_c wgmma, their red.add flushes and the B_c warps compiled out (everything else in the same order:
+// the W_3 commit group stays, empty, so the A planes are still released after the item's last wait for it; the dA tile
+// is released by the D_c waits alone).  p.dbp and p.dw_slice are not used.
+template <int PLANES, int CIN, bool WGRAD>
 __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_constant__ Bwd16Params p) {
     constexpr bool L0 = CIN > 0;
+    // threads of the dA tile's named barrier: the consumers, and the B_c warps when they sum the bias gradient
+    constexpr uint32_t kDaThreads = WGRAD ? kBDaThreads : (uint32_t)kBCons;
     constexpr int kC = (CIN == 1) ? 1 : kMaxC;
     constexpr int kNseg = L0 ? 1 : 2;
     extern __shared__ uint8_t smem_raw[];
@@ -659,7 +665,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                             if (sp1.src[sg] != 2) tma_prefetch_3d(&p.maps[sp1.src[sg]], 0, tile1 * kTileM, sp1.slice[sg] + pl);
                 }
             }
-        } else if (warp > kProdWarp && warp <= kProdWarp + kBDbWarps && n_items > 0) {
+        } else if (WGRAD && warp > kProdWarp && warp <= kProdWarp + kBDbWarps && n_items > 0) {
             // ---- B_c: bias gradient, column sums of every dA_c tile (hi + lo; rows past the end carry dA = 0) ----
             // Warp kProdWarp + 1 + h sums rows 64h .. 64h + 63, lane l the columns 2l, 2l + 1 of each chunk: a warp reads one
             // 128-byte tile row per load, conflict free.  The tile is read between store_da's second barrier (complete)
@@ -706,7 +712,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     const uint32_t w_u = smem_u32(w_sm), a_u = smem_u32(a_sm), da_u = smem_u32(da_sm);
     const uint32_t a_rows = (uint32_t)wg * 64u * 128u;             // this warpgroup's rows inside a 128-row tile
     const uint32_t wa_u = a_u + (uint32_t)(wg * 2) * kATileBytes;  // W_c's A operand: this warpgroup's kd rows
-    float* slice = p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols);
+    float* slice = WGRAD ? p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols) : nullptr;
     mbar_wait_raw(&tail->w_full, 0);
 
     for (int w = 0; w < n_items; ++w) {
@@ -726,7 +732,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         }
         // the previous item's stores (dh_rec, dc of other threads' cells) and its reads of the shared tiles are complete
         bar_sync(kBBarCons, kBCons);
-        if (L0 && (q >> 1) == 0) {
+        if (WGRAD && L0 && (q >> 1) == 0) {
             // auxiliary weight-gradient operand (seg-1 slots): row = this thread's row, columns 0..C-1 = x*s (hi / lo split)
             uint32_t hi[2], lo[2];
             split_bf16x2(xs[0], xs[1], hi[0], lo[0]);
@@ -797,7 +803,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         };
         // dpk -> the shared dA tile, once both warpgroups' W / D and the B warps of the previous chunk have read it
         auto store_da = [&]() {
-            bar_sync(kBBarDa, kBDaThreads);
+            bar_sync(kBBarDa, kDaThreads);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const uint32_t off = sw128<2>(row_in_tile, 4 * (2 * j + (q >> 1)));   // gates of unit 16c + 2j + q/2
@@ -805,7 +811,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
                 *reinterpret_cast<uint2*>(da_sm + kATileBytes + off) = make_uint2(dpk[4 * j + 2], dpk[4 * j + 3]);
             }
             fence_proxy_async_smem();
-            bar_sync(kBBarDa, kBDaThreads);                        // the dA tile (both row halves) is complete
+            bar_sync(kBBarDa, kDaThreads);                         // the dA tile (both row halves) is complete
         };
         // ---- chunk 0: R_0 alone ----
         {
@@ -833,12 +839,12 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             asm volatile("" : "+r"(a_c), "+r"(w_c), "+r"(wa_c), "+r"(da_c));
             float g[32];
             wg_fence_regs(g);
-            wg_fence_regs(wgr);
+            if constexpr (WGRAD) wg_fence_regs(wgr);
             wg_fence_regs(dacc);
             wg_fence();
             bwd_recompute_mma<PLANES, kNseg>(g, a_c, a_rows, w_c, c);
             wg_commit();
-            bwd_wgrad_mma<PLANES, L0>(wgr, wa_c, da_c);
+            if constexpr (WGRAD) bwd_wgrad_mma<PLANES, L0>(wgr, wa_c, da_c);
             bwd_dgrad_mma<PLANES, kNseg>(dacc, da_c, a_rows, w_c, c - 1);
             wg_commit();
             load_cells(c);
@@ -846,25 +852,25 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             wg_fence_regs(g);
             cell_epilogue(c, g);
             wg_wait<0>();
-            wg_fence_regs(wgr);
+            if constexpr (WGRAD) wg_fence_regs(wgr);
             wg_fence_regs(dacc);
-            bwd_wgrad_red(slice, wgr, rw0, q, c - 1);
+            if constexpr (WGRAD) bwd_wgrad_red(slice, wgr, rw0, q, c - 1);
             store_da();
         }
         // ---- chunk 3's gradients: W_3 alone first, so that the A planes go back to the producer before D_3 is done ----
-        wg_fence_regs(wgr);
+        if constexpr (WGRAD) wg_fence_regs(wgr);
         wg_fence_regs(dacc);
         wg_fence();
-        bwd_wgrad_mma<PLANES, L0>(wgr, wa_u, da_u);
+        if constexpr (WGRAD) bwd_wgrad_mma<PLANES, L0>(wgr, wa_u, da_u);
         wg_commit();
         bwd_dgrad_mma<PLANES, kNseg>(dacc, da_u, a_rows, w_u, 3);
         wg_commit();
         wg_wait<1>();
-        wg_fence_regs(wgr);
+        if constexpr (WGRAD) wg_fence_regs(wgr);
         // the A planes of this item have been read by every MMA: one arrival per warpgroup
         bar_sync(kBBarWg + wg, 128);
         if ((tid & 127) == 0) mbar_arrive(&tail->a_empty);
-        bwd_wgrad_red(slice, wgr, rw0, q, 3);
+        if constexpr (WGRAD) bwd_wgrad_red(slice, wgr, rw0, q, 3);
         wg_wait<0>();
         wg_fence_regs(dacc);
         // ---- [dx_below | dh_prev] fragment -> tile-blocked workspaces ----
@@ -1064,8 +1070,10 @@ extern "C" int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t
                                         float* dx_work, float* dw_scratch, float* dbp, const void* zero_tile, float* d_s,
                                         float* grads, const float* dh_n, const float* dc_n, float* dh0, float* dc0,
                                         float* d_xo, void* stream) {
-    STMGCN_REQUIRE(xo && s_gate && wimg && bias && hp && cs && d_top && dh_rec && dc && dw_scratch && dbp && zero_tile && d_s &&
-                       grads,
+    // grads NULL: no weight or bias gradients (dw_scratch and dbp are then unused and may be NULL too)
+    const bool wgrad = grads != nullptr;
+    STMGCN_REQUIRE(xo && s_gate && wimg && bias && hp && cs && d_top && dh_rec && dc && zero_tile && d_s &&
+                       (!wgrad || (dw_scratch && dbp)),
                    STMGCN_ERR_ARG, "lstm16_bwd: null pointer");
     if (int32_t rc = check_dims16("lstm16_bwd", t_len, n_layers, rows, c_in, b_inner, planes, wih_t, h0p, c0)) return rc;
     STMGCN_REQUIRE(t_len <= kBMaxSteps, STMGCN_ERR_SHAPE, "lstm16_bwd: T=%d (max %d)", t_len, kBMaxSteps);
@@ -1095,17 +1103,19 @@ extern "C" int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t
     // one launch covers all timesteps of a layer (t_len <= kBMaxSteps); the weight-gradient partials of every chunk are
     // added into fp32 memory, so the length of the run does not lengthen any tensor-core accumulation chain
     p.n_steps = t_len;
-    STMGCN_CUDA(cudaMemsetAsync(dbp, 0, (size_t)n_layers * kGateCols * sizeof(float), st));
+    if (wgrad) STMGCN_CUDA(cudaMemsetAsync(dbp, 0, (size_t)n_layers * kGateCols * sizeof(float), st));
     // top-down: layer l reads the dx that layer l + 1 wrote into one half of dx_work and writes its own into the other
     const float* dh_in = d_top;
     for (int l = n_layers - 1; l >= 0; --l) {
-        const auto fn = kernel_for([](auto P, auto C) { return lstm16_bwd_kernel<P.value, C.value>; }, planes, l, c_in);
+        const auto fn = kernel_for([wgrad](auto P, auto C) {
+            return wgrad ? lstm16_bwd_kernel<P.value, C.value, true> : lstm16_bwd_kernel<P.value, C.value, false>;
+        }, planes, l, c_in);
         if (int32_t rc = ensure_dyn_smem((const void*)fn, kBSmem)) return rc;
         float* dx_out = l > 0 ? dx_work + (int64_t)((n_layers - 1 - l) % 2) * t_len * cslice : nullptr;
         p.wimg = (const uint8_t*)wimg + wimg_off(l);
         p.bias = bias + (int64_t)l * kGateCols;
         p.wih = l == 0 ? wih_t : nullptr;
-        p.dbp = dbp + (int64_t)l * kGateCols;
+        p.dbp = wgrad ? dbp + (int64_t)l * kGateCols : nullptr;
         p.d_xo = l == 0 ? d_xo : nullptr;
         if (seeded) {
             // the gradients of h_n[l] / c_n[l] are what the step at T-1 reads as the incoming dh_rec / dc
@@ -1139,13 +1149,15 @@ extern "C" int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t
             sp.dx_out = l > 0 ? dx_out + (int64_t)t * cslice : nullptr;
         }
         // every CTA adds into its own slice: start from zero
-        STMGCN_CUDA(cudaMemsetAsync(dw_scratch, 0, (size_t)grid * kTileM * kGateCols * sizeof(float), st));
+        if (wgrad) STMGCN_CUDA(cudaMemsetAsync(dw_scratch, 0, (size_t)grid * kTileM * kGateCols * sizeof(float), st));
         fn<<<grid, kBThreads, kBSmem, st>>>(p);
         count_launch();
         if (int32_t rc = check_launch("lstm16_bwd")) return rc;
         // after the step at t = 0, dh_rec / dc hold the gradients of h0[l] / c0[l]: out before the next layer reuses them
         if (dh0 != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dh0 + (int64_t)l * cslice, dh_rec, slice_bytes, cudaMemcpyDeviceToDevice, st));
         if (dc0 != nullptr) STMGCN_CUDA(cudaMemcpyAsync(dc0 + (int64_t)l * cslice, dc, slice_bytes, cudaMemcpyDeviceToDevice, st));
+        dh_in = dx_out;
+        if (!wgrad) continue;
         // the slices -> this layer's d_w_ih (256, in_l) | d_w_hh (256, 64) | d_b_ih | d_b_hh, before the next layer
         // reuses dw_scratch
         const int in_l = l == 0 ? c_in : kHid;
@@ -1155,7 +1167,6 @@ extern "C" int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t
                                                                                g + kGateCols * (in_l + kHid + 1));
         count_launch();
         if (int32_t rc = check_launch("lstm16_wgrad_reduce")) return rc;
-        dh_in = dx_out;
     }
     return 0;
 }

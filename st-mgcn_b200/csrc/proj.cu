@@ -198,7 +198,9 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
                         int32_t q, int32_t act, const float* out, const float* d_out, const float* d_out_bcast,
                         float bcast_scale, int64_t b_inner, float* dz_work, float* dw, float* dbias, float* u,
                         int64_t stride_u, const float* wimg_t, void* stream) {
-    STMGCN_REQUIRE(s && out && dz_work && dw, STMGCN_ERR_ARG, "proj_bwd: null pointer");
+    STMGCN_REQUIRE(s && out && dz_work, STMGCN_ERR_ARG, "proj_bwd: null pointer");
+    // dw NULL: no dW launches; dZ (and the bias gradient / U when asked for) as before
+    STMGCN_REQUIRE(dw || dbias || u, STMGCN_ERR_ARG, "proj_bwd: dw, dbias and u all NULL (nothing to compute)");
     STMGCN_REQUIRE((d_out != nullptr) != (d_out_bcast != nullptr), STMGCN_ERR_ARG,
                    "proj_bwd: exactly one of d_out / d_out_bcast");
     STMGCN_REQUIRE(ks >= 1 && ks <= kMaxSegs, STMGCN_ERR_SHAPE, "proj_bwd: %d supports (max %d)", ks, kMaxSegs);
@@ -221,7 +223,8 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
         count_launch();
         if (int32_t rc = check_launch("proj_bwd dz")) return rc;
     }
-    if (ks * p * q <= kSmallThreads * kSmallMaxPerThread && (size_t)kSmallRows * (ks * p + q) * 4 <= 48 * 1024) {
+    const bool small = ks * p * q <= kSmallThreads * kSmallMaxPerThread && (size_t)kSmallRows * (ks * p + q) * 4 <= 48 * 1024;
+    if (dw != nullptr && small) {
         // small outputs (temporal GCN): dedicated streaming kernel instead of the 512-row-tile reduce GEMM
         int64_t blocks = ceil_div(rows, kSmallRows);
         const int64_t cap = (int64_t)sm_count() * 4;
@@ -230,7 +233,7 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
             stack_segs(s, stride_k, ks, p), rows, ks * p, dz_work, q, dw);
         count_launch();
         if (int32_t rc = check_launch("proj_bwd dW(small)")) return rc;
-    } else {   // dW (ks*p, q) += S^T dZ
+    } else if (dw != nullptr) {   // dW (ks*p, q) += S^T dZ
         const ASegs a = stack_segs(s, stride_k, ks, p);
         ReduceTime tm{};
         tm.n_t = 1;

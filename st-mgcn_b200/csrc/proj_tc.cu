@@ -413,7 +413,7 @@ int32_t launch_proj_fwd_tc(const float* s, int64_t stride_k, int ks, int64_t row
 
 // backward: dZ + bias gradient + U in one row-kernel launch per group of 4 supports (the second one re-forms dZ in its
 // loader but neither stores it nor accumulates the bias gradient again), then dW_k = S_k^T dZ, one launch per pair of
-// supports; wimg_t: stmgcn_proj_pack_tc's backward image
+// supports (none when dw is NULL); wimg_t: stmgcn_proj_pack_tc's backward image
 int32_t launch_proj_bwd_tc(const float* s, int64_t stride_k, int ks, int64_t rows, const float* d_out, const float* out_act,
                            int act, const float* wimg_t, float* dz, float* dbias, float* u, int64_t stride_u, float* dw,
                            cudaStream_t st) {
@@ -422,7 +422,7 @@ int32_t launch_proj_bwd_tc(const float* s, int64_t stride_k, int ks, int64_t row
         if (int32_t rc = launch_rows_bwd(d_out, out_act, act, rows, ks - 4, wimg_t + 2 * 2 * 256 * 32, nullptr, nullptr,
                                          u + 4 * stride_u, stride_u, st))
             return rc;
-    for (int k0 = 0; k0 < ks; k0 += 2)
+    for (int k0 = 0; k0 < ks && dw != nullptr; k0 += 2)
         if (int32_t rc = launch_wgrad(s + (int64_t)k0 * stride_k, stride_k, k0 + 1 < ks ? 128 : 64, dz, rows,
                                       dw + (int64_t)k0 * 64 * 64, st))
             return rc;

@@ -100,8 +100,9 @@ __global__ void gate_bwd_kernel(const float* __restrict__ d_s, const float* __re
         float acc = 0.f;                                     // d z[i] = sum_j da1[j] fcw[j,i]
         for (int j = 0; j < t_len; ++j) acc = fmaf(da1[j], fcw[j * t_len + i], acc);
         d_z[b * t_len + i] = acc;
-        atomicAdd(&d_fcb[i], da2[i] + da1[i]);
+        if (d_fcb != nullptr) atomicAdd(&d_fcb[i], da2[i] + da1[i]);
     }
+    if (d_fcw == nullptr) return;                            // d_z only (d_fcw and d_fcb go together)
     for (int e = threadIdx.x; e < t_len * t_len; e += blockDim.x) {
         const int j = e / t_len, i = e % t_len;              // fc used twice: both uses accumulate
         atomicAdd(&d_fcw[e], da2[j] * r1[i] + da1[j] * zs[i]);
@@ -143,6 +144,7 @@ __global__ void fuse_out_bwd_kernel(const float* __restrict__ d_y, const float* 
                                     float* __restrict__ d_fcb) {
     extern __shared__ float sacc[];          // c_out*gdim + c_out
     const int lane = threadIdx.x & 31;
+    const bool wgrad = d_fcw != nullptr;     // else d_feat only (d_fcw and d_fcb go together)
     const int n_acc = c_out * gdim + c_out;
     for (int e = threadIdx.x; e < n_acc; e += blockDim.x) sacc[e] = 0.f;
     __syncthreads();
@@ -157,13 +159,15 @@ __global__ void fuse_out_bwd_kernel(const float* __restrict__ d_y, const float* 
             for (int c = 0; c < c_out; ++c) {
                 const float dv = dyr[c];
                 acc = fmaf(dv, fcw[c * gdim + g], acc);
-                atomicAdd(&sacc[c * gdim + g], dv * fv);
+                if (wgrad) atomicAdd(&sacc[c * gdim + g], dv * fv);
             }
             d_feat[r * gdim + g] = acc;
         }
+        if (!wgrad) continue;
         if (lane < c_out) atomicAdd(&sacc[c_out * gdim + lane], dyr[lane]);
         for (int c = 32 + lane; c < c_out; c += 32) atomicAdd(&sacc[c_out * gdim + c], dyr[c]);
     }
+    if (!wgrad) return;
     __syncthreads();
     for (int e = threadIdx.x; e < c_out * gdim; e += blockDim.x) atomicAdd(&d_fcw[e], sacc[e]);
     for (int e = threadIdx.x; e < c_out; e += blockDim.x) atomicAdd(&d_fcb[e], sacc[c_out * gdim + e]);
@@ -212,7 +216,8 @@ int32_t stmgcn_gate_fwd(const float* pool, int64_t b, int32_t t, int64_t n_regio
 
 int32_t stmgcn_gate_bwd(const float* d_s, const float* z, const float* a1, const float* s, int64_t b,
                         int32_t t, const float* fcw, float* d_fcw, float* d_fcb, float* d_z, void* stream) {
-    STMGCN_REQUIRE(d_s && z && a1 && s && fcw && d_fcw && d_fcb && d_z, STMGCN_ERR_ARG, "gate_bwd: null pointer");
+    STMGCN_REQUIRE(d_s && z && a1 && s && fcw && d_z, STMGCN_ERR_ARG, "gate_bwd: null pointer");
+    STMGCN_REQUIRE((d_fcw == nullptr) == (d_fcb == nullptr), STMGCN_ERR_ARG, "gate_bwd: d_fcw and d_fcb go together");
     STMGCN_REQUIRE(b > 0 && t > 0 && t <= 2048, STMGCN_ERR_SHAPE, "gate_bwd: bad shape");
     const int threads = t <= 32 ? 32 : (t <= 128 ? 128 : 256);
     gate_bwd_kernel<<<(unsigned)b, threads, 4 * t * sizeof(float), (cudaStream_t)stream>>>(
@@ -241,7 +246,8 @@ int32_t stmgcn_fuse_out_fwd(const float* const* g, int32_t m, int64_t n, int64_t
 int32_t stmgcn_fuse_out_bwd(const float* d_y, const float* feat, int64_t n, int64_t b, int32_t gdim,
                             int32_t c, const float* fcw, float* d_feat, float* d_fcw, float* d_fcb,
                             void* stream) {
-    STMGCN_REQUIRE(d_y && feat && fcw && d_feat && d_fcw && d_fcb, STMGCN_ERR_ARG, "fuse_out_bwd: null pointer");
+    STMGCN_REQUIRE(d_y && feat && fcw && d_feat, STMGCN_ERR_ARG, "fuse_out_bwd: null pointer");
+    STMGCN_REQUIRE((d_fcw == nullptr) == (d_fcb == nullptr), STMGCN_ERR_ARG, "fuse_out_bwd: d_fcw and d_fcb go together");
     STMGCN_REQUIRE(n > 0 && b > 0 && gdim > 0 && c > 0, STMGCN_ERR_SHAPE, "fuse_out_bwd: bad shape");
     const size_t smem = ((size_t)c * gdim + c) * sizeof(float);
     STMGCN_REQUIRE(smem <= 48 * 1024, STMGCN_ERR_SHAPE, "fuse_out_bwd: C*G=%d too large", c * gdim);

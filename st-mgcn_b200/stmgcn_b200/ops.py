@@ -196,16 +196,17 @@ def _proj_fwd(s: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], ac
 
 def _proj_bwd(s: torch.Tensor, w: torch.Tensor, act: int, out: torch.Tensor, d_out: Optional[torch.Tensor],
               d_bcast: Optional[torch.Tensor], scale: float, b_inner: int, need_bias: bool, need_u: bool,
-              wimg_t: Optional[torch.Tensor] = None):
+              wimg_t: Optional[torch.Tensor] = None, need_w: bool = True):
+    """(dw, db, u), each None unless asked for (need_w, need_bias, need_u): nothing is launched for a gradient not asked for."""
     ks, n, b, p = s.shape
     q = w.shape[1]
-    dw = torch.zeros_like(w, dtype=torch.float32)
+    dw = torch.zeros_like(w, dtype=torch.float32) if need_w else None
     db = torch.zeros(q, device=s.device, dtype=torch.float32) if need_bias else None
     dz = torch.empty((n * b, q), device=s.device, dtype=torch.float32)
     u = torch.empty_like(s) if need_u else None
     wt = w.t().contiguous() if need_u else None
     _lib.check(L.stmgcn_proj_bwd(s.data_ptr(), n * b * p, ks, n * b, p, _p(wt), q, act, out.data_ptr(), _p(d_out),
-                                 _p(d_bcast), scale, b_inner, dz.data_ptr(), dw.data_ptr(), _p(db), _p(u),
+                                 _p(d_bcast), scale, b_inner, dz.data_ptr(), _p(dw), _p(db), _p(u),
                                  n * b * p, _p(wimg_t), _stream()), "proj_bwd")
     return dw, db, u
 
@@ -283,9 +284,10 @@ class ChebGCN(torch.autograd.Function):
     @staticmethod
     def backward(ctx, d_out):
         s, w, out, img_b = ctx.saved_tensors
-        need_dx = ctx.needs_input_grad[0]
+        need_dx, need_dw, need_db = ctx.needs_input_grad[:3]
         d_out = _f32c(d_out)
-        dw, db, u = _proj_bwd(s, w, ctx.act, out, d_out, None, 1.0, s.shape[2], ctx.has_bias, need_dx, img_b)
+        dw, db, u = _proj_bwd(s, w, ctx.act, out, d_out, None, 1.0, s.shape[2], ctx.has_bias and need_db, need_dx, img_b,
+                              need_w=need_dw)
         dx = adjoint_stack_(ctx.sset, u) if need_dx else None
         return dx, dw, db, None, None
 
@@ -319,8 +321,9 @@ class TemporalPool(torch.autograd.Function):
     def backward(ctx, d_pool):
         s, w, out = ctx.saved_tensors
         d_pool = _f32c(d_pool)
-        need_dx = ctx.needs_input_grad[0]
-        dw, db, u = _proj_bwd(s, w, ctx.act, out, None, d_pool, 1.0, s.shape[2], ctx.has_bias, need_dx)
+        need_dx, need_dw, need_db = ctx.needs_input_grad[:3]
+        dw, db, u = _proj_bwd(s, w, ctx.act, out, None, d_pool, 1.0, s.shape[2], ctx.has_bias and need_db, need_dx,
+                              need_w=need_dw)
         dx = None
         if need_dx:
             # the GCN's dX (adjoint Clenshaw / sum_k A_k^T U_k) plus the residual's: d_pool broadcast over regions
@@ -348,13 +351,17 @@ class ContextGate(torch.autograd.Function):
         z, a1, s, fcw = ctx.saved_tensors
         d_s = _f32c(d_s)
         b, t = s.shape
-        d_fcw = torch.zeros_like(fcw)
-        d_fcb = torch.zeros(t, device=s.device, dtype=torch.float32)
+        # the fc gradients come together from the kernel: both, or neither when the fc is frozen
+        need_fcw, need_fcb = ctx.needs_input_grad[1:3]
+        need_fc = need_fcw or need_fcb
+        d_fcw = torch.zeros_like(fcw) if need_fc else None
+        d_fcb = torch.zeros(t, device=s.device, dtype=torch.float32) if need_fc else None
         d_z = torch.empty_like(s)
         _lib.check(L.stmgcn_gate_bwd(d_s.data_ptr(), z.data_ptr(), a1.data_ptr(), s.data_ptr(), b, t,
-                                     fcw.data_ptr(), d_fcw.data_ptr(), d_fcb.data_ptr(), d_z.data_ptr(),
+                                     fcw.data_ptr(), _p(d_fcw), _p(d_fcb), d_z.data_ptr(),
                                      _stream()), "gate_bwd")
-        return d_z / float(ctx.n_regions), d_fcw, d_fcb, None
+        d_pool = d_z / float(ctx.n_regions) if ctx.needs_input_grad[0] else None
+        return d_pool, d_fcw if need_fcw else None, d_fcb if need_fcb else None, None
 
 
 def to_blocked(x: torch.Tensor) -> torch.Tensor:
@@ -495,29 +502,35 @@ def _lstm16_backward(xo, s_gate, tape, n_layers, planes, d_top):
     return _lstm16_backward_ex(xo, s_gate, tape, n_layers, planes, d_top)[:2]
 
 
-def _lstm16_backward_ex(xo, s_gate, tape, n_layers, planes, d_top, dh_n=None, dc_n=None, want=(False, False, False)):
+def _lstm16_backward_ex(xo, s_gate, tape, n_layers, planes, d_top, dh_n=None, dc_n=None, want=(False, False, False),
+                        wgrad=True):
     """:func:`_lstm16_backward` with the gradients at the inputs and the recurrent state: returns (d_s, grads, (d_xo, dh0,
     dc0)).  dh_n / dc_n (L, R, 64) or None seed the final state's gradients; ``want`` = which of d_xo, dh0, dc0 to compute
-    (None otherwise).  Without any of them the plain entry point runs."""
+    (None otherwise).  Without any of them the plain entry point runs.  ``wgrad=False``: no weight gradients (grads is a
+    list of None; the kernels' variant without the weight-gradient stage runs and no reduction is launched)."""
     hp, cs, h0p, c0b, wimg, bias, wih_t = (tape[k] for k in _TAPE16)
     n, b, t_len, c_in = xo.shape
     rows = n * b
     rows_pad = cs.shape[2]
     d_top = to_blocked(_f32c(d_top).view(rows, 64))
-    # no workspace needs initialisation: stmgcn_lstm16_bwd zeroes dw_scratch and dbp itself
+    # no workspace needs initialisation: stmgcn_lstm16_bwd zeroes dw_scratch and dbp itself (both only with wgrad)
     dh_rec = xo.new_empty((rows_pad, 64))
     dc = xo.new_empty((rows_pad, 64))
     dx_work = xo.new_empty((min(2, n_layers - 1), t_len, rows_pad, 64)) if n_layers > 1 else None
-    dw_scratch = xo.new_empty((int(L.stmgcn_lstm16_grid(rows)), 128 * 256))
-    dbp = xo.new_empty((n_layers, 256))
     d_s = xo.new_zeros((b, t_len))
     shapes = [s for l in range(n_layers) for s in ((256, c_in if l == 0 else 64), (256, 64), (256,), (256,))]
-    grads = xo.new_empty(sum(math.prod(s) for s in shapes))
+    if wgrad:
+        dw_scratch = xo.new_empty((int(L.stmgcn_lstm16_grid(rows)), 128 * 256))
+        dbp = xo.new_empty((n_layers, 256))
+        grads = xo.new_empty(sum(math.prod(s) for s in shapes))
+        w_grads = [g.view(s) for g, s in zip(grads.split([math.prod(s) for s in shapes]), shapes)]
+    else:
+        dw_scratch = dbp = grads = None
+        w_grads = [None] * len(shapes)
     args = (t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(), wimg.data_ptr(), bias.data_ptr(),
             wih_t.data_ptr(), _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(), d_top.data_ptr(), dh_rec.data_ptr(),
-            dc.data_ptr(), _p(dx_work), dw_scratch.data_ptr(), dbp.data_ptr(), _zero_tile(xo.device).data_ptr(),
-            d_s.data_ptr(), grads.data_ptr())
-    w_grads = [g.view(s) for g, s in zip(grads.split([math.prod(s) for s in shapes]), shapes)]
+            dc.data_ptr(), _p(dx_work), _p(dw_scratch), _p(dbp), _zero_tile(xo.device).data_ptr(),
+            d_s.data_ptr(), _p(grads))
     if dh_n is None and dc_n is None and not any(want):
         _lib.check(L.stmgcn_lstm16_bwd(*args, _stream()), "lstm16_bwd")
         return d_s, w_grads, (None, None, None)
@@ -557,8 +570,10 @@ def _exact_backward(xo, s_gate, tape, n_layers, hid, d_top):
     return _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top)[:2]
 
 
-def _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top, dh_n=None, dc_n=None, want=(False, False, False)):
-    """:func:`_exact_backward` with the extras of :func:`_lstm16_backward_ex`: returns (d_s, grads, (d_xo, dh0, dc0))."""
+def _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top, dh_n=None, dc_n=None, want=(False, False, False),
+                       wgrad=True):
+    """:func:`_exact_backward` with the extras and ``wgrad`` of :func:`_lstm16_backward_ex`: returns (d_s, grads, (d_xo,
+    dh0, dc0))."""
     h0, c0, hs, cs, gates, wx, wpt = tape
     n, b, t_len, c_in = xo.shape
     rows = n * b
@@ -568,12 +583,12 @@ def _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top, dh_n=None, dc_n=N
     dc = xo.new_empty((n_layers, rows, hid))
     dx_work = xo.new_empty((rows, hid))
     d_s = xo.new_zeros((b, t_len))
-    dwx = torch.zeros_like(wx)
-    dwp = torch.zeros_like(wpt)
-    dbp = xo.new_zeros((n_layers, 4 * hid))
+    dwx = torch.zeros_like(wx) if wgrad else None
+    dwp = torch.zeros_like(wpt) if wgrad else None
+    dbp = xo.new_zeros((n_layers, 4 * hid)) if wgrad else None
     args = (t_len, n_layers, rows, hid, c_in, b, xo.data_ptr(), s_gate.data_ptr(), wx.data_ptr(), wpt.data_ptr(), _p(h0),
             _p(c0), cs.data_ptr(), hs.data_ptr(), gates.data_ptr(), d_top.data_ptr(), dh_rec.data_ptr(), dc.data_ptr(),
-            dx_work.data_ptr(), d_s.data_ptr(), dwx.data_ptr(), dwp.data_ptr(), dbp.data_ptr())
+            dx_work.data_ptr(), d_s.data_ptr(), _p(dwx), _p(dwp), _p(dbp))
     extras = (None, None, None)
     if dh_n is None and dc_n is None and not any(want):
         _lib.check(L.stmgcn_lstm_bwd(*args, _stream()), "lstm_bwd")
@@ -584,7 +599,8 @@ def _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top, dh_n=None, dc_n=N
                        for w, shape in zip(want, (xo.shape, (n_layers, rows, hid), (n_layers, rows, hid))))
         _lib.check(L.stmgcn_lstm_bwd_ex(*args, _p(dh_n), _p(dc_n), _p(extras[1]), _p(extras[2]), _p(extras[0]),
                                         _stream()), "lstm_bwd_ex")
-    return d_s, _unpack_lstm_grads(dwx, dwp, dbp, n_layers, hid, c_in), extras
+    w_grads = _unpack_lstm_grads(dwx, dwp, dbp, n_layers, hid, c_in) if wgrad else [None] * (4 * n_layers)
+    return d_s, w_grads, extras
 
 
 class SharedLSTM(torch.autograd.Function):
@@ -640,15 +656,18 @@ class SharedLSTM(torch.autograd.Function):
         if d_top is None:
             d_top = xo.new_zeros((xo.shape[0], xo.shape[1], hid))
         want = (ctx.needs_input_grad[0], ctx.needs_input_grad[2], ctx.needs_input_grad[3])
+        # the weight gradients of the whole stack, or none of them when no LSTM weight requires grad
+        wgrad = any(ctx.needs_input_grad[7:])
         if ctx.planes16:
             tape16 = dict(zip(_TAPE16, tape))
-            d_s, w_grads, extras = _lstm16_backward_ex(xo, s_gate, tape16, n_layers, ctx.planes, d_top, dh_n, dc_n, want)
+            d_s, w_grads, extras = _lstm16_backward_ex(xo, s_gate, tape16, n_layers, ctx.planes, d_top, dh_n, dc_n, want,
+                                                       wgrad)
         else:
             if getattr(ctx, "tape_consumed", False):
                 raise RuntimeError("SharedLSTM (exact-fp32 kernels): the gate tape was overwritten in place by the first "
                                    "backward pass; a second backward over the same graph is not supported on this path")
             ctx.tape_consumed = True
-            d_s, w_grads, extras = _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top, dh_n, dc_n, want)
+            d_s, w_grads, extras = _exact_backward_ex(xo, s_gate, tape, n_layers, hid, d_top, dh_n, dc_n, want, wgrad)
         d_xo, dh0, dc0 = extras
         return (d_xo, d_s, dh0, dc0, None, None, None, *w_grads)
 
@@ -679,9 +698,11 @@ class FuseOut(torch.autograd.Function):
         n, b, gdim = feat.shape
         c = fcw.shape[0]
         d_feat = torch.empty_like(feat)
-        d_fcw = torch.zeros_like(fcw)
-        d_fcb = torch.zeros(c, device=feat.device, dtype=torch.float32)
+        need_fcw, need_fcb = ctx.needs_input_grad[:2]
+        need_fc = need_fcw or need_fcb                  # both from the kernel, or neither
+        d_fcw = torch.zeros_like(fcw) if need_fc else None
+        d_fcb = torch.zeros(c, device=feat.device, dtype=torch.float32) if need_fc else None
         _lib.check(L.stmgcn_fuse_out_bwd(d_y.data_ptr(), feat.data_ptr(), n, b, gdim, c, fcw.data_ptr(),
-                                         d_feat.data_ptr(), d_fcw.data_ptr(), d_fcb.data_ptr(), _stream()),
+                                         d_feat.data_ptr(), _p(d_fcw), _p(d_fcb), _stream()),
                    "fuse_out_bwd")
-        return (d_fcw, d_fcb) + tuple(d_feat for _ in range(ctx.m))
+        return (d_fcw if need_fcw else None, d_fcb if need_fcb else None) + tuple(d_feat for _ in range(ctx.m))
