@@ -586,7 +586,7 @@ class BF16ModeReference:
         self.p = {k: torch.as_tensor(v).to(self.dev, dtype) for k, v in params.items()}
         self.chains = [[torch_csr_pair(c, self.dev, dtype) for c in ch] for ch in chains]
         self.ks, self.relu, self.rounding = n_supports, relu, rounding
-        self.masks = None if relu_masks is None else [torch.as_tensor(mk).to(self.dev, dtype) for mk in relu_masks]
+        self.masks = None if relu_masks is None else [torch.as_tensor(mk).to(self.dev) for mk in relu_masks]
         self.m = len(chains)
         self.n_layers = _count_lstm_layers(self.p, "rnn_list.0.lstm.")
         assert all(ch and (n_supports - 1) % len(ch) == 0 for ch in self.chains) or n_supports == 1
@@ -621,25 +621,30 @@ class BF16ModeReference:
                 comp[seg[j]], used[seg[j]] = y, forced(seg[j], y)
         return used, comp
 
-    def _gcn(self, m, x, w, b, mask_i, spatial, tape_s=None):
-        """act(sum_k S_k W_k + b) on node-major x (N, B, p) -> (out (N, B, q), computed stack terms)."""
+    def _gcn(self, m, x, w, b, mask_i, spatial, tape_s=None, windows=None):
+        """act(sum_k S_k W_k + b) on node-major x (N, B, p) -> (out (N, B, q), computed stack terms).  ``windows``: the
+        slice of the masks' batch that x holds."""
         n, bsz, p = x.shape
         used, comp = self._stack(m, x, spatial, tape_s)
         z = sum(used[k].reshape(n, bsz, p) @ w[k * p:(k + 1) * p] for k in range(self.ks))
         if b is not None:
             z = z + b
-        if self.relu:
-            z = z * self.masks[mask_i] if self.masks is not None else torch.relu(z)
+        if self.relu and self.masks is not None:
+            mask = self.masks[mask_i] if windows is None else self.masks[mask_i][:, windows]
+            z = z * mask.to(z.dtype)
+        elif self.relu:
+            z = torch.relu(z)
         return z, comp
 
-    def cg_lstm_node_major(self, p, m, xo, tape=None, h0=None, c0=None):
+    def cg_lstm_node_major(self, p, m, xo, tape=None, h0=None, c0=None, windows=None):
         """Graph ``m``'s ``CG_LSTM`` on node-major xo (N, B, T, C) -> (h_top (N, B, H), h_n, c_n (L, R, H), (hs, cs)):
-        ``hs`` / ``cs`` the computed states of every layer-step (see :func:`lstm_planes_reference`)."""
+        ``hs`` / ``cs`` the computed states of every layer-step (see :func:`lstm_planes_reference`).  ``windows``: the
+        slice of the masks' batch that xo holds (``tape`` is taken as given, already sliced)."""
         pre = f"rnn_list.{m}."
         n, bsz, t_len, c_in = xo.shape
         xt = xo.sum(-1)
         gt, _ = self._gcn(m, xt, p[pre + "gconv_temporal_feats.W"], p.get(pre + "gconv_temporal_feats.b"), 2 * m,
-                          False)
+                          False, windows=windows)
         z = (xt + gt).sum(0) / n
         fw, fb = p[pre + "fc.weight"], p[pre + "fc.bias"]
         s = torch.sigmoid(torch.relu(z @ fw.t() + fb) @ fw.t() + fb)
@@ -661,12 +666,17 @@ class BF16ModeReference:
         to_module = lambda v: v.reshape(v.shape[0], n, bsz, -1).permute(0, 2, 1, 3).reshape(v.shape[0], bsz * n, -1)  # noqa: E731
         return h_top.permute(1, 0, 2), (to_module(h_n), to_module(c_n))
 
-    def branch(self, p, m, xo, tape=None):
+    def branch(self, p, m, xo, tape=None, windows=None):
         """Graph ``m``'s branch of ``ST_MGCN`` on node-major xo -> dict: ``out`` (N, B, G) and the computed values of
-        every rounding point -- ``hs`` / ``cs`` (per layer, per step) and ``stack`` (spatial S_k, (N, B*H) each)."""
-        h_top, _, _, (hs, cs) = self.cg_lstm_node_major(p, m, xo, tape)
+        every rounding point -- ``hs`` / ``cs`` (per layer, per step) and ``stack`` (spatial S_k, (N, B*H) each).
+
+        ``windows`` (a slice, optional): xo holds only these windows of the batch that ``relu_masks`` and ``tape``
+        describe; the masks and the tape are sliced to them."""
+        if tape is not None and windows is not None:
+            tape = _tape_windows(tape, xo.shape[0], windows)
+        h_top, _, _, (hs, cs) = self.cg_lstm_node_major(p, m, xo, tape, windows=windows)
         g, stack = self._gcn(m, h_top, p[f"gcn_list.{m}.W"], p.get(f"gcn_list.{m}.b"), 2 * m + 1, True,
-                             None if tape is None else tape["s"])
+                             None if tape is None else tape["s"], windows)
         return dict(out=g, hs=hs, cs=cs, stack=stack)
 
     def forward(self, p, obs, tapes=None):
@@ -675,22 +685,41 @@ class BF16ModeReference:
         fused = sum(self.branch(p, m, xo, None if tapes is None else tapes[m])["out"] for m in range(self.m))
         return (fused @ p["fc.weight"].t() + p["fc.bias"]).permute(1, 0, 2)
 
-    def loss_and_grads(self, obs, y, tapes=None, want_obs: bool = False, on_branch=None):
+    def loss_and_grads(self, obs, y, tapes=None, want_obs: bool = False, on_branch=None, window_chunk=None):
         """MSE(mean) loss and the gradient of every parameter (and of obs with ``want_obs``), one graph branch in memory
         at a time: the branches' outputs first (no autograd), then the fusion's gradient, then each branch's backward.
-        ``on_branch(m, branch dict)`` (optional) sees each branch's forward values.  Returns (out, loss, grads)."""
+        ``on_branch(m, branch dict)`` (optional) sees each branch's forward values.  Returns (out, loss, grads).
+
+        ``window_chunk`` (optional): each branch's forward and backward run on ``window_chunk`` windows at a time (the
+        last chunk may be shorter), so the autograd tape held at once is that of one chunk of one branch.  Windows are
+        independent (``STMGCN.py:47``: the only reductions are over the regions of one window and over graphs), so the
+        fusion's gradient is taken on the whole batch and each chunk's backward, seeded with its windows' share of it,
+        adds that chunk's exact contribution to the parameter gradients (and writes its windows' d obs)."""
         obs = torch.as_tensor(obs).to(self.dev, self.dt)
         y = torch.as_tensor(y).to(self.dev, self.dt)
+        bsz = obs.shape[0]
+        if window_chunk is None:
+            wins = [None]
+        else:
+            if window_chunk < 1:
+                raise ValueError(f"window_chunk must be at least 1, got {window_chunk}")
+            if on_branch is not None:
+                raise ValueError("on_branch sees whole-batch branch values: it does not combine with window_chunk")
+            wins = [slice(i, min(i + window_chunk, bsz)) for i in range(0, bsz, window_chunk)]
         p = self.leaves()
         xo = obs.permute(2, 0, 1, 3)
         with torch.no_grad():
             outs = []
             for m in range(self.m):
-                br = self.branch(p, m, xo, None if tapes is None else tapes[m])
-                if on_branch is not None:
-                    on_branch(m, br)
-                outs.append(br["out"])
-                del br
+                parts = []
+                for win in wins:
+                    br = self.branch(p, m, xo if win is None else xo[:, win], None if tapes is None else tapes[m], win)
+                    if on_branch is not None:
+                        on_branch(m, br)
+                    parts.append(br["out"])
+                    del br
+                outs.append(parts[0] if len(parts) == 1 else torch.cat(parts, dim=1))
+                del parts
         gs = [o.requires_grad_(True) for o in outs]
         out = (sum(gs) @ p["fc.weight"].t() + p["fc.bias"]).permute(1, 0, 2)
         loss = torch.mean((out - y) ** 2)
@@ -698,17 +727,31 @@ class BF16ModeReference:
         grads = {"fc.weight": top[-2], "fc.bias": top[-1]}
         d_obs = torch.zeros_like(obs) if want_obs else None
         for m in range(self.m):
-            ob = obs.detach().clone().requires_grad_(want_obs)
-            g = self.branch(p, m, ob.permute(2, 0, 1, 3), None if tapes is None else tapes[m])["out"]
             keys = [k for k in p if k.startswith((f"rnn_list.{m}.", f"gcn_list.{m}."))]
-            res = torch.autograd.grad(g, [p[k] for k in keys] + ([ob] if want_obs else []), grad_outputs=top[m])
-            grads.update(zip(keys, res))
-            if want_obs:
-                d_obs += res[-1]
-            del g, res
+            for win in wins:
+                ob = (obs if win is None else obs[win]).detach().clone().requires_grad_(want_obs)
+                g = self.branch(p, m, ob.permute(2, 0, 1, 3), None if tapes is None else tapes[m], win)["out"]
+                res = torch.autograd.grad(g, [p[k] for k in keys] + ([ob] if want_obs else []),
+                                          grad_outputs=top[m] if win is None else top[m][:, win])
+                for k, r in zip(keys, res):
+                    grads[k] = r if k not in grads else grads[k] + r
+                if want_obs:
+                    d_obs[slice(None) if win is None else win] += res[-1]
+                del g, res
         if want_obs:
             grads["obs"] = d_obs
         return out.detach(), loss.detach(), grads
+
+
+def _tape_windows(tape, n, windows):
+    """A :class:`BF16ModeReference` tape (rows ``r = n*B + b``) cut to the windows ``windows`` (a slice of the B)."""
+    def rows(v, axis):                  # (..., N*B, ...) -> (..., N*len(windows), ...)
+        shape = v.shape
+        v = v.reshape(shape[:axis] + (n, shape[axis] // n) + shape[axis + 1:])
+        v = v[(slice(None),) * (axis + 1) + (windows,)]
+        return v.reshape(shape[:axis] + (-1,) + shape[axis + 1:])
+    row_axis = {"h": 2, "c": 2, "h0": 1}          # h, c (L, T, R, H); h0 (L, R, H); s (Ks, N, B, H)
+    return {k: v[:, :, windows] if k == "s" else rows(v, row_axis[k]) for k, v in tape.items()}
 
 
 def laplacian_csr_from_supports(supports: torch.Tensor):

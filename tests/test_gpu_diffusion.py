@@ -1,8 +1,8 @@
 """``kernel_type='random_walk_diffusion'`` on the GPU: the two-chain sparse supports of
 ``Adj_Preprocessor.process_sparse`` through ``ST_MGCN`` / ``CG_LSTM`` against the reference's golden vectors, the dense
-``2K+1`` stack on the generic path, the fp64 sparse oracle at cfg3 size, both LSTM paths, the bf16 mode, CUDA-graph
-replay and training; negative controls that each break one part of the chain plumbing; and the launch count of an
-unchanged Chebyshev step."""
+``2K+1`` stack on the generic path, the fp64 reference on every window of a full cfg3 batch, both LSTM paths, the bf16
+mode, CUDA-graph replay and training; negative controls that each break one part of the chain plumbing; and the launch
+count of an unchanged Chebyshev step."""
 import numpy as np
 import pytest
 import scipy.sparse as sp
@@ -10,6 +10,7 @@ import torch
 from torch import nn
 
 import diffusion_oracle as D
+import full_batch
 import stmgcn_oracle as O
 from helpers import TOL, assert_close
 
@@ -118,9 +119,9 @@ def _directed_workload(name, batch):
     return w, adjs
 
 
-def _check_subbatch(name, batch, picks, order=2, tol=TOL, relu=True):
-    """test_gpu_fullsize.py's method on directed graphs with diffusion supports: the oracle (fp64, two chains) on the
-    picked windows; the other windows' targets are the run's own output, the ReLU masks those of the GPU forward."""
+def _check_full_batch(name, batch, window_chunk, order=2, tol=TOL, relu=True, **kw):
+    """test_gpu_fullsize.py's method on directed graphs with diffusion supports: one step on the full batch, every window
+    with its true target, against the fp64 reference (two chains per graph) with the GPU forward's ReLU masks."""
     import GCN
     import STMGCN
     from stmgcn_b200 import ops, synth
@@ -129,53 +130,23 @@ def _check_subbatch(name, batch, picks, order=2, tol=TOL, relu=True):
     sups_cpu = [pre.process_sparse(a) for a in adjs]
     chains = [[sp.csr_matrix(m.numpy()) for m in h.matrices_dense()] for h in sups_cpu]
     torch.manual_seed(0)
-    kw = synth.model_kwargs(w)
-    kw["sta_kernel_config"] = {"kernel_type": "random_walk_diffusion", "K": order}
+    kw_model = synth.model_kwargs(w)
+    kw_model["sta_kernel_config"] = {"kernel_type": "random_walk_diffusion", "K": order}
     if not relu:
-        kw["gconv_activation"] = None
-    model = STMGCN.ST_MGCN(**kw)
+        kw_model["gconv_activation"] = None
+    model = STMGCN.ST_MGCN(**kw_model)
     params = {k: v.detach().clone().numpy() for k, v in model.state_dict().items()}
-    model = model.to(DEV)
-    sups = [s.to(DEV) for s in sups_cpu]
     x, y = synth.make_inputs(w, seed=100, batch=batch)
-    xd = x.to(DEV)
-    with torch.no_grad():
-        out0 = model(obs_seq=xd, sta_adj_list=sups)
-    y2 = out0.detach().clone()
-    y2[picks] = y[picks].to(DEV)
-    gcn_outs = []
-    real_proj_fwd = ops._proj_fwd
-
-    def recording_proj_fwd(*a, **k):
-        out_ = real_proj_fwd(*a, **k)
-        gcn_outs.append(out_)
-        return out_
-    ops._proj_fwd = recording_proj_fwd
-    try:
-        out = model(obs_seq=xd, sta_adj_list=sups)
-    finally:
-        ops._proj_fwd = real_proj_fwd
-    assert len(gcn_outs) == 2 * w.n_graphs
-    loss = nn.MSELoss()(out, y2)
-    loss.backward()
-    torch.cuda.synchronize()
-    masks = [(g[:, picks] > 0).cpu().numpy() for g in gcn_outs] if relu else None
-    del gcn_outs
-    orc = D.ChainOracle(params, chains, 2 * order + 1, relu=relu, dtype=np.float64, relu_masks=masks)
-    o_ref, l_ref, g_ref = orc.loss_and_grads(x[picks].numpy(), y[picks].numpy())
-    scale = len(picks) / float(batch)
-    errs = {"out": O.max_rel_err(out.detach()[picks].cpu().numpy(), o_ref),
-            "loss": abs(loss.item() - l_ref * scale) / abs(l_ref * scale)}
-    for key, p in model.named_parameters():
-        errs["grad " + key] = O.max_rel_err(p.grad.cpu().numpy(), g_ref[key] * scale)
-    _assert_errs(errs, tol, f"{name} diffusion K={order} B={batch} relu={relu} planes={ops.lstm_planes()} {picks}")
-    assert bool(torch.isfinite(out).all())
+    label = f"{name} diffusion K={order} planes={ops.lstm_planes()}"
+    errs = full_batch.run(label, model.to(DEV), [s.to(DEV) for s in sups_cpu], params, chains, 2 * order + 1, x, y,
+                          relu=relu, window_chunk=window_chunk, **kw)
+    full_batch.assert_within(errs, tol, what=label)
     return errs
 
 
-def test_cfg3_full_size_diffusion_vs_fp64_oracle_on_two_windows():
+def test_cfg3_full_size_diffusion_vs_fp64_reference_on_every_window():
     """cfg3 shapes (4096 regions, 3 directed graphs, T=12, batch 64: 262 144 LSTM rows), K=2 (5 supports)."""
-    _check_subbatch("cfg3", 64, [0, 63])
+    _check_full_batch("cfg3", 64, 16)
 
 
 def test_bf16_mode_with_diffusion_supports_vs_fp64_oracle():
@@ -184,7 +155,7 @@ def test_bf16_mode_with_diffusion_supports_vs_fp64_oracle():
     old = ops.lstm_planes()
     try:
         ops.set_lstm_planes(1)
-        errs = _check_subbatch("cfg2", 32, [0, 17, 31], tol=2e-2, relu=False)
+        errs = _check_full_batch("cfg2", 32, 32, tol=2e-2, relu=False, fp32_diagnostic=False)
     finally:
         ops.set_lstm_planes(old)
     assert errs["out"] > 1e-6, "the bf16 mode produced fp32-grade results: the single-plane path did not run"

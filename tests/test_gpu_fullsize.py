@@ -1,28 +1,29 @@
 """GPU parity at the sizes that are BENCHMARKED (BASELINE.json configs[1..4]), not only at toy sizes.
 
-Windows of a batch are independent (``STMGCN.py:47``: every (window, region) pair is its own LSTM row; the only
-reductions are over regions inside one window, ``STMGCN.py:42``, and over graphs, ``STMGCN.py:116``), so the fp64 sparse
-oracle evaluated on a FEW windows pins the full-batch GPU run:
+One training step on the full batch, every window with its true target, against the fp64 reference
+(``tests/full_batch.py``: ``BF16ModeReference`` without rounding, on the GPU, a chunk of windows at a time).  Every
+window then feeds every weight-gradient reduction -- the LSTM's per-CTA slices and their sum, the projection's ``dW`` /
+``dbias`` / pool atomics, the fusion and gate ``fc`` sums, ``d_s`` -- at 262 144 LSTM rows, 2 048 tiles and > 2^31
+element tapes at cfg3.  Every window's output, the loss and every parameter gradient are held to the bar.
 
-* forward: ``out[b]`` of the full-batch run must equal the oracle's output for window ``b``;
-* backward: the targets of all other windows are set to the GPU's own forward output, so their residual -- and with it
-  their gradient contribution -- vanishes; the full-batch gradient is then exactly ``|picked| / B`` times the oracle's
-  gradient on the picked windows.  Every kernel still runs at the full size (262 144 LSTM rows, 2 048 tiles, > 2^31
-  element tapes at cfg3), with the rows of the other windows carrying zeros through the backward.
-
-Tolerance: 1e-4 max-norm relative (BASELINE.json north_star), fp32 arithmetic.
+Tolerance: 1e-4 max-norm relative (BASELINE.json north_star), fp32 arithmetic; 2e-2 for the bf16-arithmetic mode
+against the unrounded reference.
 """
-import numpy as np
 import pytest
 import scipy.sparse as sp
 import torch
 from torch import nn
 
+import full_batch
 import stmgcn_oracle as O
 from helpers import TOL, assert_close
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
+
+# windows per chunk of the fp64 reference: its autograd tape is ~1 GB per cfg3 window and graph branch, ~8 GB per cfg5
+# window (16 384 regions, T = 24)
+CHUNK = {"cfg2": 32, "cfg3": 16, "cfg5": 2}
 
 
 def _csr_of(sup):
@@ -47,89 +48,87 @@ def _build(w, batch, seed_x=100, relu=True):
     return model.to(DEV), [s.to(DEV) for s in sups_cpu], [_csr_of(s) for s in sups_cpu], params, x, y
 
 
-def _check_subbatch(w, batch, picks, tol=TOL, relu=True):
-    """ReLU: the oracle takes the ReLU masks of the GPU's own grad-enabled forward (its GCN outputs > 0, picked windows
-    only).  With a few windows carrying gradient, one pre-activation within rounding distance of zero would otherwise flip
-    its mask between fp32 and fp64 and move every gradient of that graph branch by ~1e-3; with the GPU's masks the oracle
-    follows the same branch of every ReLU, and every gradient is held to ``tol``."""
-    from stmgcn_b200 import ops
+def _run_full_batch(name, batch, relu=True, **kw):
+    """``full_batch.run`` on workload ``name`` (Chebyshev supports); returns the errors."""
+    from stmgcn_b200 import ops, synth
+    w = synth.WORKLOADS[name]
     model, sups, laps, params, x, y = _build(w, batch, relu=relu)
-    crit = nn.MSELoss(reduction="mean")
-    xd = x.to(DEV)
-    with torch.no_grad():
-        out0 = model(obs_seq=xd, sta_adj_list=sups)
-    # targets: the run's own output everywhere except the picked windows
-    y2 = out0.detach().clone()
-    y2[picks] = y[picks].to(DEV)
-    gcn_outs = []                       # per GCN call: temporal graph 0, spatial graph 0, temporal graph 1, ...
-    real_proj_fwd = ops._proj_fwd
+    label = f"{name} path={ops.lstm_path()} planes={ops.lstm_planes()}"
+    return full_batch.run(label, model, sups, params, [[lap] for lap in laps], w.n_supports, x, y, relu=relu,
+                          window_chunk=CHUNK[name], **kw)
 
-    def recording_proj_fwd(*a, **k):
-        out_ = real_proj_fwd(*a, **k)
-        gcn_outs.append(out_)
-        return out_
-    ops._proj_fwd = recording_proj_fwd
-    try:
-        out = model(obs_seq=xd, sta_adj_list=sups)
-    finally:
-        ops._proj_fwd = real_proj_fwd
-    assert len(gcn_outs) == 2 * w.n_graphs
-    loss = crit(out, y2)
-    loss.backward()
-    torch.cuda.synchronize()
-    masks = [(g[:, picks] > 0).cpu().numpy() for g in gcn_outs] if relu else None
-    del gcn_outs
-    orc = O.SparseOracle(params, laps, w.n_supports, relu=relu, dtype=np.float64, relu_masks=masks)
-    o_ref, l_ref, g_ref = orc.loss_and_grads(x[picks].numpy(), y[picks].numpy())
-    scale = len(picks) / float(batch)
-    errs = {"out": O.max_rel_err(out.detach()[picks].cpu().numpy(), o_ref),
-            "loss": abs(loss.item() - l_ref * scale) / abs(l_ref * scale)}
-    for key, p in model.named_parameters():
-        errs["grad " + key] = O.max_rel_err(p.grad.cpu().numpy(), g_ref[key] * scale)
-    print(f"{w.name} B={batch} relu={relu} planes={ops.lstm_planes()} windows {picks}: max-norm relative errors vs the "
-          f"fp64 oracle: " + ", ".join(f"{k} {v:.2e}" for k, v in sorted(errs.items(), key=lambda kv: -kv[1])[:6]))
-    bad = {k: v for k, v in errs.items() if not (v <= tol)}
-    assert not bad, f"{w.name} B={batch}: above tolerance: {bad}"
-    assert bool(torch.isfinite(out).all())                  # every window, not only the picked ones
+
+def _check_full_batch(name, batch, tol=TOL, relu=True, **kw):
+    """:func:`_run_full_batch` and every error at ``tol``."""
+    errs = _run_full_batch(name, batch, relu, **kw)
+    full_batch.assert_within(errs, tol, what=f"{name} B={batch} relu={relu}")
     return errs
 
 
 @pytest.mark.parametrize("relu", [True, False])
-def test_cfg3_full_size_vs_fp64_oracle_on_two_windows(relu):
-    """BASELINE configs[2]: 4096 regions, 3 graphs, K=3, T=12, batch 64, fp32 -- the size bench.py reports."""
-    from stmgcn_b200 import synth
-    _check_subbatch(synth.WORKLOADS["cfg3"], 64, [0, 63], relu=relu)
+def test_cfg3_full_size_vs_fp64_reference_on_every_window(relu):
+    """BASELINE configs[2]: 4096 regions, 3 graphs, K=3, T=12, batch 64, fp32 -- the size bench.py reports.  The step is
+    taken twice at the same weights, and the spread of every gradient between the two is printed beside its error."""
+    _check_full_batch("cfg3", 64, relu=relu, repeat=True)
 
 
 @pytest.mark.parametrize("relu", [True, False])
 def test_cfg2_full_size_vs_fp64_oracle(relu):
-    """BASELINE configs[1] shapes (1024 regions, 3 graphs, K=3, T=12, batch 32) in fp32 against the oracle on 3 windows."""
-    from stmgcn_b200 import synth
-    _check_subbatch(synth.WORKLOADS["cfg2"], 32, [0, 17, 31], relu=relu)
+    """BASELINE configs[1] shapes (1024 regions, 3 graphs, K=3, T=12, batch 32) in fp32, every window."""
+    _check_full_batch("cfg2", 32, relu=relu)
 
 
 @pytest.mark.parametrize("relu", [True, False])
-def test_cfg5_shapes_vs_fp64_oracle_on_one_window(relu):
+def test_cfg2_full_size_exact_fp32_path_vs_fp64_reference(relu):
+    """The exact-fp32 CUDA-core path (``ops.set_lstm_path("fma")``: FFMA LSTM and projection kernels) at cfg2 full size,
+    every window, at the same bar as the tensor-core path."""
+    from stmgcn_b200 import ops
+    old = ops.lstm_path()
+    try:
+        ops.set_lstm_path("fma")
+        _check_full_batch("cfg2", 32, relu=relu)
+    finally:
+        ops.set_lstm_path(old)
+
+
+@pytest.mark.parametrize("relu", [True, False])
+def test_cfg5_shapes_vs_fp64_reference_on_every_window(relu):
     """BASELINE configs[4] shapes: 16384 regions, 3 graphs at 1 % density, K=5 (six supports), T=24; batch 8 of 32."""
-    from stmgcn_b200 import synth
-    _check_subbatch(synth.WORKLOADS["cfg5"], 8, [5], relu=relu)
+    _check_full_batch("cfg5", 8, relu=relu)
 
 
-@pytest.mark.parametrize("cfg,batch,picks", [("cfg2", 32, [0, 17, 31]), ("cfg5", 8, [5])])
-def test_bf16_mode_at_the_quoted_sizes_vs_fp64_oracle(cfg, batch, picks):
+@pytest.mark.parametrize("cfg,batch", [("cfg2", 32), ("cfg5", 8)])
+def test_bf16_mode_at_the_quoted_sizes_vs_fp64_oracle(cfg, batch):
     """BASELINE configs[1] and [4] are quoted in the bf16 arithmetic mode (ops.set_lstm_planes(1): one bf16 hidden-state
     plane in the tensor-core LSTM, bf16 gather copies in the spatial Chebyshev recurrence, spmm_step16): the whole model at
-    those sizes against the fp64 oracle at the bf16 tolerance 2e-2 (SURVEY.md section 8(d)).  The model without the GCN
+    those sizes against the fp64 reference at the bf16 tolerance 2e-2 (SURVEY.md section 8(d)).  The model without the GCN
     activation, as in test_gpu_parity.py: bf16-level noise flips ReLU masks, which says nothing about the kernels.
     tests/test_gpu_lstm16.py is the tight check of the LSTM arithmetic in this mode; this is the end-to-end bound."""
-    from stmgcn_b200 import ops, synth
+    from stmgcn_b200 import ops
     old = ops.lstm_planes()
     try:
         ops.set_lstm_planes(1)
-        errs = _check_subbatch(synth.WORKLOADS[cfg], batch, picks, tol=2e-2, relu=False)
+        errs = _check_full_batch(cfg, batch, tol=2e-2, relu=False, fp32_diagnostic=False)
     finally:
         ops.set_lstm_planes(old)
     assert errs["out"] > 1e-6, "the bf16 mode produced fp32-grade results: the single-plane path did not run"
+
+
+def test_full_batch_check_fails_a_backward_that_drops_windows(monkeypatch):
+    """Negative control: the LSTM backward loses the gradient of windows 1 .. B-2 (their rows ``n*B + b`` of ``d_top``
+    are zeroed).  The output is untouched, so only a check in which those windows carry gradient can see it."""
+    from stmgcn_b200 import ops
+    real = ops.SharedLSTM.backward
+
+    def lossy(ctx, d_top, dh_n, dc_n):
+        d_top = d_top.clone()
+        d_top[:, 1:-1] = 0
+        return real(ctx, d_top, dh_n, dc_n)
+    monkeypatch.setattr(ops.SharedLSTM, "backward", staticmethod(lossy))
+    errs = _run_full_batch("cfg2", 32, fp32_diagnostic=False)
+    assert errs["out"] <= TOL
+    lost = {k: v for k, v in errs.items() if not v <= TOL}
+    assert any(".lstm." in k for k in lost), f"the full-batch check passed a backward that drops windows: {errs}"
 
 
 def test_lstm_tensor_core_vs_exact_fp32_at_cfg3_size():

@@ -510,21 +510,6 @@ def _tanh_gcn(supports, x, w, b, relu=True):
 _DENSE_GCN = O.dense_gcn
 
 
-def _sparse_cheb_gcn(lap, x, w, b, relu=True):
-    """``dense_gcn`` with the Chebyshev stack built on the features from the sparse L~ (fp64 autograd through
-    torch.sparse.mm): T_0 x = x, T_1 x = L~ x, T_k x = 2 L~ T_{k-1} x - T_{k-2} x."""
-    bsz, n, p = x.shape
-    ks = w.shape[0] // p
-    terms = [x.permute(1, 0, 2).reshape(n, bsz * p)]
-    for k in range(1, ks):
-        nxt = torch.sparse.mm(lap, terms[-1])
-        terms.append(nxt if k == 1 else 2.0 * nxt - terms[-2])
-    out = sum(terms[k].reshape(n, bsz, p).permute(1, 0, 2) @ w[k * p:(k + 1) * p] for k in range(ks))
-    if b is not None:
-        out = out + b
-    return torch.relu(out) if relu else out
-
-
 @pytest.mark.parametrize("kind", ["localpool", "c3", "tanh", "bf16"])
 def test_st_mgcn_obs_gradient_matches_the_dense_oracle(kind, monkeypatch):
     """localpool supports (generic stacks), C = 3, an activation the kernels do not fuse (torch applies it), and the
@@ -617,35 +602,15 @@ def test_parameter_gradients_do_not_depend_on_input_grads(path, monkeypatch):
 # ======================================================================================================================
 # full size
 # ======================================================================================================================
-def test_obs_gradient_at_cfg3_size_on_picked_windows():
-    """cfg3 (4096 regions, 3 graphs, K = 3, T = 12, batch 64, C = 1), smooth model: d obs of two picked windows against
-    fp64 torch autograd over the sparse restatement (the dense oracle with its Chebyshev stack built on the features by
-    torch.sparse.mm from L~).  The other windows' targets are the run's own output, so their loss terms and their d obs
-    vanish; windows are independent (STMGCN.py:47), so the picked windows' d obs is |picked| / B times the reference's on
-    the picked windows alone."""
+def test_obs_gradient_at_cfg3_size_on_every_window():
+    """cfg3 (4096 regions, 3 graphs, K = 3, T = 12, batch 64, C = 1), smooth model, every window with its true target:
+    d obs against the fp64 reference (tests/full_batch.py), held to the bar in max-norm, per window and per time step
+    (``per_step.worst_step`` along T), with every parameter gradient and every window's output."""
+    import full_batch
     from stmgcn_b200 import synth
-    from test_gpu_fullsize import _build
-    b, picked = 64, [3, 50]
-    model, sups, laps, params, x, y = _build(synth.WORKLOADS["cfg3"], b, relu=False)
-    xd = x.to(DEV)
-    with torch.no_grad():
-        y2 = model(obs_seq=xd, sta_adj_list=sups).clone()
-    y2[picked] = y[picked].to(DEV)
-    xg = xd.clone().requires_grad_(True)
-    nn.MSELoss()(model(obs_seq=xg, sta_adj_list=sups), y2).backward()
-    got = xg.grad[picked].double().cpu()
-    rest = float(xg.grad[[i for i in range(b) if i not in picked]].abs().max()) / float(got.abs().max())
-    p64 = {k: torch.from_numpy(v).double() for k, v in params.items()}
-    laps64 = []
-    for lap in laps:
-        coo = lap.tocoo()
-        laps64.append(torch.sparse_coo_tensor(np.vstack([coo.row, coo.col]), coo.data.astype(np.float64), lap.shape).coalesce())
-    xr = x[picked].double().requires_grad_(True)
-    with _gcn_as(_sparse_cheb_gcn):
-        out = O.dense_st_mgcn(p64, xr, laps64, relu=False)
-    loss = torch.mean((out - y[picked].double()) ** 2) * len(picked) / b
-    (ref,) = torch.autograd.grad(loss, [xr])
-    err = _err(got, ref)
-    print(f"cfg3 d obs (windows {picked}): {err:.2e}; the other windows' d obs {rest:.1e} of the picked ones'")
-    assert err <= TOL, err
-    assert rest <= TOL, rest
+    from test_gpu_fullsize import CHUNK, _build
+    w = synth.WORKLOADS["cfg3"]
+    model, sups, laps, params, x, y = _build(w, 64, relu=False)
+    errs = full_batch.run("cfg3 d obs", model, sups, params, [[lap] for lap in laps], w.n_supports, x, y, relu=False,
+                          window_chunk=CHUNK["cfg3"], want_obs=True)
+    full_batch.assert_within(errs, TOL, what="cfg3 d obs")

@@ -348,6 +348,79 @@ def test_bf16_mode_reference_without_rounding_is_the_chain_oracle():
         assert_close(grads[key].numpy(), g2[key], f"grad {key}", 1e-12)
 
 
+def _random_masks(params, chains, ks, x, seed):
+    """One random boolean ReLU mask (N, B, q) per GCN (temporal 0, spatial 0, temporal 1, ...): the model then follows
+    branches no free-running forward would, so a mask sliced on the wrong axis or to the wrong windows shows."""
+    gen = torch.Generator().manual_seed(seed)
+    b, t, n, _ = x.shape
+    g = params["gcn_list.0.W"].shape[1]
+    return [torch.rand(n, b, q, generator=gen) < 0.6 for _ in chains for q in (t, g)]
+
+
+@pytest.mark.parametrize("case", ["relu_masks", "smooth", "diffusion_relu_masks", "diffusion_smooth"])
+def test_bf16_mode_reference_in_window_chunks_is_the_sparse_oracle(case):
+    """``loss_and_grads(window_chunk=...)``: every branch's forward and backward a chunk of windows at a time, the
+    gradients summed over chunks.  Chunks of 1 window, chunks that leave a ragged last chunk, and one chunk of the whole
+    batch equal the unchunked model and SparseOracle / ChainOracle (Chebyshev / diffusion chains) to fp64 rounding:
+    output, loss, every parameter gradient and d obs, with given ReLU masks (sliced to each chunk's windows) or without
+    an activation."""
+    import diffusion_oracle as D
+    kind = "random_walk_diffusion" if case.startswith("diffusion") else "chebyshev"
+    relu = case.endswith("relu_masks")
+    params, chains, ks, x, y = _bf16_case(11, kind=kind, k=2, b=5, m=2, lyr=2)
+    masks = _random_masks(params, chains, ks, x, 12) if relu else None
+    ref = O.BF16ModeReference(params, chains, ks, relu=relu, rounding=False, relu_masks=masks)
+    out, loss, grads = ref.loss_and_grads(x, y, want_obs=True)
+    np_params = {k_: v.numpy() for k_, v in params.items()}
+    np_masks = None if masks is None else [mk.numpy() for mk in masks]
+    orc = (D.ChainOracle(np_params, chains, ks, relu=relu, relu_masks=np_masks) if kind != "chebyshev" else
+           O.SparseOracle(np_params, [ch[0] for ch in chains], ks, relu=relu, relu_masks=np_masks))
+    o2, l2, g2 = orc.loss_and_grads(x.numpy(), y.numpy())
+    assert_close(out.numpy(), o2, "unchunked forward", 1e-12)
+    for key in g2:
+        assert_close(grads[key].numpy(), g2[key], f"unchunked grad {key}", 1e-12)
+    for chunk in (1, 2, 3, x.shape[0]):                    # 2 and 3 leave a last chunk of 1 and 2 windows
+        out_c, loss_c, grads_c = ref.loss_and_grads(x, y, want_obs=True, window_chunk=chunk)
+        assert_close(out_c.numpy(), o2, f"chunk {chunk} forward", 1e-12)
+        assert abs(float(loss_c) - l2) <= 1e-12 * abs(l2)
+        assert set(grads_c) == set(g2) | {"obs"}
+        for key in g2:
+            assert_close(grads_c[key].numpy(), g2[key], f"chunk {chunk} grad {key}", 1e-12)
+        assert_close(grads_c["obs"].numpy(), grads["obs"].numpy(), f"chunk {chunk} d obs", 1e-12)
+
+
+def test_bf16_mode_reference_in_window_chunks_slices_the_tapes():
+    """Rounding on and forced with tapes (rows n*B + b, and the spatial stacks (Ks, N, B, H)): each chunk takes its own
+    windows' rows of the tapes, so the chunked model equals the unchunked one to fp64 rounding.  Forcing is per window
+    (a tape with two windows swapped moves the output), so that agreement needs every chunk to take its own windows'."""
+    params, chains, ks, x, y = _bf16_case(13, hid=16, b=5)
+    ref = O.BF16ModeReference(params, chains, ks, relu=True)
+    tapes = _own_tapes(ref, x)
+    out, loss, grads = ref.loss_and_grads(x, y, tapes=tapes, want_obs=True)
+    for chunk in (1, 2, 5):
+        out_c, loss_c, grads_c = ref.loss_and_grads(x, y, tapes=tapes, want_obs=True, window_chunk=chunk)
+        assert_close(out_c.numpy(), out.numpy(), f"chunk {chunk} forced forward", 1e-12)
+        assert abs(float(loss_c) - float(loss)) <= 1e-12 * abs(float(loss))
+        for key in grads:
+            assert_close(grads_c[key].numpy(), grads[key].numpy(), f"chunk {chunk} forced grad {key}", 1e-12)
+    n, b = x.shape[2], x.shape[0]
+    perm = torch.tensor([1, 0, 2, 3, 4])
+    swapped = [dict(h=t["h"].reshape(*t["h"].shape[:2], n, b, -1)[:, :, :, perm].reshape(t["h"].shape),
+                    c=t["c"].reshape(*t["c"].shape[:2], n, b, -1)[:, :, :, perm].reshape(t["c"].shape),
+                    s=t["s"][:, :, perm]) for t in tapes]
+    out_s, _, _ = ref.loss_and_grads(x, y, tapes=swapped, window_chunk=2)
+    assert O.max_rel_err(out_s.numpy(), out.numpy()) > 1e-6
+
+
+def test_bf16_mode_reference_window_chunk_rejects_on_branch_and_bad_sizes():
+    params, chains, ks, x, y = _bf16_case(14, b=2)
+    ref = O.BF16ModeReference(params, chains, ks, rounding=False)
+    with pytest.raises(ValueError):
+        ref.loss_and_grads(x, y, window_chunk=0)
+    with pytest.raises(ValueError):
+        ref.loss_and_grads(x, y, window_chunk=1, on_branch=lambda m, br: None)
+
+
 def _own_tapes(ref, x):
     """The tapes of ``ref``'s own free-running forward, in the layout BF16ModeReference takes."""
     tapes = {}
