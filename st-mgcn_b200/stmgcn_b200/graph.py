@@ -27,17 +27,45 @@ import torch
 
 def csr_from_coo(n: int, rows: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor):
     """int32 CSR ``(rowptr, colidx, vals)`` of the ``n x n`` matrix whose entries ``(rows, cols, vals)`` are sorted
-    row-major (by row, then column)."""
+    row-major (by row, then column).  The result shares no memory with the arguments."""
     nnz = rows.numel()
     if not 0 < n < 2 ** 30 or nnz >= 2 ** 31:
         raise ValueError(f"CSR: n={n} must be in [1, 2^30) and nnz={nnz} below 2^31 (int32 indices)")
     rowptr = torch.zeros(n + 1, dtype=torch.int32, device=rows.device)
     rowptr[1:] = torch.cumsum(torch.bincount(rows, minlength=n), 0)
-    return rowptr, cols.to(torch.int32), vals.to(torch.float32).contiguous()
+    return rowptr, cols.to(torch.int32, copy=True), vals.detach().to(torch.float32, copy=True).contiguous()
+
+
+def check_csr(n: int, rowptr: torch.Tensor, colidx: torch.Tensor, vals: torch.Tensor) -> None:
+    """Raise ``ValueError`` naming the first fault of an ``n x n`` CSR matrix: dtypes, devices, sizes, ``rowptr``
+    starting at 0, never decreasing and ending at ``nnz``, every column index in ``[0, n)``.  One host sync."""
+    if rowptr.dtype != torch.int32 or colidx.dtype != torch.int32 or vals.dtype != torch.float32:
+        raise ValueError(f"CSR: rowptr / colidx must be int32 and vals float32, got {rowptr.dtype} / {colidx.dtype} / "
+                         f"{vals.dtype}")
+    devices = {str(t.device) for t in (rowptr, colidx, vals)}
+    if len(devices) != 1:
+        raise ValueError(f"CSR: rowptr, colidx and vals are on mixed devices {sorted(devices)}")
+    if rowptr.dim() != 1 or colidx.dim() != 1 or vals.dim() != 1:
+        raise ValueError("CSR: rowptr, colidx and vals must be 1-D")
+    if rowptr.numel() != n + 1:
+        raise ValueError(f"CSR: rowptr has {rowptr.numel()} entries, n + 1 = {n + 1} expected")
+    nnz = colidx.numel()
+    if vals.numel() != nnz:
+        raise ValueError(f"CSR: vals has {vals.numel()} entries, colidx {nnz}")
+    faults = torch.stack([rowptr[0] != 0, (rowptr[1:] < rowptr[:-1]).any(), rowptr[-1] != nnz,
+                          ((colidx < 0) | (colidx >= n)).any()]).tolist()
+    names = ["rowptr[0] is not 0", "rowptr decreases", f"rowptr[-1] is not nnz = {nnz}",
+             f"a column index is outside [0, {n})"]
+    for fault, name in zip(faults, names):
+        if fault:
+            raise ValueError(f"CSR: {name}")
 
 
 class GraphHandle:
-    """CSR and CSR^T of one ``n x n`` support matrix: int32 ``rowptr`` / ``colidx`` and fp32 ``vals`` tensors."""
+    """CSR and CSR^T of one ``n x n`` support matrix: int32 ``rowptr`` / ``colidx`` and fp32 ``vals`` tensors.
+
+    The handle owns its tensors (copies of what it was built from), so the CSR and the CSR^T are one snapshot of the
+    matrix: an edit of the source after the build reaches neither."""
 
     def __init__(self, n: int, rows: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor):
         """From the matrix's entries, sorted row-major; ``rows`` and ``cols`` are int64."""
@@ -56,8 +84,9 @@ class GraphHandle:
 
     @classmethod
     def from_csr(cls, n: int, rowptr: torch.Tensor, colidx: torch.Tensor, vals: torch.Tensor) -> "GraphHandle":
-        assert rowptr.dtype == torch.int32 and colidx.dtype == torch.int32
-        assert vals.dtype == torch.float32 and rowptr.numel() == n + 1
+        """From a CSR matrix (checked by :func:`check_csr`).  Columns may be unsorted within a row, entries repeated
+        (each one is applied: repeats add up) and stored zeros kept."""
+        check_csr(n, rowptr, colidx, vals)
         rows = torch.repeat_interleave(torch.arange(n, device=rowptr.device), (rowptr[1:] - rowptr[:-1]).long(),
                                        output_size=colidx.numel())
         return cls(n, rows, colidx.long(), vals)
@@ -122,6 +151,14 @@ _CACHE: "OrderedDict[tuple, tuple]" = OrderedDict()
 _CACHE_MAX = 32
 
 
+def support_version(a) -> tuple:
+    """What a support stack's conversion is keyed on: identity and in-place version of its tensors.  Any edit of the
+    stack through a torch op changes it."""
+    if isinstance(a, SparseSupports):
+        return a.version()
+    return (a.data_ptr(), a._version, tuple(a.shape), tuple(a.stride()), str(a.device), a.dtype)
+
+
 def supports_from_dense(a: torch.Tensor) -> SupportSet:
     """Cached conversion of a dense support stack (keyed on tensor identity + in-place version)."""
     if isinstance(a, SparseSupports):
@@ -131,7 +168,7 @@ def supports_from_dense(a: torch.Tensor) -> SupportSet:
     if not a.is_cuda:
         raise RuntimeError("stmgcn_b200 has no CPU path: supports must live on a CUDA device "
                            "(the reference moves them there at Main.py:54)")
-    key = (a.data_ptr(), a._version, tuple(a.shape), tuple(a.stride()), str(a.device), a.dtype)
+    key = support_version(a)
     hit = _CACHE.get(key)
     if hit is not None:
         _CACHE.move_to_end(key)
@@ -171,6 +208,7 @@ class SparseSupports:
         self.mode, self.n, self.ks = mode, int(n), int(ks)
         self.mats = [(rp.to(torch.int32), ci.to(torch.int32), v.float()) for rp, ci, v in mats]
         self._sset: Optional[SupportSet] = None
+        self._sset_version: tuple = ()
 
     @property
     def shape(self):
@@ -199,13 +237,21 @@ class SparseSupports:
     def cuda(self, device=None):
         return self.to(torch.device("cuda", torch.cuda.current_device() if device is None else device))
 
+    def version(self) -> tuple:
+        """Identity and in-place version of every stored tensor: changes with any edit through a torch op."""
+        return tuple((t.data_ptr(), t._version) for m in self.mats for t in m)
+
     def support_set(self) -> SupportSet:
-        if self._sset is None:
+        """The kernels' copy of the stored matrices, built again whenever :meth:`version` has changed since the last
+        build (as :func:`supports_from_dense` does for a dense stack)."""
+        version = self.version()
+        if self._sset is None or self._sset_version != version:
             if not self.is_cuda:
                 raise RuntimeError(f"{type(self).__name__} must be moved to a CUDA device before use (.to(device))")
             mats = self.mats if self.mode == "generic" or self.ks > 1 else []
             graphs = [GraphHandle.from_csr(self.n, *m) for m in mats]
             self._sset = SupportSet(self.mode, self.n, self.ks, graphs, self.device)
+            self._sset_version = version
         return self._sset
 
     def matrices_dense(self) -> List[torch.Tensor]:

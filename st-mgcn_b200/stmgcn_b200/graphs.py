@@ -8,6 +8,10 @@ once into a CUDA graph and replayed: ``GraphedStep(model, criterion, x, y, suppo
 The kernels launched through the C ABI take the stream from ``torch.cuda.current_stream()``, so they are captured
 like any torch op; every buffer they touch comes from torch's allocator and therefore from the graph's private pool.
 Gradients are accumulated into ``GradBucket`` views (static addresses).  The optimizer step stays outside the graph.
+
+The supports are baked in too: the graph reads the CSR tensors of the support sets converted at capture.  The step holds
+those sets (so their memory stays valid whatever happens to the conversion cache) and the supports' versions
+(``graph.support_version``); a call after any support was edited raises instead of replaying the old supports.
 """
 from __future__ import annotations
 
@@ -16,6 +20,7 @@ from typing import Callable, Optional, Sequence
 import torch
 
 from .dp import GradBucket
+from .graph import support_version, supports_from_dense
 
 
 class GraphedStep:
@@ -36,6 +41,9 @@ class GraphedStep:
                 self._eager()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
+        # the conversions the warm-up cached, which the capture below reads
+        self.support_sets = [supports_from_dense(s) for s in self.supports]
+        self.support_versions = [support_version(s) for s in self.supports]
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.loss = self._eager()
@@ -52,7 +60,12 @@ class GraphedStep:
 
     def __call__(self, x: Optional[torch.Tensor] = None, y: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Copy the batch into the static buffers (host or device source) and replay. Returns the loss tensor
-        (static buffer: read it before the next call)."""
+        (static buffer: read it before the next call).  Raises ``RuntimeError`` if a support was edited since the
+        capture (build a new ``GraphedStep`` then)."""
+        changed = [m for m, s in enumerate(self.supports) if support_version(s) != self.support_versions[m]]
+        if changed:
+            raise RuntimeError(f"GraphedStep: supports {changed} were edited after the step was captured; the captured "
+                               f"graph would replay the supports of capture time: capture a new GraphedStep")
         if x is not None and tuple(x.shape) != tuple(self.x.shape):
             # a batch of another size (the reference's DataLoader yields one short last batch, Data_Container.py:122):
             # shapes are baked into the captured graph, so this batch runs eagerly

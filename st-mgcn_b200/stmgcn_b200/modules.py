@@ -176,11 +176,11 @@ class ST_MGCN(nn.Module):
     def forward(self, obs_seq: torch.Tensor, sta_adj_list: list):
         """``obs_seq``: (B,T,N,C); ``sta_adj_list``: M support stacks -> (B,N,C).  ``STMGCN.py:100-119``."""
         assert len(sta_adj_list) == self.M
-        xo, xt = ops.obs_to_node_major(obs_seq)          # shared by all graphs
-        ssets = []
+        ssets = []                                        # first: a malformed support raises before any launch
         for m in range(self.M):
             assert self.sta_K == sta_adj_list[m].shape[0]
             ssets.append(supports_from_dense(sta_adj_list[m]))
+        xo, xt = ops.obs_to_node_major(obs_seq)          # shared by all graphs
         feats = []
         if self.M > 1 and _graph_streams_enabled():
             # the M graph branches are independent until the fusion: one CUDA stream per branch keeps the device's work
