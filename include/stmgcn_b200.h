@@ -89,7 +89,7 @@ int32_t stmgcn_obs_grad(const float* d_xo, const float* d_xt, float* d_obs, int6
 
 /* ---- K2: stacked-K projection (GCN.py:37-42) --------------------------------------------------------
  * out[r,:] = act( sum_k S_k[r,:] W[k*p:(k+1)*p, :] + bias ),  r in [0, rows), S_k = s + k*stride_k
- * (rows x p, row-major), W: (ks*p, q) row-major, bias: q or NULL.
+ * (rows x p, row-major), W: (ks*p, q) row-major, bias: q or NULL.  ks <= 8 and q <= 8192 in both directions.
  * Optional gate pooling (STMGCN.py:41-42), requires q == p: pool[(r % b_inner)*q + j] +=
  * S_0[r,j] + out[r,j]  (caller zeroes pool; sum over regions of x_hat, not yet divided by N). */
 int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t rows, int32_t p,
@@ -114,7 +114,8 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
                         void* stream);
 
 /* ---- K3a: context gate (STMGCN.py:42-43) -----------------------------------------------------------
- * z = pool / n_regions; a1 = z fcw^T + fcb; s = sigmoid(relu(a1) fcw^T + fcb).  All (B, T); fcw (T,T). */
+ * z = pool / n_regions; a1 = z fcw^T + fcb; s = sigmoid(relu(a1) fcw^T + fcb).  All (B, T); fcw (T,T).
+ * Both directions take T <= 2048 (the backward's shared memory); beyond it STMGCN_ERR_SHAPE. */
 int32_t stmgcn_gate_fwd(const float* pool, int64_t b, int32_t t, int64_t n_regions, const float* fcw,
                         const float* fcb, float* z, float* a1, float* s, void* stream);
 /* d_s -> d_fcw (+=), d_fcb (+=), d_z (B,T).  d_fcw and d_fcb may be NULL together (a frozen fc): d_z only.  One of
@@ -231,7 +232,8 @@ int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t rows, int3
                              float* d_xo, void* stream);
 
 /* ---- fusion over graphs + output FC (STMGCN.py:116-118) ------------------------------------------
- * feat = sum_m g[m] (each (R, G) node-major); y[b, n, c] = feat[n*B+b, :] . fcw[c, :] + fcb[c]. */
+ * feat = sum_m g[m] (each (R, G) node-major); y[b, n, c] = feat[n*B+b, :] . fcw[c, :] + fcb[c].
+ * M <= 8.  Both directions take C*G + C <= 12288 (the backward's 48 KB shared-memory accumulator). */
 int32_t stmgcn_fuse_out_fwd(const float* const* g, int32_t m, int64_t n, int64_t b, int32_t gdim,
                             int32_t c, const float* fcw, const float* fcb, float* feat, float* y,
                             void* stream);

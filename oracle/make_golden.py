@@ -3,10 +3,11 @@
 TEST INFRASTRUCTURE.  Needs a checkout of the reference (its ``GCN.py`` / ``STMGCN.py``); the fixtures it writes are
 committed, so the tests never need the reference itself:
 
-    python oracle/make_golden.py /path/to/reference
+    python oracle/make_golden.py /path/to/reference [fixture names]       (default: every fixture)
 
 Each fixture stores: the adjacency matrices, the reference's supports ``Adj_Preprocessor.process``
-(``GCN.py:57-97``), the reference model's ``state_dict`` after ``torch.manual_seed(seed)`` construction,
+(``GCN.py:57-97``), the model configuration (``kernel_type``, ``gconv_use_bias``, the activation class name or
+``"None"``), the reference model's ``state_dict`` after ``torch.manual_seed(seed)`` construction,
 inputs ``x, y``, the forward output of ``ST_MGCN.forward`` (``STMGCN.py:100-119``), the MSE loss and the
 autograd gradient of every parameter.  Reference modules are imported under their own names from a
 temporary ``sys.path`` entry and removed again so they can never shadow the repo's drop-in modules.
@@ -40,7 +41,10 @@ def import_reference():
     return ref_gcn, ref_stmgcn
 
 
-def build_case(name, n, m, k, t, b, c, hid, layers, gcn_hid, density, seed, weighted=False):
+def build_case(name, n, m, k, t, b, c, hid, layers, gcn_hid, density, seed, weighted=False, kernel_type="chebyshev",
+               gconv_use_bias=True, gconv_activation=nn.ReLU):
+    """``k``: the ``K`` of ``sta_kernel_config`` (1 for ``localpool``); the supports are the reference's own
+    ``Adj_Preprocessor(kernel_type, k).process``."""
     sys.path.insert(0, os.path.join(REPO, "st-mgcn_b200"))
     from stmgcn_b200 import synth
     ref_gcn, ref_stmgcn = import_reference()
@@ -48,12 +52,12 @@ def build_case(name, n, m, k, t, b, c, hid, layers, gcn_hid, density, seed, weig
     if weighted:                                    # asymmetric, weighted => asymmetric L~
         gen = torch.Generator().manual_seed(77)
         adjs = [a * (0.25 + torch.rand(n, n, generator=gen)) for a in adjs]
-    sups = [ref_gcn.Adj_Preprocessor("chebyshev", k).process(a) for a in adjs]
+    sups = [ref_gcn.Adj_Preprocessor(kernel_type, k).process(a) for a in adjs]
     torch.manual_seed(seed)
     model = ref_stmgcn.ST_MGCN(M=m, seq_len=t, n_nodes=n, input_dim=c, lstm_hidden_dim=hid,
                                lstm_num_layers=layers, gcn_hidden_dim=gcn_hid,
-                               sta_kernel_config={"kernel_type": "chebyshev", "K": k},
-                               gconv_use_bias=True, gconv_activation=nn.ReLU)
+                               sta_kernel_config={"kernel_type": kernel_type, "K": k},
+                               gconv_use_bias=gconv_use_bias, gconv_activation=gconv_activation)
     x = torch.randn(b, t, n, c)
     y = torch.randn(b, n, c)
     out = model(obs_seq=x, sta_adj_list=sups)
@@ -61,7 +65,9 @@ def build_case(name, n, m, k, t, b, c, hid, layers, gcn_hid, density, seed, weig
     loss.backward()
     blob = {"meta": np.array([n, m, k, t, b, c, hid, layers, gcn_hid], dtype=np.int64),
             "x": x.numpy(), "y": y.numpy(), "out": out.detach().numpy(),
-            "loss": np.array(loss.item(), dtype=np.float64)}
+            "loss": np.array(loss.item(), dtype=np.float64), "kernel_type": np.array(kernel_type),
+            "gconv_use_bias": np.array(gconv_use_bias),
+            "gconv_activation": np.array("None" if gconv_activation is None else gconv_activation.__name__)}
     for g, (a, s) in enumerate(zip(adjs, sups)):
         blob[f"adj.{g}"] = a.numpy()
         blob[f"supports.{g}"] = s.numpy()
@@ -80,13 +86,25 @@ if __name__ == "__main__":
     if not os.path.exists(os.path.join(REF, "STMGCN.py")):
         sys.exit("usage: python oracle/make_golden.py /path/to/reference  (the directory with GCN.py and STMGCN.py)")
     torch.set_num_threads(1)
-    # BASELINE.json configs[0]: 64 regions, 1 graph, K=2, seq_len=4, batch=8, H=G=64, L=3, C=1.
-    build_case("cfg1_ref", 64, 1, 2, 4, 8, 1, 64, 3, 64, 0.10, seed=0)
-    # ragged/small case: 3 graphs, weighted asymmetric adjacency, C=2, odd sizes.
-    build_case("ragged_ref", 37, 3, 3, 5, 3, 2, 16, 2, 24, 0.15, seed=1, weighted=True)
-    # BASELINE.json configs[1]/[2] hyper-parameters (3 graphs, K=3, seq_len=12, H=G=64, L=3, C=1) at a size the reference
-    # finishes in seconds: 96 regions x batch 6 = 576 LSTM rows (4.5 tiles of 128: ragged last tile on the GPU).
-    build_case("cfg3_small_ref", 96, 3, 3, 12, 6, 1, 64, 3, 64, 0.05, seed=2)
-    # two graphs, two LSTM layers, narrow hidden sizes (H=16, G=8): pins the oracle's dense restatement to the reference
-    # modules away from the H=64 shapes of the other fixtures.
-    build_case("small_ref", 30, 2, 3, 5, 2, 1, 16, 2, 8, 0.2, seed=3)
+    cases = {
+        # BASELINE.json configs[0]: 64 regions, 1 graph, K=2, seq_len=4, batch=8, H=G=64, L=3, C=1.
+        "cfg1_ref": lambda: build_case("cfg1_ref", 64, 1, 2, 4, 8, 1, 64, 3, 64, 0.10, seed=0),
+        # ragged/small case: 3 graphs, weighted asymmetric adjacency, C=2, odd sizes.
+        "ragged_ref": lambda: build_case("ragged_ref", 37, 3, 3, 5, 3, 2, 16, 2, 24, 0.15, seed=1, weighted=True),
+        # BASELINE.json configs[1]/[2] hyper-parameters (3 graphs, K=3, seq_len=12, H=G=64, L=3, C=1) at a size the
+        # reference finishes in seconds: 96 regions x batch 6 = 576 LSTM rows (4.5 tiles of 128: ragged last tile on the GPU).
+        "cfg3_small_ref": lambda: build_case("cfg3_small_ref", 96, 3, 3, 12, 6, 1, 64, 3, 64, 0.05, seed=2),
+        # two graphs, two LSTM layers, narrow hidden sizes (H=16, G=8): pins the oracle's dense restatement to the
+        # reference modules away from the H=64 shapes of the other fixtures.
+        "small_ref": lambda: build_case("small_ref", 30, 2, 3, 5, 2, 1, 16, 2, 8, 0.2, seed=3),
+        # no GCN bias, a Tanh activation (applied by torch, outside the kernels), localpool supports (one generic
+        # support, not I: the temporal pooling's residual is added by torch), C=2, two graphs; H=G=64 (tensor cores).
+        "localpool_tanh_ref": lambda: build_case("localpool_tanh_ref", 48, 2, 1, 8, 3, 2, 64, 2, 64, 0.12, seed=4,
+                                                 weighted=True, kernel_type="localpool", gconv_use_bias=False,
+                                                 gconv_activation=nn.Tanh),
+        # no GCN bias, no activation, Chebyshev K=7 (8 supports: the projections' maximum), one LSTM layer, H=G=64.
+        "cheb7_linear_ref": lambda: build_case("cheb7_linear_ref", 40, 2, 7, 12, 4, 1, 64, 1, 64, 0.12, seed=5,
+                                               gconv_use_bias=False, gconv_activation=None),
+    }
+    for name in (sys.argv[2:] or cases):
+        cases[name]()

@@ -70,10 +70,25 @@ def chebyshev_supports_dense(adj: torch.Tensor, order: int, lambda_max: float = 
 # --------------------------------------------------------------------------------------------------
 # dense restatement (torch CPU; autograd supplies the backward)
 # --------------------------------------------------------------------------------------------------
+def _activate(z: torch.Tensor, relu, mask: Optional[torch.Tensor]) -> torch.Tensor:
+    """The GCN activation ``relu`` of the dense restatement on the pre-activation ``z`` (B, N, q): True = ReLU, False or
+    None = none, anything else a callable applied to ``z`` (a torch module such as ``nn.Tanh()``, as the reference's
+    ``self.activation``).  ``mask`` (ReLU only): a boolean ReLU mask in the kernels' node-major layout (N, B, q) used in
+    place of ``z > 0``: ``out = z * mask``."""
+    if relu is True:
+        return torch.relu(z) if mask is None else z * mask.permute(1, 0, 2).to(z.dtype)
+    if mask is not None:
+        raise ValueError("a forced ReLU mask needs the ReLU activation")
+    if relu is False or relu is None:
+        return z
+    return relu(z)
+
+
 def dense_gcn(supports: torch.Tensor, x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor],
-              relu: bool = True) -> torch.Tensor:
+              relu=True, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``GCN.forward`` (``GCN.py:24-43``): ``act(cat_k(A_k x) W + b)``; rows ``[k p,(k+1) p)`` of W
-    pair with support k."""
+    pair with support k.  ``relu`` / ``mask``: the activation and an optional forced ReLU mask (:func:`_activate`).
+    Runs on the device and in the dtype of its arguments (fp64 on the GPU for the model-level sweeps)."""
     n_sup = supports.shape[0]
     p = x.shape[-1]
     assert w.shape[0] == n_sup * p                      # GCN.py:31 in spirit
@@ -84,7 +99,7 @@ def dense_gcn(supports: torch.Tensor, x: torch.Tensor, w: torch.Tensor, b: Optio
         out = term if out is None else out + term
     if b is not None:
         out = out + b
-    return torch.relu(out) if relu else out
+    return _activate(out, relu, mask)
 
 
 def lstm_explicit(x: torch.Tensor, layers: Sequence[Tuple[torch.Tensor, ...]],
@@ -215,14 +230,24 @@ def _count_lstm_layers(params: Params, prefix: str) -> int:
     return n
 
 
+def _gcn(supports, x, w, b, relu, mask):
+    """:func:`dense_gcn` as the model functions call it: through the module attribute, and with ``mask`` only when one
+    is forced, so a caller that puts a graph convolution of the five-argument form ``(supports, x, w, b, relu)`` in
+    place of ``dense_gcn`` still runs the model on it."""
+    if mask is None:
+        return dense_gcn(supports, x, w, b, relu)
+    return dense_gcn(supports, x, w, b, relu, mask)
+
+
 def dense_cg_lstm(supports: torch.Tensor, obs: torch.Tensor, params: Params, prefix: str,
-                  relu: bool = True, lstm=lstm_explicit, hidden=None):
+                  relu=True, lstm=lstm_explicit, hidden=None, mask: Optional[torch.Tensor] = None):
     """``CG_LSTM.forward`` (``STMGCN.py:24-51``).  ``params`` uses the reference ``state_dict`` names
-    under ``prefix`` (e.g. ``rnn_list.0.``).  Returns ``(out (B,N,H), (h_n, c_n))``."""
+    under ``prefix`` (e.g. ``rnn_list.0.``).  ``relu`` / ``mask``: the temporal GCN's activation and forced ReLU mask
+    (:func:`_activate`).  Returns ``(out (B,N,H), (h_n, c_n))``."""
     b_sz, t_len, n, c_in = obs.shape
     x_seq = obs.sum(dim=-1).permute(0, 2, 1)                                    # :36, :39  (B,N,T)
-    gconv = dense_gcn(supports, x_seq, params[prefix + "gconv_temporal_feats.W"],
-                      params.get(prefix + "gconv_temporal_feats.b"), relu)        # :40
+    gconv = _gcn(supports, x_seq, params[prefix + "gconv_temporal_feats.W"],
+                 params.get(prefix + "gconv_temporal_feats.b"), relu, mask)       # :40
     x_hat = x_seq + gconv                                                        # :41
     z = x_hat.sum(dim=1) / n                                                     # :42  (B,T)
     fw, fb = params[prefix + "fc.weight"], params[prefix + "fc.bias"]
@@ -236,24 +261,33 @@ def dense_cg_lstm(supports: torch.Tensor, obs: torch.Tensor, params: Params, pre
 
 
 def dense_st_mgcn(params: Params, obs: torch.Tensor, supports_list: Sequence[torch.Tensor],
-                  relu: bool = True, lstm=lstm_explicit) -> torch.Tensor:
-    """``ST_MGCN.forward`` (``STMGCN.py:100-119``) -> ``(B,N,C)``."""
+                  relu=True, lstm=lstm_explicit, masks=None) -> torch.Tensor:
+    """``ST_MGCN.forward`` (``STMGCN.py:100-119``) -> ``(B,N,C)``.  ``relu``: every GCN's activation (:func:`_activate`);
+    ``masks`` (ReLU only, optional): the forced ReLU masks of the 2M GCNs, boolean (N, B, q) each, in the kernels' order
+    temporal 0, spatial 0, temporal 1, ... (as :class:`SparseOracle` takes them)."""
+    if masks is not None and len(masks) != 2 * len(supports_list):
+        raise ValueError(f"{len(masks)} ReLU masks for {len(supports_list)} graphs (two GCNs each)")
     fused = None
     for m, sup in enumerate(supports_list):                                       # :112
-        cg, _ = dense_cg_lstm(sup, obs, params, f"rnn_list.{m}.", relu, lstm)      # :113
-        g = dense_gcn(sup, cg, params[f"gcn_list.{m}.W"], params.get(f"gcn_list.{m}.b"), relu)  # :114
+        mt, ms = (None, None) if masks is None else masks[2 * m:2 * m + 2]
+        cg, _ = dense_cg_lstm(sup, obs, params, f"rnn_list.{m}.", relu, lstm, mask=mt)  # :113
+        g = _gcn(sup, cg, params[f"gcn_list.{m}.W"], params.get(f"gcn_list.{m}.b"), relu, ms)   # :114
         fused = g if fused is None else fused + g                                 # :116
     return fused @ params["fc.weight"].t() + params["fc.bias"]                   # :118
 
 
 def dense_loss_and_grads(params: Params, obs: torch.Tensor, y: torch.Tensor,
-                         supports_list: Sequence[torch.Tensor], relu: bool = True, lstm=lstm_explicit):
-    """MSE(mean) loss (``Main.py:66-67``, ``Model_Trainer.py:38``) + gradient of every parameter."""
+                         supports_list: Sequence[torch.Tensor], relu=True, lstm=lstm_explicit, masks=None,
+                         want_obs: bool = False):
+    """MSE(mean) loss (``Main.py:66-67``, ``Model_Trainer.py:38``) + gradient of every parameter (and, with ``want_obs``,
+    of ``obs`` under the key ``"obs"``).  ``relu`` / ``masks`` as for :func:`dense_st_mgcn`."""
     leaves = {k: v.detach().clone().requires_grad_(True) for k, v in params.items()}
-    out = dense_st_mgcn(leaves, obs, supports_list, relu, lstm)
+    obs_leaf = obs.detach().clone().requires_grad_(want_obs)
+    out = dense_st_mgcn(leaves, obs_leaf, supports_list, relu, lstm, masks)
     loss = torch.mean((out - y) ** 2)
-    grads = torch.autograd.grad(loss, list(leaves.values()), allow_unused=True)
-    return out.detach(), loss.detach(), {k: g for k, g in zip(leaves.keys(), grads)}
+    grads = torch.autograd.grad(loss, list(leaves.values()) + ([obs_leaf] if want_obs else []), allow_unused=True)
+    res = {k: g for k, g in zip(list(leaves.keys()) + (["obs"] if want_obs else []), grads)}
+    return out.detach(), loss.detach(), res
 
 
 def init_params(n_graphs: int, seq_len: int, c_in: int, hid: int, n_layers: int, gcn_hid: int,

@@ -109,6 +109,7 @@ dz_kernel(const float* __restrict__ out, const float* __restrict__ d_out, const 
 
 // dW (kd x q) += S^T dZ for SMALL kd*q (the temporal GCN: kd = Ks*T = 48, q = T = 12): each CTA streams row chunks of
 // S and dZ through shared memory; thread e owns outputs e, e + blockDim, ...  (i = out / q, j = out % q).
+constexpr int kMaxProjCols = 8192;                  // q: dz_kernel keeps q floats in shared memory
 constexpr int kSmallRows = 64;
 constexpr int kSmallThreads = 256;
 constexpr int kSmallMaxPerThread = 8;
@@ -171,6 +172,8 @@ int32_t stmgcn_proj_fwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     STMGCN_REQUIRE(s && w && out, STMGCN_ERR_ARG, "proj_fwd: null pointer");
     STMGCN_REQUIRE(ks >= 1 && ks <= kMaxSegs, STMGCN_ERR_SHAPE, "proj_fwd: %d supports (max %d)", ks, kMaxSegs);
     STMGCN_REQUIRE(rows > 0 && p > 0 && q > 0, STMGCN_ERR_SHAPE, "proj_fwd: bad shape");
+    // the backward's limit (its dZ kernel keeps q floats in shared memory), so no shape runs its forward only
+    STMGCN_REQUIRE(q <= kMaxProjCols, STMGCN_ERR_SHAPE, "proj_fwd: q=%d (max %d)", q, kMaxProjCols);
     STMGCN_REQUIRE(act == STMGCN_ACT_NONE || act == STMGCN_ACT_RELU, STMGCN_ERR_ARG, "proj_fwd: act=%d", act);
     STMGCN_REQUIRE(!pool || q == p, STMGCN_ERR_SHAPE, "proj_fwd: pooling needs q == p (got %d, %d)", q, p);
     STMGCN_REQUIRE(!pool || (b_inner > 0 && rows % b_inner == 0), STMGCN_ERR_SHAPE, "proj_fwd: rows %% b_inner != 0");
@@ -204,7 +207,8 @@ int32_t stmgcn_proj_bwd(const float* s, int64_t stride_k, int32_t ks, int64_t ro
     STMGCN_REQUIRE((d_out != nullptr) != (d_out_bcast != nullptr), STMGCN_ERR_ARG,
                    "proj_bwd: exactly one of d_out / d_out_bcast");
     STMGCN_REQUIRE(ks >= 1 && ks <= kMaxSegs, STMGCN_ERR_SHAPE, "proj_bwd: %d supports (max %d)", ks, kMaxSegs);
-    STMGCN_REQUIRE(rows > 0 && p > 0 && q > 0 && q <= 8192, STMGCN_ERR_SHAPE, "proj_bwd: bad shape");
+    STMGCN_REQUIRE(rows > 0 && p > 0 && q > 0, STMGCN_ERR_SHAPE, "proj_bwd: bad shape");
+    STMGCN_REQUIRE(q <= kMaxProjCols, STMGCN_ERR_SHAPE, "proj_bwd: q=%d (max %d)", q, kMaxProjCols);
     STMGCN_REQUIRE(!d_out_bcast || (b_inner > 0 && rows % b_inner == 0), STMGCN_ERR_SHAPE, "proj_bwd: b_inner");
     STMGCN_REQUIRE(!u || wt, STMGCN_ERR_ARG, "proj_bwd: u requested without wt");
     cudaStream_t st = (cudaStream_t)stream;

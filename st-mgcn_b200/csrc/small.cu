@@ -45,6 +45,9 @@ __global__ void obs_grad_kernel(const float* __restrict__ d_xo, const float* __r
 }
 
 // ---- context gate ----------------------------------------------------------------------------------
+// one limit for both directions: the backward keeps 4*T floats in (default, 48 KB) dynamic shared memory
+constexpr int kMaxGateSteps = 2048;
+
 // one CTA per window b; T threads-worth of work looped over blockDim
 __global__ void gate_fwd_kernel(const float* __restrict__ pool, int t_len, float inv_n,
                                 const float* __restrict__ fcw, const float* __restrict__ fcb,
@@ -111,6 +114,9 @@ __global__ void gate_bwd_kernel(const float* __restrict__ d_s, const float* __re
 
 // ---- fusion over graphs + output FC -------------------------------------------------------------------
 constexpr int kMaxGraphs = 8;
+// C*G + C floats: the backward's shared-memory accumulator (48 KB); the forward takes the same limit, so no shape runs its
+// forward and is then refused by its backward
+constexpr int kMaxFuseFloats = 48 * 1024 / 4;
 struct GraphPtrs {
     const float* g[kMaxGraphs];
 };
@@ -206,7 +212,8 @@ int32_t stmgcn_obs_grad(const float* d_xo, const float* d_xt, float* d_obs, int6
 int32_t stmgcn_gate_fwd(const float* pool, int64_t b, int32_t t, int64_t n_regions, const float* fcw,
                         const float* fcb, float* z, float* a1, float* s, void* stream) {
     STMGCN_REQUIRE(pool && fcw && fcb && z && a1 && s, STMGCN_ERR_ARG, "gate_fwd: null pointer");
-    STMGCN_REQUIRE(b > 0 && t > 0 && t <= 4096 && n_regions > 0, STMGCN_ERR_SHAPE, "gate_fwd: bad shape");
+    STMGCN_REQUIRE(b > 0 && t > 0 && n_regions > 0, STMGCN_ERR_SHAPE, "gate_fwd: bad shape");
+    STMGCN_REQUIRE(t <= kMaxGateSteps, STMGCN_ERR_SHAPE, "gate_fwd: T=%d (max %d)", t, kMaxGateSteps);
     const int threads = t <= 32 ? 32 : (t <= 128 ? 128 : 256);
     gate_fwd_kernel<<<(unsigned)b, threads, 2 * t * sizeof(float), (cudaStream_t)stream>>>(
         pool, t, 1.0f / (float)n_regions, fcw, fcb, z, a1, s);
@@ -218,7 +225,8 @@ int32_t stmgcn_gate_bwd(const float* d_s, const float* z, const float* a1, const
                         int32_t t, const float* fcw, float* d_fcw, float* d_fcb, float* d_z, void* stream) {
     STMGCN_REQUIRE(d_s && z && a1 && s && fcw && d_z, STMGCN_ERR_ARG, "gate_bwd: null pointer");
     STMGCN_REQUIRE((d_fcw == nullptr) == (d_fcb == nullptr), STMGCN_ERR_ARG, "gate_bwd: d_fcw and d_fcb go together");
-    STMGCN_REQUIRE(b > 0 && t > 0 && t <= 2048, STMGCN_ERR_SHAPE, "gate_bwd: bad shape");
+    STMGCN_REQUIRE(b > 0 && t > 0, STMGCN_ERR_SHAPE, "gate_bwd: bad shape");
+    STMGCN_REQUIRE(t <= kMaxGateSteps, STMGCN_ERR_SHAPE, "gate_bwd: T=%d (max %d)", t, kMaxGateSteps);
     const int threads = t <= 32 ? 32 : (t <= 128 ? 128 : 256);
     gate_bwd_kernel<<<(unsigned)b, threads, 4 * t * sizeof(float), (cudaStream_t)stream>>>(
         d_s, z, a1, s, t, fcw, d_fcw, d_fcb, d_z);
@@ -231,6 +239,8 @@ int32_t stmgcn_fuse_out_fwd(const float* const* g, int32_t m, int64_t n, int64_t
     STMGCN_REQUIRE(g && fcw && fcb && feat && y, STMGCN_ERR_ARG, "fuse_out_fwd: null pointer");
     STMGCN_REQUIRE(m >= 1 && m <= kMaxGraphs, STMGCN_ERR_SHAPE, "fuse_out_fwd: M=%d (max %d)", m, kMaxGraphs);
     STMGCN_REQUIRE(n > 0 && b > 0 && gdim > 0 && c > 0, STMGCN_ERR_SHAPE, "fuse_out_fwd: bad shape");
+    STMGCN_REQUIRE((int64_t)c * gdim + c <= kMaxFuseFloats, STMGCN_ERR_SHAPE, "fuse_out_fwd: C*G=%lld too large (C*G + C "
+                   "<= %d)", (long long)c * gdim, kMaxFuseFloats);
     GraphPtrs gp;
     for (int k = 0; k < kMaxGraphs; ++k) gp.g[k] = k < m ? g[k] : nullptr;
     for (int k = 0; k < m; ++k) STMGCN_REQUIRE(gp.g[k], STMGCN_ERR_ARG, "fuse_out_fwd: g[%d] null", k);
@@ -249,8 +259,9 @@ int32_t stmgcn_fuse_out_bwd(const float* d_y, const float* feat, int64_t n, int6
     STMGCN_REQUIRE(d_y && feat && fcw && d_feat, STMGCN_ERR_ARG, "fuse_out_bwd: null pointer");
     STMGCN_REQUIRE((d_fcw == nullptr) == (d_fcb == nullptr), STMGCN_ERR_ARG, "fuse_out_bwd: d_fcw and d_fcb go together");
     STMGCN_REQUIRE(n > 0 && b > 0 && gdim > 0 && c > 0, STMGCN_ERR_SHAPE, "fuse_out_bwd: bad shape");
+    STMGCN_REQUIRE((int64_t)c * gdim + c <= kMaxFuseFloats, STMGCN_ERR_SHAPE, "fuse_out_bwd: C*G=%lld too large (C*G + C "
+                   "<= %d)", (long long)c * gdim, kMaxFuseFloats);
     const size_t smem = ((size_t)c * gdim + c) * sizeof(float);
-    STMGCN_REQUIRE(smem <= 48 * 1024, STMGCN_ERR_SHAPE, "fuse_out_bwd: C*G=%d too large", c * gdim);
     const int64_t rows = n * b;
     const int64_t blocks = ceil_div(rows, 8);
     const int64_t cap = (int64_t)sm_count() * 4;

@@ -65,6 +65,7 @@ class GCN(nn.Module):
         """``A``: (K, N, N) supports (dense tensor as in the reference, or a ``SparseSupports`` handle);
         ``x``: (batch, N, input_dim) -> (batch, N, hidden_dim).  Reference ``GCN.py:24-43``."""
         assert self.K == A.shape[0]
+        ops.check_limits(ks=self.K, gcn_hid=self.hidden_dim)
         sset = supports_from_dense(A)
         x_nm = x.permute(1, 0, 2).contiguous()
         return self.forward_node_major(sset, x_nm).permute(1, 0, 2)
@@ -116,6 +117,8 @@ class CG_LSTM(nn.Module):
     def forward(self, adj, obs_seq: torch.Tensor, hidden: tuple):
         """Reference ``STMGCN.py:24-51``: returns ``(output (B,N,H), (h_n, c_n) each (L, B*N, H))``."""
         b, t, n, c = obs_seq.shape
+        ops.check_limits(ks=self.gconv_temporal_feats.K, c_in=c, n_layers=self.lstm_num_layers, hid=self.lstm_hidden_dim,
+                         t_len=t)
         sset = supports_from_dense(adj)
         xo, xt = ops.obs_to_node_major(obs_seq)
         lyr, hid = self.lstm_num_layers, self.lstm_hidden_dim
@@ -176,6 +179,10 @@ class ST_MGCN(nn.Module):
     def forward(self, obs_seq: torch.Tensor, sta_adj_list: list):
         """``obs_seq``: (B,T,N,C); ``sta_adj_list``: M support stacks -> (B,N,C).  ``STMGCN.py:100-119``."""
         assert len(sta_adj_list) == self.M
+        ops.check_limits(m=self.M)
+        rnn = self.rnn_list[0]
+        ops.check_limits(ks=self.sta_K, c_in=obs_seq.shape[3], n_layers=rnn.lstm_num_layers,
+                         hid=rnn.lstm_hidden_dim, t_len=obs_seq.shape[1], gcn_hid=self.fc.in_features)
         ssets = []                                        # first: a malformed support raises before any launch
         for m in range(self.M):
             assert self.sta_K == sta_adj_list[m].shape[0]

@@ -45,6 +45,47 @@ def set_lstm_path(path: str) -> None:
     _LSTM_PATH = path
 
 
+# The module-level limits of the kernels, the numbers the C entry points enforce (include/stmgcn_b200.h).  The modules
+# check them before a step's first launch (check_limits), so a configuration beyond one raises at once, naming the limit,
+# instead of failing after some kernels ran or, worse, only in its backward.
+LIMITS = {
+    "M": 8,                 # graph branches fused by stmgcn_fuse_out_*
+    "supports": 8,          # supports per GCN (the projections' segments)
+    "C": 4,                 # input_dim of the shared LSTM (both kernel families)
+    "L": 8,                 # LSTM layers (both kernel families)
+    "H": 128,               # lstm_hidden_dim, a multiple of 4 (exact-fp32 LSTM; the tensor cores take H = 64)
+    "T": 2048,              # seq_len: the context gate (stmgcn_gate_*)
+    "q": 8192,              # output width of a GCN projection (stmgcn_proj_*)
+    "C*G+C": 12288,         # the output layer's weights and bias in the fusion backward's 48 KB of shared memory
+}
+
+
+def check_limits(m: Optional[int] = None, ks: Optional[int] = None, c_in: Optional[int] = None,
+                 n_layers: Optional[int] = None, hid: Optional[int] = None, t_len: Optional[int] = None,
+                 gcn_hid: Optional[int] = None) -> None:
+    """Raise ``ValueError`` naming every limit of :data:`LIMITS` the given sizes exceed (None: not checked).  ``gcn_hid``
+    with ``c_in`` also checks the fusion's ``C*G + C``.  Launches nothing."""
+    faults = []
+    if m is not None and not 1 <= m <= LIMITS["M"]:
+        faults.append(f"M={m} graphs (at most {LIMITS['M']})")
+    if ks is not None and not 1 <= ks <= LIMITS["supports"]:
+        faults.append(f"{ks} supports per GCN (at most {LIMITS['supports']})")
+    if c_in is not None and not 1 <= c_in <= LIMITS["C"]:
+        faults.append(f"input_dim C={c_in} (at most {LIMITS['C']})")
+    if n_layers is not None and not 1 <= n_layers <= LIMITS["L"]:
+        faults.append(f"lstm_num_layers L={n_layers} (at most {LIMITS['L']})")
+    if hid is not None and not (hid > 0 and hid % 4 == 0 and hid <= LIMITS["H"]):
+        faults.append(f"lstm_hidden_dim H={hid} (a multiple of 4, at most {LIMITS['H']})")
+    if t_len is not None and not 1 <= t_len <= LIMITS["T"]:
+        faults.append(f"seq_len T={t_len} (at most {LIMITS['T']})")
+    if gcn_hid is not None and not 1 <= gcn_hid <= LIMITS["q"]:
+        faults.append(f"GCN hidden_dim {gcn_hid} (at most {LIMITS['q']})")
+    if gcn_hid is not None and c_in is not None and c_in * gcn_hid + c_in > LIMITS["C*G+C"]:
+        faults.append(f"output layer C*G + C = {c_in * gcn_hid + c_in} floats (at most {LIMITS['C*G+C']})")
+    if faults:
+        raise ValueError("stmgcn_b200: configuration beyond the kernels' limits: " + "; ".join(faults))
+
+
 def _p(t: Optional[torch.Tensor]):
     return None if t is None else t.data_ptr()
 
@@ -485,15 +526,11 @@ def _lstm16_forward(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes,
     return h_top.view(n, b, 64), h_n, c_n, tape
 
 
-_ZERO_TILES: dict = {}
-
-
 def _zero_tile(dev: torch.device) -> torch.Tensor:
-    """16 KB of zeros per device: the h_prev operand tile at t = 0 without an initial state."""
-    key = str(dev)
-    if key not in _ZERO_TILES:
-        _ZERO_TILES[key] = torch.zeros(128 * 64, device=dev, dtype=torch.bfloat16)
-    return _ZERO_TILES[key]
+    """16 KB of zeros, the h_prev operand tile at t = 0 without an initial state, made on the current stream for each
+    call.  (Not cached: a tile filled on one graph branch's stream would be read by the other branches' backward kernels
+    with nothing ordering the read after the fill.)"""
+    return torch.zeros(128 * 64, device=dev, dtype=torch.bfloat16)
 
 
 def _lstm16_backward(xo, s_gate, tape, n_layers, planes, d_top):
@@ -527,9 +564,10 @@ def _lstm16_backward_ex(xo, s_gate, tape, n_layers, planes, d_top, dh_n=None, dc
     else:
         dw_scratch = dbp = grads = None
         w_grads = [None] * len(shapes)
+    zero_tile = _zero_tile(xo.device)              # held until the launches below are enqueued
     args = (t_len, n_layers, rows, c_in, b, planes, xo.data_ptr(), s_gate.data_ptr(), wimg.data_ptr(), bias.data_ptr(),
             wih_t.data_ptr(), _p(h0p), _p(c0b), hp.data_ptr(), cs.data_ptr(), d_top.data_ptr(), dh_rec.data_ptr(),
-            dc.data_ptr(), _p(dx_work), _p(dw_scratch), _p(dbp), _zero_tile(xo.device).data_ptr(),
+            dc.data_ptr(), _p(dx_work), _p(dw_scratch), _p(dbp), zero_tile.data_ptr(),
             d_s.data_ptr(), _p(grads))
     if dh_n is None and dc_n is None and not any(want):
         _lib.check(L.stmgcn_lstm16_bwd(*args, _stream()), "lstm16_bwd")

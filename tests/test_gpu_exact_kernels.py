@@ -507,15 +507,15 @@ def test_fuse_out_matches_fp64(m, gdim, c_out, rows_id):
     assert control > FWD_TOL, f"the reference without fcb is within the bar ({control:.2e})"
 
 
-def test_fuse_out_backward_beyond_shared_memory_raises():
-    """The backward accumulates C*G + C floats in 48 KB of shared memory: C = 40, G = 400 (16 040 floats) raises."""
+def test_fuse_out_beyond_shared_memory_raises_in_the_forward():
+    """The backward accumulates C*G + C floats in 48 KB of shared memory, and the forward takes the same limit: C = 40,
+    G = 400 (16 040 floats) raises in the forward, so no step runs a forward its backward would refuse."""
     from stmgcn_b200 import ops
     gs = [torch.randn(3, 2, 400, device=DEV, requires_grad=True)]
     fcw = torch.randn(40, 400, device=DEV, requires_grad=True)
     fcb = torch.randn(40, device=DEV, requires_grad=True)
-    y = ops.FuseOut.apply(fcw, fcb, *gs)
-    with pytest.raises(RuntimeError, match="C\\*G=16000 too large"):
-        y.sum().backward()
+    with pytest.raises(RuntimeError, match="fuse_out_fwd: C\\*G=16000 too large"):
+        ops.FuseOut.apply(fcw, fcb, *gs)
 
 
 @pytest.mark.parametrize("c", [1, 3])

@@ -82,9 +82,11 @@ def test_spmm_step_with_bf16_gather_copy(n, f, transpose):
     assert torch.equal(y16, y.to(torch.bfloat16))
 
 
-@pytest.mark.parametrize("name", ["cfg1_ref", "ragged_ref", "cfg3_small_ref"])
+@pytest.mark.parametrize("name", ["cfg1_ref", "ragged_ref", "cfg3_small_ref", "localpool_tanh_ref", "cheb7_linear_ref"])
 def test_model_matches_reference_golden(name):
-    """Forward output, loss and EVERY parameter gradient vs vectors produced by the unmodified reference."""
+    """Forward output, loss and EVERY parameter gradient vs vectors produced by the unmodified reference.  The model is
+    built as the fixture's reference model was: ``localpool_tanh_ref`` without GCN bias, with ``nn.Tanh`` (applied by
+    torch, outside the kernels) and localpool supports; ``cheb7_linear_ref`` without bias or activation, 8 supports."""
     meta, params, grads, supports, _, blob = load_golden(name)
     model = build_model(meta, DEV)
     model.load_state_dict(params)

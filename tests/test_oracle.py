@@ -37,6 +37,95 @@ def test_sparse_oracle_matches_reference_golden(name, dtype):
         assert_close(g[key], grads[key], f"grad {key}", 2e-5)
 
 
+NEW_GOLDENS = ["localpool_tanh_ref", "cheb7_linear_ref"]
+
+
+@pytest.mark.parametrize("name", NEW_GOLDENS)
+def test_dense_oracle_matches_configured_reference_golden(name):
+    """The dense restatement with the fixture's configuration (no GCN bias; ``nn.Tanh`` or no activation; localpool or
+    Chebyshev K = 7) in fp64 reproduces the unmodified reference's fp32 forward, loss and every gradient."""
+    from helpers import oracle_activation
+    meta, params, grads, supports, adjs, blob = load_golden(name)
+    assert not meta["bias"] and not any(k.endswith(".b") for k in params)
+    x, y = torch.from_numpy(blob["x"]).double(), torch.from_numpy(blob["y"]).double()
+    out, loss, g = O.dense_loss_and_grads({k: v.double() for k, v in params.items()}, x, y,
+                                          [s.double() for s in supports], relu=oracle_activation(meta["activation"]))
+    assert_close(out.numpy(), blob["out"], "forward", 1e-5)
+    assert abs(float(loss) - float(blob["loss"])) < 1e-6
+    assert set(g) == set(grads)
+    for key in grads:
+        assert_close(g[key].numpy(), grads[key], f"grad {key}", 2e-5)
+    for a, s in zip(adjs, supports):            # support construction (GCN.py:57-97) restated
+        if meta["kernel_type"] == "localpool":
+            d = a.sum(1).pow(-0.5)
+            want = (torch.eye(a.shape[0]) + d[:, None] * a * d[None, :])[None]
+        else:
+            want = O.chebyshev_supports_dense(a, meta["k"])
+        assert_close(want.numpy(), s.numpy(), "supports", 1e-6)
+
+
+def _small_model(relu_case, seed=0):
+    from stmgcn_b200 import synth
+    n, m, k, t, b, c, hid, lyr, g = 14, 2, 2, 4, 3, 2, 8, 2, 6
+    adjs = [synth.make_adjacency(n, i, 0.3) for i in range(m)]
+    sups = [O.chebyshev_supports_dense(a.double(), k, lambda_max=1.8) for a in adjs]
+    params = {kk: v.double() for kk, v in O.init_params(m, t, c, hid, lyr, g, k + 1, seed=seed).items()}
+    gen = torch.Generator().manual_seed(seed)
+    x = torch.randn(b, t, n, c, generator=gen).double()
+    y = torch.randn(b, n, c, generator=gen).double()
+    return sups, params, x, y, k + 1
+
+
+@pytest.mark.parametrize("relu", [True, False])
+def test_dense_restatement_with_relu_or_none_is_the_sparse_oracle(relu):
+    """The activation argument at ReLU (True, or an ``nn.ReLU()`` module) and at none (False, or None) gives the model of
+    :class:`O.SparseOracle` at 1e-12 in fp64: forward, loss, every gradient and d obs."""
+    sups, params, x, y, ks = _small_model(relu)
+    orc = O.SparseOracle({k: v.numpy() for k, v in params.items()}, [O.laplacian_csr_from_supports(s) for s in sups],
+                         ks, relu=relu, dtype=np.float64)
+    o_ref, l_ref, g_ref = orc.loss_and_grads(x.numpy(), y.numpy())
+    for act in ([True, torch.nn.ReLU()] if relu else [False, None]):
+        out, loss, g = O.dense_loss_and_grads(params, x, y, sups, relu=act, want_obs=True)
+        assert_close(out.numpy(), o_ref, "forward", 1e-12)
+        assert abs(float(loss) - l_ref) <= 1e-12 * l_ref
+        for key in g_ref:
+            assert_close(g[key].numpy(), g_ref[key], f"grad {key}", 1e-12)
+        # d obs against autograd through the restatement itself (the sparse oracle has no d obs)
+        xd = x.clone().requires_grad_(True)
+        (d_obs,) = torch.autograd.grad(torch.mean((O.dense_st_mgcn(params, xd, sups, relu) - y) ** 2), [xd])
+        assert_close(g["obs"].numpy(), d_obs.numpy(), "d obs", 1e-12)
+
+
+def test_dense_restatement_forced_with_its_own_relu_masks_changes_nothing():
+    """Masks equal to the restatement's own ``z > 0``, handed back in the kernels' order and layout (temporal 0,
+    spatial 0, temporal 1, ...; node-major (N, B, q)), change no value and no gradient; other masks do."""
+    sups, params, x, y, _ = _small_model(True, seed=1)
+    masks, real = [], O.dense_gcn
+
+    def recording(supports, x_, w, b, relu=True, mask=None):
+        z = real(supports, x_, w, b, False)
+        masks.append((z > 0).permute(1, 0, 2))
+        return real(supports, x_, w, b, relu, mask)
+    O.dense_gcn = recording
+    try:
+        out0, loss0, g0 = O.dense_loss_and_grads(params, x, y, sups, want_obs=True)
+    finally:
+        O.dense_gcn = real
+    assert len(masks) == 4 and [tuple(mk.shape) for mk in masks[:2]] == [(14, 3, 4), (14, 3, 6)]
+    out1, loss1, g1 = O.dense_loss_and_grads(params, x, y, sups, masks=masks, want_obs=True)
+    assert torch.equal(out1, out0) and float(loss1) == float(loss0)
+    for key in g0:
+        assert torch.allclose(g1[key], g0[key], rtol=0, atol=1e-15), key
+    flipped = [mk.clone() for mk in masks]
+    flipped[1][0] = ~flipped[1][0]              # one region of graph 0's spatial GCN takes the other branch
+    out2, _, _ = O.dense_loss_and_grads(params, x, y, sups, masks=flipped)
+    assert O.max_rel_err(out2.numpy(), out0.numpy()) > 1e-3
+    with pytest.raises(ValueError, match="ReLU masks for 2 graphs"):
+        O.dense_st_mgcn(params, x, sups, masks=masks[:3])
+    with pytest.raises(ValueError, match="needs the ReLU activation"):
+        O.dense_st_mgcn(params, x, sups, relu=False, masks=masks)
+
+
 def test_lstm_explicit_equals_library_lstm():
     gen = torch.Generator().manual_seed(0)
     layers = []
