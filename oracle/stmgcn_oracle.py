@@ -67,6 +67,19 @@ def chebyshev_supports_dense(adj: torch.Tensor, order: int, lambda_max: float = 
     return torch.stack(polys, dim=0)
 
 
+def chain_stack_dense(mats: Sequence[torch.Tensor], order: int) -> torch.Tensor:
+    """Dense stack of Chebyshev recurrence chains sharing ``T_0 = I``: ``[I, T_1(X_0)..T_K(X_0), T_1(X_1)..]`` for the
+    chain matrices ``X_c`` of ``mats`` (in their dtype), ``K = order``: the stack a support set of chains stands for."""
+    eye = torch.eye(mats[0].shape[0], dtype=mats[0].dtype)
+    out = [eye]
+    for x in mats:
+        polys = [eye, x]
+        for _ in range(2, order + 1):
+            polys.append(2.0 * (x @ polys[-1]) - polys[-2])
+        out += polys[1:order + 1]
+    return torch.stack(out)
+
+
 # --------------------------------------------------------------------------------------------------
 # dense restatement (torch CPU; autograd supplies the backward)
 # --------------------------------------------------------------------------------------------------

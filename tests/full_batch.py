@@ -21,16 +21,8 @@ import torch
 from torch import nn
 
 import stmgcn_oracle as O
+from helpers import DEV, rel_err
 from per_step import per_step_rel_err, worst_step
-
-DEV = "cuda:0"
-
-
-def _err(a, b):
-    """max-norm relative error (``O.max_rel_err``), on the device."""
-    a, b = a.detach().double(), b.detach().double().to(a.device)
-    den = float(b.abs().max())
-    return float((a - b).abs().max()) / (den if den > 0 else 1.0)
 
 
 def _errors(got, ref, want_obs):
@@ -40,9 +32,9 @@ def _errors(got, ref, want_obs):
             "loss": abs(got["loss"] - ref["loss"]) / abs(ref["loss"])}
     for key, g in got["grads"].items():
         if key != "obs":
-            errs["grad " + key] = _err(g, ref["grads"][key])
+            errs["grad " + key] = rel_err(g, ref["grads"][key])
     if want_obs:
-        errs["d obs"] = _err(got["d_obs"], ref["grads"]["obs"])
+        errs["d obs"] = rel_err(got["d_obs"], ref["grads"]["obs"])
         errs["d obs (worst window)"] = float(np.max(per_step_rel_err(got["d_obs"], ref["grads"]["obs"], 0)))
         errs["d obs (worst step)"] = worst_step(got["d_obs"], ref["grads"]["obs"], 1)[0]
     return errs
@@ -118,8 +110,8 @@ def run(label, model, sups, params, chains, ks, x, y, *, relu, window_chunk, wan
     spread = None
     if repeat:
         first, second = steps
-        spread = {"grad " + k: _err(second["grads"][k], g) for k, g in first["grads"].items()}
-        spread["out"] = _err(second["out"], first["out"])
+        spread = {"grad " + k: rel_err(second["grads"][k], g) for k, g in first["grads"].items()}
+        spread["out"] = rel_err(second["out"], first["out"])
         if relu:
             flips = [int((a != b).sum()) for a, b in zip(first["masks"], second["masks"])]
             lines.append(f"  ReLU mask entries that differ between the two steps, per GCN (temporal 0, spatial 0, "

@@ -8,7 +8,28 @@ from torch import nn
 import stmgcn_oracle as O
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+DEV = "cuda:0"
 TOL = 1e-4          # BASELINE.json north_star: "within 1e-4 relative fp32" (max-norm form, SURVEY 8(d))
+FWD_TOL, GRAD_TOL = 2e-5, 5e-5      # the kernel-level bars: forward values, gradients (max-norm relative)
+
+
+def rel_err(a, b):
+    """``max|a - b| / max|b|`` in fp64, with 1 as the denominator when ``max|b| = 0``, as ``O.max_rel_err``.  ``a`` and
+    ``b`` are tensors (on any device) or numpy arrays; tensors are compared on ``a``'s device."""
+    a, b = (torch.as_tensor(v).detach().double() for v in (a, b))
+    b = b.to(a.device)
+    den = float(b.abs().max())
+    return float((a - b).abs().max()) / (den if den > 0 else 1.0)
+
+
+def lib():
+    """The library's ctypes handle (``_lib.lib``)."""
+    from stmgcn_b200 import _lib
+    return _lib.lib
+
+
+def sm_count():
+    return int(lib().stmgcn_sm_count())
 
 
 def load_golden(name):

@@ -23,14 +23,12 @@ mistakes the 2e-2 bar can miss.
 import pytest
 import scipy.sparse as sp
 import torch
-from torch import nn
 
 import stmgcn_oracle as O
-from helpers import TOL, build_model, load_golden
-from test_gpu_lstm16 import _step_local_error
+from helpers import DEV, TOL, build_model, load_golden, rel_err
+from model_cases import Recorder, cheb_workload, directed_workload, forced_errors, gpu_run
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 
 
 @pytest.fixture
@@ -42,126 +40,9 @@ def bf16_mode(monkeypatch):
     return ops
 
 
-def _err(a, b):
-    """max-norm relative error (``O.max_rel_err``) of two tensors, on the device."""
-    a, b = a.detach().double(), b.detach().double().to(a.device)
-    den = float(b.abs().max())
-    return float((a - b).abs().max()) / (den if den > 0 else 1.0)
-
-
 # ======================================================================================================================
 # recording the kernels' values
 # ======================================================================================================================
-class Recorder:
-    """Wraps ``ops`` for one forward and keeps, for the rows of the windows ``picks``, the kernels' values at the
-    rounding points: per shared LSTM its tape, per spatial GCN its Chebyshev stack, per GCN its ReLU mask (GCN order
-    temporal 0, spatial 0, temporal 1, ...)."""
-
-    def __init__(self, picks):
-        self.picks = list(picks)
-        self.lstm, self.stacks, self.masks = [], [], []
-
-    def __enter__(self):
-        from stmgcn_b200 import ops
-        self.ops = ops
-        self.real = (ops._lstm16_forward, ops.build_stack, ops._proj_fwd)
-        real_lstm, real_stack, real_proj = self.real
-
-        def lstm(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes, keep_tape):
-            res = real_lstm(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes, keep_tape)
-            tape = res[3]
-            assert tape is not None, "record the forward with autograd on"
-            n, b = xo.shape[:2]
-            rows = (torch.arange(n, device=xo.device)[:, None] * b
-                    + torch.tensor(self.picks, device=xo.device)[None, :]).reshape(-1)
-            lyr, t_len, rows_pad, _ = tape["cs"].shape
-            # cs is tile-blocked [tile][unit/4][128][4] (ops.to_blocked): gather the picked rows without unblocking
-            cs = tape["cs"].view(lyr, t_len, rows_pad // 128, 16, 128, 4)[:, :, rows // 128, :, rows % 128, :]
-            rec = dict(hp=tape["hp"].index_select(3, rows), c=cs.permute(1, 2, 0, 3, 4).reshape(lyr, t_len, -1, 64))
-            if tape["h0p"] is not None:
-                rec["h0p"] = tape["h0p"].index_select(2, rows)
-            self.lstm.append(rec)
-            return res
-
-        def stack(sset, x, gather16=False):
-            s = real_stack(sset, x, gather16)
-            if gather16:                                # the spatial GCN (ChebGCN); the temporal one passes False
-                self.stacks.append(s[:, :, self.picks].clone())
-            return s
-
-        def proj(*a, **k):
-            out = real_proj(*a, **k)
-            self.masks.append(out[:, self.picks] > 0)
-            return out
-
-        ops._lstm16_forward, ops.build_stack, ops._proj_fwd = lstm, stack, proj
-        return self
-
-    def __exit__(self, *exc):
-        self.ops._lstm16_forward, self.ops.build_stack, self.ops._proj_fwd = self.real
-
-    def tapes(self):
-        """Per graph the tape :class:`O.BF16ModeReference` takes (fp64): h (planes summed), c, h0 and s."""
-        out = []
-        for m, rec in enumerate(self.lstm):
-            assert rec["hp"].shape[2] == 1, "the LSTM ran with two planes: not the bf16 mode"
-            tape = dict(h=rec["hp"].double().sum(dim=2), c=rec["c"].double())
-            if "h0p" in rec:
-                tape["h0"] = rec["h0p"].double().sum(dim=1)
-            if m < len(self.stacks):
-                tape["s"] = self.stacks[m].double()
-            out.append(tape)
-        return out
-
-
-def gpu_run(model, sups, x, y, picks, want_obs=False):
-    """One forward (recorded) and backward of ``model`` on the full batch ``x``; the targets of the windows not picked
-    are the run's own output.  Returns the picked windows' output, the loss, every parameter gradient, d obs of the
-    picked windows (``want_obs``) and the recording."""
-    rec = Recorder(picks)
-    xd = x.to(DEV).requires_grad_(want_obs)
-    with rec:
-        out = model(obs_seq=xd, sta_adj_list=sups)
-    y2 = out.detach().clone()
-    y2[picks] = y[picks].to(DEV)
-    loss = nn.MSELoss()(out, y2)
-    loss.backward()
-    torch.cuda.synchronize()
-    return dict(out=out.detach()[picks], loss=loss.item(), rec=rec,
-                grads={k: p.grad.detach().clone() for k, p in model.named_parameters()},
-                d_obs=xd.grad[picks] if want_obs else None)
-
-
-def forced_errors(run, params, chains, ks, x, y, picks, relu, rounding=True, want_obs=False):
-    """The GPU run against :class:`O.BF16ModeReference` forced with its recording.  Returns (step-local errors: every
-    layer-step of each LSTM, its h_top and every spatial S_k; whole-model errors: output, loss, every parameter gradient
-    and d obs with ``want_obs``)."""
-    rec = run["rec"]
-    tapes = rec.tapes()
-    ref = O.BF16ModeReference(params, chains, ks, relu=relu, rounding=rounding,
-                              relu_masks=rec.masks if relu else None, device=DEV)
-    step = {}
-
-    def on_branch(m, br):
-        tape = tapes[m]
-        n = tape["s"].shape[1]
-        step[f"g{m} LSTM layer-steps"] = _step_local_error(tape, br["hs"], br["cs"], 1)
-        step[f"g{m} h_top"] = _err(tape["s"][0].reshape(n, -1), br["hs"][-1][-1].reshape(n, -1))
-        for k in range(1, ks):
-            step[f"g{m} S_{k}"] = _err(tape["s"][k].reshape(n, -1), br["stack"][k])
-    batch = x.shape[0]
-    out, loss, grads = ref.loss_and_grads(x[picks], y[picks], tapes=tapes, want_obs=want_obs, on_branch=on_branch)
-    scale = len(picks) / float(batch)
-    errs = {"out": _err(run["out"], out), "loss": abs(run["loss"] - float(loss) * scale) / abs(float(loss) * scale)}
-    for key, g in run["grads"].items():
-        errs["grad " + key] = _err(g, grads[key] * scale)
-    if want_obs:
-        errs["d obs"] = _err(run["d_obs"], grads["obs"] * scale)
-    del ref, grads
-    torch.cuda.empty_cache()
-    return step, errs
-
-
 def _summary(errs, n=6):
     return ", ".join(f"{k} {v:.2e}" for k, v in sorted(errs.items(), key=lambda kv: -kv[1])[:n])
 
@@ -180,9 +61,8 @@ def _golden_case(relu):
 
 def _workload_case(name, batch, picks, relu):
     from stmgcn_b200 import synth
-    from test_gpu_fullsize import _build
     w = synth.WORKLOADS[name]
-    model, sups, laps, params, x, y = _build(w, batch, relu=relu)
+    model, sups, laps, params, x, y = cheb_workload(w, batch, relu=relu)
     return model, sups, [[lap] for lap in laps], w.n_supports, params, x, y, picks
 
 
@@ -191,8 +71,7 @@ def _diffusion_case(batch, picks, relu, order=2):
     import GCN
     import STMGCN
     from stmgcn_b200 import synth
-    from test_gpu_diffusion import _directed_workload
-    w, adjs = _directed_workload("cfg2", batch)
+    w, adjs = directed_workload("cfg2", batch)
     sups_cpu = [GCN.Adj_Preprocessor("random_walk_diffusion", order).process_sparse(a) for a in adjs]
     chains = [[sp.csr_matrix(m.numpy()) for m in h.matrices_dense()] for h in sups_cpu]
     torch.manual_seed(0)
@@ -268,9 +147,9 @@ def test_cg_lstm_with_an_initial_state_matches_the_forced_reference(bf16_mode):
     loss = (r_out * w_out.double().to(DEV)).sum() + (r_hn * r1.double().to(DEV)).sum() + (r_cn * r2.double().to(DEV)).sum()
     names = [key for key, _ in model.named_parameters()]
     g = torch.autograd.grad(loss, r_leaves + [p["rnn_list.0." + key] for key in names])
-    errs = {"out": _err(out, r_out), "h_n": _err(h_n, r_hn), "c_n": _err(c_n, r_cn)}
-    errs.update({f"d {v}": _err(leaf.grad, gr) for v, leaf, gr in zip(("obs", "h0", "c0"), leaves, g[:3])})
-    errs.update({"grad " + key: _err(prm.grad, gr) for (key, prm), gr in zip(model.named_parameters(), g[3:])})
+    errs = {"out": rel_err(out, r_out), "h_n": rel_err(h_n, r_hn), "c_n": rel_err(c_n, r_cn)}
+    errs.update({f"d {v}": rel_err(leaf.grad, gr) for v, leaf, gr in zip(("obs", "h0", "c0"), leaves, g[:3])})
+    errs.update({"grad " + key: rel_err(prm.grad, gr) for (key, prm), gr in zip(model.named_parameters(), g[3:])})
     print(f"\nbf16 mode CG_LSTM with (h0, c0): worst {max(errs.values()):.2e} ({_summary(errs)})")
     bad = {key: v for key, v in errs.items() if not v <= TOL}
     assert not bad, f"above {TOL:.0e}: {bad}"

@@ -31,9 +31,8 @@ import torch
 from torch import nn
 
 import stmgcn_oracle as O
-from helpers import TOL
+from helpers import DEV, TOL, sm_count
 
-DEV = "cuda:0"
 
 FACTORS = {
     "M": ["1", "2", "3", "8"],
@@ -209,18 +208,6 @@ def region_batch(rows_kind, sms):
     return n, b
 
 
-def _dense_chains(mats, k):
-    """[I, T_1(X_c) .. T_K(X_c) for each chain matrix X_c] in fp64 (the stack a support set of chains stands for)."""
-    eye = torch.eye(mats[0].shape[0], dtype=torch.float64)
-    out = [eye]
-    for x in mats:
-        polys = [eye, x]
-        for _ in range(2, k + 1):
-            polys.append(2.0 * (x @ polys[-1]) - polys[-2])
-        out += polys[1:k + 1]
-    return torch.stack(out)
-
-
 def make_supports(case, n, m):
     """(supports the model takes, their dense fp64 stacks on the device) for each of the ``m`` graphs."""
     import GCN
@@ -241,7 +228,7 @@ def make_supports(case, n, m):
         if form == "handle":
             h = pre.process_sparse(adj).to(DEV)
             mats = [v.double().cpu() for v in h.matrices_dense()]
-            ref = mats[0][None] if kind == "localpool" else _dense_chains(mats if h.ks > 1 else [mats[0]], k)
+            ref = mats[0][None] if kind == "localpool" else O.chain_stack_dense(mats if h.ks > 1 else [mats[0]], k)
             model_sups.append(h)
         elif kind == "random_walk_diffusion":     # the 2K+1 bidirectional stack, dense (the generic path)
             ref = D.diffusion_supports_dense(adj.double(), k)
@@ -249,7 +236,7 @@ def make_supports(case, n, m):
         else:
             dense = pre.process(adj)
             model_sups.append(dense.to(DEV))
-            ref = dense.double() if kind == "localpool" else _dense_chains([dense[1].double()], k) if k else dense.double()
+            ref = dense.double() if kind == "localpool" else O.chain_stack_dense([dense[1].double()], k) if k else dense.double()
         ref_sups.append(ref.to(DEV))
     return model_sups, ref_sups
 
@@ -371,8 +358,7 @@ def test_config_sweep_case_matches_fp64(case, monkeypatch):
     """One training step of the row against the fp64 dense restatement at the kernels' own ReLU masks: every window's
     output, the loss, every parameter gradient and (where the row asks) d obs, at 1e-4; and the row ran the kernel
     families and streams it claims."""
-    from stmgcn_b200 import _lib
-    sms = int(_lib.lib.stmgcn_sm_count())
+    sms = sm_count()
     seed = int(case["id"][1:])
     want_obs = case["d_obs"] == "yes"
     torch.cuda.synchronize()

@@ -12,10 +12,10 @@ from torch import nn
 import diffusion_oracle as D
 import full_batch
 import stmgcn_oracle as O
-from helpers import TOL, assert_close
+from helpers import DEV, TOL, assert_close
+from model_cases import directed_workload
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 
 
 def _model(meta, relu=True):
@@ -108,24 +108,13 @@ def test_handle_equals_the_dense_stack_on_the_generic_path():
         assert_close(a.cpu().numpy(), b.cpu().numpy(), f"handle vs dense stack, tensor {i}", 1e-5)
 
 
-def _directed_workload(name, batch):
-    """The workload's shapes on directed graphs; in each, region 0 is made a sink and region 1 a source."""
-    from stmgcn_b200 import synth
-    w = synth.WORKLOADS[name]
-    adjs = [synth.make_directed_adjacency(w.n_regions, m, w.density) for m in range(w.n_graphs)]
-    for a in adjs:
-        a[0, :] = 0.0
-        a[:, 1] = 0.0
-    return w, adjs
-
-
 def _check_full_batch(name, batch, window_chunk, order=2, tol=TOL, relu=True, **kw):
     """test_gpu_fullsize.py's method on directed graphs with diffusion supports: one step on the full batch, every window
     with its true target, against the fp64 reference (two chains per graph) with the GPU forward's ReLU masks."""
     import GCN
     import STMGCN
     from stmgcn_b200 import ops, synth
-    w, adjs = _directed_workload(name, batch)
+    w, adjs = directed_workload(name, batch)
     pre = GCN.Adj_Preprocessor("random_walk_diffusion", order)
     sups_cpu = [pre.process_sparse(a) for a in adjs]
     chains = [[sp.csr_matrix(m.numpy()) for m in h.matrices_dense()] for h in sups_cpu]
@@ -167,7 +156,7 @@ def test_exact_and_tensor_core_paths_agree():
     import GCN
     import STMGCN
     from stmgcn_b200 import ops, synth
-    w, adjs = _directed_workload("cfg2", 16)
+    w, adjs = directed_workload("cfg2", 16)
     sups = [GCN.Adj_Preprocessor("random_walk_diffusion", 2).process_sparse(a).to(DEV) for a in adjs]
     kw = synth.model_kwargs(w)
     kw["sta_kernel_config"] = {"kernel_type": "random_walk_diffusion", "K": 2}

@@ -18,21 +18,12 @@ import torch
 from torch import nn
 
 import stmgcn_oracle as O
-from test_gpu_abi_contract import (GRAD_TOL, Buf, Call, _bits, _drive, _fuse_calls, _gate_calls, _lstm_calls,
-                                   _lstm16_calls, _proj_calls, _run, run_captured, run_contract)
-from test_gpu_input_grads import _lstm16_ex_calls, _lstm_ex_calls
+from abi_harness import (LSTM16_CASES, Buf, Call, bits, drive, fuse_calls, gate_calls, lstm16_calls, lstm16_ex_calls,
+                         lstm_calls, lstm_ex_calls, proj_calls, run_captured, run_contract, run_once)
+from helpers import DEV, GRAD_TOL, lib, rel_err
+from model_cases import cheb_workload
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-
-
-def _lib():
-    from stmgcn_b200 import _lib as lib
-    return lib.lib
-
-
-def _rel(a, b):
-    return O.max_rel_err(a.detach().double().cpu().numpy(), b.detach().double().cpu().numpy())
 
 
 # ======================================================================================================================
@@ -66,7 +57,7 @@ def _lstm_saved(call):
     return _LSTM_LAYERS                            # one reduce GEMM per layer
 
 
-_LSTM_LAYERS = 3                                   # _lstm_calls / _lstm_ex_calls: L = 3
+_LSTM_LAYERS = 3                                   # lstm_calls / lstm_ex_calls: L = 3
 
 
 def _frozen_variant(call, null, keep=()):
@@ -103,13 +94,13 @@ ENTRIES = {
 
 
 def _frozen_driver(which, keep_ws, runner=run_contract, proj_saved=None):
-    """A _drive runner: the calls before the backward ``which`` run clean; the backward runs in full (contract), then
+    """A drive runner: the calls before the backward ``which`` run clean; the backward runs in full (contract), then
     with its weight outputs NULL (and, with ``keep_ws``, its weight-only workspaces given but required untouched):
     the contract again, the per-row outputs bit-identical to the full call's, the launch count lower by exactly the
     skipped launches."""
     def run(call):
         if call.name != which:
-            return _run(call, "clean")
+            return run_once(call, "clean")
         if which == "proj_bwd":
             weights, ws_only, rows_prep, saved = ("dw",), (), None, lambda c: proj_saved
         else:
@@ -124,10 +115,10 @@ def _frozen_driver(which, keep_ws, runner=run_contract, proj_saved=None):
         for k, v in got.items():
             b = call.bufs[k]
             if b.role == "acc" or not b.exact:       # d_s, the bias gradient of the projection: sums of atomics
-                err = _rel(v, full[k])
+                err = rel_err(v, full[k])
                 assert err <= GRAD_TOL, f"{frozen.name}: {k} is {err:.2e} off the full call"
             else:
-                assert torch.equal(_bits(v), _bits(full[k])), f"{frozen.name}: {k} differs from the full call"
+                assert torch.equal(bits(v), bits(full[k])), f"{frozen.name}: {k} differs from the full call"
         return full
     return run
 
@@ -136,9 +127,8 @@ def _frozen_driver(which, keep_ws, runner=run_contract, proj_saved=None):
 @pytest.mark.parametrize("planes", [1, 2])
 @pytest.mark.parametrize("case", ["one_row", "l1_no_dx_work", "c3_l4_state", "waves_b37_state"])
 def test_tensor_core_lstm_backward_without_weight_gradients(case, planes, keep_ws):
-    from test_gpu_abi_contract import LSTM16_CASES
     spec = next(c for c in LSTM16_CASES if c[0] == case)
-    _drive(_lstm16_calls(spec, planes), _frozen_driver("lstm16_bwd", keep_ws))
+    drive(lstm16_calls(spec, planes), _frozen_driver("lstm16_bwd", keep_ws))
 
 
 @pytest.mark.parametrize("planes", [1, 2])
@@ -146,14 +136,14 @@ def test_tensor_core_lstm_backward_without_weight_gradients(case, planes, keep_w
                          ids=["one_row", "c3_l4_state", "l1_c4"])
 def test_tensor_core_extended_backward_without_weight_gradients(shape, planes):
     """dh0, dc0, d_xo and the seeded state: bit-identical to the full call's."""
-    _drive(_lstm16_ex_calls(*shape, planes), _frozen_driver("lstm16_bwd_ex", False))
+    drive(lstm16_ex_calls(*shape, planes), _frozen_driver("lstm16_bwd_ex", False))
 
 
 @pytest.mark.parametrize("state", [False, True])
 def test_exact_lstm_backward_without_weight_gradients(state):
     n, b_sz = (7, 5) if state else (61, 5)
-    _drive(_lstm_calls(n, b_sz, state), _frozen_driver("lstm_bwd", False))
-    _drive(_lstm_ex_calls(7, 5, state), _frozen_driver("lstm_bwd_ex", False))
+    drive(lstm_calls(n, b_sz, state), _frozen_driver("lstm_bwd", False))
+    drive(lstm_ex_calls(7, 5, state), _frozen_driver("lstm_bwd_ex", False))
 
 
 # (name, ks, p, q, regions N, batch B, gap, weight images, broadcast dOut, ReLU, bias)
@@ -172,27 +162,27 @@ def test_projection_backward_without_weight_gradient(case):
     _, ks, p, q, n, b_sz, gap, tc, bcast, relu, bias = case
     on_tc = tc and not bcast and gap % 4 == 0
     saved = (ks + 1) // 2 if on_tc else 1
-    _drive(_proj_calls(ks, p, q, n, b_sz, gap, tc, bcast, relu, bias, seed=300 + PROJ.index(case)),
+    drive(proj_calls(ks, p, q, n, b_sz, gap, tc, bcast, relu, bias, seed=300 + PROJ.index(case)),
            _frozen_driver("proj_bwd", False, proj_saved=saved))
 
 
 @pytest.mark.parametrize("t", [12, 300])
 def test_context_gate_backward_without_fc_gradients(t):
-    _drive(_gate_calls(t, 5), _frozen_driver("gate_bwd", False))
+    drive(gate_calls(t, 5), _frozen_driver("gate_bwd", False))
 
 
 @pytest.mark.parametrize("c", [1, 40])
 def test_fuse_out_backward_without_fc_gradients(c):
-    _drive(_fuse_calls(3, c), _frozen_driver("fuse_out_bwd", False))
+    drive(fuse_calls(3, c), _frozen_driver("fuse_out_bwd", False))
 
 
 CAPTURED = {
-    "tensor_core_lstm": (lambda: _lstm16_calls(("c3_l4_state", 5, 60, 5, 4, 3, True), 2), "lstm16_bwd", None),
-    "tensor_core_lstm_ex": (lambda: _lstm16_ex_calls(5, 60, 5, 4, 3, True, 1), "lstm16_bwd_ex", None),
-    "exact_lstm_ex": (lambda: _lstm_ex_calls(7, 5, True), "lstm_bwd_ex", None),
-    "projection_tensor_cores": (lambda: _proj_calls(5, 64, 64, 40, 37, 0, True, False, True, True, seed=1), "proj_bwd", 3),
-    "context_gate": (lambda: _gate_calls(12, 5), "gate_bwd", None),
-    "fuse_out": (lambda: _fuse_calls(3, 40), "fuse_out_bwd", None),
+    "tensor_core_lstm": (lambda: lstm16_calls(("c3_l4_state", 5, 60, 5, 4, 3, True), 2), "lstm16_bwd", None),
+    "tensor_core_lstm_ex": (lambda: lstm16_ex_calls(5, 60, 5, 4, 3, True, 1), "lstm16_bwd_ex", None),
+    "exact_lstm_ex": (lambda: lstm_ex_calls(7, 5, True), "lstm_bwd_ex", None),
+    "projection_tensor_cores": (lambda: proj_calls(5, 64, 64, 40, 37, 0, True, False, True, True, seed=1), "proj_bwd", 3),
+    "context_gate": (lambda: gate_calls(12, 5), "gate_bwd", None),
+    "fuse_out": (lambda: fuse_calls(3, 40), "fuse_out_bwd", None),
 }
 
 
@@ -201,7 +191,7 @@ def test_backward_without_weight_gradients_replays_from_a_cuda_graph(family):
     """The NULL-weight call eagerly on a side stream, then captured and replayed (test_gpu_abi_contract.run_captured);
     both equal the full call's per-row outputs."""
     calls, which, saved = CAPTURED[family]
-    _drive(calls(), _frozen_driver(which, False, runner=run_captured, proj_saved=saved))
+    drive(calls(), _frozen_driver(which, False, runner=run_captured, proj_saved=saved))
 
 
 # (what, call(lib, a, b, c, d, e, f)): one NULL weight output where its partner is given, or nothing to compute
@@ -236,14 +226,14 @@ def test_mixed_null_weight_outputs_are_rejected_without_a_launch(case):
     gen = torch.Generator().manual_seed(0)
     bufs = [Buf("in", torch.randn(1 << 16, generator=gen)) for _ in range(6)]
     torch.cuda.synchronize()
-    n0 = _lib().stmgcn_launch_count()
-    rc = call(_lib(), *(x.p for x in bufs))
+    n0 = lib().stmgcn_launch_count()
+    rc = call(lib(), *(x.p for x in bufs))
     torch.cuda.synchronize()
     assert rc < 0, f"{what}: rc={rc}"
-    assert _lib().stmgcn_last_error(), f"{what}: no message"
-    assert _lib().stmgcn_launch_count() == n0, f"{what}: a kernel was launched"
+    assert lib().stmgcn_last_error(), f"{what}: no message"
+    assert lib().stmgcn_launch_count() == n0, f"{what}: a kernel was launched"
     for i, x in enumerate(bufs):
-        assert x.guards_intact() and torch.equal(_bits(x.t), _bits(x.init)), f"{what}: buffer {i} changed"
+        assert x.guards_intact() and torch.equal(bits(x.t), bits(x.init)), f"{what}: buffer {i} changed"
 
 
 # ======================================================================================================================
@@ -325,8 +315,8 @@ def _check_pattern(model, frozen, leaves, run, what):
     assert set(got) == set(base[0]) - set(frozen), what
     errs = {}
     for k, g in got.items():
-        spread = _rel(base[1][k], base[0][k])
-        err = _rel(g, base[0][k])
+        spread = rel_err(base[1][k], base[0][k])
+        err = rel_err(g, base[0][k])
         # within the atomics' run-to-run spread (x4: two runs are a small sample of it), and never further than fp32
         # summation-order noise (1e-5, a fifth of the 5e-5 gradient bar) where the two runs happen to agree bit for bit
         bound = max(4 * spread, 1e-5)
@@ -382,8 +372,7 @@ def test_freeze_pattern_at_cfg3_size(pattern):
     (with it, cfg3's obs gradient is vanishing and a flipped ReLU mask moves it by up to 6e-2 between two all-trainable
     runs, measured on an H100)."""
     from stmgcn_b200 import synth
-    from test_gpu_fullsize import _build
-    model, sups, _, _, x, y = _build(synth.WORKLOADS["cfg3"], 16, relu=False)
+    model, sups, _, _, x, y = cheb_workload(synth.WORKLOADS["cfg3"], 16, relu=False)
     xd, yd = x.to(DEV), y.to(DEV)
     pred, obs_grad = PATTERNS[pattern]
     frozen = {name for name, p in model.named_parameters() if pred(model, p)}
@@ -417,10 +406,10 @@ def test_launch_count_drops_by_the_skipped_launches(mode, monkeypatch):
             p.grad = None
         loss = nn.MSELoss()(model(obs_seq=x, sta_adj_list=sups), y)
         torch.cuda.synchronize()
-        n0 = _lib().stmgcn_launch_count()
+        n0 = lib().stmgcn_launch_count()
         loss.backward()
         torch.cuda.synchronize()
-        return _lib().stmgcn_launch_count() - n0
+        return lib().stmgcn_launch_count() - n0
 
     full = backward_launches(None)
     assert full - backward_launches("lstm_frozen") == M * LAYERS
@@ -459,4 +448,4 @@ def test_fine_tuning_with_the_lstms_frozen():
     assert losses[-1] < 0.8 * losses[0], losses
     for n, p in model.named_parameters():
         if n in lstm:
-            assert p.grad is None and torch.equal(_bits(p.detach()), _bits(lstm[n])), f"{n} changed"
+            assert p.grad is None and torch.equal(bits(p.detach()), bits(lstm[n])), f"{n} changed"

@@ -10,49 +10,22 @@ Tolerance: 1e-4 max-norm relative (BASELINE.json north_star), fp32 arithmetic; 2
 against the unrounded reference.
 """
 import pytest
-import scipy.sparse as sp
 import torch
 from torch import nn
 
 import full_batch
 import stmgcn_oracle as O
-from helpers import TOL, assert_close
+from helpers import DEV, TOL, assert_close
+from model_cases import CHUNK, cheb_workload
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-
-# windows per chunk of the fp64 reference: its autograd tape is ~1 GB per cfg3 window and graph branch, ~8 GB per cfg5
-# window (16 384 regions, T = 24)
-CHUNK = {"cfg2": 32, "cfg3": 16, "cfg5": 2}
-
-
-def _csr_of(sup):
-    """scipy CSR of L~ from a ChebSupports handle (CPU copy)."""
-    rp, ci, va = sup.rowptr.cpu().numpy(), sup.colidx.cpu().numpy(), sup.vals.cpu().numpy()
-    return sp.csr_matrix((va, ci, rp), shape=(sup.n, sup.n))
-
-
-def _build(w, batch, seed_x=100, relu=True):
-    import GCN
-    import STMGCN
-    from stmgcn_b200 import synth
-    pre = GCN.Adj_Preprocessor("chebyshev", w.cheb_order)
-    sups_cpu = [pre.process_sparse(a) for a in synth.make_adjacency_list(w)]
-    torch.manual_seed(0)
-    kw = synth.model_kwargs(w)
-    if not relu:
-        kw["gconv_activation"] = None
-    model = STMGCN.ST_MGCN(**kw)
-    params = {k: v.detach().clone().numpy() for k, v in model.state_dict().items()}
-    x, y = synth.make_inputs(w, seed=seed_x, batch=batch)
-    return model.to(DEV), [s.to(DEV) for s in sups_cpu], [_csr_of(s) for s in sups_cpu], params, x, y
 
 
 def _run_full_batch(name, batch, relu=True, **kw):
     """``full_batch.run`` on workload ``name`` (Chebyshev supports); returns the errors."""
     from stmgcn_b200 import ops, synth
     w = synth.WORKLOADS[name]
-    model, sups, laps, params, x, y = _build(w, batch, relu=relu)
+    model, sups, laps, params, x, y = cheb_workload(w, batch, relu=relu)
     label = f"{name} path={ops.lstm_path()} planes={ops.lstm_planes()}"
     return full_batch.run(label, model, sups, params, [[lap] for lap in laps], w.n_supports, x, y, relu=relu,
                           window_chunk=CHUNK[name], **kw)

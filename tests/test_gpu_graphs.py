@@ -6,10 +6,9 @@ import torch
 from torch import nn
 
 import stmgcn_oracle as O
-from helpers import assert_close, build_model
+from helpers import DEV, assert_close, build_model
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 
 
 def _eager(model, crit, x, y, sups):

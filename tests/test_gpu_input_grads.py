@@ -6,89 +6,24 @@ their arithmetic forced with the kernel's own tape, as in test_gpu_lstm16.py / t
 contract of test_gpu_abi_contract.py for every new entry point.  Module level: the drop-in modules against the
 reference's own gradients (tests/golden/inputgrad_ref.npz) and the dense fp64 oracle, and d obs at cfg3 size.
 """
-import math
-
 import numpy as np
 import pytest
 import torch
 from torch import nn
 
 import stmgcn_oracle as O
-from helpers import GOLDEN, TOL
-from test_gpu_abi_contract import Buf, Call, _blocked_pads, _drive, run_captured, run_contract
-from test_gpu_exact_kernels import lstm_inputs
-from test_gpu_lstm16 import CASES, _inputs, _wave_regions
+from abi_harness import Buf, bits, drive, lstm16_ex_calls, lstm_ex_calls, obs_grad_calls, run_captured, run_contract
+from helpers import DEV, GOLDEN, GRAD_TOL, TOL, lib, rel_err
+from lstm_cases import (CASES, EXACT_CASES, HID, exact_run, grad_errors, lstm16_inputs, lstm16_run, lstm_inputs, seeds,
+                        state_gradients, wave_regions)
+from model_cases import CHUNK, cheb_workload, dense_grads, forced_errors, gpu_run, small_model
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-HID = 64
-GRAD_TOL = 5e-5
-
-
-def _err(a, b):
-    return O.max_rel_err(a.detach().double().cpu().numpy(), b.detach().double().cpu().numpy())
-
-
-def _lib():
-    from stmgcn_b200 import _lib as lib
-    return lib.lib
-
-
-# ======================================================================================================================
-# fp64 reference with the extra leaves
-# ======================================================================================================================
-def _state_reference(xo, s, h0, c0, ws, lyr, planes, tape, d_top, dh_n, dc_n):
-    """``O.lstm_planes_reference`` in fp64, forced with ``tape``; leaves xo, s, h0, c0 (zeros when None: the gradient at
-    a zero initial state) and the weights.  Returns the gradients of <h_top, d_top> + <h_n, dh_n> + <c_n, dc_n>
-    (dh_n / dc_n may be None) as a dict."""
-    n, b, t, c = xo.shape
-    rows, hid = n * b, ws[1].shape[1]
-    xo64 = xo.double().requires_grad_(True)
-    s64 = s.double().requires_grad_(True)
-    h0d = (h0.double() if h0 is not None else xo64.new_zeros(lyr, rows, hid)).requires_grad_(True)
-    c0d = (c0.double() if c0 is not None else xo64.new_zeros(lyr, rows, hid)).requires_grad_(True)
-    tape = dict(tape)
-    if "h0" not in tape:
-        tape["h0"] = h0d.detach()
-    layers = [tuple(w.double().requires_grad_(True) for w in ws[4 * l:4 * l + 4]) for l in range(lyr)]
-    x = xo64.reshape(rows, t, c) * s64.repeat(n, 1)[:, :, None]
-    _, _, (hs, cs) = O.lstm_planes_reference(x, layers, planes, h0d, c0d, tape)
-    loss = (hs[-1][-1] * d_top.double()).sum()
-    if dh_n is not None:
-        loss = loss + sum((hs[l][-1] * dh_n[l].double()).sum() for l in range(lyr))
-    if dc_n is not None:
-        loss = loss + sum((cs[l][-1] * dc_n[l].double()).sum() for l in range(lyr))
-    flat = [w for layer in layers for w in layer]
-    g = torch.autograd.grad(loss, [xo64, s64, h0d, c0d] + flat)
-    return dict(d_xo=g[0], d_s=g[1], dh0=g[2], dc0=g[3], params=list(g[4:]))
-
-
-def _errors(got, ref):
-    errs = {k: _err(got[k], ref[k]) for k in ("d_xo", "d_s", "dh0", "dc0")}
-    errs.update({f"param {i}": _err(a, r) for i, (a, r) in enumerate(zip(got["params"], ref["params"]))})
-    return errs
-
-
-def _seeds(lyr, rows, hid, seed):
-    gen = torch.Generator().manual_seed(seed)
-    return (torch.randn(lyr, rows, hid, generator=gen).to(DEV), torch.randn(lyr, rows, hid, generator=gen).to(DEV))
 
 
 # ======================================================================================================================
 # tensor-core kernels
 # ======================================================================================================================
-def _lstm16_run(xo, s, h0, c0, ws, lyr, planes, d_top, dh_n, dc_n):
-    from stmgcn_b200 import ops
-    rows = xo.shape[0] * xo.shape[1]
-    _, _, _, tape = ops._lstm16_forward(xo, s, h0, c0, lyr, h0 is not None, ws, planes, True)
-    d_s, grads, (d_xo, dh0, dc0) = ops._lstm16_backward_ex(xo, s, tape, lyr, planes, d_top, dh_n, dc_n, (True, True, True))
-    torch.cuda.synchronize()
-    ktape = dict(h=tape["hp"].double().sum(dim=2), c=ops.from_blocked(tape["cs"], rows).double())
-    if h0 is not None:
-        ktape["h0"] = tape["h0p"].double().sum(dim=1)
-    return dict(d_xo=d_xo, d_s=d_s, dh0=dh0, dc0=dc0, params=grads), ktape, tape
-
-
 @pytest.mark.parametrize("planes", [1, 2])
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 def test_tensor_core_input_and_state_gradients(case, planes):
@@ -103,15 +38,15 @@ def test_tensor_core_input_and_state_gradients(case, planes):
     with one plane, whose reference rounds like the kernel, the same case holds 5e-5."""
     name, n, b, t, lyr, c, state = case
     if n is None:
-        n = _wave_regions(b)
-    xo, s, h0, c0, ws, d_top = _inputs(n, b, t, lyr, c, state, seed=10 * CASES.index(case) + planes + 500,
+        n = wave_regions(b)
+    xo, s, h0, c0, ws, d_top = lstm16_inputs(n, b, t, lyr, c, state, seed=10 * CASES.index(case) + planes + 500,
                                        saturate=name == "saturated")
-    dh_n, dc_n = _seeds(lyr, n * b, HID, seed=CASES.index(case))
-    got, ktape, _ = _lstm16_run(xo, s, h0, c0, ws, lyr, planes, d_top, dh_n, dc_n)
-    ref = _state_reference(xo, s, h0, c0, ws, lyr, planes, ktape, d_top, dh_n, dc_n)
-    errs = _errors(got, ref)
-    unseeded, _, _ = _lstm16_run(xo, s, h0, c0, ws, lyr, planes, d_top, None, None)
-    control = max(_errors(unseeded, ref).values())
+    dh_n, dc_n = seeds(lyr, n * b, HID, seed=CASES.index(case))
+    got, ktape, _ = lstm16_run(xo, s, h0, c0, ws, lyr, planes, d_top, dh_n, dc_n)
+    ref = state_gradients(xo, s, h0, c0, ws, lyr, planes, ktape, d_top, dh_n, dc_n)
+    errs = grad_errors(got, ref)
+    unseeded, _, _ = lstm16_run(xo, s, h0, c0, ws, lyr, planes, d_top, None, None)
+    control = max(grad_errors(unseeded, ref).values())
     print(f"lstm16 extras {name} P={planes}: worst {max(errs.values()):.2e} ({max(errs, key=errs.get)}), "
           f"d_xo {errs['d_xo']:.2e} dh0 {errs['dh0']:.2e} dc0 {errs['dc0']:.2e}; control (no seeds) {control:.2e}")
     w_bar = 2e-4 if (name == "saturated" and planes == 2) else GRAD_TOL
@@ -123,35 +58,17 @@ def test_tensor_core_input_and_state_gradients(case, planes):
 # ======================================================================================================================
 # exact-fp32 kernels
 # ======================================================================================================================
-# (name, H, L, T, C, regions N, batch B, initial state)
-EXACT_CASES = [("h16_c1", 16, 2, 5, 1, 7, 5, False),
-               ("h48_c3_state", 48, 3, 6, 3, 9, 4, True),
-               ("h128_l8_c4_state", 128, 8, 3, 4, 3, 11, True),
-               ("h48_t1_c2", 48, 1, 1, 2, 5, 3, False)]
-
-
-def _exact_run(xo, s, h0, c0, ws, lyr, hid, d_top, dh_n, dc_n):
-    from stmgcn_b200 import ops
-    _, _, _, tape = ops._exact_forward(xo, s, h0, c0, lyr, hid, True, ws, True)
-    ktape = dict(h=tape[2].double(), c=tape[3].double())
-    if h0 is not None:
-        ktape["h0"] = h0.double()
-    d_s, grads, (d_xo, dh0, dc0) = ops._exact_backward_ex(xo, s, tape, lyr, hid, d_top, dh_n, dc_n, (True, True, True))
-    torch.cuda.synchronize()
-    return dict(d_xo=d_xo, d_s=d_s, dh0=dh0, dc0=dc0, params=grads), ktape
-
-
 @pytest.mark.parametrize("case", EXACT_CASES, ids=[c[0] for c in EXACT_CASES])
 def test_exact_input_and_state_gradients(case):
     name, hid, lyr, t, c, n, b, state = case
     xo, s, h0, c0, ws, d_top = (None if v is None else v.to(DEV) if torch.is_tensor(v) else [w.to(DEV) for w in v]
                                 for v in lstm_inputs(n, b, t, lyr, c, hid, state, seed=700 + EXACT_CASES.index(case)))
-    dh_n, dc_n = _seeds(lyr, n * b, hid, seed=40 + EXACT_CASES.index(case))
-    got, ktape = _exact_run(xo, s, h0, c0, ws, lyr, hid, d_top, dh_n, dc_n)
-    ref = _state_reference(xo, s, h0, c0, ws, lyr, 2, ktape, d_top, dh_n, dc_n)
-    errs = _errors(got, ref)
-    unseeded, _ = _exact_run(xo, s, h0, c0, ws, lyr, hid, d_top, None, None)
-    control = max(_errors(unseeded, ref).values())
+    dh_n, dc_n = seeds(lyr, n * b, hid, seed=40 + EXACT_CASES.index(case))
+    got, ktape = exact_run(xo, s, h0, c0, ws, lyr, hid, d_top, dh_n, dc_n)
+    ref = state_gradients(xo, s, h0, c0, ws, lyr, 2, ktape, d_top, dh_n, dc_n)
+    errs = grad_errors(got, ref)
+    unseeded, _ = exact_run(xo, s, h0, c0, ws, lyr, hid, d_top, None, None)
+    control = max(grad_errors(unseeded, ref).values())
     print(f"lstm extras {name}: worst {max(errs.values()):.2e} ({max(errs, key=errs.get)}); control {control:.2e}")
     assert max(errs.values()) <= GRAD_TOL, errs
     assert control > GRAD_TOL, control
@@ -161,11 +78,11 @@ def test_exact_input_and_state_gradients(case):
 def test_tensor_core_and_exact_extras_agree(state):
     """H = 64, two planes: the two kernel families give the same d_xo, dh0, dc0 and weight gradients."""
     n, b, t, lyr, c = 6, 30, 7, 3, 2
-    xo, s, h0, c0, ws, d_top = _inputs(n, b, t, lyr, c, state, seed=77)
-    dh_n, dc_n = _seeds(lyr, n * b, HID, seed=78)
-    tc, _, _ = _lstm16_run(xo, s, h0, c0, ws, lyr, 2, d_top, dh_n, dc_n)
-    ex, _ = _exact_run(xo, s, h0, c0, ws, lyr, HID, d_top, dh_n, dc_n)
-    errs = _errors(tc, ex)
+    xo, s, h0, c0, ws, d_top = lstm16_inputs(n, b, t, lyr, c, state, seed=77)
+    dh_n, dc_n = seeds(lyr, n * b, HID, seed=78)
+    tc, _, _ = lstm16_run(xo, s, h0, c0, ws, lyr, 2, d_top, dh_n, dc_n)
+    ex, _ = exact_run(xo, s, h0, c0, ws, lyr, HID, d_top, dh_n, dc_n)
+    errs = grad_errors(tc, ex)
     print(f"tensor cores vs exact (state={state}): worst {max(errs.values()):.2e}")
     assert max(errs.values()) <= GRAD_TOL, errs
 
@@ -191,10 +108,10 @@ class _ViaEx:
 
 def _backward_outputs(run):
     torch.cuda.synchronize()
-    n0 = _lib().stmgcn_launch_count()
+    n0 = lib().stmgcn_launch_count()
     d_s, grads = run()
     torch.cuda.synchronize()
-    return [d_s] + list(grads), _lib().stmgcn_launch_count() - n0
+    return [d_s] + list(grads), lib().stmgcn_launch_count() - n0
 
 
 # How the backward kernels write each output decides what two runs can be asked to agree on:
@@ -212,8 +129,8 @@ def _path_runs(path, seeded):
     ``seeded``)."""
     from stmgcn_b200 import ops
     n, b, t, lyr, c = 5, 60, 7, 3, 2
-    xo, s, h0, c0, ws, d_top = _inputs(n, b, t, lyr, c, True, seed=9)
-    dh_n, dc_n = _seeds(lyr, n * b, HID, seed=10) if seeded else (None, None)
+    xo, s, h0, c0, ws, d_top = lstm16_inputs(n, b, t, lyr, c, True, seed=9)
+    dh_n, dc_n = seeds(lyr, n * b, HID, seed=10) if seeded else (None, None)
     if path == "tc":
         _, _, _, tape = ops._lstm16_forward(xo, s, h0, c0, lyr, True, ws, 2, True)
         old = lambda: ops._lstm16_backward(xo, s, tape, lyr, 2, d_top)      # noqa: E731
@@ -239,7 +156,7 @@ def test_extended_entry_points_with_null_extras_equal_the_old_ones(path, monkeyp
     new, n_new = _backward_outputs(run)
     assert n_new == n_old
     for i, (a, o) in enumerate(zip(new, old)):
-        assert _err(a, o) <= GRAD_TOL, f"{path} output {i}: {_err(a, o):.2e}"
+        assert rel_err(a, o) <= GRAD_TOL, f"{path} output {i}: {rel_err(a, o):.2e}"
 
 
 @pytest.mark.parametrize("path", ["tc", "exact"])
@@ -253,160 +170,55 @@ def test_extended_entry_points_store_the_input_and_state_gradients_reproducibly(
         torch.cuda.synchronize()
         runs.append(dict(zip(("d_xo", "dh0", "dc0"), (v.clone() for v in extras))))
     for k in _PLAIN_STORES:
-        assert torch.equal(runs[0][k], runs[1][k]), f"{path} {k}: two runs differ ({_err(runs[0][k], runs[1][k]):.1e})"
+        assert torch.equal(runs[0][k], runs[1][k]), f"{path} {k}: two runs differ ({rel_err(runs[0][k], runs[1][k]):.1e})"
 
 
 # ======================================================================================================================
 # memory contract of the new entry points (harness of test_gpu_abi_contract.py)
 # ======================================================================================================================
-def _obs_grad_calls(c, which):
-    b_sz, t, n = 5, 7, 33
-    gen = torch.Generator().manual_seed(c)
-    d_xo, d_xt = torch.randn(n, b_sz, t, c, generator=gen), torch.randn(n, b_sz, t, generator=gen)
-    bufs = dict(d_obs=Buf("out", shape=(b_sz, t, n, c)))
-    if "xo" in which:
-        bufs["d_xo"] = Buf("in", d_xo)
-    if "xt" in which:
-        bufs["d_xt"] = Buf("in", d_xt)
-    opt = lambda k: bufs[k].p if k in bufs else None      # noqa: E731
-
-    def ref(res):
-        want = torch.zeros(b_sz, t, n, c, dtype=torch.float64)
-        if "xo" in which:
-            want += d_xo.double().permute(1, 2, 0, 3)
-        if "xt" in which:
-            want += d_xt.double().permute(1, 2, 0)[..., None]
-        assert torch.equal(res["d_obs"].double().cpu(), want.float().double())
-
-    yield Call("obs_grad", bufs, lambda st: _lib().stmgcn_obs_grad(opt("d_xo"), opt("d_xt"), bufs["d_obs"].p, b_sz, t, n,
-                                                                    c, st), ref, 1)
-
-
 @pytest.mark.parametrize("c,which", [(1, ("xt",)), (3, ("xo", "xt")), (2, ("xo",))])
 def test_obs_grad_keeps_the_memory_contract(c, which):
-    _drive(_obs_grad_calls(c, which), run_contract)
-
-
-def _lstm16_ex_calls(n, b_sz, t, lyr, c, state, planes):
-    """Forward through ops (not under test), then stmgcn_lstm16_bwd_ex with every extra: seeds with poisoned padding
-    rows, dh0 / dc0 with unspecified padding rows, d_xo."""
-    from stmgcn_b200 import ops
-    rows = n * b_sz
-    rp = -(-rows // 128) * 128
-    xo, s, h0, c0, ws, d_top = _inputs(n, b_sz, t, lyr, c, state, seed=n + planes)
-    dh_n, dc_n = _seeds(lyr, rows, HID, seed=n)
-    _, _, _, tape = ops._lstm16_forward(xo, s, h0, c0, lyr, state, ws, planes, True)
-    ktape = dict(h=tape["hp"].double().sum(dim=2), c=ops.from_blocked(tape["cs"], rows).double())
-    if state:
-        ktape["h0"] = tape["h0p"].double().sum(dim=1)
-    pads = lambda v: _blocked_pads(v, rows)      # noqa: E731
-    blocked = lambda v: ops.from_blocked(v, rows)      # noqa: E731
-    shapes = [sh for l in range(lyr) for sh in ((256, c if l == 0 else 64), (256, 64), (256,), (256,))]
-    grid = int(_lib().stmgcn_lstm16_grid(rows))
-    d = dict(xo=Buf("in", xo), s=Buf("in", s), wimg=Buf("in", tape["wimg"].view(torch.bfloat16)), bias=Buf("in", tape["bias"]),
-             wih_t=Buf("in", tape["wih_t"]), hp=Buf("in", tape["hp"]), cs=Buf("in", tape["cs"]),
-             d_top=Buf("in", ops.to_blocked(d_top), pad=pads), dh_rec=Buf("ws", shape=(rp, 64)),
-             dc=Buf("ws", shape=(rp, 64)), dw_scratch=Buf("ws", shape=(grid, 128 * 256)), dbp=Buf("ws", shape=(lyr, 256)),
-             zero_tile=Buf("in", torch.zeros(128 * 64, dtype=torch.bfloat16)), d_s=Buf("acc", shape=(b_sz, t)),
-             grads=Buf("out", shape=(sum(math.prod(sh) for sh in shapes),), exact=False),
-             dh_n=Buf("in", ops.to_blocked(dh_n), pad=pads), dc_n=Buf("in", ops.to_blocked(dc_n), pad=pads),
-             dh0=Buf("out", shape=(lyr, rp, 64), part=blocked), dc0=Buf("out", shape=(lyr, rp, 64), part=blocked),
-             d_xo=Buf("out", shape=xo.shape))
-    if state:
-        d.update(h0p=Buf("in", tape["h0p"]), c0=Buf("in", tape["c0b"], pad=pads))
-    if lyr > 1:
-        d["dx_work"] = Buf("ws", shape=(min(2, lyr - 1), t, rp, 64))
-    opt = lambda k: d[k].p if k in d else None      # noqa: E731
-
-    def ref(res):
-        r = _state_reference(xo, s, h0, c0, ws, lyr, planes, ktape, d_top, dh_n, dc_n)
-        got = dict(d_xo=res["d_xo"], d_s=res["d_s"], dh0=res["dh0"], dc0=res["dc0"],
-                   params=[g.view(sh) for g, sh in zip(res["grads"].split([math.prod(sh) for sh in shapes]), shapes)])
-        errs = _errors(got, r)
-        assert max(errs.values()) <= GRAD_TOL, f"lstm16_bwd_ex rows={rows} P={planes}: {errs}"
-
-    yield Call("lstm16_bwd_ex", d, lambda st: _lib().stmgcn_lstm16_bwd_ex(
-        t, lyr, rows, c, b_sz, planes, d["xo"].p, d["s"].p, d["wimg"].p, d["bias"].p, d["wih_t"].p, opt("h0p"), opt("c0"),
-        d["hp"].p, d["cs"].p, d["d_top"].p, d["dh_rec"].p, d["dc"].p, opt("dx_work"), d["dw_scratch"].p, d["dbp"].p,
-        d["zero_tile"].p, d["d_s"].p, d["grads"].p, d["dh_n"].p, d["dc_n"].p, d["dh0"].p, d["dc0"].p, d["d_xo"].p, st),
-        ref, 2 * lyr)
-
-
-def _lstm_ex_calls(n, b_sz, state):
-    from stmgcn_b200 import ops
-    hid, lyr, t, c = 48, 3, 5, 2
-    rows = n * b_sz
-    xo, s, h0, c0, ws, d_top = (None if v is None else v.to(DEV) if torch.is_tensor(v) else [w.to(DEV) for w in v]
-                                for v in lstm_inputs(n, b_sz, t, lyr, c, hid, state, seed=rows))
-    dh_n, dc_n = _seeds(lyr, rows, hid, seed=rows)
-    _, _, _, tape = ops._exact_forward(xo, s, h0, c0, lyr, hid, True, ws, True)
-    _, _, hs, cs, gates, wx, wpt = tape
-    ktape = dict(h=hs.double(), c=cs.double())
-    if state:
-        ktape["h0"] = h0.double()
-    bp = ops._pack_lstm(ws, lyr, hid)[2]
-    d = dict(xo=Buf("in", xo), s=Buf("in", s), wx=Buf("in", wx), wpt=Buf("in", wpt), cs=Buf("in", cs), hs=Buf("in", hs),
-             gates=Buf("inout", gates), d_top=Buf("in", d_top), dh_rec=Buf("ws", shape=(lyr, rows, hid)),
-             dc=Buf("ws", shape=(lyr, rows, hid)), dx_work=Buf("ws", shape=(rows, hid)), d_s=Buf("acc", shape=(b_sz, t)),
-             dwx=Buf("acc", shape=wx.shape), dwp=Buf("acc", shape=wpt.shape), dbp=Buf("acc", shape=bp.shape),
-             dh_n=Buf("in", dh_n), dc_n=Buf("in", dc_n), dh0=Buf("out", shape=(lyr, rows, hid)),
-             dc0=Buf("out", shape=(lyr, rows, hid)), d_xo=Buf("out", shape=xo.shape))
-    if state:
-        d.update(h0=Buf("in", h0), c0=Buf("in", c0))
-    opt = lambda k: d[k].p if k in d else None      # noqa: E731
-
-    def ref(res):
-        r = _state_reference(xo, s, h0, c0, ws, lyr, 2, ktape, d_top, dh_n, dc_n)
-        got = dict(d_xo=res["d_xo"], d_s=res["d_s"], dh0=res["dh0"], dc0=res["dc0"],
-                   params=ops._unpack_lstm_grads(res["dwx"], res["dwp"], res["dbp"], lyr, hid, c))
-        errs = _errors(got, r)
-        assert max(errs.values()) <= GRAD_TOL, f"lstm_bwd_ex rows={rows}: {errs}"
-
-    yield Call("lstm_bwd_ex", d, lambda st: _lib().stmgcn_lstm_bwd_ex(
-        t, lyr, rows, hid, c, b_sz, d["xo"].p, d["s"].p, d["wx"].p, d["wpt"].p, opt("h0"), opt("c0"), d["cs"].p, d["hs"].p,
-        d["gates"].p, d["d_top"].p, d["dh_rec"].p, d["dc"].p, d["dx_work"].p, d["d_s"].p, d["dwx"].p, d["dwp"].p,
-        d["dbp"].p, d["dh_n"].p, d["dc_n"].p, d["dh0"].p, d["dc0"].p, d["d_xo"].p, st), ref, 2 * lyr * t + lyr)
+    drive(obs_grad_calls(c, which), run_contract)
 
 
 @pytest.mark.parametrize("planes", [1, 2])
 @pytest.mark.parametrize("shape", [(1, 1, 3, 2, 1, False), (5, 60, 5, 4, 3, True), (3, 43, 4, 1, 4, False)],
                          ids=["one_row", "c3_l4_state", "l1_c4"])
 def test_tensor_core_extended_backward_keeps_the_memory_contract(shape, planes):
-    _drive(_lstm16_ex_calls(*shape, planes), run_contract)
+    drive(lstm16_ex_calls(*shape, planes), run_contract)
 
 
 @pytest.mark.parametrize("state", [False, True])
 def test_exact_extended_backward_keeps_the_memory_contract(state):
-    _drive(_lstm_ex_calls(7, 5, state), run_contract)
+    drive(lstm_ex_calls(7, 5, state), run_contract)
 
 
 @pytest.mark.parametrize("family", ["obs_grad", "lstm16_bwd_ex", "lstm_bwd_ex"])
 def test_new_entry_points_replay_from_a_cuda_graph(family):
-    calls = {"obs_grad": lambda: _obs_grad_calls(3, ("xo", "xt")),
-             "lstm16_bwd_ex": lambda: _lstm16_ex_calls(5, 60, 5, 4, 3, True, 2),
-             "lstm_bwd_ex": lambda: _lstm_ex_calls(7, 5, True)}[family]
-    _drive(calls(), run_captured)
+    calls = {"obs_grad": lambda: obs_grad_calls(3, ("xo", "xt")),
+             "lstm16_bwd_ex": lambda: lstm16_ex_calls(5, 60, 5, 4, 3, True, 2),
+             "lstm_bwd_ex": lambda: lstm_ex_calls(7, 5, True)}[family]
+    drive(calls(), run_captured)
 
 
 def test_new_entry_points_reject_bad_calls_without_launching():
-    from test_gpu_abi_contract import _bits
     gen = torch.Generator().manual_seed(0)
     bufs = [Buf("in", torch.randn(1 << 16, generator=gen)) for _ in range(4)]
     a, b, c, d = (x.p for x in bufs)
-    calls = {"obs_grad: n = 0": lambda: _lib().stmgcn_obs_grad(a, b, c, 2, 3, 0, 1, None),
-             "lstm16_bwd_ex: T = 65": lambda: _lib().stmgcn_lstm16_bwd_ex(
+    calls = {"obs_grad: n = 0": lambda: lib().stmgcn_obs_grad(a, b, c, 2, 3, 0, 1, None),
+             "lstm16_bwd_ex: T = 65": lambda: lib().stmgcn_lstm16_bwd_ex(
                  65, 2, 100, 1, 4, 2, *([a, b, c, d] * 5)[:18], a, b, c, d, a, None),
-             "lstm_bwd_ex: H = 6": lambda: _lib().stmgcn_lstm_bwd_ex(
+             "lstm_bwd_ex: H = 6": lambda: lib().stmgcn_lstm_bwd_ex(
                  3, 2, 8, 6, 1, 2, *([a, b, c, d] * 5)[:17], a, b, c, d, a, None)}
     for what, call in calls.items():
         torch.cuda.synchronize()
-        n0 = _lib().stmgcn_launch_count()
+        n0 = lib().stmgcn_launch_count()
         rc = call()
         torch.cuda.synchronize()
         assert rc < 0, f"{what}: rc={rc}"
-        assert _lib().stmgcn_launch_count() == n0, what
+        assert lib().stmgcn_launch_count() == n0, what
         for i, x in enumerate(bufs):
-            assert x.guards_intact() and torch.equal(_bits(x.t), _bits(x.init)), f"{what}: buffer {i} changed"
+            assert x.guards_intact() and torch.equal(bits(x.t), bits(x.init)), f"{what}: buffer {i} changed"
 
 
 # ======================================================================================================================
@@ -432,9 +244,9 @@ def test_st_mgcn_obs_gradient_matches_the_reference():
     sups = [torch.from_numpy(blob[f"st.supports.{g}"]).to(DEV) for g in range(m)]
     out = model(obs_seq=x, sta_adj_list=sups)
     nn.MSELoss()(out, torch.from_numpy(blob["st.y"]).to(DEV)).backward()
-    errs = {"out": _err(out, torch.from_numpy(blob["st.out"])),
-            "d obs": _err(x.grad, torch.from_numpy(blob["st.grad_obs"]))}
-    errs.update({key: _err(p.grad, torch.from_numpy(blob["st.grad." + key])) for key, p in model.named_parameters()})
+    errs = {"out": rel_err(out, torch.from_numpy(blob["st.out"])),
+            "d obs": rel_err(x.grad, torch.from_numpy(blob["st.grad_obs"]))}
+    errs.update({key: rel_err(p.grad, torch.from_numpy(blob["st.grad." + key])) for key, p in model.named_parameters()})
     print(f"ST_MGCN vs reference: d obs {errs['d obs']:.2e}, worst {max(errs.values()):.2e}")
     assert max(errs.values()) <= TOL, errs
 
@@ -451,63 +263,12 @@ def test_cg_lstm_obs_and_state_gradients_match_the_reference():
     out, (h_n, c_n) = model(g("supports"), x, (h0, c0))
     loss = nn.MSELoss()(out, g("y")) + (h_n * g("r1")).sum() + (c_n * g("r2")).sum()
     loss.backward()
-    errs = {"h_n": _err(h_n, g("h_n")), "c_n": _err(c_n, g("c_n"))}
-    errs.update({f"d {v}": _err(t_.grad, g("grad_" + v)) for v, t_ in (("obs", x), ("h0", h0), ("c0", c0))})
-    errs.update({key: _err(p.grad, g("grad." + key)) for key, p in model.named_parameters()})
+    errs = {"h_n": rel_err(h_n, g("h_n")), "c_n": rel_err(c_n, g("c_n"))}
+    errs.update({f"d {v}": rel_err(t_.grad, g("grad_" + v)) for v, t_ in (("obs", x), ("h0", h0), ("c0", c0))})
+    errs.update({key: rel_err(p.grad, g("grad." + key)) for key, p in model.named_parameters()})
     print(f"CG_LSTM vs reference: d obs {errs['d obs']:.2e}, d h0 {errs['d h0']:.2e}, d c0 {errs['d c0']:.2e}, "
           f"worst {max(errs.values()):.2e}")
     assert max(errs.values()) <= TOL, errs
-
-
-def _small_model(m, c, kernel, relu, seed, hid=64, t=5):
-    import STMGCN
-    n = 19
-    torch.manual_seed(seed)
-    cfg = {"kernel_type": kernel, "K": 1 if kernel == "localpool" else 2}
-    act = nn.ReLU if relu == "relu" else (nn.Tanh if relu == "tanh" else None)
-    model = STMGCN.ST_MGCN(M=m, seq_len=t, n_nodes=n, input_dim=c, lstm_hidden_dim=hid, lstm_num_layers=2,
-                           gcn_hidden_dim=24, sta_kernel_config=cfg, gconv_use_bias=True, gconv_activation=act).to(DEV)
-    gen = torch.Generator().manual_seed(seed)
-    adjs = [(torch.rand(n, n, generator=gen) < 0.3).float() * (0.5 + torch.rand(n, n, generator=gen)) for _ in range(m)]
-    if kernel == "localpool":
-        sups = []
-        for a in adjs:
-            a = a + torch.eye(n)
-            d = a.sum(1) ** -0.5
-            sups.append((d[:, None] * a * d[None, :])[None])
-    else:
-        sups = [O.chebyshev_supports_dense(a.double(), cfg["K"]).float() for a in adjs]
-    return model, sups, n, t
-
-
-def _dense_grads(model, sups, x, y, act):
-    params = {k: v.detach().double().cpu().requires_grad_(True) for k, v in model.state_dict().items()}
-    xd = x.detach().double().cpu().requires_grad_(True)
-    with _gcn_as(_tanh_gcn if act == "tanh" else O.dense_gcn):
-        out = O.dense_st_mgcn(params, xd, [s.double() for s in sups], relu=act == "relu")
-    loss = torch.mean((out - y.double().cpu()) ** 2)
-    g = torch.autograd.grad(loss, [xd] + list(params.values()))
-    return g[0], dict(zip(params, g[1:]))
-
-
-class _gcn_as:
-    """Run the dense oracle with another graph convolution in place of ``O.dense_gcn``."""
-
-    def __init__(self, fn):
-        self.fn, self.real = fn, O.dense_gcn
-
-    def __enter__(self):
-        O.dense_gcn = self.fn
-
-    def __exit__(self, *exc):
-        O.dense_gcn = self.real
-
-
-def _tanh_gcn(supports, x, w, b, relu=True):
-    return torch.tanh(_DENSE_GCN(supports, x, w, b, False))
-
-
-_DENSE_GCN = O.dense_gcn
 
 
 @pytest.mark.parametrize("kind", ["localpool", "c3", "tanh", "bf16"])
@@ -522,12 +283,11 @@ def test_st_mgcn_obs_gradient_matches_the_dense_oracle(kind, monkeypatch):
         monkeypatch.setattr(ops, "_LSTM_PATH", "tc")
     c = 3 if kind == "c3" else 1
     act = {"tanh": "tanh", "bf16": "none"}.get(kind, "relu")
-    model, sups, n, t = _small_model(2, c, "localpool" if kind == "localpool" else "chebyshev", act, seed=5)
+    model, sups, n, t = small_model(2, c, "localpool" if kind == "localpool" else "chebyshev", act, seed=5)
     gen = torch.Generator().manual_seed(6)
     x = torch.randn(4, t, n, c, generator=gen)
     y = torch.randn(4, n, c, generator=gen)
     if kind == "bf16":
-        from test_gpu_bf16_mode import forced_errors, gpu_run
         params = {k: v.detach().clone() for k, v in model.state_dict().items()}
         picks = list(range(x.shape[0]))
         run = gpu_run(model, [s.to(DEV) for s in sups], x, y, picks, want_obs=True)
@@ -538,9 +298,9 @@ def test_st_mgcn_obs_gradient_matches_the_dense_oracle(kind, monkeypatch):
         x, y = x.to(DEV).requires_grad_(True), y.to(DEV)
         out = model(obs_seq=x, sta_adj_list=[s.to(DEV) for s in sups])
         nn.MSELoss()(out, y).backward()
-        d_obs, d_params = _dense_grads(model, sups, x, y, act)
-        errs = {"d obs": _err(x.grad, d_obs)}
-        errs.update({k: _err(p.grad, d_params[k]) for k, p in model.named_parameters()})
+        d_obs, d_params = dense_grads(model, sups, x, y, act)
+        errs = {"d obs": rel_err(x.grad, d_obs)}
+        errs.update({k: rel_err(p.grad, d_params[k]) for k, p in model.named_parameters()})
     print(f"ST_MGCN {kind} vs {'forced bf16-mode' if kind == 'bf16' else 'dense'} oracle: d obs {errs['d obs']:.2e}, "
           f"worst {max(errs.values()):.2e}")
     assert max(errs.values()) <= TOL, errs
@@ -548,7 +308,7 @@ def test_st_mgcn_obs_gradient_matches_the_dense_oracle(kind, monkeypatch):
 
 def test_two_step_rollout_matches_the_dense_oracle():
     """Step 1's prediction is appended to the window of step 2; the loss is on both predictions."""
-    model, sups, n, t = _small_model(2, 1, "chebyshev", "relu", seed=8)
+    model, sups, n, t = small_model(2, 1, "chebyshev", "relu", seed=8)
     gen = torch.Generator().manual_seed(9)
     x = torch.randn(3, t, n, 1, generator=gen).to(DEV).requires_grad_(True)
     y1, y2 = (torch.randn(3, n, 1, generator=gen).to(DEV) for _ in range(2))
@@ -564,8 +324,8 @@ def test_two_step_rollout_matches_the_dense_oracle():
     xd = x.detach().double().cpu().requires_grad_(True)
     loss = rollout(lambda v: O.dense_st_mgcn(params, v, [s.double() for s in sups]), xd)
     g = torch.autograd.grad(loss, [xd] + list(params.values()))
-    errs = {"d obs": _err(x.grad, g[0])}
-    errs.update({k: _err(p.grad, r) for (k, p), r in zip(model.named_parameters(), g[1:])})
+    errs = {"d obs": rel_err(x.grad, g[0])}
+    errs.update({k: rel_err(p.grad, r) for (k, p), r in zip(model.named_parameters(), g[1:])})
     print(f"two-step rollout: d obs {errs['d obs']:.2e}, worst {max(errs.values()):.2e}")
     assert max(errs.values()) <= TOL, errs
 
@@ -595,7 +355,7 @@ def test_parameter_gradients_do_not_depend_on_input_grads(path, monkeypatch):
         runs.append({k: p.grad.clone() for k, p in model.named_parameters()})
         if grad:
             assert xs.grad is not None and hs.grad is not None and cs.grad is not None
-    errs = {k: _err(runs[1][k], runs[0][k]) for k in runs[0]}
+    errs = {k: rel_err(runs[1][k], runs[0][k]) for k in runs[0]}
     assert max(errs.values()) <= GRAD_TOL, errs
 
 
@@ -608,9 +368,8 @@ def test_obs_gradient_at_cfg3_size_on_every_window():
     (``per_step.worst_step`` along T), with every parameter gradient and every window's output."""
     import full_batch
     from stmgcn_b200 import synth
-    from test_gpu_fullsize import CHUNK, _build
     w = synth.WORKLOADS["cfg3"]
-    model, sups, laps, params, x, y = _build(w, 64, relu=False)
+    model, sups, laps, params, x, y = cheb_workload(w, 64, relu=False)
     errs = full_batch.run("cfg3 d obs", model, sups, params, [[lap] for lap in laps], w.n_supports, x, y, relu=False,
                           window_chunk=CHUNK["cfg3"], want_obs=True)
     full_batch.assert_within(errs, TOL, what="cfg3 d obs")

@@ -9,9 +9,8 @@ import pytest
 import torch
 from torch import nn
 
-from helpers import TOL
+from helpers import DEV, TOL
 
-DEV = "cuda:0"
 
 
 def test_check_limits_names_each_limit_and_accepts_each_bound():

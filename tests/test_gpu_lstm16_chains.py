@@ -9,27 +9,22 @@ import pytest
 import torch
 
 import stmgcn_oracle as O
-from test_gpu_lstm16 import FWD_TOL, GRAD_TOL, _inputs, _kernel, _reference, _step_local_error, _wave_regions
+from helpers import FWD_TOL, GRAD_TOL
+from lstm_cases import CHAIN_CASES, lstm16_inputs, lstm16_kernel, reference, step_local_error, wave_regions
 
 pytestmark = pytest.mark.gpu
 
-# (name, batch B (b_inner), channels C, initial state)
-CASES = [
-    ("b64", 64, 1, False),           # b_inner divides 128: every tile's rows cover the same windows
-    ("b37_state", 37, 2, True),      # b_inner does not divide 128; h0 / c0; runtime-C layer-0 variant
-]
-
 
 @pytest.mark.parametrize("planes", [1, 2])
-@pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
+@pytest.mark.parametrize("case", CHAIN_CASES, ids=[c[0] for c in CHAIN_CASES])
 def test_lstm16_t64_chains_over_several_tiles_per_cta(case, planes):
     name, b, c, state = case
     t, lyr = 64, 2
-    n = _wave_regions(b)
-    xo, s, h0, c0, ws, d_top = _inputs(n, b, t, lyr, c, state, seed=1000 + 10 * CASES.index(case) + planes)
-    h_top, hc_n, ktape, d_s, grads = _kernel(xo, s, h0, c0, ws, lyr, planes, d_top)
-    hs, cs, layers, s64 = _reference(xo, s, h0, c0, ws, lyr, planes, ktape)
-    errs = {"step-local forward": _step_local_error(ktape, hs, cs, planes),
+    n = wave_regions(b)
+    xo, s, h0, c0, ws, d_top = lstm16_inputs(n, b, t, lyr, c, state, seed=1000 + 10 * CHAIN_CASES.index(case) + planes)
+    h_top, hc_n, ktape, d_s, grads = lstm16_kernel(xo, s, h0, c0, ws, lyr, planes, d_top)
+    hs, cs, layers, s64 = reference(xo, s, h0, c0, ws, lyr, planes, ktape)
+    errs = {"step-local forward": step_local_error(ktape, hs, cs, planes),
             "h_top": O.max_rel_err(h_top.cpu().numpy(), hs[-1][-1].detach().cpu().numpy())}
     if state:
         errs["c_n"] = O.max_rel_err(hc_n[1].cpu().numpy(), torch.stack([v[-1] for v in cs]).detach().cpu().numpy())

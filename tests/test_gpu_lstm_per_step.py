@@ -25,36 +25,12 @@ from torch import nn
 
 import stmgcn_oracle as O
 from per_step import per_step_rel_err, worst_step
-from test_gpu_exact_kernels import LSTM_CASES, _sms, lstm_inputs
-from test_gpu_input_grads import (EXACT_CASES, _dense_grads, _errors, _exact_run, _lstm16_run, _seeds, _small_model,
-                                  _state_reference)
-from test_gpu_lstm16 import CASES, _inputs, _wave_regions
-from test_gpu_lstm16_chains import CASES as CHAIN_CASES
+from helpers import DEV, GRAD_TOL, sm_count
+from lstm_cases import (EXACT, HID, PREMISE, TC_CASES, exact_run, grad_errors, lstm16_inputs, lstm16_run, lstm_inputs,
+                        seeds, state_gradients, wave_regions, with_long_memory)
+from model_cases import dense_grads, small_model
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-HID = 64
-GRAD_TOL = 5e-5
-FORGET_BIAS = 3.0           # long-memory cases: added to b_ih's forget-gate rows [H, 2H)
-PREMISE = 1e-2              # long-memory cases: max|d_s[:, 0]| / max|d_s| of the reference at least this
-
-# (name, regions N (None: multi-wave, from the SM count), batch B, T, layers L, channels C, initial state, long memory)
-TC_CASES = ([(name, n, b, t, lyr, c, state, False) for name, n, b, t, lyr, c, state in CASES]
-            + [("chain_" + name, None, b, 64, 2, c, state, False) for name, b, c, state in CHAIN_CASES]
-            + [("long_waves_b64", None, 64, 64, 2, 1, False, True),        # several tiles per CTA
-               ("long_t64_l1_c4_state", 3, 43, 64, 1, 4, True, True),
-               ("long_l3_c3_b37_state", 7, 37, 64, 3, 3, True, True)])     # 259 rows: a ragged third tile
-# (name, H, L, T, C, regions N (None: multi-wave), batch B, initial state, long memory)
-EXACT = ([(name, hid, lyr, t, c, n, b, state, False) for name, hid, lyr, t, c, n, b, state, _ in LSTM_CASES]
-         + [(name, hid, lyr, t, c, n, b, state, False) for name, hid, lyr, t, c, n, b, state in EXACT_CASES]
-         + [("long_h64_t70_b2100", 64, 2, 70, 1, 2, 2100, False, True),   # b_inner > 2048: d_s atomics in global memory
-            ("long_h48_t40_state", 48, 3, 40, 2, 9, 20, True, True)])
-
-
-def _long_memory(ws, hid):
-    for l in range(len(ws) // 4):
-        ws[4 * l + 2][hid:2 * hid] += FORGET_BIAS
-    return ws
 
 
 def _per_step(got, ref):
@@ -69,20 +45,20 @@ def _truncated_reference(xo, s, ws, lyr, planes, ktape, d_top, dh_n, dc_n):
     k = t // 2
     h_k, c_k = ktape["h"][:, k - 1].clone(), ktape["c"][:, k - 1].clone()
     tape = dict(h=ktape["h"][:, k:], c=ktape["c"][:, k:], h0=h_k)
-    r = _state_reference(xo[:, :, k:], s[:, k:], h_k, c_k, ws, lyr, planes, tape, d_top, dh_n, dc_n)
+    r = state_gradients(xo[:, :, k:], s[:, k:], h_k, c_k, ws, lyr, planes, tape, d_top, dh_n, dc_n)
     r["d_s"] = torch.cat([r["d_s"].new_zeros(s.shape[0], k), r["d_s"]], dim=1)
     r["d_xo"] = torch.cat([r["d_xo"].new_zeros(xo.shape[:2] + (k,) + xo.shape[3:]), r["d_xo"]], dim=2)
     return r
 
 
 def _check(what, xo, s, h0, c0, ws, lyr, planes, d_top, dh_n, dc_n, got, ktape, long_memory, bars=None):
-    ref = _state_reference(xo, s, h0, c0, ws, lyr, planes, ktape, d_top, dh_n, dc_n)
+    ref = state_gradients(xo, s, h0, c0, ws, lyr, planes, ktape, d_top, dh_n, dc_n)
     steps = _per_step(got, ref)
     line = f"{what}: per step " + ", ".join(f"{k} {e:.2e} (step {i})" for k, (e, i) in steps.items())
     bad = {k: e for k, (e, _) in steps.items() if not e <= (bars or {}).get(k, GRAD_TOL)}
     if long_memory:
         share = float(ref["d_s"][:, 0].abs().max()) / float(ref["d_s"].abs().max())
-        errs = _errors(got, ref)
+        errs = grad_errors(got, ref)
         line += f"; max-norm worst {max(errs.values()):.2e} ({max(errs, key=errs.get)}); d_s[:, 0] share {share:.2f}"
         assert share >= PREMISE, f"{what}: the long-memory premise fails: d_s[:, 0] is {share:.1e} of max|d_s|"
         bad.update({k: e for k, e in errs.items() if not e <= GRAD_TOL})
@@ -91,7 +67,7 @@ def _check(what, xo, s, h0, c0, ws, lyr, planes, d_top, dh_n, dc_n, got, ktape, 
         trunc = _truncated_reference(xo, s, ws, lyr, planes, ktape, d_top, dh_n, dc_n)
         tr_step = worst_step(trunc["d_s"], ref["d_s"], 1)[0]
         tr_old = O.max_rel_err(trunc["d_s"].cpu().numpy(), ref["d_s"].cpu().numpy())
-        tr_w = max(v for k, v in _errors(trunc, ref).items() if k.startswith("param"))
+        tr_w = max(v for k, v in grad_errors(trunc, ref).items() if k.startswith("param"))
         swapped = got["d_s"].clone()
         swapped[:, [0, 1]] = swapped[:, [1, 0]]
         sw_step = worst_step(swapped, ref["d_s"], 1)[0]
@@ -121,13 +97,13 @@ SATURATED_DH0_BAR = 2e-3
 def test_tensor_core_backward_per_step(case, planes):
     name, n, b, t, lyr, c, state, long_memory = case
     if n is None:
-        n = _wave_regions(b)
-    xo, s, h0, c0, ws, d_top = _inputs(n, b, t, lyr, c, state, seed=3000 + 10 * TC_CASES.index(case) + planes,
+        n = wave_regions(b)
+    xo, s, h0, c0, ws, d_top = lstm16_inputs(n, b, t, lyr, c, state, seed=3000 + 10 * TC_CASES.index(case) + planes,
                                        saturate=name == "saturated")
     if long_memory:
-        ws = _long_memory(ws, HID)
-    dh_n, dc_n = _seeds(lyr, n * b, HID, seed=3000 + TC_CASES.index(case))
-    got, ktape, _ = _lstm16_run(xo, s, h0, c0, ws, lyr, planes, d_top, dh_n, dc_n)
+        ws = with_long_memory(ws, HID)
+    dh_n, dc_n = seeds(lyr, n * b, HID, seed=3000 + TC_CASES.index(case))
+    got, ktape, _ = lstm16_run(xo, s, h0, c0, ws, lyr, planes, d_top, dh_n, dc_n)
     _check(f"lstm16 {name} P={planes} rows={n * b}", xo, s, h0, c0, ws, lyr, planes, d_top, dh_n, dc_n, got, ktape,
            long_memory, bars={"dh0": SATURATED_DH0_BAR} if name == "saturated" else None)
 
@@ -136,16 +112,16 @@ def test_tensor_core_backward_per_step(case, planes):
 def test_exact_backward_per_step(case):
     name, hid, lyr, t, c, n, b, state, long_memory = case
     if n is None:
-        n = (2 * 32 * _sms()) // b + 1
+        n = (2 * 32 * sm_count()) // b + 1
     xo, s, h0, c0, ws, d_top = lstm_inputs(n, b, t, lyr, c, hid, state, seed=4000 + EXACT.index(case),
                                            saturate=name == "saturated")
     if long_memory:
-        ws = _long_memory(ws, hid)
+        ws = with_long_memory(ws, hid)
     xo, s, d_top = xo.to(DEV), s.to(DEV), d_top.to(DEV)
     h0, c0 = (None, None) if h0 is None else (h0.to(DEV), c0.to(DEV))
     ws = [w.to(DEV) for w in ws]
-    dh_n, dc_n = _seeds(lyr, n * b, hid, seed=4000 + EXACT.index(case))
-    got, ktape = _exact_run(xo, s, h0, c0, ws, lyr, hid, d_top, dh_n, dc_n)
+    dh_n, dc_n = seeds(lyr, n * b, hid, seed=4000 + EXACT.index(case))
+    got, ktape = exact_run(xo, s, h0, c0, ws, lyr, hid, d_top, dh_n, dc_n)
     _check(f"lstm {name} rows={n * b}", xo, s, h0, c0, ws, lyr, 2, d_top, dh_n, dc_n, got, ktape, long_memory)
 
 
@@ -168,7 +144,7 @@ def test_shared_lstm_input_gradients_per_step(t_len, monkeypatch):
     monkeypatch.setattr(ops, "_PLANES", 2)
     monkeypatch.setattr(ops, "_LSTM_PATH", "tc")
     n, b, lyr, c = 3, 50, 3, 2
-    xo, s, _, _, ws, d_top = _inputs(n, b, t_len, lyr, c, False, seed=5000 + t_len)
+    xo, s, _, _, ws, d_top = lstm16_inputs(n, b, t_len, lyr, c, False, seed=5000 + t_len)
     xo_g, s_g = xo.clone().requires_grad_(True), s.clone().requires_grad_(True)
     h_top, _, _ = ops.SharedLSTM.apply(xo_g, s_g, None, None, lyr, HID, False, *ws)
     (h_top.reshape(n * b, HID) * d_top).sum().backward()
@@ -188,13 +164,13 @@ def test_shared_lstm_input_gradients_per_step(t_len, monkeypatch):
 def test_st_mgcn_obs_gradient_per_step():
     """ST_MGCN (two Chebyshev graphs, ReLU, H = 64 on the tensor cores) at T = 24 with obs_seq requiring grad: d obs
     per step against the dense fp64 oracle."""
-    model, sups, n, t = _small_model(2, 1, "chebyshev", "relu", seed=21, t=24)
+    model, sups, n, t = small_model(2, 1, "chebyshev", "relu", seed=21, t=24)
     gen = torch.Generator().manual_seed(22)
     x = torch.randn(4, t, n, 1, generator=gen).to(DEV).requires_grad_(True)
     y = torch.randn(4, n, 1, generator=gen).to(DEV)
     out = model(obs_seq=x, sta_adj_list=[v.to(DEV) for v in sups])
     nn.MSELoss()(out, y).backward()
-    d_obs, _ = _dense_grads(model, sups, x, y, "relu")
+    d_obs, _ = dense_grads(model, sups, x, y, "relu")
     errs = per_step_rel_err(x.grad, d_obs, 1)
     share = (d_obs.abs().amax(dim=(0, 2, 3)) / d_obs.abs().max()).min()
     print(f"ST_MGCN T={t} d obs per step: worst {errs.max():.2e} (step {int(errs.argmax())}), "

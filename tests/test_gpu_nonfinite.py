@@ -27,16 +27,12 @@ import torch
 from torch import nn
 
 import stmgcn_oracle as O
-from test_gpu_exact_kernels import _fuse_rows, _proj_rows, isolated_matrix
-from test_gpu_lstm16 import _inputs as lstm_inputs
-from test_gpu_lstm16 import _wave_regions
-from test_gpu_proj_tc import _shape as tc_shape
+from helpers import DEV, FWD_TOL, GRAD_TOL
+from kernel_cases import fuse_rows, isolated_matrix, proj_rows, tc_shape
+from lstm_cases import HID, lstm16_inputs, wave_regions
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-FWD_TOL, GRAD_TOL = 2e-5, 5e-5
 LEAK_TOL = 5e-6
-HID = 64
 NAN = math.nan
 
 
@@ -121,7 +117,7 @@ def _proj_case(path, ks, p, q, rows_id, seed):
     if path == "tc":
         n, b = tc_shape(rows_id)
     else:
-        n, b = _proj_rows(rows_id), 1
+        n, b = proj_rows(rows_id), 1
     gen = torch.Generator().manual_seed(seed)
     s = torch.randn(ks, n, b, p, generator=gen)
     s[:, 1::5] = 0.0                                 # rows whose stack is exactly zero
@@ -327,8 +323,8 @@ def test_lstm_nan_in_one_input_row_stays_in_that_row(family, c, state, where, mo
     size (several 128-row tiles per CTA), 3 layers, T = 12."""
     _family_setup(monkeypatch, family)
     b, t, lyr = 37, 12, 3
-    n = _wave_regions(b)
-    inputs = lstm_inputs(n, b, t, lyr, c, state, seed=7 * c + state)
+    n = wave_regions(b)
+    inputs = lstm16_inputs(n, b, t, lyr, c, state, seed=7 * c + state)
     rows = n * b
     r = _position(rows, where)
     xo_bad = inputs[0].clone()
@@ -347,8 +343,8 @@ def test_lstm_nan_in_one_initial_state_row_stays_in_that_row(family, which, laye
     the layers below and every other row are the clean run's bit for bit."""
     _family_setup(monkeypatch, family)
     b, t, lyr = 64, 6, 3
-    n = _wave_regions(b)
-    inputs = lstm_inputs(n, b, t, lyr, 2, True, seed=11 + layer)
+    n = wave_regions(b)
+    inputs = lstm16_inputs(n, b, t, lyr, 2, True, seed=11 + layer)
     r = _position(n * b, "second_warpgroup")
     h0, c0 = inputs[2].clone(), inputs[3].clone()
     (h0 if which == "h0" else c0)[layer, r, 9] = NAN
@@ -367,7 +363,7 @@ def test_lstm_nan_in_a_recurrent_weight_reaches_every_row(family, state, monkeyp
     _family_setup(monkeypatch, family)
     b, t, lyr = 40, 7, 3
     n = 9
-    inputs = lstm_inputs(n, b, t, lyr, 1, state, seed=13 + state)
+    inputs = lstm16_inputs(n, b, t, lyr, 1, state, seed=13 + state)
     ws = [w.clone() for w in inputs[4]]
     ws[5][2 * HID + 3, 17] = NAN                     # layer 1, W_hh: the g gate of unit 3, from h unit 17
     clean = None
@@ -386,7 +382,7 @@ def test_lstm_products_skipped_with_a_zero_initial_state(family, monkeypatch):
     form the product and give NaN as torch does.  With an h0 of zeros every family gives NaN."""
     _family_setup(monkeypatch, family)
     b, t, lyr = 40, 1, 2
-    xo, s, _, _, ws, d_top = lstm_inputs(3, b, t, lyr, 1, False, seed=3)
+    xo, s, _, _, ws, d_top = lstm16_inputs(3, b, t, lyr, 1, False, seed=3)
     ws = [w.clone() for w in ws]
     ws[1][7, 7] = NAN                                # layer 0 W_hh
     res, _, _ = _lstm_run(family, xo, s, None, None, ws, lyr, d_top)
@@ -407,7 +403,7 @@ def test_lstm16_saturated_gates_keep_their_cap_and_trace_nan(family, monkeypatch
     with c beyond 15 (the NaN-keeping cap saturates as before), and a NaN in xo[r, 3] stays in row r."""
     _family_setup(monkeypatch, family)
     n, b, t, lyr, c = 5, 40, 20, 3, 1
-    inputs = lstm_inputs(n, b, t, lyr, c, True, seed=70, saturate=True)
+    inputs = lstm16_inputs(n, b, t, lyr, c, True, seed=70, saturate=True)
     r = 150
     xo_bad = inputs[0].clone()
     xo_bad.view(n * b, t, c)[r, 3, 0] = NAN
@@ -453,7 +449,7 @@ def test_fuse_out_nan_in_one_feature():
     column g of d_fcw is NaN; d_g (which does not read the features) is the clean run's bit for bit and d_fcb within
     LEAK_TOL (atomics)."""
     from stmgcn_b200 import ops
-    n, b = _fuse_rows("waves")
+    n, b = fuse_rows("waves")
     m, gdim, c_out = 3, 64, 2
     gen = torch.Generator().manual_seed(5)
     gs = [torch.randn(n, b, gdim, generator=gen).to(DEV) for _ in range(m)]

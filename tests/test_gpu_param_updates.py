@@ -41,10 +41,9 @@ from torch import nn
 
 import diffusion_oracle as D
 import stmgcn_oracle as O
-from helpers import TOL
+from helpers import DEV, TOL
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 
 META = dict(n=96, m=3, k=3, t=12, b=8, c=1, hid=64, layers=3, gcn_hid=64)     # LSTM and projection on the tensor cores
 LR, WD = 2e-3, 1e-4             # Main.py

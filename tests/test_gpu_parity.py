@@ -7,10 +7,9 @@ import torch
 from torch import nn
 
 import stmgcn_oracle as O
-from helpers import TOL, assert_close, build_model, load_golden
+from helpers import DEV, TOL, assert_close, build_model, load_golden
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 
 
 def _rand_csr(n, density, seed, asym=True):

@@ -6,19 +6,10 @@ import pytest
 import torch
 
 import stmgcn_oracle as O
+from helpers import DEV, FWD_TOL, GRAD_TOL
+from kernel_cases import tc_shape
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-FWD_TOL, GRAD_TOL = 2e-5, 5e-5
-
-
-def _shape(rows_id):
-    """(N, B) with N * B rows."""
-    if rows_id == "waves":
-        from stmgcn_b200 import _lib
-        n = (128 * (2 * int(_lib.lib.stmgcn_sm_count()) + 1) + 77) // 7 + 1
-        return n, 7
-    return {1: (1, 1), 31: (31, 1), 33: (11, 3), 129: (43, 3)}[rows_id]
 
 
 @pytest.mark.parametrize("bias", [True, False])
@@ -29,7 +20,7 @@ def test_projection_tensor_core_kernels_match_fp64(ks, rows_id, relu, bias):
     """out = act(sum_k S_k W_k + b); dZ = d_out * mask with the kernel's own mask (out > 0); db = sum dZ; dW_k = S_k^T dZ;
     U_k = dZ W_k^T.  Measured on an H100 (max over all 160 cases): out 6.3e-6, gradients 3.2e-6."""
     from stmgcn_b200 import ops
-    n, b = _shape(rows_id)
+    n, b = tc_shape(rows_id)
     p = q = 64
     gen = torch.Generator().manual_seed(100 * ks + (rows_id if isinstance(rows_id, int) else 999) + 2 * relu + bias)
     s = torch.randn(ks, n, b, p, generator=gen).to(DEV)

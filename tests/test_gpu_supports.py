@@ -28,38 +28,18 @@ import weakref
 
 import numpy as np
 import pytest
-import scipy.sparse as sp
 import torch
 from torch import nn
 
 import diffusion_oracle as D
 import stmgcn_oracle as O
-from helpers import TOL
-from test_supports_host import MALFORMED, _malformed, handmade_csr, scipy_of
+from helpers import DEV, FWD_TOL, GRAD_TOL, TOL, rel_err
+from kernel_cases import MALFORMED, handmade_csr, malformed, scipy_of
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-SPMM_TOL, FWD_TOL, GRAD_TOL = 1e-5, 2e-5, 5e-5
+SPMM_TOL = 1e-5
 ADJ_TOL = 1e-8           # 10x the largest residual measured (9.3e-10); a forward and backward of different matrices: >= 6.9e-4
 N_ROUTE, B_ROUTE = 200, 3
-
-
-def _err(new, ref):
-    return O.max_rel_err(new.detach().double().cpu().numpy(), ref.detach().double().cpu().numpy())
-
-
-def _chain_stack64(mats, ks):
-    """fp64 dense (Ks, N, N) stack of recurrence chains sharing T_0 = I: [I, T_1(X_0) .. T_K(X_0), T_1(X_1) ..]."""
-    n = mats[0].shape[0] if mats else None
-    eye = np.eye(n)
-    out = [eye]
-    for x in mats:
-        x = x.toarray() if sp.issparse(x) else x
-        terms = [eye, x]
-        for _ in range(2, (ks - 1) // len(mats) + 1):
-            terms.append(2.0 * (x @ terms[-1]) - terms[-2])
-        out += terms[1:]
-    return torch.from_numpy(np.stack(out))
 
 
 def dense64(sup):
@@ -73,7 +53,7 @@ def dense64(sup):
         return torch.from_numpy(np.stack([m.toarray() for m in mats]))
     if sup.ks == 1:
         return torch.eye(sup.n, dtype=torch.float64)[None]
-    return _chain_stack64(mats, sup.ks)
+    return O.chain_stack_dense([torch.from_numpy(m.toarray()) for m in mats], (sup.ks - 1) // len(mats))
 
 
 ROUTES = {  # name: (mode, number of graphs of the support set)
@@ -117,8 +97,8 @@ def stack_and_adjoint(sset, s64, x, u):
     torch.cuda.synchronize()
     x64, u64 = x.double().cpu().reshape(n, -1), u.double().cpu().reshape(ks, n, -1)
     st64, dx64 = stack.double().cpu().reshape(ks, n, -1), dx.double().cpu().reshape(n, -1)
-    errs = {f"S_{k} X": _err(st64[k], s64[k] @ x64) for k in range(ks)}
-    errs["adjoint"] = _err(dx64, sum(s64[k].t() @ u64[k] for k in range(ks)))
+    errs = {f"S_{k} X": rel_err(st64[k], s64[k] @ x64) for k in range(ks)}
+    errs["adjoint"] = rel_err(dx64, sum(s64[k].t() @ u64[k] for k in range(ks)))
     lhs = float((st64 * u64).sum())
     rhs = float((x64 * dx64).sum())
     scale = float(sum(((s64[k].abs() @ x64.abs()) * u64[k].abs()).sum() for k in range(ks)))
@@ -148,8 +128,8 @@ def gcn_vs_fp64(sup, s64, p, seed, relu=True):
     mask = (out.detach().cpu() > 0).double() if relu else 1.0
     ref = z * mask
     grads = torch.autograd.grad((ref * probe.double()).sum(), [x64, w64, b64])
-    gerrs = {"dX": _err(xd.grad, grads[0]), "dW": _err(layer.W.grad, grads[1]), "db": _err(layer.b.grad, grads[2])}
-    return _err(out, ref), gerrs
+    gerrs = {"dX": rel_err(xd.grad, grads[0]), "dW": rel_err(layer.W.grad, grads[1]), "db": rel_err(layer.b.grad, grads[2])}
+    return rel_err(out, ref), gerrs
 
 
 # ======================================================================================================================
@@ -268,7 +248,7 @@ def test_malformed_handle_raises_before_any_launch(case):
         rp, ci, v = handmade_csr(n, 7)
         bad = ChebSupports(n, 3, rp.to(DEV), ci.to(DEV), v)
     else:
-        n, rp, ci, v, msg = _malformed(case)
+        n, rp, ci, v, msg = malformed(case)
         bad = ChebSupports(n, 3, rp.to(DEV), ci.to(DEV), v.to(DEV))
     model, _, x, _ = _model(3, n)
     xd = x.to(DEV)
@@ -316,8 +296,8 @@ def model_errors(model, sup, params, x, y):
     loss = nn.MSELoss()(out, y.to(DEV))
     loss.backward()
     o_ref, l_ref, g_ref = dense_reference(params, [dense64(sup)], x, y)
-    errs = {"out": _err(out, o_ref), "d obs": _err(xd.grad, g_ref["d obs"])}
-    errs.update({k: _err(p.grad, g_ref[k]) for k, p in model.named_parameters()})
+    errs = {"out": rel_err(out, o_ref), "d obs": rel_err(xd.grad, g_ref["d obs"])}
+    errs.update({k: rel_err(p.grad, g_ref[k]) for k, p in model.named_parameters()})
     return errs
 
 
@@ -421,8 +401,8 @@ def test_graphed_step_holds_its_support_sets_and_matches_fp64():
     loss = gstep(x2.to(DEV), y2.to(DEV))
     torch.cuda.synchronize()
     o_ref, l_ref, g_ref = dense_reference(params, [dense64(s) for s in sups], x2, y2)
-    errs = {"out": _err(gstep.out, o_ref), "loss": abs(loss.item() - l_ref) / abs(l_ref)}
-    errs.update({k: _err(p.grad, g_ref[k]) for k, p in model.named_parameters()})
+    errs = {"out": rel_err(gstep.out, o_ref), "loss": abs(loss.item() - l_ref) / abs(l_ref)}
+    errs.update({k: rel_err(p.grad, g_ref[k]) for k, p in model.named_parameters()})
     worst = max(errs, key=errs.get)
     print(f"graphed step after clear_cache + 40 conversions: worst {errs[worst]:.2e} ({worst})")
     assert errs[worst] <= TOL, errs

@@ -180,6 +180,17 @@ def test_known_answer_ring_graph_spectrum():
         assert np.allclose(np.sort(np.linalg.eigvalsh(sup[k].numpy())), want, atol=1e-10)
 
 
+def test_chain_stack_of_one_chain_is_the_chebyshev_stack():
+    """``chain_stack_dense`` of the single chain L~ is ``chebyshev_supports_dense`` of the adjacency, T_0 .. T_K."""
+    from stmgcn_b200 import synth
+    adj = synth.make_adjacency(40, 0, 0.2).double()
+    for order in (1, 2, 5):
+        want = O.chebyshev_supports_dense(adj, order)
+        got = O.chain_stack_dense([O.rescaled_laplacian_dense(adj)], order)
+        assert got.shape == want.shape, (order, got.shape, want.shape)
+        assert_close(got.numpy(), want.numpy(), f"chain stack, K = {order}", 1e-12)
+
+
 def test_known_answer_order_zero_gcn_is_a_linear_layer():
     x = torch.randn(3, 9, 4)
     w, b = torch.randn(4, 5), torch.randn(5)

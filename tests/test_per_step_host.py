@@ -6,9 +6,8 @@ import torch
 
 import stmgcn_oracle as O
 from per_step import per_step_rel_err, worst_step
-from test_gpu_lstm16 import _inputs
-from test_gpu_lstm_per_step import EXACT, GRAD_TOL, PREMISE, TC_CASES, _long_memory
-from test_gpu_exact_kernels import lstm_inputs
+from helpers import GRAD_TOL
+from lstm_cases import EXACT, PREMISE, TC_CASES, lstm16_inputs, lstm_inputs, with_long_memory
 
 
 # ======================================================================================================================
@@ -101,7 +100,7 @@ def test_truncated_bptt_passes_the_max_norm_bar_and_fails_the_per_step_one():
     (With this seed, skipping T/2 = 32 steps puts d_s 9.2e-5 off in max-norm, 30 steps 6.1e-5, 28 steps 3.8e-5.)"""
     n, b, t, lyr, c = 3, 43, 64, 1, 4
     cut = 28
-    xo, s, _, _, ws, d_top = _inputs(n, b, t, lyr, c, False, seed=21, device="cpu")
+    xo, s, _, _, ws, d_top = lstm16_inputs(n, b, t, lyr, c, False, seed=21, device="cpu")
     d_s, _ = _reference(xo, s, ws, lyr, d_top)
     d_s_cut, _ = _reference(xo, s, ws, lyr, d_top, cut=cut)
     old = O.max_rel_err(d_s_cut.numpy(), d_s.numpy())
@@ -115,14 +114,14 @@ def test_truncated_bptt_passes_the_max_norm_bar_and_fails_the_per_step_one():
 def _tc_long_inputs(case, planes, n_waves=4):
     name, n, b, t, lyr, c, state, _ = case
     seed = 3000 + 10 * TC_CASES.index(case) + planes
-    xo, s, h0, c0, ws, d_top = _inputs(n or n_waves, b, t, lyr, c, state, seed=seed, device="cpu")
-    return xo, s, h0, c0, _long_memory(ws, 64), d_top, lyr
+    xo, s, h0, c0, ws, d_top = lstm16_inputs(n or n_waves, b, t, lyr, c, state, seed=seed, device="cpu")
+    return xo, s, h0, c0, with_long_memory(ws, 64), d_top, lyr
 
 
 def _exact_long_inputs(case):
     name, hid, lyr, t, c, n, b, state, _ = case
     xo, s, h0, c0, ws, d_top = lstm_inputs(n, b, t, lyr, c, hid, state, seed=4000 + EXACT.index(case))
-    return xo, s, h0, c0, _long_memory(ws, hid), d_top, lyr
+    return xo, s, h0, c0, with_long_memory(ws, hid), d_top, lyr
 
 
 LONG = ([("tc", c) for c in TC_CASES if c[-1]] + [("exact", c) for c in EXACT if c[-1]])
@@ -147,7 +146,7 @@ def test_without_the_forget_bias_the_early_steps_vanish():
     what the forget bias is there to change."""
     case = next(c for c in TC_CASES if c[-1])
     name, n, b, t, lyr, c, state, _ = case
-    xo, s, h0, c0, ws, d_top = _inputs(n or 4, b, t, lyr, c, state, seed=3000 + 10 * TC_CASES.index(case) + 2,
+    xo, s, h0, c0, ws, d_top = lstm16_inputs(n or 4, b, t, lyr, c, state, seed=3000 + 10 * TC_CASES.index(case) + 2,
                                        device="cpu")
     d_s, _ = _reference(xo, s, ws, lyr, d_top, h0, c0)
     share = float(d_s[:, 0].abs().max() / d_s.abs().max())

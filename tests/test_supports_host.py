@@ -13,47 +13,7 @@ import pytest
 import scipy.sparse as sp
 import torch
 
-import stmgcn_oracle as O
-
-
-def handmade_csr(n, seed, hub_row=0, hub_col=1, scale=True):
-    """int32 / float32 CSR ``(rowptr, colidx, vals)`` of an ``n x n`` matrix as a caller might hand-make it: row ``i`` has
-    ``i % 10`` entries (every tail length of the SpMM's 4-way unroll, empty rows included), row ``hub_row`` has ``n - 1``
-    and column ``hub_col`` is in almost every row; columns are shuffled within each row, every third non-empty row
-    repeats one of its entries, and some stored values are ``0.0`` and ``-0.0``.  With ``scale`` each value is divided by
-    the larger of its row's and its column's absolute sum (entries counted one by one), so the matrix's 1- and inf-norms,
-    and with them its spectral radius, are at most 1."""
-    rng = np.random.default_rng(seed)
-    rows = []
-    for i in range(n):
-        deg = n - 1 if i == hub_row else i % 10
-        cols = list(rng.choice(n, size=min(deg, n), replace=False))
-        if i != hub_row and hub_col not in cols and i % 10 > 1:
-            cols[0] = hub_col
-        if cols and i % 3 == 0:
-            cols.append(cols[int(rng.integers(len(cols)))])             # a repeated (i, j) entry
-        cols = list(rng.permutation(cols))
-        rows.append(cols)
-    vals = [rng.standard_normal(len(c)) for c in rows]
-    for i, v in enumerate(vals):
-        if len(v) >= 3 and i % 4 == 1:
-            v[1] = 0.0
-        if len(v) >= 3 and i % 4 == 3:
-            v[2] = -0.0
-    rowptr = np.concatenate([[0], np.cumsum([len(c) for c in rows])]).astype(np.int32)
-    colidx = np.concatenate([np.asarray(c, np.int64) for c in rows]).astype(np.int32)
-    data = np.concatenate(vals)
-    if scale:
-        a, row_of = np.abs(data), np.repeat(np.arange(n), np.diff(rowptr))
-        r = np.bincount(row_of, weights=a, minlength=n)
-        c = np.bincount(colidx, weights=a, minlength=n)
-        data = data / np.maximum(np.maximum(r[row_of], c[colidx]), 1e-30)
-    return torch.from_numpy(rowptr), torch.from_numpy(colidx), torch.from_numpy(data.astype(np.float32))
-
-
-def scipy_of(rowptr, colidx, vals, n):
-    """fp64 scipy CSR of a CSR triple, entries verbatim (repeats are summed by every product scipy computes)."""
-    return sp.csr_matrix((vals.double().cpu().numpy(), colidx.cpu().numpy(), rowptr.cpu().numpy()), shape=(n, n))
+from kernel_cases import MALFORMED, handmade_csr, malformed, scipy_of, valid_csr
 
 
 def test_handmade_csr_has_the_advertised_edges():
@@ -147,45 +107,10 @@ def test_handmade_csr_exports_scipys_csr_and_transpose(n):
         assert (np.diff(row) >= 0).all(), f"CSR^T row {i} is not sorted"
 
 
-def _valid(n=40):
-    return handmade_csr(n, 7)
-
-
-def _malformed(case):
-    """(n, rowptr, colidx, vals, message) of one malformed CSR, made from a valid one."""
-    n = 40
-    rp, ci, v = (t.clone() for t in _valid(n))
-    if case == "rowptr_start":
-        rp[0] = 1
-        return n, rp, ci, v, "rowptr\\[0\\] is not 0"
-    if case == "rowptr_decreasing":
-        rp[20] = rp[21] + 1
-        return n, rp, ci, v, "rowptr decreases"
-    if case == "rowptr_end":
-        return n, rp, ci[:-1].clone(), v[:-1].clone(), "rowptr\\[-1\\] is not nnz"
-    if case == "short_vals":
-        return n, rp, ci, v[:-2].clone(), "vals has .* entries, colidx"
-    if case == "col_negative":
-        ci[5] = -1
-        return n, rp, ci, v, "column index is outside \\[0, 40\\)"
-    if case == "col_n":
-        ci[-1] = n
-        return n, rp, ci, v, "column index is outside \\[0, 40\\)"
-    if case == "rowptr_length":
-        return n, rp[:-1].clone(), ci, v, "rowptr has 40 entries, n \\+ 1 = 41"
-    if case == "dtype":
-        return n, rp, ci, v.double(), "must be int32 and vals float32"
-    raise KeyError(case)
-
-
-MALFORMED = ["rowptr_start", "rowptr_decreasing", "rowptr_end", "short_vals", "col_negative", "col_n", "rowptr_length",
-             "dtype"]
-
-
 @pytest.mark.parametrize("case", MALFORMED)
 def test_malformed_csr_raises_a_value_error_naming_the_fault(case):
     from stmgcn_b200.graph import GraphHandle
-    n, rp, ci, v, msg = _malformed(case)
+    n, rp, ci, v, msg = malformed(case)
     with pytest.raises(ValueError, match=msg):
         GraphHandle.from_csr(n, rp, ci, v)
 
@@ -193,7 +118,7 @@ def test_malformed_csr_raises_a_value_error_naming_the_fault(case):
 def test_the_valid_csr_the_malformed_ones_come_from_is_accepted():
     from stmgcn_b200.graph import GraphHandle
     n = 40
-    assert GraphHandle.from_csr(n, *_valid(n)).nnz == _valid(n)[1].numel()
+    assert GraphHandle.from_csr(n, *valid_csr(n)).nnz == valid_csr(n)[1].numel()
 
 
 TOL_CHEB = 5e-5          # graph._is_chebyshev_stack's default tolerance
