@@ -507,7 +507,7 @@ struct Bwd16Params {
     float* dh_rec;             // blocked, in (unless first) / out, in place through the steps
     float* dc;                 // blocked, in (unless first) / out, in place through the steps
     float* dbp;                // (256) +=  gate-interleaved bias gradient
-    float* dw_slice;           // gridDim.x slices of 128 x 256 floats (row-major [kd][gate column]), +=
+    float* dw_slice;           // gridDim.x slices of 128 x 256 floats (fragment order, see bwd_wgrad_red), +=
     int64_t rows;
     int n_tiles;
     Bwd16Step steps[kBMaxSteps];   // in execution order: steps[0] is t = T-1
@@ -577,14 +577,24 @@ __device__ __forceinline__ void bwd_dgrad_mma(float (&dacc)[32 * NSEG], uint32_t
     }
 }
 
-// weight-gradient fragment of chunk c -> this CTA's slice (row-major [kd][256]); rw0: the fragment's first row
-__device__ __forceinline__ void bwd_wgrad_red(float* slice, const float (&wgr)[32], uint32_t rw0, int q, int c) {
+// The per-CTA weight-gradient slice is kept in FRAGMENT order: float4 (c, j, consumer thread) holds wgr[4j .. 4j+3] of
+// chunk c, i.e. the four accumulator values a consumer thread owns for every item of the launch, at float offset
+// ((8c + j) * kBCons + thread) * 4.  A warp's flush of one j is then one red.v4 over 512 contiguous bytes, four whole
+// L2 lines; row-major [kd][256], the same adds took two red.v2 that each touched eight lines.
+// lstm16_wgrad_reduce_kernel maps it back (wgrad_slice_row_col).
+constexpr int kWgrSliceFloats = kTileM * kGateCols;
+__device__ __forceinline__ void wgrad_slice_row_col(int e, int& m, int& n) {
+    const int v = e & 3, thr = (e >> 2) % kBCons, cj = (e >> 2) / kBCons;
+    const int lane = thr & 31, q = lane & 3;
+    m = 64 * (thr >> 7) + 16 * ((thr >> 5) & 3) + (lane >> 2) + 8 * (v >> 1);      // fragment rows rw0, rw0 + 8
+    n = 8 * cj + 2 * q + (v & 1);                                                     // 64 c + 8 j + 2 q + {0, 1}
+}
+// weight-gradient fragment of chunk c -> this CTA's slice; slice_t: the slice + 4 * (this consumer thread)
+__device__ __forceinline__ void bwd_wgrad_red(float* slice_t, const float (&wgr)[32], int c) {
+    float* dst = slice_t + (size_t)c * (8 * 4 * kBCons);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const uint32_t n = (uint32_t)(64 * c + 8 * j + 2 * q);
-        red_add_f32x2(slice + (size_t)rw0 * kGateCols + n, wgr[4 * j], wgr[4 * j + 1]);
-        red_add_f32x2(slice + (size_t)(rw0 + 8) * kGateCols + n, wgr[4 * j + 2], wgr[4 * j + 3]);
-    }
+    for (int j = 0; j < 8; ++j)
+        red_add_f32x4(dst + j * (4 * kBCons), wgr[4 * j], wgr[4 * j + 1], wgr[4 * j + 2], wgr[4 * j + 3]);
 }
 
 // CIN: see lstm16_fwd_kernel.  WGRAD = false: the variant for a caller that wants no weight gradients -- the schedule
@@ -712,7 +722,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
     const uint32_t w_u = smem_u32(w_sm), a_u = smem_u32(a_sm), da_u = smem_u32(da_sm);
     const uint32_t a_rows = (uint32_t)wg * 64u * 128u;             // this warpgroup's rows inside a 128-row tile
     const uint32_t wa_u = a_u + (uint32_t)(wg * 2) * kATileBytes;  // W_c's A operand: this warpgroup's kd rows
-    float* slice = WGRAD ? p.dw_slice + (size_t)blockIdx.x * (kTileM * kGateCols) : nullptr;
+    float* slice_t = WGRAD ? p.dw_slice + (size_t)blockIdx.x * kWgrSliceFloats + 4 * tid : nullptr;
     mbar_wait_raw(&tail->w_full, 0);
 
     for (int w = 0; w < n_items; ++w) {
@@ -854,7 +864,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
             wg_wait<0>();
             if constexpr (WGRAD) wg_fence_regs(wgr);
             wg_fence_regs(dacc);
-            if constexpr (WGRAD) bwd_wgrad_red(slice, wgr, rw0, q, c - 1);
+            if constexpr (WGRAD) bwd_wgrad_red(slice_t, wgr, c - 1);
             store_da();
         }
         // ---- chunk 3's gradients: W_3 alone first, so that the A planes go back to the producer before D_3 is done ----
@@ -870,7 +880,7 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
         // the A planes of this item have been read by every MMA: one arrival per warpgroup
         bar_sync(kBBarWg + wg, 128);
         if ((tid & 127) == 0) mbar_arrive(&tail->a_empty);
-        if constexpr (WGRAD) bwd_wgrad_red(slice, wgr, rw0, q, 3);
+        if constexpr (WGRAD) bwd_wgrad_red(slice_t, wgr, 3);
         wg_wait<0>();
         wg_fence_regs(dacc);
         // ---- [dx_below | dh_prev] fragment -> tile-blocked workspaces ----
@@ -914,16 +924,17 @@ __global__ void __launch_bounds__(kBThreads, 1) lstm16_bwd_kernel(const __grid_c
 
 // Sum the per-CTA weight-gradient slices of one layer and write nn.LSTM-native gradients:
 //   d_w_ih (256, in), d_w_hh (256, 64), d_b_ih = d_b_hh (256); native row of gate-interleaved column n: (n & 3) * 64 + (n >> 2).
-// Slice row m = kd index: layers > 0: m < 64 -> W_ih[:, m], m >= 64 -> W_hh[:, m - 64]; layer 0: m < 64 -> W_hh[:, m],
-// m = 64 + c -> W_ih[:, c].
+// Slice element e holds kd row m, gate column n (wgrad_slice_row_col): layers > 0: m < 64 -> W_ih[:, m], m >= 64 ->
+// W_hh[:, m - 64]; layer 0: m < 64 -> W_hh[:, m], m = 64 + c -> W_ih[:, c].
 __global__ void lstm16_wgrad_reduce_kernel(const float* __restrict__ slices, int n_slices, int layer, int c_in,
                                            const float* __restrict__ dbp, float* __restrict__ d_w_ih,
                                            float* __restrict__ d_w_hh, float* __restrict__ d_b_ih, float* __restrict__ d_b_hh) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;           // index in the slice layout
-    if (e < kTileM * kGateCols) {
+    if (e < kWgrSliceFloats) {
         float s = 0.f;
-        for (int i = 0; i < n_slices; ++i) s += slices[(size_t)i * (kTileM * kGateCols) + e];
-        const int m = e / kGateCols, n = e % kGateCols;
+        for (int i = 0; i < n_slices; ++i) s += slices[(size_t)i * kWgrSliceFloats + e];
+        int m, n;
+        wgrad_slice_row_col(e, m, n);
         const int nat = (n & 3) * kHid + (n >> 2);
         if (layer > 0) {
             if (m < 64) d_w_ih[(size_t)nat * kHid + m] = s;
@@ -1149,7 +1160,7 @@ extern "C" int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t
             sp.dx_out = l > 0 ? dx_out + (int64_t)t * cslice : nullptr;
         }
         // every CTA adds into its own slice: start from zero
-        if (wgrad) STMGCN_CUDA(cudaMemsetAsync(dw_scratch, 0, (size_t)grid * kTileM * kGateCols * sizeof(float), st));
+        if (wgrad) STMGCN_CUDA(cudaMemsetAsync(dw_scratch, 0, (size_t)grid * kWgrSliceFloats * sizeof(float), st));
         fn<<<grid, kBThreads, kBSmem, st>>>(p);
         count_launch();
         if (int32_t rc = check_launch("lstm16_bwd")) return rc;
@@ -1162,9 +1173,9 @@ extern "C" int32_t stmgcn_lstm16_bwd_ex(int32_t t_len, int32_t n_layers, int64_t
         // reuses dw_scratch
         const int in_l = l == 0 ? c_in : kHid;
         float* g = grads + (l == 0 ? 0 : (int64_t)kGateCols * (c_in + kHid + 2 + (l - 1) * (2 * kHid + 2)));
-        lstm16_wgrad_reduce_kernel<<<(kTileM * kGateCols) / 256, 256, 0, st>>>(dw_scratch, grid, l, c_in, p.dbp, g, g + kGateCols * in_l,
-                                                                               g + kGateCols * (in_l + kHid),
-                                                                               g + kGateCols * (in_l + kHid + 1));
+        lstm16_wgrad_reduce_kernel<<<kWgrSliceFloats / 256, 256, 0, st>>>(dw_scratch, grid, l, c_in, p.dbp, g, g + kGateCols * in_l,
+                                                                          g + kGateCols * (in_l + kHid),
+                                                                          g + kGateCols * (in_l + kHid + 1));
         count_launch();
         if (int32_t rc = check_launch("lstm16_wgrad_reduce")) return rc;
     }

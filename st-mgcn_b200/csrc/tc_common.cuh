@@ -123,9 +123,9 @@ __device__ __forceinline__ bool elect_one_sync() {
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-// fire-and-forget 8-byte reduction into global memory (the add happens in L2, nothing returns)
-__device__ __forceinline__ void red_add_f32x2(float* dst, float a, float b) {
-    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
+// fire-and-forget 16-byte reduction into global memory (the add happens in L2, nothing returns); dst 16-byte aligned
+__device__ __forceinline__ void red_add_f32x4(float* dst, float a, float b, float c, float d) {
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 // L2 prefetch of a contiguous global range (no registers, no shared memory)
 __device__ __forceinline__ void prefetch_l2(const void* gmem, uint32_t bytes) {
