@@ -619,7 +619,7 @@ class BF16ModeReference:
     ``relu``: ReLU after both GCNs (else no activation); ``relu_masks`` as for :class:`SparseOracle` (boolean
     ``(N, B, q)`` arrays or tensors, order temporal 0, spatial 0, temporal 1, ...): ``out = z * mask``.
 
-    ``tapes`` (optional, per graph): the kernels' values at every rounding point, in this model's dtype, rows
+    ``tapes`` (optional, per graph): the kernels' values at every rounding point, in any precision, rows
     ``r = n*B + b`` of the windows this model is given -- ``h``, ``c`` (L, T, R, H) and ``h0`` (L, R, H) as
     :func:`lstm_planes_reference` takes them, and ``s`` (Ks, N, B, H): the spatial stack, ``s[0]`` the fp32 h_top.
     Every operand of the spatial recurrence, and every stack term the projection reads, then takes the tape's value with
@@ -718,9 +718,10 @@ class BF16ModeReference:
         every rounding point -- ``hs`` / ``cs`` (per layer, per step) and ``stack`` (spatial S_k, (N, B*H) each).
 
         ``windows`` (a slice, optional): xo holds only these windows of the batch that ``relu_masks`` and ``tape``
-        describe; the masks and the tape are sliced to them."""
-        if tape is not None and windows is not None:
-            tape = _tape_windows(tape, xo.shape[0], windows)
+        describe; the masks and the tape are sliced to them.  The tape may be in any precision (the kernels' own: h in
+        bf16, c and s in fp32): only the slice taken is cast to this model's dtype."""
+        if tape is not None:
+            tape = _tape_windows(tape, xo.shape[0], slice(None) if windows is None else windows, self.dt)
         h_top, _, _, (hs, cs) = self.cg_lstm_node_major(p, m, xo, tape, windows=windows)
         g, stack = self._gcn(m, h_top, p[f"gcn_list.{m}.W"], p.get(f"gcn_list.{m}.b"), 2 * m + 1, True,
                              None if tape is None else tape["s"], windows)
@@ -735,7 +736,9 @@ class BF16ModeReference:
     def loss_and_grads(self, obs, y, tapes=None, want_obs: bool = False, on_branch=None, window_chunk=None):
         """MSE(mean) loss and the gradient of every parameter (and of obs with ``want_obs``), one graph branch in memory
         at a time: the branches' outputs first (no autograd), then the fusion's gradient, then each branch's backward.
-        ``on_branch(m, branch dict)`` (optional) sees each branch's forward values.  Returns (out, loss, grads).
+        ``on_branch(m, branch dict)`` (optional) sees each branch's forward values, once per chunk with ``window_chunk``;
+        ``branch["windows"]`` is the slice of the batch they belong to (all of it without chunks).  Returns (out, loss,
+        grads).
 
         ``window_chunk`` (optional): each branch's forward and backward run on ``window_chunk`` windows at a time (the
         last chunk may be shorter), so the autograd tape held at once is that of one chunk of one branch.  Windows are
@@ -750,8 +753,6 @@ class BF16ModeReference:
         else:
             if window_chunk < 1:
                 raise ValueError(f"window_chunk must be at least 1, got {window_chunk}")
-            if on_branch is not None:
-                raise ValueError("on_branch sees whole-batch branch values: it does not combine with window_chunk")
             wins = [slice(i, min(i + window_chunk, bsz)) for i in range(0, bsz, window_chunk)]
         p = self.leaves()
         xo = obs.permute(2, 0, 1, 3)
@@ -762,6 +763,7 @@ class BF16ModeReference:
                 for win in wins:
                     br = self.branch(p, m, xo if win is None else xo[:, win], None if tapes is None else tapes[m], win)
                     if on_branch is not None:
+                        br["windows"] = slice(0, bsz) if win is None else win
                         on_branch(m, br)
                     parts.append(br["out"])
                     del br
@@ -790,15 +792,17 @@ class BF16ModeReference:
         return out.detach(), loss.detach(), grads
 
 
-def _tape_windows(tape, n, windows):
-    """A :class:`BF16ModeReference` tape (rows ``r = n*B + b``) cut to the windows ``windows`` (a slice of the B)."""
+def _tape_windows(tape, n, windows, dtype=None):
+    """A :class:`BF16ModeReference` tape (rows ``r = n*B + b``) cut to the windows ``windows`` (a slice of the B), in
+    ``dtype`` (given): a tape kept in the kernels' precision is widened one slice at a time."""
     def rows(v, axis):                  # (..., N*B, ...) -> (..., N*len(windows), ...)
         shape = v.shape
         v = v.reshape(shape[:axis] + (n, shape[axis] // n) + shape[axis + 1:])
         v = v[(slice(None),) * (axis + 1) + (windows,)]
         return v.reshape(shape[:axis] + (-1,) + shape[axis + 1:])
     row_axis = {"h": 2, "c": 2, "h0": 1}          # h, c (L, T, R, H); h0 (L, R, H); s (Ks, N, B, H)
-    return {k: v[:, :, windows] if k == "s" else rows(v, row_axis[k]) for k, v in tape.items()}
+    cut = {k: v[:, :, windows] if k == "s" else rows(v, row_axis[k]) for k, v in tape.items()}
+    return cut if dtype is None else {k: v.to(dtype) for k, v in cut.items()}
 
 
 def laplacian_csr_from_supports(supports: torch.Tensor):

@@ -13,6 +13,9 @@ pre-activation within rounding distance of the kink follows the same branch in b
 
 Diagnostic (printed, not asserted): the same reference in fp32 (no TF32), i.e. what fp32 arithmetic of this model gets
 at this size, next to the kernels' error of every gradient.
+
+The bf16-arithmetic mode is checked by :func:`run_forced`: the reference rounds where the kernels round and is forced
+with the step's own values at every rounding point, recorded for every row of the batch.
 """
 import time
 
@@ -22,6 +25,8 @@ from torch import nn
 
 import stmgcn_oracle as O
 from helpers import DEV, rel_err
+from lstm_cases import step_local_error
+from model_cases import FullBatchRecorder
 from per_step import per_step_rel_err, worst_step
 
 
@@ -129,6 +134,77 @@ def run(label, model, sups, params, chains, ks, x, y, *, relu, window_chunk, wan
     for got in steps:
         assert bool(torch.isfinite(got["out"]).all())
     return {k: max(e[k] for e in step_errs) for k in step_errs[0]}
+
+
+def _windows_rolled(tape, n, shift):
+    """``tape`` with window b holding the recording of window (b + shift) mod B (rows ``n*B + b``)."""
+    def roll(v, axis):
+        shape = v.shape
+        v = v.reshape(shape[:axis] + (n, shape[axis] // n) + shape[axis + 1:])
+        return torch.roll(v, -shift, axis + 1).reshape(shape)
+    return {k: torch.roll(v, -shift, 2) if k == "s" else roll(v, 1 if k == "h0" else 2) for k, v in tape.items()}
+
+
+def run_forced(label, model, sups, params, chains, ks, x, y, *, relu, window_chunk, want_obs=False, window_offset=0):
+    """The bf16-arithmetic mode on the full batch: one GPU step, every window with its true target, recorded for every
+    row (:class:`FullBatchRecorder`), against :class:`O.BF16ModeReference` forced with that recording and the step's
+    ReLU masks, ``window_chunk`` windows at a time.  The recording stays in the kernels' precision; each chunk's slice is
+    widened to fp64 only when the reference reaches it.
+
+    Returns (step-local errors: every LSTM layer-step and h_top of each graph, every spatial S_k, each the worst over
+    the chunks; whole-model errors as :func:`_errors`; the worst whole-model error of the same step against the
+    unrounded reference, which says the single-plane arithmetic ran).  Prints them with the peak memory and wall time.
+
+    ``window_offset`` (negative controls only): the reference for window b is forced with window b + offset's
+    recording."""
+    n = x.shape[2]
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    t0 = time.perf_counter()
+    with FullBatchRecorder() as rec:
+        got = gpu_step(model, sups, x, y, want_obs, keep_masks=relu)
+    rec.check_intact()
+    assert len(rec.lstm) == len(rec.stacks) == len(chains), "a graph branch ran without the bf16 mode's LSTM or stack"
+    tapes = rec.take_tapes()
+    if window_offset:
+        tapes = [_windows_rolled(t, n, window_offset) for t in tapes]
+    torch.cuda.synchronize()
+    t1 = time.perf_counter()
+    ref = O.BF16ModeReference(params, chains, ks, relu=relu, relu_masks=got["masks"] if relu else None, device=DEV)
+    step = {}
+
+    def worst(key, v):
+        step[key] = float(np.maximum(step.get(key, 0.0), v))          # NaN stays NaN
+
+    def on_branch(m, br):
+        tape = O._tape_windows(tapes[m], n, br["windows"], torch.float64)
+        worst(f"g{m} LSTM layer-steps", step_local_error(tape, br["hs"], br["cs"], 1))
+        worst(f"g{m} h_top", rel_err(tape["s"][0].reshape(n, -1), br["hs"][-1][-1].reshape(n, -1)))
+        for k in range(1, ks):
+            worst(f"g{m} S_{k}", rel_err(tape["s"][k].reshape(n, -1), br["stack"][k]))
+    out, loss, grads = ref.loss_and_grads(x, y, tapes=tapes, want_obs=want_obs, on_branch=on_branch,
+                                          window_chunk=window_chunk)
+    errs = _errors(got, dict(out=out, loss=float(loss), grads=grads), want_obs)
+    del ref, tapes, out, grads
+    torch.cuda.empty_cache()
+    torch.cuda.synchronize()
+    t2 = time.perf_counter()
+    unrounded = max(_errors(got, reference(params, chains, ks, x, y, relu, got["masks"], window_chunk, want_obs),
+                            want_obs).values())
+    torch.cuda.synchronize()
+    t3 = time.perf_counter()
+    peak = torch.cuda.max_memory_allocated() / 2 ** 30
+    lines = [f"{label}: B={x.shape[0]} relu={relu}, every window against the forced fp64 reference in chunks of "
+             f"{window_chunk}" + (f", tapes {window_offset} window(s) off" if window_offset else ""),
+             f"  step-local worst {max(step.values()):.2e}; whole model worst {max(errs.values()):.2e}; against the "
+             f"unrounded reference {unrounded:.2e}"]
+    for k, v in sorted({**step, **errs}.items(), key=lambda kv: -kv[1])[:8]:
+        lines.append(f"  {k:<44} {v:9.2e}")
+    lines.append(f"  peak memory {peak:.1f} GiB; wall time: GPU step and recording {t1 - t0:.1f} s, forced fp64 "
+                 f"reference {t2 - t1:.1f} s, unrounded reference {t3 - t2:.1f} s")
+    print("\n".join(lines))
+    assert bool(torch.isfinite(got["out"]).all())
+    return step, errs, unrounded
 
 
 def assert_within(errs, tol, what=""):

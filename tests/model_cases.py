@@ -1,6 +1,7 @@
 """Shared model-level cases: the benchmarked workloads with Chebyshev or diffusion supports, the small models of the
 input-gradient checks with their dense fp64 gradients, and the recording of the bf16-arithmetic mode's rounding points
 for its forced fp64 reference."""
+import pytest
 import scipy.sparse as sp
 import torch
 from torch import nn
@@ -12,7 +13,7 @@ from lstm_cases import step_local_error
 
 # windows per chunk of the fp64 reference: its autograd tape is ~1 GB per cfg3 window and graph branch, ~8 GB per cfg5
 # window (16 384 regions, T = 24)
-CHUNK = {"cfg2": 32, "cfg3": 16, "cfg5": 2}
+CHUNK = {"cfg2": 32, "cfg3": 16, "cfg4": 8, "cfg5": 2}
 
 
 def _csr_of(sup):
@@ -46,6 +47,117 @@ def directed_workload(name, batch):
         a[0, :] = 0.0
         a[:, 1] = 0.0
     return w, adjs
+
+
+def workload_case(name, batch, relu):
+    """Workload ``name`` with Chebyshev supports (:func:`cheb_workload`, inputs of seed 100) -> (model, supports, chains,
+    n_supports, params, x, y)."""
+    from stmgcn_b200 import synth
+    w = synth.WORKLOADS[name]
+    model, sups, laps, params, x, y = cheb_workload(w, batch, relu=relu)
+    return model, sups, [[lap] for lap in laps], w.n_supports, params, x, y
+
+
+def diffusion_case(batch, relu, order=2):
+    """cfg2 shapes on directed graphs with random_walk_diffusion supports: two chains per graph -> (model, supports,
+    chains, n_supports, params, x, y)."""
+    import GCN
+    import STMGCN
+    from stmgcn_b200 import synth
+    w, adjs = directed_workload("cfg2", batch)
+    sups_cpu = [GCN.Adj_Preprocessor("random_walk_diffusion", order).process_sparse(a) for a in adjs]
+    chains = [[sp.csr_matrix(m.numpy()) for m in h.matrices_dense()] for h in sups_cpu]
+    torch.manual_seed(0)
+    kw = synth.model_kwargs(w)
+    kw["sta_kernel_config"] = {"kernel_type": "random_walk_diffusion", "K": order}
+    if not relu:
+        kw["gconv_activation"] = None
+    model = STMGCN.ST_MGCN(**kw)
+    params = {k: v.detach().clone() for k, v in model.state_dict().items()}
+    x, y = synth.make_inputs(w, seed=100, batch=batch)
+    return model.to(DEV), [s.to(DEV) for s in sups_cpu], chains, 2 * order + 1, params, x, y
+
+
+@pytest.fixture
+def bf16_mode(monkeypatch):
+    """One-plane tensor-core LSTM and bf16 gather copies: the bf16-arithmetic mode."""
+    from stmgcn_b200 import ops
+    monkeypatch.setattr(ops, "_PLANES", 1)
+    monkeypatch.setattr(ops, "_LSTM_PATH", "tc")
+    return ops
+
+
+def _bits_sum(t):
+    """The sum of ``t``'s bit patterns as integers, on the device (no synchronisation): a write to any element moves
+    it, barring an exact cancellation."""
+    bits = t.reshape(-1).view({torch.bfloat16: torch.int16, torch.float32: torch.int32}[t.dtype])
+    return torch.stack([part.sum(dtype=torch.int64) for part in bits.split(1 << 26)]).sum()
+
+
+class FullBatchRecorder:
+    """Wraps ``ops`` for one training step and keeps, for every row, the kernels' values at the bf16 mode's rounding
+    points: per shared LSTM its tape (``hp``, ``cs``, ``h0p``), per spatial GCN its Chebyshev stack ``s`` (graph order).
+
+    These are the very tensors the step saves for its backward, held by reference in the kernels' precision, not
+    copied: the tensor-core LSTM backward only reads ``hp`` and ``cs`` (``const`` at the C ABI, so a second backward
+    over the same forward is allowed on that path), and ``ChebGCN.backward`` runs its adjoint Clenshaw in the
+    projection's fresh ``u``, not in ``s``.  :meth:`check_intact` holds the backward to that: it compares a checksum of
+    each tensor, taken as it was recorded, with one taken after the step."""
+
+    def __init__(self):
+        self.lstm, self.stacks, self.sums = [], [], []
+
+    def _keep(self, t):
+        self.sums.append((t, _bits_sum(t)))
+
+    def __enter__(self):
+        from stmgcn_b200 import ops
+        self.ops = ops
+        self.real = (ops._lstm16_forward, ops.build_stack)
+        real_lstm, real_stack = self.real
+
+        def lstm(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes, keep_tape):
+            res = real_lstm(xo, s_gate, h0c, c0c, n_layers, want_state, weights, planes, keep_tape)
+            tape = res[3]
+            assert tape is not None, "record the forward with autograd on"
+            rec = dict(hp=tape["hp"], cs=tape["cs"], h0p=tape["h0p"], rows=xo.shape[0] * xo.shape[1])
+            for key in ("hp", "cs", "h0p"):
+                if rec[key] is not None:
+                    self._keep(rec[key])
+            self.lstm.append(rec)
+            return res
+
+        def stack(sset, x, gather16=False):
+            s = real_stack(sset, x, gather16)
+            if gather16:                                # the spatial GCN (ChebGCN); the temporal one passes False
+                self._keep(s)
+                self.stacks.append(s)
+            return s
+
+        ops._lstm16_forward, ops.build_stack = lstm, stack
+        return self
+
+    def __exit__(self, *exc):
+        self.ops._lstm16_forward, self.ops.build_stack = self.real
+
+    def check_intact(self):
+        """Every recorded tensor holds what it held when recorded."""
+        for i, (t, before) in enumerate(self.sums):
+            assert torch.equal(_bits_sum(t), before), f"recorded tensor {i} {tuple(t.shape)} changed after it was taken"
+
+    def take_tapes(self):
+        """Per graph the tape :class:`O.BF16ModeReference` takes, still in the kernels' precision: ``h`` the one bf16
+        plane (L, T, R, 64), ``c`` fp32 unblocked (L, T, R, 64), ``h0`` (with an initial state) and ``s``.  The blocked
+        cell states are released as each branch's is unblocked, so the recording can be taken once."""
+        out = []
+        for rec, s in zip(self.lstm, self.stacks):
+            assert rec["hp"].shape[2] == 1, "the LSTM ran with two planes: not the bf16 mode"
+            tape = dict(h=rec.pop("hp")[:, :, 0], c=self.ops.from_blocked(rec.pop("cs"), rec["rows"]), s=s)
+            if rec["h0p"] is not None:
+                tape["h0"] = rec["h0p"][:, 0]
+            out.append(tape)
+        self.lstm, self.stacks, self.sums = [], [], []
+        return out
 
 
 class Recorder:

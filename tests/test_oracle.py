@@ -512,13 +512,66 @@ def test_bf16_mode_reference_in_window_chunks_slices_the_tapes():
     assert O.max_rel_err(out_s.numpy(), out.numpy()) > 1e-6
 
 
-def test_bf16_mode_reference_window_chunk_rejects_on_branch_and_bad_sizes():
+def test_bf16_mode_reference_window_chunk_rejects_bad_sizes():
     params, chains, ks, x, y = _bf16_case(14, b=2)
     ref = O.BF16ModeReference(params, chains, ks, rounding=False)
-    with pytest.raises(ValueError):
-        ref.loss_and_grads(x, y, window_chunk=0)
-    with pytest.raises(ValueError):
-        ref.loss_and_grads(x, y, window_chunk=1, on_branch=lambda m, br: None)
+    for bad in (0, -1):
+        with pytest.raises(ValueError):
+            ref.loss_and_grads(x, y, window_chunk=bad)
+
+
+def test_bf16_mode_reference_takes_tapes_in_kernel_precision():
+    """Tapes in the kernels' precision (h bf16, c and s fp32), whole-batch, are widened one chunk's slice at a time:
+    output, loss, every gradient and d obs are bit-identical to those of the same tapes given in fp64, unchunked, in
+    chunks of 1, in ragged chunks and in one whole-batch chunk."""
+    params, chains, ks, x, y = _bf16_case(15, hid=16, b=5)
+    ref = O.BF16ModeReference(params, chains, ks, relu=True)
+    native = [dict(h=t["h"].to(torch.bfloat16), c=t["c"].float(), s=t["s"].float()) for t in _own_tapes(ref, x)]
+    wide = [{k: v.double() for k, v in t.items()} for t in native]
+    for chunk in (None, 1, 2, 5):
+        out_n, loss_n, grads_n = ref.loss_and_grads(x, y, tapes=native, want_obs=True, window_chunk=chunk)
+        out_w, loss_w, grads_w = ref.loss_and_grads(x, y, tapes=wide, want_obs=True, window_chunk=chunk)
+        assert torch.equal(out_n, out_w) and torch.equal(loss_n, loss_w), f"chunk {chunk}"
+        assert set(grads_n) == set(grads_w)
+        for key in grads_w:
+            assert torch.equal(grads_n[key], grads_w[key]), f"chunk {chunk} grad {key}"
+
+
+def test_bf16_mode_reference_on_branch_per_chunk_is_the_whole_branch():
+    """``on_branch`` with ``window_chunk``: called once per chunk and branch, ``branch["windows"]`` that chunk's.  Each value it
+    sees (every LSTM layer-step's h and c, every spatial S_k, the branch output), put back together over the chunks,
+    equals the unchunked branch's value to fp64 rounding -- with chunks of 1, ragged chunks and one whole-batch chunk.
+    The model is forced with another model's tapes, so every chunk's values depend on it taking its own windows' rows."""
+    params, chains, ks, x, y = _bf16_case(16, hid=16, b=5, m=2)
+    params_other, chains_other, _, _, _ = _bf16_case(17, hid=16, b=5, m=2)
+    tapes = _own_tapes(O.BF16ModeReference(params_other, chains_other, ks, relu=True), x)
+    ref = O.BF16ModeReference(params, chains, ks, relu=True)
+    n, bsz = x.shape[2], x.shape[0]
+
+    def values(chunk):
+        seen = {m: [] for m in range(ref.m)}
+
+        def keep(m, br):
+            win = br["windows"]
+            nb = win.stop - win.start
+            lstm = [torch.stack([torch.stack(v) for v in br[k]]) for k in ("hs", "cs")]       # (L, T, N*nb, H)
+            seen[m].append((win, [v.reshape(*v.shape[:2], n, nb, -1) for v in lstm]
+                            + [torch.stack(br["stack"]).reshape(ks, n, nb, -1), br["out"]]))
+        ref.loss_and_grads(x, y, tapes=tapes, on_branch=keep, window_chunk=chunk)
+        out = {}
+        for m, parts in seen.items():
+            wins = [w for w, _ in parts]
+            assert [(w.start, w.stop) for w in wins] == [(i, min(i + (chunk or bsz), bsz))
+                                                        for i in range(0, bsz, chunk or bsz)], f"chunk {chunk}: {wins}"
+            # window axes: h and c (L, T, N, b, H) -> 3; S_k (Ks, N, b, H) -> 2; out (N, b, G) -> 1
+            out[m] = [torch.cat([v[i] for _, v in parts], dim=axis) for i, axis in enumerate((3, 3, 2, 1))]
+        return out
+    whole = values(None)
+    for chunk in (1, 2, bsz):
+        got = values(chunk)
+        for m in whole:
+            for name, a, b in zip(("h", "c", "S", "out"), got[m], whole[m]):
+                assert_close(a.detach().numpy(), b.detach().numpy(), f"chunk {chunk} branch {m} {name}", 1e-12)
 
 
 def _own_tapes(ref, x):
