@@ -78,6 +78,25 @@ int32_t stmgcn_cheb_spmm_step16(int64_t n, const int32_t* rowptr, const int32_t*
                                 float* y, void* y16, int64_t f_total, void* stream);
 int32_t stmgcn_to_bf16(const float* x, void* y16, int64_t count, void* stream);
 
+/* ---- K1b: gradient of a support's stored values (CSR SDDMM) ------------------------------------------
+ *   dvals[e] += sum_t coef[t] * < A_t[i, :], B_t[j, :] >   for every stored entry e = (i, j) of the CSR (rowptr, colidx),
+ * i the row that owns e and j = colidx[e]; nnz = rowptr[n] entries, dvals in the CSR's storage order (a repeated (i, j)
+ * gets the same value at each of its entries).  A_t, B_t: (N, f_total) fp32 row-major, nterms = 1..8 term pairs given as
+ * host arrays a[nterms], b[nterms] of device pointers and coef[nterms] of host floats.  Chebyshev chain X with
+ * T_1 = X T_0, T_k = 2 X T_{k-1} - T_{k-2}: A_t = G_k (the total adjoint dL/dT_k), B_t = T_{k-1}, coef 1 for k = 1 and 2
+ * otherwise; a generic support S = A x: one term, A_0 = dL/dS, B_0 = x.  round_b_bf16 = 1 rounds every B element to bf16
+ * (to nearest even) before the product: the operand stmgcn_cheb_spmm_step16 multiplied by.
+ * f_total % 4 == 0 takes the float4 kernel (every A_t and B_t 16-byte aligned, else STMGCN_ERR_ALIGN), any other width
+ * the scalar one.  Column tiles: tiles = ceil(f_total / 128) (float4) or ceil(f_total / 32) (scalar); with tiles > 1,
+ * work (tiles * nnz floats, work_count >= that) receives one partial per tile and entry and a second launch adds them
+ * to dvals in tile order; with tiles == 1 work may be NULL.  Every sum has one owner in a fixed order: two calls with
+ * the same inputs give bit-identical dvals.  A_t and B_t may alias one another.  dvals (nnz floats) and work (work_count
+ * floats) share no byte with any A_t / B_t (n * f_total floats each) or with each other: the byte ranges are checked.
+ * nnz == 0 enqueues nothing (colidx and dvals may then be NULL). */
+int32_t stmgcn_csr_sddmm(int64_t n, const int32_t* rowptr, const int32_t* colidx, int64_t nnz, int32_t nterms,
+                         const float* const* a, const float* const* b, const float* coef, int32_t round_b_bf16,
+                         int64_t f_total, float* work, int64_t work_count, float* dvals, void* stream);
+
 /* ---- layout: obs (B,T,N,C) -> node-major (STMGCN.py:36,39 sum over C + permute; :47 row order) ----
  * xo: (N,B,T,C) copy of obs;  xt: (N,B,T) = sum_c obs.  xo may be NULL when C == 1 (xt is then xo). */
 int32_t stmgcn_obs_to_node_major(const float* obs, float* xo, float* xt, int64_t b, int64_t t,

@@ -171,6 +171,134 @@ spmm_row_gather16_kernel(int64_t n, const int32_t* __restrict__ rowptr, const in
     }
 }
 
+// ---- K1b: CSR SDDMM, the gradient of a support's stored values ---------------------------------------------------
+//   dvals[e] += sum_t coef[t] * < A_t[row(e), :], B_t[colidx[e], :] >
+// The SpMM's gather, transposed: one warp owns one row x one column tile; lanes hold the row's own A_t run in registers
+// (one vector per term) and every entry gathers B_t[colidx[e]]'s run (one coalesced 512 B read per warp, as the forward's
+// X), then a fixed xor-tree warp sum.  Same column-tile-major grid as the SpMM (the resident CTAs share one column strip
+// of every B_t in L2).  Each (entry, tile) partial has one owner; with more than one tile the partials go to the caller's
+// workspace [tile][e] and a second pass adds them in tile order: no float atomics, two runs agree bit for bit.
+constexpr int kMaxSddmmTerms = 8;
+struct SddmmTerms {
+    const float* a[kMaxSddmmTerms];
+    const float* b[kMaxSddmmTerms];
+    float coef[kMaxSddmmTerms];
+};
+
+__device__ __forceinline__ float round_bf16(float v) {
+    return __uint_as_float(pack2_bf16(v, 0.f) << 16);
+}
+__device__ __forceinline__ float dot_vec(const float4& a, float4 b, bool rnd) {
+    if (rnd) {
+        b.x = round_bf16(b.x);
+        b.y = round_bf16(b.y);
+        b.z = round_bf16(b.z);
+        b.w = round_bf16(b.w);
+    }
+    return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.y, b.y, a.x * b.x)));
+}
+__device__ __forceinline__ float dot_vec(float a, float b, bool rnd) { return a * (rnd ? round_bf16(b) : b); }
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// out[e] = partial of entry e over this CTA's column tile (accumulate: out[e] += it, the single-tile case)
+template <int VEC, bool ROUND>
+__global__ void __launch_bounds__(kWarpsPerCta * 32)
+sddmm_row_gather_kernel(int64_t n, const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, int nterms,
+                        const SddmmTerms terms, int64_t f_total, float* __restrict__ out, int64_t tile_stride,
+                        bool accumulate) {
+    using V = typename VecT<VEC>::type;
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const int64_t f = ((int64_t)blockIdx.y * 32 + lane) * VEC;
+    const bool live = f < f_total;
+    float* __restrict__ dst = out + (int64_t)blockIdx.y * tile_stride;
+    const int64_t row0 = (int64_t)blockIdx.x * kRowsPerCta;
+    for (int r = warp; r < kRowsPerCta; r += kWarpsPerCta) {
+        const int64_t row = row0 + r;
+        if (row >= n) break;
+        const int32_t beg = rowptr[row], end = rowptr[row + 1];
+        if (beg == end) continue;
+        V a[kMaxSddmmTerms];
+#pragma unroll
+        for (int t = 0; t < kMaxSddmmTerms; ++t) {
+            a[t] = zero_vec((V*)nullptr);
+            if (t < nterms && live) a[t] = *reinterpret_cast<const V*>(terms.a[t] + row * f_total + f);
+        }
+        int32_t i = beg;
+        for (; i + 4 <= end; i += 4) {
+            const int64_t c0 = __ldg(colidx + i), c1 = __ldg(colidx + i + 1);
+            const int64_t c2 = __ldg(colidx + i + 2), c3 = __ldg(colidx + i + 3);
+            float p0 = 0.f, p1 = 0.f, p2 = 0.f, p3 = 0.f;
+            if (live) {
+#pragma unroll
+                for (int t = 0; t < kMaxSddmmTerms; ++t) {
+                    if (t >= nterms) break;
+                    const float* __restrict__ b = terms.b[t] + f;
+                    const V b0 = *reinterpret_cast<const V*>(b + c0 * f_total);
+                    const V b1 = *reinterpret_cast<const V*>(b + c1 * f_total);
+                    const V b2 = *reinterpret_cast<const V*>(b + c2 * f_total);
+                    const V b3 = *reinterpret_cast<const V*>(b + c3 * f_total);
+                    const float cf = terms.coef[t];
+                    p0 = fmaf(cf, dot_vec(a[t], b0, ROUND), p0);
+                    p1 = fmaf(cf, dot_vec(a[t], b1, ROUND), p1);
+                    p2 = fmaf(cf, dot_vec(a[t], b2, ROUND), p2);
+                    p3 = fmaf(cf, dot_vec(a[t], b3, ROUND), p3);
+                }
+            }
+            p0 = warp_sum(p0);
+            p1 = warp_sum(p1);
+            p2 = warp_sum(p2);
+            p3 = warp_sum(p3);
+            if (lane == 0) {
+                if (accumulate) {
+                    dst[i] += p0;
+                    dst[i + 1] += p1;
+                    dst[i + 2] += p2;
+                    dst[i + 3] += p3;
+                } else {
+                    dst[i] = p0;
+                    dst[i + 1] = p1;
+                    dst[i + 2] = p2;
+                    dst[i + 3] = p3;
+                }
+            }
+        }
+        for (; i < end; ++i) {
+            const int64_t c0 = __ldg(colidx + i);
+            float p0 = 0.f;
+            if (live) {
+#pragma unroll
+                for (int t = 0; t < kMaxSddmmTerms; ++t) {
+                    if (t >= nterms) break;
+                    const V b0 = *reinterpret_cast<const V*>(terms.b[t] + c0 * f_total + f);
+                    p0 = fmaf(terms.coef[t], dot_vec(a[t], b0, ROUND), p0);
+                }
+            }
+            p0 = warp_sum(p0);
+            if (lane == 0) {
+                if (accumulate)
+                    dst[i] += p0;
+                else
+                    dst[i] = p0;
+            }
+        }
+    }
+}
+
+// second pass: dvals[e] += sum over tiles, in tile order
+__global__ void sddmm_tiles_sum_kernel(const float* __restrict__ work, int64_t tiles, int64_t nnz,
+                                       float* __restrict__ dvals) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x) {
+        float s = work[e];
+        for (int64_t t = 1; t < tiles; ++t) s += work[t * nnz + e];
+        dvals[e] += s;
+    }
+}
+
 __global__ void to_bf16_kernel(const float* __restrict__ x, uint16_t* __restrict__ y, int64_t n8) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (int64_t)gridDim.x * blockDim.x) {
         const float4 a = *reinterpret_cast<const float4*>(x + 8 * i), b = *reinterpret_cast<const float4*>(x + 8 * i + 4);
@@ -209,6 +337,77 @@ extern "C" int32_t stmgcn_cheb_spmm_step16(int64_t n, const int32_t* rowptr, con
                                                                                 beta, z, gamma, u, y, (uint16_t*)y16, f_total);
     count_launch();
     return check_launch("cheb_spmm_step16");
+}
+
+// whether the byte ranges [p, p + pb) and [q, q + qb) share a byte (a NULL or empty range shares none)
+static bool overlaps(const void* p, int64_t pb, const void* q, int64_t qb) {
+    if (p == nullptr || q == nullptr || pb <= 0 || qb <= 0) return false;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
+    return a < b + (uintptr_t)qb && b < a + (uintptr_t)pb;
+}
+
+extern "C" int32_t stmgcn_csr_sddmm(int64_t n, const int32_t* rowptr, const int32_t* colidx, int64_t nnz, int32_t nterms,
+                                    const float* const* a, const float* const* b, const float* coef,
+                                    int32_t round_b_bf16, int64_t f_total, float* work, int64_t work_count,
+                                    float* dvals, void* stream) {
+    STMGCN_REQUIRE(rowptr && a && b && coef, STMGCN_ERR_ARG, "csr_sddmm: null pointer");
+    STMGCN_REQUIRE(n > 0 && nnz >= 0 && nnz < ((int64_t)1 << 31), STMGCN_ERR_SHAPE, "csr_sddmm: n=%lld nnz=%lld",
+                   (long long)n, (long long)nnz);
+    STMGCN_REQUIRE(nnz == 0 || (colidx && dvals), STMGCN_ERR_ARG, "csr_sddmm: colidx / dvals null with nnz=%lld",
+                   (long long)nnz);
+    STMGCN_REQUIRE(nterms >= 1 && nterms <= kMaxSddmmTerms, STMGCN_ERR_SHAPE, "csr_sddmm: nterms=%d (1..%d)", (int)nterms,
+                   kMaxSddmmTerms);
+    STMGCN_REQUIRE(f_total > 0, STMGCN_ERR_SHAPE, "csr_sddmm: f_total=%lld", (long long)f_total);
+    STMGCN_REQUIRE(round_b_bf16 == 0 || round_b_bf16 == 1, STMGCN_ERR_ARG, "csr_sddmm: round_b_bf16=%d", (int)round_b_bf16);
+    const bool vec4 = f_total % 4 == 0;
+    SddmmTerms terms{};
+    for (int t = 0; t < nterms; ++t) {
+        STMGCN_REQUIRE(a[t] && b[t], STMGCN_ERR_ARG, "csr_sddmm: null operand of term %d", t);
+        STMGCN_REQUIRE(!vec4 || (aligned16(a[t]) && aligned16(b[t])), STMGCN_ERR_ALIGN,
+                       "csr_sddmm: f_total=%lld is a multiple of 4: the operands of term %d must be 16-byte aligned",
+                       (long long)f_total, t);
+        const int64_t op_bytes = n * f_total * 4;
+        STMGCN_REQUIRE(!overlaps(a[t], op_bytes, dvals, nnz * 4) && !overlaps(b[t], op_bytes, dvals, nnz * 4) &&
+                           !overlaps(a[t], op_bytes, work, work_count * 4) && !overlaps(b[t], op_bytes, work, work_count * 4),
+                       STMGCN_ERR_ARG, "csr_sddmm: dvals / work must not overlap the operands of term %d", t);
+        terms.a[t] = a[t];
+        terms.b[t] = b[t];
+        terms.coef[t] = coef[t];
+    }
+    const int64_t tiles = ceil_div(f_total, 32 * (vec4 ? 4 : 1));
+    STMGCN_REQUIRE(tiles <= 65535, STMGCN_ERR_SHAPE, "csr_sddmm: f_total=%lld too wide", (long long)f_total);
+    STMGCN_REQUIRE(tiles == 1 || nnz == 0 || (work && work_count >= tiles * nnz && !overlaps(work, work_count * 4, dvals, nnz * 4)),
+                   STMGCN_ERR_ARG,
+                   "csr_sddmm: %lld column tiles need a workspace of %lld floats distinct from dvals (work_count=%lld)",
+                   (long long)tiles, (long long)(tiles * nnz), (long long)work_count);
+    if (nnz == 0) return 0;             // no entry, nothing to add: nothing is enqueued
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool one = tiles == 1;
+    float* out = one ? dvals : work;
+    const int64_t stride = one ? 0 : nnz;
+    dim3 grid((unsigned)ceil_div(n, kRowsPerCta), (unsigned)tiles);
+    const int blk = kWarpsPerCta * 32;
+    if (vec4) {
+        if (round_b_bf16)
+            sddmm_row_gather_kernel<4, true><<<grid, blk, 0, st>>>(n, rowptr, colidx, nterms, terms, f_total, out, stride, one);
+        else
+            sddmm_row_gather_kernel<4, false><<<grid, blk, 0, st>>>(n, rowptr, colidx, nterms, terms, f_total, out, stride, one);
+    } else {
+        if (round_b_bf16)
+            sddmm_row_gather_kernel<1, true><<<grid, blk, 0, st>>>(n, rowptr, colidx, nterms, terms, f_total, out, stride, one);
+        else
+            sddmm_row_gather_kernel<1, false><<<grid, blk, 0, st>>>(n, rowptr, colidx, nterms, terms, f_total, out, stride, one);
+    }
+    count_launch();
+    if (!one) {
+        int32_t rc = check_launch("csr_sddmm");
+        if (rc != 0) return rc;
+        const int64_t cap = (int64_t)sm_count() * 8;
+        const int blocks = (int)(ceil_div(nnz, 256) < cap ? ceil_div(nnz, 256) : cap);
+        sddmm_tiles_sum_kernel<<<blocks, 256, 0, st>>>(work, tiles, nnz, dvals);
+        count_launch();
+    }
+    return check_launch("csr_sddmm");
 }
 
 extern "C" int32_t stmgcn_cheb_spmm_step(int64_t n, const int32_t* rowptr, const int32_t* colidx, const float* vals,

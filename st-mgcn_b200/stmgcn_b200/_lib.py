@@ -26,6 +26,8 @@ SIGNATURES = [
     ("stmgcn_cheb_spmm_step16", c_int32, [c_int64, _P, _P, _P, c_float, _P, c_float, _P, c_float, _P, _P, _P, c_int64,
                                           _P]),
     ("stmgcn_to_bf16", c_int32, [_P, _P, c_int64, _P]),
+    ("stmgcn_csr_sddmm", c_int32, [c_int64, _P, _P, c_int64, c_int32, POINTER(c_void_p), POINTER(c_void_p),
+                                   POINTER(c_float), c_int32, c_int64, _P, c_int64, _P, _P]),
     ("stmgcn_obs_to_node_major", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),
     ("stmgcn_obs_grad", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),
     ("stmgcn_proj_fwd", c_int32, [_P, c_int64, c_int32, c_int64, c_int32, _P, _P, c_int32, c_int32, _P, _P,
@@ -87,6 +89,11 @@ def ptr_array(ptrs):
     for i, p in enumerate(ptrs):
         arr[i] = p
     return arr
+
+
+def float_array(vals):
+    """Host array of floats for ``const float*`` parameters read on the host."""
+    return (c_float * len(vals))(*vals)
 
 
 def launch_count() -> int:

@@ -73,6 +73,16 @@ class GraphHandle:
         # CSR^T: the entries in column-major order (stable: repeated (row, col) entries keep their order)
         order = torch.argsort(cols * n + rows, stable=True)
         self._csr = (csr_from_coo(n, rows, cols, vals), csr_from_coo(n, cols[order], rows[order], vals[order]))
+        self._order = order
+
+    def with_values(self, vals: torch.Tensor) -> "GraphHandle":
+        """The same structure (shared index tensors) with the values ``vals``, given in this handle's CSR entry order
+        (a CSR source's storage order), copied -- the matrix a learnable support has at one forward."""
+        new = copy.copy(self)
+        v = vals.detach().to(torch.float32, copy=True).contiguous()
+        (rp, ci, _), (rpt, cit, _) = self._csr
+        new._csr = ((rp, ci, v), (rpt, cit, v[self._order]))
+        return new
 
     @classmethod
     def from_dense(cls, mat: torch.Tensor) -> "GraphHandle":
@@ -102,12 +112,25 @@ class SupportSet:
     ``"cheb"``: ``graphs`` are the recurrence matrices ``X_c`` of chains that share ``T_0 = I``; chain ``c`` owns the
     segments ``1 + cK .. (c+1)K``, ``T_k(X_c)`` with ``K = (Ks - 1) / len(graphs)`` (no graph when ``Ks == 1``).
     ``"generic"``: ``graphs[k]`` is ``A_k``.
+
+    ``values`` (optional): the source tensors of the graphs' stored values, one per graph in CSR entry order, when some
+    of them require grad (a learnable :class:`SparseSupports`).  The graphs hold detached copies; the graph
+    convolutions take these tensors as inputs, so their gradients reach them.
     """
 
-    def __init__(self, mode: str, n: int, ks: int, graphs: List[GraphHandle], device: torch.device):
+    def __init__(self, mode: str, n: int, ks: int, graphs: List[GraphHandle], device: torch.device,
+                 values: Optional[List[torch.Tensor]] = None):
         assert mode in ("cheb", "generic")
         assert len(graphs) == ks if mode == "generic" else (ks - 1) % max(len(graphs), 1) == 0 and (ks == 1) == (not graphs)
+        assert values is None or len(values) == len(graphs)
         self.mode, self.n, self.ks, self.graphs, self.device = mode, n, ks, graphs, device
+        self.values = values
+
+    def grad_values(self) -> tuple:
+        """The value tensors the graph convolutions take as inputs: ``values`` when one of them requires grad, else ()."""
+        if self.values is not None and any(v.requires_grad for v in self.values):
+            return tuple(self.values)
+        return ()
 
     @property
     def order(self) -> int:
@@ -209,6 +232,8 @@ class SparseSupports:
         self.mats = [(rp.to(torch.int32), ci.to(torch.int32), v.float()) for rp, ci, v in mats]
         self._sset: Optional[SupportSet] = None
         self._sset_version: tuple = ()
+        self._structure: Optional[List[GraphHandle]] = None
+        self._structure_key: tuple = ()
 
     @property
     def shape(self):
@@ -232,6 +257,7 @@ class SparseSupports:
         moved = copy.copy(self)
         moved.mats = [tuple(t.to(device) for t in m) for m in self.mats]
         moved._sset = None
+        moved._structure = None
         return moved
 
     def cuda(self, device=None):
@@ -241,9 +267,21 @@ class SparseSupports:
         """Identity and in-place version of every stored tensor: changes with any edit through a torch op."""
         return tuple((t.data_ptr(), t._version) for m in self.mats for t in m)
 
+    @property
+    def requires_grad(self) -> bool:
+        """Whether some stored values require grad (learnable edge weights on the fixed sparsity pattern)."""
+        return any(v.requires_grad for _, _, v in self.mats)
+
     def support_set(self) -> SupportSet:
         """The kernels' copy of the stored matrices, built again whenever :meth:`version` has changed since the last
-        build (as :func:`supports_from_dense` does for a dense stack)."""
+        build (as :func:`supports_from_dense` does for a dense stack).
+
+        With values that require grad the structure (CSR and CSR^T indices, the transpose's permutation) is cached on the
+        index tensors only, and the values are copied again on every call: an optimizer may change them without a
+        version bump (fused optimizers, ``.data`` writes), and each forward must multiply by the values it differentiates
+        at.  The returned set carries the value tensors (:attr:`SupportSet.values`)."""
+        if self.requires_grad:
+            return self._learnable_support_set()
         version = self.version()
         if self._sset is None or self._sset_version != version:
             if not self.is_cuda:
@@ -254,9 +292,22 @@ class SparseSupports:
             self._sset_version = version
         return self._sset
 
+    def _learnable_support_set(self) -> SupportSet:
+        if not self.is_cuda:
+            raise RuntimeError(f"{type(self).__name__} must be moved to a CUDA device before use (.to(device))")
+        # a one-support Chebyshev stack ([I], K = 0) multiplies by no matrix: its values are not an input of any
+        # convolution and their .grad stays None, as for any tensor the loss does not use
+        mats = self.mats if self.mode == "generic" or self.ks > 1 else []
+        key = tuple((rp.data_ptr(), rp._version, ci.data_ptr(), ci._version, v.numel()) for rp, ci, v in mats)
+        if self._structure is None or self._structure_key != key:
+            self._structure = [GraphHandle.from_csr(self.n, rp, ci, v.detach()) for rp, ci, v in mats]
+            self._structure_key = key
+        graphs = [h.with_values(v) for h, (_, _, v) in zip(self._structure, mats)]
+        return SupportSet(self.mode, self.n, self.ks, graphs, self.device, values=[v for _, _, v in mats])
+
     def matrices_dense(self) -> List[torch.Tensor]:
         """The stored matrices as dense ``(N, N)`` tensors (tests / small graphs only)."""
-        return [torch.sparse_csr_tensor(rp.long(), ci.long(), v, size=(self.n, self.n)).to_dense()
+        return [torch.sparse_csr_tensor(rp.long(), ci.long(), v.detach(), size=(self.n, self.n)).to_dense()
                 for rp, ci, v in self.mats]
 
 

@@ -12,6 +12,8 @@ Gradients are accumulated into ``GradBucket`` views (static addresses).  The opt
 The supports are baked in too: the graph reads the CSR tensors of the support sets converted at capture.  The step holds
 those sets (so their memory stays valid whatever happens to the conversion cache) and the supports' versions
 (``graph.support_version``); a call after any support was edited raises instead of replaying the old supports.
+Learnable supports (a ``SparseSupports`` whose values require grad) are refused at construction: their values are read
+again at every forward, which a replayed graph cannot do.
 """
 from __future__ import annotations
 
@@ -20,13 +22,17 @@ from typing import Callable, Optional, Sequence
 import torch
 
 from .dp import GradBucket
-from .graph import support_version, supports_from_dense
+from .graph import SparseSupports, support_version, supports_from_dense
 
 
 class GraphedStep:
     def __init__(self, model: torch.nn.Module, criterion: Callable, x: torch.Tensor, y: torch.Tensor,
                  supports: Sequence, bucket: Optional[GradBucket] = None, all_reduce: bool = False,
                  warmup: int = 3):
+        learnable = [m for m, s in enumerate(supports) if isinstance(s, SparseSupports) and s.requires_grad]
+        if learnable:
+            raise ValueError(f"GraphedStep: supports {learnable} have values that require grad; a captured step replays "
+                             f"the values of capture time, so learnable supports run eagerly")
         self.model, self.criterion, self.supports = model, criterion, list(supports)
         self.bucket = bucket if bucket is not None else GradBucket(model)
         self.all_reduce = all_reduce

@@ -58,7 +58,7 @@ class GCN(nn.Module):
         """x (N,B,p) node-major -> (N,B,hidden) node-major (internal fast path, no permutes)."""
         code = _act_code(self.activation)
         bias = self.b if self.bias else None
-        out = ops.ChebGCN.apply(x_nm, self.W, bias, sset, _lib.ACT_NONE if code is None else code)
+        out = ops.ChebGCN.apply(x_nm, self.W, bias, sset, _lib.ACT_NONE if code is None else code, *sset.grad_values())
         return self.activation(out) if code is None else out
 
     def forward(self, A, x: torch.Tensor):
@@ -107,7 +107,7 @@ class CG_LSTM(nn.Module):
         n = xt.shape[0]
         code = _act_code(gc.activation)
         if code is not None:
-            pool = ops.TemporalPool.apply(xt, gc.W, gc.b if gc.bias else None, sset, code)
+            pool = ops.TemporalPool.apply(xt, gc.W, gc.b if gc.bias else None, sset, code, *sset.grad_values())
         else:       # exotic activation class: kernel does the GCN, torch applies the module + pooling
             pool = (xt + gc.forward_node_major(sset, xt)).sum(dim=0)
         s = ops.ContextGate.apply(pool, self.fc.weight, self.fc.bias, n)

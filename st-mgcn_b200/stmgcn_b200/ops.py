@@ -181,16 +181,24 @@ def build_stack(sset: SupportSet, x: torch.Tensor, gather16: bool = False) -> to
     return cheb_stack_generic(sset, x)
 
 
-def adjoint_stack_(sset: SupportSet, u: torch.Tensor) -> torch.Tensor:
+def adjoint_stack_(sset: SupportSet, u: torch.Tensor, need_dx: bool = True) -> Optional[torch.Tensor]:
     """Given U_k = dZ W_k^T stacked in ``u`` (Ks, N, B, p) return dX (N, B, p); ``u`` is clobbered.
 
     cheb: one adjoint Clenshaw per chain with X_c^T (SURVEY.md section 8(a)), each adding its part into U_0 (T_0 = I is
-    shared); generic: sum_k A_k^T U_k.
+    shared); generic: sum_k A_k^T U_k.  Afterwards ``u[k]`` holds, for every segment k >= 1 of a chain, the total adjoint
+    G_k = dL/dT_k that :func:`support_value_grads` needs.  ``need_dx=False``: only that (cheb: each chain's last step
+    into U_0 is skipped; generic: nothing to do); returns None.
     """
     if sset.mode == "cheb":
         for c, g in enumerate(sset.graphs):
-            _adjoint_chain_(g, [u[i] for i in sset.chain_segments(c)])
-        return u[0]
+            segs = [u[i] for i in sset.chain_segments(c)]
+            if need_dx:
+                _adjoint_chain_(g, segs)
+            else:
+                _adjoint_chain_(g, segs, False)
+        return u[0] if need_dx else None
+    if not need_dx:
+        return None
     out = torch.empty_like(u[0])
     acc = None
     for k in range(sset.ks):
@@ -200,8 +208,9 @@ def adjoint_stack_(sset: SupportSet, u: torch.Tensor) -> torch.Tensor:
     return acc
 
 
-def _adjoint_chain_(g, u: List[torch.Tensor]) -> None:
-    """Adjoint of :func:`_cheb_chain_`: ``u[0] += sum_{k>=1} T_k(X)^T u[k]``; ``u[1:]`` is clobbered."""
+def _adjoint_chain_(g, u: List[torch.Tensor], into_u0: bool = True) -> None:
+    """Adjoint of :func:`_cheb_chain_`: ``u[0] += sum_{k>=1} T_k(X)^T u[k]``; ``u[1:]`` is overwritten with the Clenshaw
+    b_k, which is G_k = dL/dT_k.  ``into_u0=False`` stops there (``u[0]`` untouched)."""
     k_ord = len(u) - 1
     # b_K = U_K (in place).  b_k = U_k + 2 X^T b_{k+1} - b_{k+2}  written over U_k.
     # (always fp32 gathers here, also in the bf16-arithmetic mode: rounding b_{k+1} to bf16 before every gather puts
@@ -210,8 +219,55 @@ def _adjoint_chain_(g, u: List[torch.Tensor]) -> None:
     for k in range(k_ord - 1, 0, -1):
         z = u[k + 2] if k + 2 <= k_ord else None
         spmm_step(g, True, 2.0, u[k + 1], -1.0 if z is not None else 0.0, z, 1.0, u[k], u[k])
+    if not into_u0:
+        return
     z = u[2] if k_ord >= 2 else None
     spmm_step(g, True, 1.0, u[1], -1.0 if z is not None else 0.0, z, 1.0, u[0], u[0])
+
+
+def sddmm_tiles(f_total: int) -> int:
+    """Column tiles of :func:`csr_sddmm_` (include/stmgcn_b200.h, stmgcn_csr_sddmm): float4 lanes when f_total % 4 == 0."""
+    width = 128 if f_total % 4 == 0 else 32
+    return (f_total + width - 1) // width
+
+
+def csr_sddmm_(g, terms, dvals: torch.Tensor, round_b16: bool = False) -> None:
+    """``dvals[e] += sum_t coef_t <A_t[i, :], B_t[j, :]>`` over the stored entries e = (i, j) of ``g``'s CSR, in its
+    entry order; ``terms``: (A_t, B_t, coef_t) with A_t, B_t (N, ...) fp32 contiguous.  ``round_b16``: B rounded to bf16."""
+    rowptr, colidx, _ = g.export(False)
+    f_total = terms[0][0].numel() // g.n
+    tiles = sddmm_tiles(f_total)
+    work = torch.empty(tiles * g.nnz, device=dvals.device, dtype=torch.float32) if tiles > 1 and g.nnz else None
+    a = _lib.ptr_array([t[0].data_ptr() for t in terms])
+    b = _lib.ptr_array([t[1].data_ptr() for t in terms])
+    coef = _lib.float_array([float(t[2]) for t in terms])
+    _lib.check(L.stmgcn_csr_sddmm(g.n, rowptr.data_ptr(), colidx.data_ptr(), g.nnz, len(terms), a, b, coef,
+                                  int(round_b16), f_total, _p(work), 0 if work is None else work.numel(),
+                                  dvals.data_ptr(), _stream()), "csr_sddmm")
+
+
+def support_value_grads(sset: SupportSet, s: torch.Tensor, u: torch.Tensor, x: Optional[torch.Tensor],
+                        round_b16: bool, need: Sequence[bool]) -> List[Optional[torch.Tensor]]:
+    """The gradient of each graph's stored values (CSR entry order), None where ``need`` is False.  ``u`` after
+    :func:`adjoint_stack_`; ``s`` the forward stack; ``x`` the input (generic supports only).
+
+    cheb, chain X with terms T_0 .. T_K:  d vals[e] = sum_k c_k <G_k[i], T_{k-1}[j]>, c_1 = 1, c_k = 2 (k >= 2), one
+    SDDMM launch per chain over its own segments (``round_b16``: the bf16 copies the forward gathered from);
+    generic S_k = A_k x:  d vals_k[e] = <U_k[i], x[j]>."""
+    grads: List[Optional[torch.Tensor]] = []
+    for c, g in enumerate(sset.graphs):
+        if not need[c]:
+            grads.append(None)
+            continue
+        dv = torch.zeros(g.nnz, device=u.device, dtype=torch.float32)
+        if sset.mode == "cheb":
+            seg = sset.chain_segments(c)
+            terms = [(u[seg[k]], s[seg[k - 1]], 1.0 if k == 1 else 2.0) for k in range(1, len(seg))]
+            csr_sddmm_(g, terms, dv, round_b16)
+        else:
+            csr_sddmm_(g, [(u[c], x, 1.0)], dv)
+        grads.append(dv)
+    return grads
 
 
 def _proj_images(w: torch.Tensor, ks: int, p: int, need_bwd: bool):
@@ -302,10 +358,13 @@ class ObsToNodeMajor(torch.autograd.Function):
 
 
 class ChebGCN(torch.autograd.Function):
-    """out (N,B,q) = act( sum_k (T_k x) W_k + b ),  x (N,B,p) node-major."""
+    """out (N,B,q) = act( sum_k (T_k x) W_k + b ),  x (N,B,p) node-major.
+
+    ``vals``: the support set's value tensors (``sset.grad_values()``), inputs only so that their gradients reach them:
+    the kernels read the set's own copies."""
 
     @staticmethod
-    def forward(ctx, x, w, bias, sset: SupportSet, act: int):
+    def forward(ctx, x, w, bias, sset: SupportSet, act: int, *vals):
         _require_cuda(x, w)
         x, w = _f32c(x), _f32c(w)
         bias_c = _f32c(bias) if bias is not None else None
@@ -318,26 +377,40 @@ class ChebGCN(torch.autograd.Function):
         img_f, img_b = _proj_images(w, sset.ks, x.shape[2], need_grad)
         out = _proj_fwd(s, w, bias_c, act, None, x.shape[1], img_f)
         ctx.sset, ctx.act, ctx.has_bias = sset, act, bias is not None
+        # the value gradients' B operand is what the recurrence gathered: bf16(T_{k-1}) where it read bf16 copies (asked
+        # only when a value needs grad: such a set has a graph, and a set without values runs nothing new)
+        ctx.round16 = any(ctx.needs_input_grad[5:]) and _gather16(sset, x)
         if need_grad:
-            ctx.save_for_backward(s, w, out, img_b)
+            # x (generic supports' value gradients only) is saved last, and only then
+            need_x = any(ctx.needs_input_grad[5:]) and sset.mode == "generic"
+            ctx.save_for_backward(s, w, out, img_b, *([x] if need_x else []))
         return out
 
     @staticmethod
     def backward(ctx, d_out):
-        s, w, out, img_b = ctx.saved_tensors
+        s, w, out, img_b, *x = ctx.saved_tensors
+        x = x[0] if x else None
         need_dx, need_dw, need_db = ctx.needs_input_grad[:3]
+        need_v = ctx.needs_input_grad[5:]
         d_out = _f32c(d_out)
-        dw, db, u = _proj_bwd(s, w, ctx.act, out, d_out, None, 1.0, s.shape[2], ctx.has_bias and need_db, need_dx, img_b,
+        need_u = need_dx or any(need_v)
+        dw, db, u = _proj_bwd(s, w, ctx.act, out, d_out, None, 1.0, s.shape[2], ctx.has_bias and need_db, need_u, img_b,
                               need_w=need_dw)
-        dx = adjoint_stack_(ctx.sset, u) if need_dx else None
-        return dx, dw, db, None, None
+        dx = None
+        if need_dx:
+            dx = adjoint_stack_(ctx.sset, u)
+        elif need_u:
+            adjoint_stack_(ctx.sset, u, False)          # G_k into u for the value gradients only
+        dvals = support_value_grads(ctx.sset, s, u, x, ctx.round16, need_v) if any(need_v) else [None] * len(need_v)
+        return (dx, dw, db, None, None, *dvals)
 
 
 class TemporalPool(torch.autograd.Function):
-    """pool (B,T) = sum_n ( x + act(GCN_T(x)) )[n,b,:]  (STMGCN.py:40-42 before the division by N)."""
+    """pool (B,T) = sum_n ( x + act(GCN_T(x)) )[n,b,:]  (STMGCN.py:40-42 before the division by N).  ``vals`` as for
+    :class:`ChebGCN`."""
 
     @staticmethod
-    def forward(ctx, x, w, bias, sset: SupportSet, act: int):
+    def forward(ctx, x, w, bias, sset: SupportSet, act: int, *vals):
         _require_cuda(x, w)
         x, w = _f32c(x), _f32c(w)
         bias_c = _f32c(bias) if bias is not None else None
@@ -355,21 +428,28 @@ class TemporalPool(torch.autograd.Function):
             pool = (x + out).sum(dim=0)
         ctx.act, ctx.has_bias, ctx.sset = act, bias is not None, sset
         if any(ctx.needs_input_grad):
-            ctx.save_for_backward(s, w, out)
+            need_x = any(ctx.needs_input_grad[5:]) and sset.mode == "generic"
+            ctx.save_for_backward(s, w, out, *([x] if need_x else []))
         return pool
 
     @staticmethod
     def backward(ctx, d_pool):
-        s, w, out = ctx.saved_tensors
+        s, w, out, *x = ctx.saved_tensors
+        x = x[0] if x else None
         d_pool = _f32c(d_pool)
         need_dx, need_dw, need_db = ctx.needs_input_grad[:3]
-        dw, db, u = _proj_bwd(s, w, ctx.act, out, None, d_pool, 1.0, s.shape[2], ctx.has_bias and need_db, need_dx,
+        need_v = ctx.needs_input_grad[5:]
+        need_u = need_dx or any(need_v)
+        dw, db, u = _proj_bwd(s, w, ctx.act, out, None, d_pool, 1.0, s.shape[2], ctx.has_bias and need_db, need_u,
                               need_w=need_dw)
         dx = None
         if need_dx:
             # the GCN's dX (adjoint Clenshaw / sum_k A_k^T U_k) plus the residual's: d_pool broadcast over regions
             dx = adjoint_stack_(ctx.sset, u) + d_pool.unsqueeze(0)
-        return dx, dw, db, None, None
+        elif need_u:
+            adjoint_stack_(ctx.sset, u, False)          # G_k into u for the value gradients only
+        dvals = support_value_grads(ctx.sset, s, u, x, False, need_v) if any(need_v) else [None] * len(need_v)
+        return (dx, dw, db, None, None, *dvals)
 
 
 class ContextGate(torch.autograd.Function):

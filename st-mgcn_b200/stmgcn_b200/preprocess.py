@@ -95,6 +95,10 @@ class Adj_Preprocessor(object):
           8 supports (``K <= 3``): the projection kernels take up to 8;
         * ``localpool``: ``I + D^-1/2 A D^-1/2`` as one generic support.
 
+        When ``adj`` (dense) or its values (sparse COO) require grad, the handle's stored values keep the autograd graph
+        back to them: rebuilt every step, the supports carry the loss's gradient to the adjacency's entries through the
+        normalisations (``lambda_max`` is a constant).  The gradient lives on the stored pattern: an absent edge, or an
+        entry dropped as an exact zero, gets none (a dense ``process()`` stack would give one there).
         ``adj`` may be dense ``(N,N)`` or a sparse COO/CSR tensor.  The result is accepted wherever the
         dense stack is (``GCN.forward``, ``ST_MGCN.forward``'s ``sta_adj_list``)."""
         coo = adj.to_sparse_coo().coalesce() if adj.layout != torch.sparse_coo else adj.coalesce()
@@ -129,7 +133,7 @@ class Adj_Preprocessor(object):
         elif isinstance(self.lambda_max, (int, float)):
             lam = float(self.lambda_max)
         else:
-            lam = self._lambda_sparse(n, row, col, a_norm)
+            lam = self._lambda_sparse(n, row, col, a_norm.detach())      # a constant: no gradient through it
         scale = 2.0 / lam
         # L~ = scale * (I - A_norm) - I  => off-diagonal -scale*A_norm, diagonal (scale - 1) - scale*A_norm_ii
         diag_val = scale - 1.0
@@ -153,7 +157,11 @@ class Adj_Preprocessor(object):
 
 
 def _csr(n: int, rows: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor):
-    """CSR of the ``n x n`` matrix with entries ``(rows, cols, vals)`` in any order (repeats summed, exact zeros dropped)."""
+    """CSR of the ``n x n`` matrix with entries ``(rows, cols, vals)`` in any order (repeats summed, exact zeros dropped).
+    With ``vals`` requiring grad the CSR's values are the differentiable values (the indices are copies)."""
     m = torch.sparse_coo_tensor(torch.stack([rows, cols]), vals, (n, n)).coalesce()
     keep = m.values() != 0
-    return csr_from_coo(n, m.indices()[0][keep], m.indices()[1][keep], m.values()[keep])
+    rowptr, colidx, v = csr_from_coo(n, m.indices()[0][keep], m.indices()[1][keep], m.values()[keep])
+    if vals.requires_grad:
+        v = m.values()[keep].to(torch.float32)
+    return rowptr, colidx, v
