@@ -97,6 +97,41 @@ int32_t stmgcn_csr_sddmm(int64_t n, const int32_t* rowptr, const int32_t* colidx
                          const float* const* a, const float* const* b, const float* coef, int32_t round_b_bf16,
                          int64_t f_total, float* work, int64_t work_count, float* dvals, void* stream);
 
+/* ---- K1c: the supports of a learnable adjacency on a fixed sparsity pattern ----------------------------------------
+ * The pattern is an n x n CSR (rowptr, colidx; nnz = rowptr[n] entries, no repeated (i, j)) and its transpose's structure
+ * rowptr_t, colidx_t with perm_t: CSR^T position p holds CSR entry perm_t[p].  widx (int32 per pattern entry) gives the
+ * entry's index in w, or -1 for a slot with no weight of its own (a diagonal slot that holds only the diagonal term);
+ * it maps onto [0, nnz_w) one to one.  widx NULL: the pattern's entries are w's, in order (nnz_w == nnz).  w (fp32): the
+ * edge weights; D below sums them per row (d_out) or per column (d_in), over the entries that have one.  kind:
+ *   STMGCN_NORM_CHEBYSHEV  vals[e] = -scale * D^-1/2 A D^-1/2 + (scale - 1) I     (scale = 2 / lambda_max, finite)
+ *   STMGCN_NORM_LOCALPOOL  vals[e] =  I + D^-1/2 A D^-1/2
+ *   STMGCN_NORM_DIFFUSION  vals[e]   = P_b^T = w * d_in^-1[col]   (CSR order)
+ *                          vals_t[p] = P_f^T = w * d_out^-1[row]  (CSR^T order), an infinite d^-1 taken as 0 (GCN.py:100-104)
+ * D^-1/2 is torch's pow(D, -0.5): +inf at a zero sum, NaN at a negative one.  The backward is torch autograd's chain
+ * through these formulas, non-finite values included: at a zero sum the degree term is NaN (0 * -inf for DIFFUSION, whose
+ * masked reciprocal passes 0 into pow(D, -1)'s -D^-2), so a row or column of stored entries that sum to zero (stored
+ * zeros, say) gets NaN in dw; an empty row or column has no entry to pass it to.  The diagonal terms go into the pattern's
+ * diagonal slot of each row (added to a stored self-loop); the caller's pattern has one in every row for the symmetric
+ * kinds (unless scale == 1 for CHEBYSHEV).  vals_t / dvals_t are for DIFFUSION only (NULL otherwise).
+ * Every sum has one owner and a fixed order (no float atomics): two calls give bit-identical results.  Nothing is
+ * allocated and nothing synchronises; the workspace (work_count floats) needs no initialisation: 2n floats forward,
+ * 3n + nnz backward.  Outputs (work, vals, vals_t, dw) share no byte with any input or with one another (checked).  The
+ * forward enqueues 2 launches (none when nnz == 0), the backward 3 (none when nnz_w == 0). */
+#define STMGCN_NORM_CHEBYSHEV 0
+#define STMGCN_NORM_LOCALPOOL 1
+#define STMGCN_NORM_DIFFUSION 2
+int32_t stmgcn_adj_norm_fwd(int32_t kind, int64_t n, const int32_t* rowptr, const int32_t* colidx, const int32_t* rowptr_t,
+                            const int32_t* colidx_t, const int32_t* perm_t, int64_t nnz, const int32_t* widx, const float* w,
+                            int64_t nnz_w, float scale, float* work, int64_t work_count, float* vals, float* vals_t,
+                            void* stream);
+/* The backward: dw (nnz_w, overwritten) from the values' gradients dvals (CSR order) and, DIFFUSION, dvals_t (CSR^T
+ * order): the direct term plus the degree terms (a row segment sum over the CSR, a column segment sum over the CSR^T,
+ * then one pass over the entries).  Same pattern, w and scale as the forward. */
+int32_t stmgcn_adj_norm_bwd(int32_t kind, int64_t n, const int32_t* rowptr, const int32_t* colidx, const int32_t* rowptr_t,
+                            const int32_t* colidx_t, const int32_t* perm_t, int64_t nnz, const int32_t* widx, const float* w,
+                            int64_t nnz_w, float scale, const float* dvals, const float* dvals_t, float* work,
+                            int64_t work_count, float* dw, void* stream);
+
 /* ---- layout: obs (B,T,N,C) -> node-major (STMGCN.py:36,39 sum over C + permute; :47 row order) ----
  * xo: (N,B,T,C) copy of obs;  xt: (N,B,T) = sum_c obs.  xo may be NULL when C == 1 (xt is then xo). */
 int32_t stmgcn_obs_to_node_major(const float* obs, float* xo, float* xt, int64_t b, int64_t t,

@@ -17,10 +17,21 @@ import torch.distributed as dist
 
 
 class GradBucket:
-    """All parameter gradients of a module as views into one flat contiguous buffer."""
+    """All parameter gradients of one or more modules as views into one flat contiguous buffer: ``GradBucket(model)``,
+    or ``GradBucket(model, *adjacencies)`` to reduce learnable graphs (``LearnableAdjacency``, held outside the model so
+    its ``state_dict`` keys stay the reference's) in the same single collective.  A parameter shared by two modules is
+    taken once."""
 
-    def __init__(self, module: torch.nn.Module):
-        self.params = [p for p in module.parameters() if p.requires_grad]
+    def __init__(self, module: torch.nn.Module, *more: torch.nn.Module):
+        self.params, seen = [], set()
+        for mod in (module,) + more:
+            for p in mod.parameters():
+                if p.requires_grad and id(p) not in seen:
+                    seen.add(id(p))
+                    self.params.append(p)
+        kinds = {(p.dtype, p.device) for p in self.params}
+        if len(kinds) > 1:
+            raise ValueError(f"GradBucket: the parameters must share one dtype and device, got {sorted(map(str, kinds))}")
         total = sum(p.numel() for p in self.params)
         ref = self.params[0]
         self.flat = torch.zeros(total, dtype=ref.dtype, device=ref.device)

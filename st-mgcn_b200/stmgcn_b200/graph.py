@@ -15,6 +15,9 @@ for ``chebyshev``): it quacks like the reference's tensor where ``Main.py`` touc
 ``.shape``) but never materialises ``N x N`` polynomials (SURVEY.md section 8(f)-1).  Its ``"cheb"`` stacks are one or
 more recurrence chains that share ``T_0 = I``: one for ``chebyshev`` (``L~``), two for ``random_walk_diffusion``
 (``P_f^T`` and ``P_b^T``, DCRNN's dual random-walk diffusion).
+
+``LearnableAdjacency`` (``Adj_Preprocessor.process_learnable``) is a learnable graph on a fixed pattern: an ``nn.Module``
+whose edge weights are normalised into such a handle's values on the device at every forward.
 """
 from __future__ import annotations
 
@@ -23,6 +26,7 @@ from collections import OrderedDict
 from typing import List, Optional
 
 import torch
+from torch import nn
 
 
 def csr_from_coo(n: int, rows: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor):
@@ -177,14 +181,14 @@ _CACHE_MAX = 32
 def support_version(a) -> tuple:
     """What a support stack's conversion is keyed on: identity and in-place version of its tensors.  Any edit of the
     stack through a torch op changes it."""
-    if isinstance(a, SparseSupports):
+    if isinstance(a, (SparseSupports, LearnableAdjacency)):
         return a.version()
     return (a.data_ptr(), a._version, tuple(a.shape), tuple(a.stride()), str(a.device), a.dtype)
 
 
 def supports_from_dense(a: torch.Tensor) -> SupportSet:
     """Cached conversion of a dense support stack (keyed on tensor identity + in-place version)."""
-    if isinstance(a, SparseSupports):
+    if isinstance(a, (SparseSupports, LearnableAdjacency)):
         return a.support_set()
     if not isinstance(a, torch.Tensor) or a.dim() != 3 or a.shape[1] != a.shape[2]:
         raise ValueError(f"supports must be a (K, N, N) tensor, got {type(a)} {getattr(a, 'shape', None)}")
@@ -293,22 +297,180 @@ class SparseSupports:
         return self._sset
 
     def _learnable_support_set(self) -> SupportSet:
+        return self.support_set_with([v for _, _, v in self.mats])
+
+    def support_set_with(self, values) -> SupportSet:
+        """The kernels' set for this handle's index structure with the stored values ``values`` (one tensor per matrix,
+        in its CSR entry order) copied in; the set carries ``values`` as the convolutions' inputs, so their gradients
+        reach them.  The structure (CSR and CSR^T indices, the transpose's permutation) is cached on the index tensors:
+        only the first call converts it (one host sync); the later ones copy values and never synchronise."""
         if not self.is_cuda:
             raise RuntimeError(f"{type(self).__name__} must be moved to a CUDA device before use (.to(device))")
         # a one-support Chebyshev stack ([I], K = 0) multiplies by no matrix: its values are not an input of any
         # convolution and their .grad stays None, as for any tensor the loss does not use
         mats = self.mats if self.mode == "generic" or self.ks > 1 else []
-        key = tuple((rp.data_ptr(), rp._version, ci.data_ptr(), ci._version, v.numel()) for rp, ci, v in mats)
+        values = list(values)[:len(mats)]
+        key = tuple((rp.data_ptr(), rp._version, ci.data_ptr(), ci._version, v.numel())
+                    for (rp, ci, _), v in zip(mats, values))
         if self._structure is None or self._structure_key != key:
-            self._structure = [GraphHandle.from_csr(self.n, rp, ci, v.detach()) for rp, ci, v in mats]
+            self._structure = [GraphHandle.from_csr(self.n, rp, ci, v.detach().float()) for (rp, ci, _), v in zip(mats, values)]
             self._structure_key = key
-        graphs = [h.with_values(v) for h, (_, _, v) in zip(self._structure, mats)]
-        return SupportSet(self.mode, self.n, self.ks, graphs, self.device, values=[v for _, _, v in mats])
+        graphs = [h.with_values(v) for h, v in zip(self._structure, values)]
+        return SupportSet(self.mode, self.n, self.ks, graphs, self.device, values=values)
 
     def matrices_dense(self) -> List[torch.Tensor]:
         """The stored matrices as dense ``(N, N)`` tensors (tests / small graphs only)."""
         return [torch.sparse_csr_tensor(rp.long(), ci.long(), v.detach(), size=(self.n, self.n)).to_dense()
                 for rp, ci, v in self.mats]
+
+
+def _stored_entries(adj: torch.Tensor):
+    """``(n, rows, cols, vals)`` of a square adjacency, row-major: a dense one's non-zero entries, a sparse (COO / CSR)
+    one's stored entries, stored zeros included (repeats summed)."""
+    if adj.dim() != 2 or adj.shape[0] != adj.shape[1]:
+        raise ValueError(f"the adjacency must be (N, N), got {tuple(adj.shape)}")
+    if adj.layout == torch.strided:
+        rows, cols = (adj != 0).nonzero(as_tuple=True)
+        vals = adj[rows, cols]
+    else:
+        coo = adj.coalesce() if adj.layout == torch.sparse_coo else adj.to_sparse_coo().coalesce()
+        (rows, cols), vals = coo.indices(), coo.values()
+    return adj.shape[0], rows, cols, vals.detach().to(torch.float32)
+
+
+class LearnableAdjacency(nn.Module):
+    """A learnable adjacency on a fixed sparsity pattern: ``weight`` (one per stored edge) is its only parameter, and each
+    forward normalises it on the device into the supports ``Adj_Preprocessor.process_sparse`` would build from it
+    (``ops.AdjNorm``: no host synchronisation, fixed-order sums), so a step that learns the graph can be captured
+    (``GraphedStep``) and its edge weights reduced with the model's gradients (``GradBucket(model, adjacency)``).
+
+    Built by ``Adj_Preprocessor.process_learnable``.  The pattern -- the stored entries plus a diagonal slot in every row
+    that lacks one when the kind has a diagonal term (``localpool``; ``chebyshev`` with ``2 / lambda_max != 1``) -- is
+    built once, as CSR and CSR^T on the module's buffers; ``lambda_max`` is a constant.  Stands in for the support stack
+    wherever one goes (``ST_MGCN.forward``'s ``sta_adj_list``, ``GCN.forward``, ``CG_LSTM.forward``): ``.shape ==
+    (Ks, N, N)``, ``len``, ``.device``, and ``nn.Module.to``.  The supports are fed to the kernels through a
+    :class:`SparseSupports` handle on the module's own index tensors, so the structure is converted once and every
+    forward only copies the new values in."""
+
+    def __init__(self, kind: str, order: int, adj: torch.Tensor, scale: float = 1.0, lambda_max: float = 2.0):
+        super().__init__()
+        if kind not in ("chebyshev", "localpool", "random_walk_diffusion"):
+            raise ValueError(f"kind={kind!r}")
+        n, rows, cols, vals = _stored_entries(adj)
+        nnz_w = rows.numel()
+        self.kind, self.order, self.n = kind, int(order), int(n)
+        self.ks = {"chebyshev": self.order + 1, "localpool": 1, "random_walk_diffusion": 2 * self.order + 1}[kind]
+        if kind == "random_walk_diffusion" and self.ks > 8:
+            raise ValueError(f"LearnableAdjacency: random_walk_diffusion with K={self.order} needs {self.ks} supports; the "
+                             f"projection kernels take at most 8 supports (K <= 3)")
+        self.scale, self.lambda_max = float(scale), float(lambda_max)
+        dev = rows.device
+        prow, pcol, src = rows, cols, None
+        if kind == "localpool" or (kind == "chebyshev" and self.scale != 1.0):
+            has = torch.zeros(n, dtype=torch.bool, device=dev)
+            has[rows[rows == cols]] = True
+            extra = (~has).nonzero().flatten()
+            if extra.numel():
+                order_ = torch.argsort(torch.cat([rows, extra]) * n + torch.cat([cols, extra]))
+                prow, pcol = torch.cat([rows, extra])[order_], torch.cat([cols, extra])[order_]
+                src = torch.cat([torch.arange(nnz_w, device=dev), torch.full_like(extra, -1)])[order_]
+        nnz = prow.numel()
+        if not 0 < n < 2 ** 30 or nnz >= 2 ** 31:
+            raise ValueError(f"LearnableAdjacency: n={n} must be in [1, 2^30) and nnz={nnz} below 2^31 (int32 indices)")
+        rowptr = torch.zeros(n + 1, dtype=torch.int32, device=dev)
+        rowptr[1:] = torch.cumsum(torch.bincount(prow, minlength=n), 0)
+        tord = torch.argsort(pcol * n + prow)
+        rowptr_t = torch.zeros(n + 1, dtype=torch.int32, device=dev)
+        rowptr_t[1:] = torch.cumsum(torch.bincount(pcol, minlength=n), 0)
+        self.register_buffer("rowptr", rowptr)
+        self.register_buffer("colidx", pcol.to(torch.int32))
+        self.register_buffer("rowptr_t", rowptr_t)
+        self.register_buffer("colidx_t", prow[tord].to(torch.int32))
+        self.register_buffer("perm_t", tord.to(torch.int32))
+        self.register_buffer("widx", None if src is None else src.to(torch.int32))
+        self.weight = nn.Parameter(vals.clone())
+        self._handle: Optional[SparseSupports] = None
+        self._handle_key: tuple = ()
+
+    def extra_repr(self) -> str:
+        return f"{self.kind}, Ks={self.ks}, N={self.n}, edges={self.weight.numel()}, lambda_max={self.lambda_max:g}"
+
+    @property
+    def shape(self):
+        return torch.Size((self.ks, self.n, self.n))
+
+    @property
+    def device(self):
+        return self.weight.device
+
+    @property
+    def is_cuda(self):
+        return self.weight.is_cuda
+
+    def __len__(self):
+        return self.ks
+
+    def pattern(self) -> tuple:
+        """``(rowptr, colidx, rowptr_t, colidx_t, perm_t, widx)``: the pattern the normalisation runs on (widx: each
+        pattern entry's index in ``weight``, -1 for an added diagonal slot; None when there is no such slot)."""
+        return self.rowptr, self.colidx, self.rowptr_t, self.colidx_t, self.perm_t, self.widx
+
+    def version(self) -> tuple:
+        """Identity and in-place version of the pattern's tensors (not of ``weight``: its values are read at every
+        forward)."""
+        return tuple((t.data_ptr(), t._version) for t in self.pattern() if t is not None)
+
+    def edges(self):
+        """int64 ``(rows, cols)`` of the stored edges, in ``weight``'s order (row-major), read off the pattern."""
+        rows = torch.repeat_interleave(torch.arange(self.n, device=self.rowptr.device),
+                                       (self.rowptr[1:] - self.rowptr[:-1]).long(), output_size=self.colidx.numel())
+        cols = self.colidx.long()
+        if self.widx is not None:            # the stored entries keep their row-major order among the added slots
+            keep = self.widx >= 0
+            rows, cols = rows[keep], cols[keep]
+        return rows, cols
+
+    def learned_adjacency(self) -> torch.Tensor:
+        """The current edge weights as a sparse COO ``(N, N)`` tensor on the stored pattern (a detached copy)."""
+        return torch.sparse_coo_tensor(torch.stack(self.edges()), self.weight.detach().clone(), (self.n, self.n),
+                                       is_coalesced=True)
+
+    def _supports_handle(self) -> SparseSupports:
+        key = self.version()
+        if self._handle is None or self._handle_key != key:
+            blank = torch.empty(self.colidx.numel(), device=self.device)
+            if self.kind == "random_walk_diffusion":
+                self._handle = SparseSupports("cheb", self.n, self.ks, [(self.rowptr_t, self.colidx_t, blank),
+                                                                         (self.rowptr, self.colidx, blank)])
+            elif self.kind == "chebyshev":
+                self._handle = ChebSupports(self.n, self.ks, self.rowptr, self.colidx, blank)
+            else:
+                self._handle = SparseSupports("generic", self.n, 1, [(self.rowptr, self.colidx, blank)])
+            self._handle_key = key
+        return self._handle
+
+    def _values(self):
+        """The stored values of the supports' matrices at the current weights, in the handle's matrix order."""
+        from . import ops
+        vals = ops.AdjNorm.apply(self.weight, self.kind, self.scale, *self.pattern())
+        return list(vals) if isinstance(vals, tuple) else [vals]
+
+    def forward(self) -> SupportSet:
+        """The kernels' support set at the current weights: one normalisation launch pair, then the values copied into
+        the cached structure (:meth:`SparseSupports.support_set_with`)."""
+        if not self.is_cuda:
+            raise RuntimeError("LearnableAdjacency must be moved to a CUDA device before use (.to(device))")
+        return self._supports_handle().support_set_with(self._values())
+
+    def supports(self) -> SparseSupports:
+        """The supports at the current weights as a fixed handle (detached copies of the values): what
+        ``process_sparse`` would return for the learned graph."""
+        with torch.no_grad():
+            vals = self._values()
+        h = self._supports_handle()
+        return SparseSupports(h.mode, h.n, h.ks, [(rp, ci, v) for (rp, ci, _), v in zip(h.mats, vals)])
+
+    support_set = forward
 
 
 class ChebSupports(SparseSupports):

@@ -14,6 +14,12 @@ those sets (so their memory stays valid whatever happens to the conversion cache
 (``graph.support_version``); a call after any support was edited raises instead of replaying the old supports.
 Learnable supports (a ``SparseSupports`` whose values require grad) are refused at construction: their values are read
 again at every forward, which a replayed graph cannot do.
+
+A ``LearnableAdjacency`` is accepted: its normalisation (``ops.AdjNorm``) is captured with the step and reads ``weight``
+at its own address, so each replay runs at the weights the optimizer left there (fused optimizers included).  Its
+``support_version`` is the version of its pattern tensors.  The default bucket covers the model and these modules; an
+explicit ``bucket`` must hold their parameters (else ``ValueError``: their gradients would land outside the reduced
+buffer).
 """
 from __future__ import annotations
 
@@ -22,7 +28,7 @@ from typing import Callable, Optional, Sequence
 import torch
 
 from .dp import GradBucket
-from .graph import SparseSupports, support_version, supports_from_dense
+from .graph import LearnableAdjacency, SparseSupports, support_version, supports_from_dense
 
 
 class GraphedStep:
@@ -34,7 +40,18 @@ class GraphedStep:
             raise ValueError(f"GraphedStep: supports {learnable} have values that require grad; a captured step replays "
                              f"the values of capture time, so learnable supports run eagerly")
         self.model, self.criterion, self.supports = model, criterion, list(supports)
-        self.bucket = bucket if bucket is not None else GradBucket(model)
+        adjs = []
+        for s in self.supports:
+            if isinstance(s, LearnableAdjacency) and all(s is not a for a in adjs):
+                adjs.append(s)
+        if bucket is not None:
+            held = {id(p) for p in bucket.params}
+            lacking = [m for m, s in enumerate(self.supports) if isinstance(s, LearnableAdjacency)
+                       and any(p.requires_grad and id(p) not in held for p in s.parameters())]
+            if lacking:
+                raise ValueError(f"GraphedStep: the bucket lacks the parameters of the learnable adjacencies {lacking}; "
+                                 f"build it as GradBucket(model, *adjacencies)")
+        self.bucket = bucket if bucket is not None else GradBucket(model, *adjs)
         self.all_reduce = all_reduce
         self.x = torch.empty_like(x)
         self.y = torch.empty_like(y)
@@ -47,8 +64,9 @@ class GraphedStep:
                 self._eager()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
-        # the conversions the warm-up cached, which the capture below reads
-        self.support_sets = [supports_from_dense(s) for s in self.supports]
+        # the conversions the warm-up cached, which the capture below reads (a learnable adjacency holds its own structure
+        # and is normalised inside the capture)
+        self.support_sets = [s if isinstance(s, LearnableAdjacency) else supports_from_dense(s) for s in self.supports]
         self.support_versions = [support_version(s) for s in self.supports]
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):

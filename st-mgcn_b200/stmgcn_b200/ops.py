@@ -11,6 +11,7 @@ Functions (reference lines they replace):
   ContextGate      STMGCN.py:42-43: /N, fc, relu, fc (same weights), sigmoid -> s (B,T)
   SharedLSTM       STMGCN.py:44,47-50: modulate + 3-layer shared LSTM (lstm16.cu / lstm.cu: one call each way)
   FuseOut          STMGCN.py:116-118: sum over graphs + output FC -> (B,N,C)
+  AdjNorm          GCN.py:99-111 on a fixed pattern: a learnable adjacency's weights -> its supports' stored values
 """
 from __future__ import annotations
 
@@ -268,6 +269,52 @@ def support_value_grads(sset: SupportSet, s: torch.Tensor, u: torch.Tensor, x: O
             csr_sddmm_(g, [(u[c], x, 1.0)], dv)
         grads.append(dv)
     return grads
+
+
+NORM_KINDS = {"chebyshev": 0, "localpool": 1, "random_walk_diffusion": 2}      # STMGCN_NORM_* of the C ABI
+
+
+def _norm_args(kind: str, pattern, w: torch.Tensor, scale: float):
+    """The pattern and weight arguments stmgcn_adj_norm_fwd / _bwd share: ``pattern`` is (rowptr, colidx, rowptr_t,
+    colidx_t, perm_t, widx or None) int32 on the device."""
+    rowptr, colidx, rowptr_t, colidx_t, perm_t, widx = pattern
+    return (NORM_KINDS[kind], rowptr.numel() - 1, rowptr.data_ptr(), colidx.data_ptr(), rowptr_t.data_ptr(),
+            colidx_t.data_ptr(), perm_t.data_ptr(), colidx.numel(), _p(widx), w.data_ptr(), w.numel(), scale)
+
+
+class AdjNorm(torch.autograd.Function):
+    """The stored values of a learnable adjacency's supports from its edge weights, on its fixed pattern
+    (stmgcn_adj_norm_fwd / _bwd): ``L~`` (chebyshev) or ``I + D^-1/2 A D^-1/2`` (localpool) in CSR order, or
+    ``(P_f^T in CSR^T order, P_b^T in CSR order)`` (random_walk_diffusion).  Backward: d weight, the direct and the
+    degree terms, in a fixed order.  Allocates through torch and never synchronises, so it is captured by a CUDA graph;
+    the kernels read ``weight`` at its own address, so a replay sees in-place optimizer updates."""
+
+    @staticmethod
+    def forward(ctx, weight, kind: str, scale: float, *pattern):
+        _require_cuda(weight, pattern[0])
+        w = _f32c(weight.detach())
+        n, nnz = pattern[0].numel() - 1, pattern[1].numel()
+        diff = kind == "random_walk_diffusion"
+        work = torch.empty(2 * n, device=w.device, dtype=torch.float32)
+        vals = torch.empty(nnz, device=w.device, dtype=torch.float32)
+        vals_t = torch.empty(nnz, device=w.device, dtype=torch.float32) if diff else None
+        _lib.check(L.stmgcn_adj_norm_fwd(*_norm_args(kind, pattern, w, scale), work.data_ptr(), work.numel(),
+                                         vals.data_ptr(), _p(vals_t), _stream()), "adj_norm_fwd")
+        ctx.kind, ctx.scale, ctx.pattern = kind, scale, pattern
+        ctx.save_for_backward(w)
+        return (vals_t, vals) if diff else vals
+
+    @staticmethod
+    def backward(ctx, *grads):
+        (w,) = ctx.saved_tensors
+        pattern = ctx.pattern
+        n, nnz = pattern[0].numel() - 1, pattern[1].numel()
+        g_t, g = (_f32c(grads[0]), _f32c(grads[1])) if ctx.kind == "random_walk_diffusion" else (None, _f32c(grads[0]))
+        work = torch.empty(3 * n + nnz, device=w.device, dtype=torch.float32)
+        dw = torch.empty_like(w)
+        _lib.check(L.stmgcn_adj_norm_bwd(*_norm_args(ctx.kind, pattern, w, ctx.scale), g.data_ptr(), _p(g_t),
+                                         work.data_ptr(), work.numel(), dw.data_ptr(), _stream()), "adj_norm_bwd")
+        return (dw, None, None) + (None,) * len(pattern)
 
 
 def _proj_images(w: torch.Tensor, ks: int, p: int, need_bwd: bool):

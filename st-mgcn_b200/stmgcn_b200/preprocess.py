@@ -17,7 +17,7 @@ from typing import Union
 
 import torch
 
-from .graph import ChebSupports, SparseSupports, csr_from_coo
+from .graph import ChebSupports, LearnableAdjacency, SparseSupports, _stored_entries, csr_from_coo
 
 
 class Adj_Preprocessor(object):
@@ -142,6 +142,25 @@ class Adj_Preprocessor(object):
             idx_r, idx_c = torch.cat([idx_r, ar]), torch.cat([idx_c, ar])
             vals = torch.cat([vals, torch.full((n,), diag_val, dtype=torch.float32, device=dev)])
         return ChebSupports(n, self.K + 1, *_csr(n, idx_r, idx_c, vals))
+
+    def process_learnable(self, adj: torch.Tensor) -> LearnableAdjacency:
+        """A learnable graph on the fixed pattern of ``adj``: a :class:`~stmgcn_b200.graph.LearnableAdjacency` whose only
+        parameter ``weight`` holds one value per stored edge (initialised to ``adj``'s values; a dense ``adj``'s non-zero
+        entries, a sparse one's stored entries, stored zeros included).  Every forward normalises the weights on the
+        device into the supports :meth:`process_sparse` would build from them (``lambda_max`` is evaluated once, here, and
+        held constant).  It stands in for the supports wherever they go; train it by giving ``module.parameters()`` to
+        the optimizer (and to ``dp.GradBucket`` / ``GraphedStep``'s bucket under data parallelism)."""
+        lam = 2.0
+        if self.kernel_type == "chebyshev":
+            if self.lambda_max == "reference":
+                lam = 2.0
+            elif isinstance(self.lambda_max, (int, float)):
+                lam = float(self.lambda_max)
+            else:
+                n, row, col, val = _stored_entries(adj)
+                d = torch.zeros(n, dtype=torch.float32, device=val.device).index_add_(0, row, val).pow(-0.5)
+                lam = self._lambda_sparse(n, row, col, d[row] * val * d[col])
+        return LearnableAdjacency(self.kernel_type, self.K, adj, scale=2.0 / lam, lambda_max=lam)
 
     @staticmethod
     def _lambda_sparse(n, row, col, a_norm) -> float:
