@@ -132,6 +132,17 @@ int32_t stmgcn_adj_norm_bwd(int32_t kind, int64_t n, const int32_t* rowptr, cons
                             int64_t nnz_w, float scale, const float* dvals, const float* dvals_t, float* work,
                             int64_t work_count, float* dw, void* stream);
 
+/* ---- input pipeline: training windows gathered from a device-resident series (Data_Container.py:114-146) ----------
+ *   obs[k, t, :] = series[wrap(first + k - lags[t]), :],   y[k, :] = series[first + k, :]      (k < b, t < t_len)
+ * A row is `row` = N*C fp32 values; series is (s_len, row) row-major; obs is (b, t_len, row); y is (b, row).
+ * wrap(r) = r + s_len for -s_len <= r < 0 (numpy's negative indexing, which the reference's periodic windows hit).
+ * lags: host array of t_len int32 values, read at enqueue.  A plain copy: output bits equal input bits (NaN payloads, -0).
+ * Requires s_len, row, b > 0, 0 < t_len <= 2048, 0 <= first, first + b <= s_len, every lags[t] >= 0 and
+ * first - lags[t] >= -s_len; obs and y share no byte with the series or with each other.  One launch: 16-byte loads and
+ * stores when row % 4 == 0 and series, obs and y are 16-byte aligned, scalar ones otherwise. */
+int32_t stmgcn_window_gather(const float* series, int64_t s_len, int64_t row, const int32_t* lags, int32_t t_len,
+                             int64_t first, int64_t b, float* obs, float* y, void* stream);
+
 /* ---- layout: obs (B,T,N,C) -> node-major (STMGCN.py:36,39 sum over C + permute; :47 row order) ----
  * xo: (N,B,T,C) copy of obs;  xt: (N,B,T) = sum_c obs.  xo may be NULL when C == 1 (xt is then xo). */
 int32_t stmgcn_obs_to_node_major(const float* obs, float* xo, float* xt, int64_t b, int64_t t,

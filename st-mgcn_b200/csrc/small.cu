@@ -1,5 +1,6 @@
-// Small memory-bound kernels around the three hot kernels: layout change of the observations, the context
-// gate's tiny FC (STMGCN.py:42-43) and the fusion over graphs + output FC (STMGCN.py:116-118).
+// Small memory-bound kernels around the three hot kernels: the training windows gathered from a resident series
+// (Data_Container.py:114-146), layout change of the observations, the context gate's tiny FC (STMGCN.py:42-43) and the
+// fusion over graphs + output FC (STMGCN.py:116-118).
 #include "common.cuh"
 
 using namespace stmgcn;
@@ -179,9 +180,102 @@ __global__ void fuse_out_bwd_kernel(const float* __restrict__ d_y, const float* 
     for (int e = threadIdx.x; e < c_out; e += blockDim.x) atomicAdd(&d_fcb[e], sacc[c_out * gdim + e]);
 }
 
+// ---- training windows gathered from a resident series ---------------------------------------------------
+// One limit with the context gate: T <= 2048.  The lags travel by value in the kernel's parameter block (8 KB at the
+// limit, above the classic 4 KB: CUDA >= 12.1 on sm_70+), read from the constant bank through __grid_constant__.
+constexpr int kMaxGatherSteps = 2048;
+struct GatherLags {
+    int32_t v[kMaxGatherSteps];
+};
+constexpr int kGatherThreads = 256;
+constexpr int kGatherUnroll = 4;                        // elements per thread per tile: loads issued before stores
+constexpr int64_t kGatherTile = kGatherThreads * kGatherUnroll;
+
+// A tile is one destination row (an obs row (k, t) or the target row k) times one span of kGatherTile elements of V
+// (float4 or float).  Slot j < t_len of window k reads series row wrap(first + k - lags[j]), slot t_len reads first + k.
+// A plain copy: loads and stores only, so output bits are input bits.
+template <typename V>
+__global__ void __launch_bounds__(kGatherThreads)
+window_gather_kernel(const V* __restrict__ series, int64_t s_len, int64_t row, const __grid_constant__ GatherLags lags,
+                     int t_len, int64_t first, int64_t b, V* __restrict__ obs, V* __restrict__ y) {
+    const int64_t spans = (row + kGatherTile - 1) / kGatherTile;
+    const int64_t tiles = b * (t_len + 1) * spans;
+    for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int64_t slot = tile / spans;
+        const int64_t c0 = (tile - slot * spans) * kGatherTile + threadIdx.x;
+        const int64_t k = slot / (t_len + 1);
+        const int j = (int)(slot - k * (t_len + 1));
+        int64_t src_row = first + k;
+        V* dst = y + k * row;
+        if (j < t_len) {
+            src_row -= lags.v[j];
+            if (src_row < 0) src_row += s_len;             // numpy's negative index (checked >= -s_len at enqueue)
+            dst = obs + (k * t_len + j) * row;
+        }
+        const V* src = series + src_row * row;
+        V v[kGatherUnroll];
+#pragma unroll
+        for (int u = 0; u < kGatherUnroll; ++u) {
+            const int64_t c = c0 + u * kGatherThreads;
+            if (c < row) v[u] = src[c];
+        }
+#pragma unroll
+        for (int u = 0; u < kGatherUnroll; ++u) {
+            const int64_t c = c0 + u * kGatherThreads;
+            if (c < row) dst[c] = v[u];
+        }
+    }
+}
+
+// whether the byte ranges [p, p + pb) and [q, q + qb) share a byte
+bool overlaps(const void* p, int64_t pb, const void* q, int64_t qb) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p), c = reinterpret_cast<uintptr_t>(q);
+    return a < c + (uintptr_t)qb && c < a + (uintptr_t)pb;
+}
+
 }  // namespace
 
 extern "C" {
+
+int32_t stmgcn_window_gather(const float* series, int64_t s_len, int64_t row, const int32_t* lags, int32_t t_len,
+                             int64_t first, int64_t b, float* obs, float* y, void* stream) {
+    STMGCN_REQUIRE(series && lags && obs && y, STMGCN_ERR_ARG, "window_gather: null pointer");
+    STMGCN_REQUIRE(s_len > 0 && row > 0 && b > 0 && t_len > 0, STMGCN_ERR_SHAPE,
+                   "window_gather: bad shape (s_len=%lld row=%lld b=%lld t_len=%d)", (long long)s_len, (long long)row,
+                   (long long)b, (int)t_len);
+    STMGCN_REQUIRE(t_len <= kMaxGatherSteps, STMGCN_ERR_SHAPE, "window_gather: T=%d (max %d)", (int)t_len, kMaxGatherSteps);
+    // byte counts below must fit in int64: series s_len*row floats, obs b*t_len*row floats (b <= s_len by the next check)
+    STMGCN_REQUIRE(row <= INT64_MAX / 4 / s_len / (kMaxGatherSteps + 1), STMGCN_ERR_SHAPE,
+                   "window_gather: s_len=%lld x row=%lld too large", (long long)s_len, (long long)row);
+    STMGCN_REQUIRE(first >= 0 && first <= s_len && b <= s_len - first, STMGCN_ERR_SHAPE,
+                   "window_gather: windows [%lld, %lld) run past the series (s_len=%lld)", (long long)first,
+                   (long long)first + (long long)b, (long long)s_len);
+    GatherLags lv;
+    for (int t = 0; t < t_len; ++t) {
+        STMGCN_REQUIRE(lags[t] >= 0, STMGCN_ERR_ARG, "window_gather: lags[%d]=%d is negative", t, (int)lags[t]);
+        STMGCN_REQUIRE(first - lags[t] >= -s_len, STMGCN_ERR_SHAPE,
+                       "window_gather: lags[%d]=%d reaches row %lld, before -s_len=%lld", t, (int)lags[t],
+                       (long long)(first - lags[t]), (long long)-s_len);
+        lv.v[t] = lags[t];
+    }
+    const int64_t s_bytes = s_len * row * 4, obs_bytes = b * t_len * row * 4, y_bytes = b * row * 4;
+    STMGCN_REQUIRE(!overlaps(obs, obs_bytes, series, s_bytes) && !overlaps(y, y_bytes, series, s_bytes), STMGCN_ERR_ARG,
+                   "window_gather: obs / y overlap the series");
+    STMGCN_REQUIRE(!overlaps(obs, obs_bytes, y, y_bytes), STMGCN_ERR_ARG, "window_gather: obs and y overlap");
+    const bool vec4 = row % 4 == 0 && aligned16(series) && aligned16(obs) && aligned16(y);
+    const int64_t row_v = vec4 ? row / 4 : row;
+    const int64_t tiles = b * (t_len + 1) * ceil_div(row_v, kGatherTile);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const unsigned grid = (unsigned)(tiles < cap ? tiles : cap);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (vec4)
+        window_gather_kernel<float4><<<grid, kGatherThreads, 0, st>>>((const float4*)series, s_len, row_v, lv, t_len, first,
+                                                                      b, (float4*)obs, (float4*)y);
+    else
+        window_gather_kernel<float><<<grid, kGatherThreads, 0, st>>>(series, s_len, row_v, lv, t_len, first, b, obs, y);
+    count_launch();
+    return check_launch("window_gather");
+}
 
 int32_t stmgcn_obs_to_node_major(const float* obs, float* xo, float* xt, int64_t b, int64_t t, int64_t n,
                                  int64_t c, void* stream) {

@@ -32,6 +32,7 @@ SIGNATURES = [
                                       c_int64, _P, _P, _P]),
     ("stmgcn_adj_norm_bwd", c_int32, [c_int32, c_int64, _P, _P, _P, _P, _P, c_int64, _P, _P, c_int64, c_float, _P, _P,
                                       _P, c_int64, _P, _P]),
+    ("stmgcn_window_gather", c_int32, [_P, c_int64, c_int64, POINTER(c_int32), c_int32, c_int64, c_int64, _P, _P, _P]),
     ("stmgcn_obs_to_node_major", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),
     ("stmgcn_obs_grad", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),
     ("stmgcn_proj_fwd", c_int32, [_P, c_int64, c_int32, c_int64, c_int32, _P, _P, c_int32, c_int32, _P, _P,
