@@ -17,30 +17,10 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
 import statistics
-import subprocess
 import sys
 
-REPO = os.path.dirname(os.path.abspath(__file__))
-for _p in (REPO, os.path.join(REPO, "st-mgcn_b200"), os.path.join(REPO, "oracle")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
-
-
-def card():
-    """(name, power limit) of the device, read with nvidia-smi (queried only, nothing is set)."""
-    import torch
-    name, limit = torch.cuda.get_device_name(0), "unknown"
-    try:
-        idx = os.environ.get("CUDA_VISIBLE_DEVICES", "0").split(",")[0] or "0"
-        q = subprocess.run(["nvidia-smi", "-i", idx, "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30)
-        if q.returncode == 0 and q.stdout.strip():
-            name, limit = (v.strip() for v in q.stdout.strip().splitlines()[0].split(",", 1))
-    except (OSError, subprocess.SubprocessError):
-        pass
-    return name, limit
+from benchlib import alternate, device_record, require_cuda, setup_paths
 
 
 def main():
@@ -51,14 +31,13 @@ def main():
     ap.add_argument("--order", type=int, default=2)
     ap.add_argument("--workload", default="cfg3")
     args = ap.parse_args()
+    require_cuda("bench_diffusion.py")
+    setup_paths()
 
     import numpy as np
     import scipy.sparse as sp
     import torch
     from torch import nn
-
-    if not torch.cuda.is_available():
-        sys.exit("bench_diffusion.py needs a CUDA device (an H100)")
     import GCN
     import STMGCN
     import diffusion_oracle as D
@@ -107,23 +86,9 @@ def main():
                      f"(relative error {checks[kind]:.2e} > 1e-4): no time reported")
         del out
 
-    for kind in kinds:
-        for _ in range(args.warmup):
-            step(kind)
-    torch.cuda.synchronize()
-    times = {kind: [] for kind in kinds}
-    for _ in range(args.rounds):
-        for kind in kinds:
-            start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            start.record()
-            for _ in range(args.steps):
-                loss = step(kind)
-            end.record()
-            torch.cuda.synchronize()
-            assert bool(torch.isfinite(loss))
-            times[kind].append(start.elapsed_time(end) / args.steps)
-
-    name, limit = card()
+    times, _ = alternate({kind: lambda kind=kind: step(kind) for kind in kinds}, args.rounds, args.steps, args.warmup)
+    assert all(bool(torch.isfinite(step(kind))) for kind in kinds)     # every timed step computes this same loss
+    name, limit = device_record()
     ms = {kind: statistics.median(t) for kind, t in times.items()}
     result = {
         "workload": args.workload, "n_regions": w.n_regions, "graphs": w.n_graphs, "seq_len": w.seq_len,

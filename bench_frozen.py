@@ -18,25 +18,10 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 
-REPO = os.path.dirname(os.path.abspath(__file__))
-for _p in (REPO, os.path.join(REPO, "st-mgcn_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+from benchlib import alternate, device_record, require_cuda, setup_paths
 
 VARIANTS = ("all_trainable", "frozen_obs", "lstm_frozen")
-
-
-def _power_limit():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                             capture_output=True, text=True, timeout=30)
-        return out.stdout.strip() or None
-    except (OSError, subprocess.SubprocessError):
-        return None
 
 
 def main() -> None:
@@ -46,12 +31,15 @@ def main() -> None:
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
+    require_cuda("bench_frozen.py")
+    setup_paths()
 
     import torch
     from torch import nn
     import GCN
     import STMGCN
-    from stmgcn_b200 import _lib, ops, synth
+    import stmgcn_oracle as O
+    from stmgcn_b200 import ops, synth
 
     w = synth.WORKLOADS[args.workload]
     dev = torch.device("cuda:0")
@@ -77,9 +65,6 @@ def main() -> None:
         crit(model(obs_seq=xs, sta_adj_list=sups), y).backward()
         return xs
 
-    def rel(a, b):
-        return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
-
     # ---- the requested gradients against the all-trainable run's (which also takes d obs) ----
     model = make(gconv_activation=None)
     params = dict(model.named_parameters())
@@ -94,24 +79,11 @@ def main() -> None:
         if variant == "frozen_obs":
             got["obs"] = xs.grad
         assert all(params[k].grad is None for k in frozen), f"{variant}: a frozen parameter has a gradient"
-        errs = {k: rel(g, base[k]) for k, g in got.items()}
+        errs = {k: O.max_rel_err(g.cpu(), base[k].cpu()) for k, g in got.items()}
         check[variant] = max(errs.values())
         assert check[variant] <= 1e-4, f"{variant}: {max(errs, key=errs.get)} is {check[variant]:.2e} off"
     del model, params, base, base_x
     model = make()                                  # the timed model: the workload's own activation
-
-    def timed(fn):
-        for _ in range(args.warmup):
-            fn()
-        torch.cuda.synchronize()
-        n0 = _lib.launch_count()
-        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        start.record()
-        for _ in range(args.steps):
-            fn()
-        end.record()
-        torch.cuda.synchronize()
-        return start.elapsed_time(end) / args.steps, (_lib.launch_count() - n0) // args.steps
 
     # ---- the LSTM backward alone: one CG_LSTM's stack, the tape of one forward, backward with / without wgrad ----
     cg = model.rnn_list[0]
@@ -132,28 +104,20 @@ def main() -> None:
             _, _, _, tape = ops._exact_forward(xo, s_gate, None, None, lyr, hid, False, ws, True)
             return ops._exact_backward_ex(xo, s_gate, tape, lyr, hid, d_top, wgrad=wgrad)
     full, part = lstm_bwd(True), lstm_bwd(False)
-    check["lstm_bwd_d_s"] = rel(part[0], full[0])
+    check["lstm_bwd_d_s"] = O.max_rel_err(part[0].cpu(), full[0].cpu())
     assert check["lstm_bwd_d_s"] <= 1e-4 and all(g is None for g in part[1])
 
-    runs = {v: [] for v in VARIANTS}
-    launches = {}
-    lstm_runs = {True: [], False: []}
-    lstm_launches = {}
-    for _ in range(args.rounds):
-        for v in VARIANTS:
-            ms, launches[v] = timed(lambda: step(model, v))
-            runs[v].append(ms)
-        for wgrad in (True, False):
-            ms, lstm_launches[wgrad] = timed(lambda: lstm_bwd(wgrad))
-            lstm_runs[wgrad].append(ms)
+    lstm = {"with_wgrad": lambda: lstm_bwd(True), "without_wgrad": lambda: lstm_bwd(False)}
+    runs, launches = alternate({**{v: lambda v=v: step(model, v) for v in VARIANTS}, **lstm},
+                               args.rounds, args.steps, args.warmup)
+    name, power_limit = device_record()
     print(json.dumps({
-        "workload": w.name, "device": torch.cuda.get_device_name(dev), "power_limit": _power_limit(),
+        "workload": w.name, "device": name, "power_limit": power_limit,
         "lstm_path": ops.lstm_path(), "planes": ops.lstm_planes() if on_tc else None, "steps": args.steps,
         "ms_per_step": {v: [round(r, 3) for r in runs[v]] for v in VARIANTS},
-        "gpu_launches": launches,
-        "lstm_bwd_ms": {"with_wgrad": [round(r, 3) for r in lstm_runs[True]],
-                        "without_wgrad": [round(r, 3) for r in lstm_runs[False]]},
-        "lstm_bwd_launches": {"with_wgrad": lstm_launches[True], "without_wgrad": lstm_launches[False]},
+        "gpu_launches": {v: launches[v] for v in VARIANTS},
+        "lstm_bwd_ms": {k: [round(r, 3) for r in runs[k]] for k in lstm},
+        "lstm_bwd_launches": {k: launches[k] for k in lstm},
         "lstm_bwd_includes_forward": not on_tc,
         "max_rel_err_vs_all_trainable": {k: float(f"{v:.3e}") for k, v in check.items()}}))
 

@@ -1,5 +1,6 @@
 """Extra cost of the input gradient: one cfg3 training step (forward, MSE, backward) with and without
-``obs_seq.requires_grad``, timed alternately with CUDA events on one GPU.  Prints one JSON line.
+``obs_seq.requires_grad``, timed alternately with CUDA events on one GPU.  Prints one JSON line with the card's name
+and power limit.
 
     python bench_input_grad.py [--workload cfg3] [--steps 20] [--rounds 3]
 
@@ -10,13 +11,8 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import sys
 
-REPO = os.path.dirname(os.path.abspath(__file__))
-for _p in (REPO, os.path.join(REPO, "st-mgcn_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+from benchlib import alternate, device_record, require_cuda, setup_paths
 
 
 def main() -> None:
@@ -26,12 +22,14 @@ def main() -> None:
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
+    require_cuda("bench_input_grad.py")
+    setup_paths()
 
     import torch
     from torch import nn
     import GCN
     import STMGCN
-    from stmgcn_b200 import _lib, synth
+    from stmgcn_b200 import synth
 
     w = synth.WORKLOADS[args.workload]
     dev = torch.device("cuda:0")
@@ -47,31 +45,14 @@ def main() -> None:
         xs = x.detach().requires_grad_(grad)
         crit(model(obs_seq=xs, sta_adj_list=sups), y).backward()
 
-    def timed(grad: bool):
-        for _ in range(args.warmup):
-            step(grad)
-        torch.cuda.synchronize()
-        n0 = _lib.launch_count()
-        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        start.record()
-        for _ in range(args.steps):
-            step(grad)
-        end.record()
-        torch.cuda.synchronize()
-        return start.elapsed_time(end) / args.steps, (_lib.launch_count() - n0) // args.steps
-
-    runs = {False: [], True: []}
-    launches = {}
-    for _ in range(args.rounds):
-        for grad in (False, True):
-            ms, launches[grad] = timed(grad)
-            runs[grad].append(ms)
-    base, with_dx = min(runs[False]), min(runs[True])
-    print(json.dumps({"workload": w.name, "device": torch.cuda.get_device_name(dev), "steps": args.steps,
-                      "ms_per_step": [round(v, 3) for v in runs[False]],
-                      "ms_per_step_obs_grad": [round(v, 3) for v in runs[True]],
-                      "extra_ms": round(with_dx - base, 3), "gpu_launches": launches[False],
-                      "gpu_launches_obs_grad": launches[True]}))
+    runs, launches = alternate({"base": lambda: step(False), "obs_grad": lambda: step(True)},
+                               args.rounds, args.steps, args.warmup)
+    name, power_limit = device_record()
+    print(json.dumps({"workload": w.name, "device": name, "power_limit": power_limit, "steps": args.steps,
+                      "ms_per_step": [round(v, 3) for v in runs["base"]],
+                      "ms_per_step_obs_grad": [round(v, 3) for v in runs["obs_grad"]],
+                      "extra_ms": round(min(runs["obs_grad"]) - min(runs["base"]), 3),
+                      "gpu_launches": launches["base"], "gpu_launches_obs_grad": launches["obs_grad"]}))
 
 
 if __name__ == "__main__":

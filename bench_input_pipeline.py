@@ -7,8 +7,9 @@ Two shapes: cfg3's (4096 regions, C = 1, batch 64, cpt (8, 2, 2): T = 12) on fiv
 (58 regions, batch 32, cpt (3, 1, 1), its default dates) on one year.  Before any time is measured, every batch of the
 first and last few of each mode is compared bit for bit with the reference loader's.  Then, per shape:
 
-* ``ms_per_batch``: wall time of a full pass over the training mode divided by its batches, the device synchronised at
-  the end, for each loader; the two alternate for ``--rounds`` rounds and the median round is reported;
+* ``ms_per_batch``: a full pass over the training mode between CUDA events, the device idle at the start and
+  synchronised at the end (so the host's iteration is inside the window), divided by its batches, for each loader; the
+  two alternate for ``--rounds`` rounds and the median round is reported;
 * ``gather_us`` / ``gather_gbs_written``: one batch's ``stmgcn_window_gather`` alone, CUDA events over ``--launches``
   launches, and the bytes it writes (x and y) over that time;
 * ``construction``: host peak RSS growth (sampled every ~1 ms) and device peak memory of ``get_data_loader`` for each
@@ -27,10 +28,8 @@ import subprocess
 import sys
 import time
 
-REPO = os.path.dirname(os.path.abspath(__file__))
-for _p in (REPO, os.path.join(REPO, "st-mgcn_b200")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+from benchlib import REPO, alternate, device_record, require_cuda, setup_paths, timed
+
 REF_DC = os.path.join(REPO, "oracle", "_ref", "Data_Container.pyc")
 
 # (name, regions, series rows, cpt, dates, batch)
@@ -124,20 +123,11 @@ def measure(shape: str, rounds: int, launches: int) -> dict:
     checked = _check_bits(loaders["reference"], loaders["device"])
 
     def epoch(kind):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        count = 0
         for _x, _y in loaders[kind]["train"]:
-            count += 1
-        torch.cuda.synchronize()
-        return (time.perf_counter() - t0) * 1e3 / count
+            pass
 
-    for kind in loaders:
-        epoch(kind)                                      # warm-up
-    times = {kind: [] for kind in loaders}
-    for _ in range(rounds):
-        for kind in loaders:
-            times[kind].append(epoch(kind))
+    ms, _ = alternate({kind: lambda kind=kind: epoch(kind) for kind in loaders}, rounds, 1, 1)
+    times = {kind: [t / len(loaders[kind]["train"]) for t in v] for kind, v in ms.items()}
 
     # one full batch's gather alone
     dev = loaders["device"]["train"]
@@ -151,15 +141,7 @@ def measure(shape: str, rounds: int, launches: int) -> dict:
     def gather():
         _lib.check(_lib.lib.stmgcn_window_gather(series.data_ptr(), series.shape[0], row, dev.lags, dev.t_len, first,
                                                  b, x.data_ptr(), y.data_ptr(), st), "window_gather")
-    for _ in range(10):
-        gather()
-    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    start.record()
-    for _ in range(launches):
-        gather()
-    end.record()
-    torch.cuda.synchronize()
-    us = start.elapsed_time(end) * 1e3 / launches
+    us = timed(gather, launches, 10)[0] * 1e3
     written = (x.numel() + y.numel()) * 4
 
     construction = {}
@@ -176,31 +158,19 @@ def measure(shape: str, rounds: int, launches: int) -> dict:
             "gather_gbs_written": round(written / us / 1e3, 1), "construction": construction}
 
 
-def _card():
-    import torch
-    out = {"device": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30)
-        out["nvidia_smi"] = q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else None
-    except (OSError, subprocess.TimeoutExpired):
-        out["nvidia_smi"] = None
-    return out
-
-
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--construction", nargs=2, metavar=("KIND", "SHAPE"), help=argparse.SUPPRESS)
     args = ap.parse_args()
+    require_cuda("bench_input_pipeline.py")
+    setup_paths()
     if args.construction:
         construction_child(*args.construction)
         return
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_input_pipeline.py needs a CUDA device")
-    result = _card()
+    name, limit = device_record()
+    result = {"device": name, "power_limit": limit, "nvidia_smi": f"{name}, {limit}"}
     for shape in SHAPES:
         result[shape] = measure(shape, args.rounds, args.launches)
     print(json.dumps(result))

@@ -16,36 +16,8 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 
-REPO = os.path.dirname(os.path.abspath(__file__))
-for _p in (REPO, os.path.join(REPO, "st-mgcn_b200"), os.path.join(REPO, "oracle")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
-
-
-def _card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = (s.strip() for s in q.split(","))
-        return name, power
-    except Exception:           # the timing stands without the record; say so
-        import torch
-        return torch.cuda.get_device_name(0), "unknown"
-
-
-def _laplacian64(adj, w):
-    """Dense fp64 ``L~`` of a chebyshev ``LearnableAdjacency`` at the weights ``w`` (differentiable in ``w``)."""
-    import torch
-    n = adj.n
-    rows, cols = adj.edges()
-    a = torch.zeros(n, dtype=w.dtype, device=w.device).index_add(0, rows, w).pow(-0.5)
-    lap = torch.zeros(n, n, dtype=w.dtype, device=w.device).index_put((rows, cols), -adj.scale * ((a[rows] * w) * a[cols]),
-                                                                      accumulate=True)
-    return lap + (adj.scale - 1.0) * torch.eye(n, dtype=w.dtype, device=w.device)
+from benchlib import alternate, device_record, require_cuda, setup_paths
 
 
 def main():
@@ -54,6 +26,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=4)
     ap.add_argument("--reps", type=int, default=50)
     args = ap.parse_args()
+    require_cuda("bench_learnable_adjacency.py")
+    setup_paths()
 
     import torch
     from torch import nn
@@ -63,8 +37,6 @@ def main():
     from stmgcn_b200 import _lib, ops, synth
     from stmgcn_b200.graphs import GraphedStep
 
-    if not torch.cuda.is_available():
-        raise RuntimeError("bench_learnable_adjacency.py needs a CUDA device")
     dev = torch.device("cuda:0")
     w = synth.WORKLOADS["cfg3"]
     ops.set_lstm_planes(2)
@@ -110,11 +82,8 @@ def main():
     leaves, stacks = [], []
     for m in mods:
         leaf = m.weight.detach().double().clone().requires_grad_(True)
-        lap = _laplacian64(m, leaf)
-        polys = [torch.eye(m.n, dtype=torch.float64, device=dev), lap]
-        while len(polys) < m.ks:
-            polys.append(2.0 * (lap @ polys[-1]) - polys[-2])
-        stacks.append(torch.stack(polys))
+        adj64 = torch.zeros(m.n, m.n, dtype=torch.float64, device=dev).index_put(m.edges(), leaf, accumulate=True)
+        stacks.append(O.chain_stack_dense([O.rescaled_laplacian_dense(adj64, m.lambda_max)], m.order))
         leaves.append(leaf)
     out64 = O.dense_st_mgcn(params, x2.double(), stacks, masks=masks)
     loss64 = ((out64 - y2.double()) ** 2).mean()
@@ -127,28 +96,12 @@ def main():
         raise SystemExit(f"bench_learnable_adjacency: parity failed: loss {err_loss:.3e}, d weight {err_grad:.3e}")
 
     # ---- the step, five ways, alternating -----------------------------------------------------------------------------
-    def timed(fn, steps):
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / steps
-
     graphed_fixed = GraphedStep(model, crit, x, y, fixed)
     graphed_mods = GraphedStep(model, crit, x, y, mods)
     variants = {"fixed": lambda: step(fixed), "process_sparse_per_step": lambda: step(rebuilt),
                 "module_eager": lambda: step(mods), "module_graphed": lambda: graphed_mods(),
                 "fixed_graphed": lambda: graphed_fixed()}
-    for _ in range(3):
-        for fn in variants.values():
-            fn()
-    ms = {k: [] for k in variants}
-    for _ in range(args.rounds):
-        for k, fn in variants.items():
-            ms[k].append(timed(fn, args.steps))
+    ms, _ = alternate(variants, args.rounds, args.steps, 3)
 
     # ---- the normalisation's launches alone ---------------------------------------------------------------------------
     m = mods[0]
@@ -166,18 +119,15 @@ def main():
     def bwd():
         _lib.check(ops.L.stmgcn_adj_norm_bwd(*head, g.data_ptr(), None, work_b.data_ptr(), work_b.numel(), dw.data_ptr(),
                                              ops._stream()), "adj_norm_bwd")
-    for _ in range(5):
-        fwd()
-        bwd()
-    t_f = [timed(fwd, args.reps) * 1e3 for _ in range(args.rounds)]
-    t_b = [timed(bwd, args.reps) * 1e3 for _ in range(args.rounds)]
+    norm_ms, _ = alternate({"fwd": fwd, "bwd": bwd}, args.rounds, args.reps, 5)
 
-    name, power = _card()
+    name, power = device_record()
     med = lambda v: sorted(v)[len(v) // 2]      # noqa: E731
     print(json.dumps(dict(
         bench="learnable_adjacency", workload="cfg3", card=name, power_limit=power, learnable_graphs=len(mods),
         nnz_per_graph=[int(i.shape[1]) for i in idx], step_ms_median={k: med(v) for k, v in ms.items()},
-        step_ms_rounds=ms, norm_fwd_us_median=med(t_f), norm_bwd_us_median=med(t_b),
+        step_ms_rounds=ms, norm_fwd_us_median=med(norm_ms["fwd"]) * 1e3,
+        norm_bwd_us_median=med(norm_ms["bwd"]) * 1e3,
         parity=dict(windows=2, loss_rel_err=err_loss, d_weight_rel_err=err_grad))))
 
 

@@ -16,29 +16,12 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
 import statistics
-import subprocess
-import sys
 
-REPO = os.path.dirname(os.path.abspath(__file__))
-for _p in (REPO, os.path.join(REPO, "st-mgcn_b200"), os.path.join(REPO, "oracle")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+from benchlib import device_record, require_cuda, setup_paths, timed
 
 CASES = (("cfg2", 1), ("cfg3", 2))      # (workload, bf16 planes of the LSTM)
 SAME = 2e-5                             # two-plane bar of two fresh copies of one model (tests/test_gpu_param_updates.py)
-
-
-def card() -> dict:
-    """Name and power limit of GPU 0 (read-only query)."""
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                             capture_output=True, text=True, timeout=30).stdout.strip()
-        name, limit = (v.strip() for v in out.split(","))
-        return {"gpu": name, "power_limit": limit}
-    except Exception as e:          # the numbers still stand; say why the card is not named
-        return {"gpu": f"unknown ({e})", "power_limit": "unknown"}
 
 
 def memoised(ops):
@@ -66,6 +49,8 @@ def main() -> None:
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     args = ap.parse_args()
+    require_cuda("bench_pack.py")
+    setup_paths()
 
     import torch
     from torch import nn
@@ -74,9 +59,9 @@ def main() -> None:
     import stmgcn_oracle as O
     from stmgcn_b200 import ops, synth
 
-    assert torch.cuda.is_available(), "bench_pack.py needs a CUDA device"
     dev = torch.device("cuda:0")
-    result = dict(card(), steps_per_variant=args.steps * args.rounds)
+    gpu, limit = device_record()
+    result = dict(gpu=gpu, power_limit=limit, steps_per_variant=args.steps * args.rounds)
     real = (ops._lstm16_images, ops._proj_images)
     old_planes = ops.lstm_planes()
     for name, planes in CASES:
@@ -113,20 +98,14 @@ def main() -> None:
             del res
             assert diff <= max(SAME, 4 * spread), f"{name}: old and new differ by {diff:.2e} (new vs new: {spread:.2e})"
 
+            # one sample per step, not per round: the summary is a distribution over steps (median, p10, p90)
             times = {"new": [], "old": []}
             for _ in range(args.rounds):
                 for variant in ("old", "new"):
                     use(variant)
                     for _ in range(args.warmup):
                         step()
-                    torch.cuda.synchronize()
-                    for _ in range(args.steps):
-                        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                        a.record()
-                        step()
-                        b.record()
-                        b.synchronize()
-                        times[variant].append(a.elapsed_time(b))
+                    times[variant] += [timed(step, 1)[0] for _ in range(args.steps)]
         finally:
             ops._lstm16_images, ops._proj_images = real
             memo.clear()
@@ -139,15 +118,7 @@ def main() -> None:
                 ops._lstm16_images([wt.detach() for wt in cg._lstm_weights()], cg.lstm_num_layers, cg.input_dim)
                 ops._proj_images(gcn.W.detach(), ks, gcn.input_dim, True)
 
-        for _ in range(args.warmup):
-            packs()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        reps = 50
-        a.record()
-        for _ in range(reps):
-            packs()
-        b.record()
-        b.synchronize()
+        pack_ms, _ = timed(packs, 50, args.warmup)
 
         def summary(v):
             q = statistics.quantiles(v, n=10)
@@ -155,7 +126,7 @@ def main() -> None:
 
         result[name] = {"planes": planes, "old": summary(times["old"]), "new": summary(times["new"]),
                         "new_minus_old_median_ms": round(statistics.median(times["new"]) - statistics.median(times["old"]), 3),
-                        "pack_ms_per_step_serial": round(a.elapsed_time(b) / reps, 4),
+                        "pack_ms_per_step_serial": round(pack_ms, 4),
                         "max_rel_diff_old_vs_new": float(f"{diff:.2e}"),
                         "max_rel_diff_new_vs_new": float(f"{spread:.2e}")}
         del model, sups, x, y

@@ -17,25 +17,8 @@ from __future__ import annotations
 
 import argparse
 import json
-import os
-import subprocess
-import sys
 
-REPO = os.path.dirname(os.path.abspath(__file__))
-for _p in (REPO, os.path.join(REPO, "st-mgcn_b200"), os.path.join(REPO, "oracle")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
-
-
-def _card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = (s.strip() for s in q.split(","))
-        return name, power
-    except Exception:           # the timing stands without the record; say so
-        import torch
-        return torch.cuda.get_device_name(0), "unknown"
+from benchlib import alternate, device_record, require_cuda, setup_paths
 
 
 def main():
@@ -44,6 +27,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=4)
     ap.add_argument("--reps", type=int, default=50)
     args = ap.parse_args()
+    require_cuda("bench_support_grad.py")
+    setup_paths()
 
     import torch
     from torch import nn
@@ -52,8 +37,6 @@ def main():
     import stmgcn_oracle as O
     from stmgcn_b200 import ops, synth
 
-    if not torch.cuda.is_available():
-        raise RuntimeError("bench_support_grad.py needs a CUDA device")
     dev = torch.device("cuda:0")
     w = synth.WORKLOADS["cfg3"]
     ops.set_lstm_planes(2)
@@ -106,11 +89,8 @@ def main():
         leaf = h.vals.detach().double().clone().requires_grad_(True)
         rows = torch.repeat_interleave(torch.arange(n, device=dev), (h.rowptr[1:] - h.rowptr[:-1]).long())
         lap = torch.zeros(n, n, dtype=torch.float64, device=dev).index_put((rows, h.colidx.long()), leaf, accumulate=True)
-        polys = [torch.eye(n, dtype=torch.float64, device=dev), lap]
-        while len(polys) < h.ks:
-            polys.append(2.0 * (lap @ polys[-1]) - polys[-2])
         leaves.append(leaf)
-        stacks.append(torch.stack(polys))
+        stacks.append(O.chain_stack_dense([lap], h.ks - 1))
     # the reference takes the step's ReLU masks: a pre-activation within rounding distance of the kink takes the same
     # branch in both (one flipped entry moves a d vals entry, a sum over one row's B*64 features, by about 1/64)
     out64 = O.dense_st_mgcn(params, x2.double(), stacks, masks=masks)
@@ -124,23 +104,9 @@ def main():
         raise SystemExit(f"bench_support_grad: parity failed: loss {err_loss:.3e}, d vals {err_grad:.3e}")
 
     # ---- the step, alternating learnable and fixed handles ------------------------------------------------------------
-    def timed(fn, steps):
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / steps
-
-    for _ in range(3):
-        step(learnable)
-        step(fixed)
-    ms_learn, ms_fixed = [], []
-    for _ in range(args.rounds):
-        ms_learn.append(timed(lambda: step(learnable), args.steps))
-        ms_fixed.append(timed(lambda: step(fixed), args.steps))
+    step_ms, _ = alternate({"learnable": lambda: step(learnable), "fixed": lambda: step(fixed)},
+                           args.rounds, args.steps, 3)
+    ms_learn, ms_fixed = step_ms["learnable"], step_ms["fixed"]
 
     # ---- the SDDMM launches of one GCN against its K forward SpMM launches ------------------------------------------
     g = fixed[0].support_set().graphs[0]
@@ -161,17 +127,11 @@ def main():
             for j in range(2, k + 1):
                 ops.spmm_step(g, False, 2.0, s[j - 1], -1.0, s[j - 2], 0.0, None, s[j])
 
-        for _ in range(5):
-            sddmm()
-            spmm()
-        t_sd, t_sp = [], []
-        for _ in range(args.rounds):
-            t_sd.append(timed(sddmm, args.reps) * 1e3)
-            t_sp.append(timed(spmm, args.reps) * 1e3)
-        kernels[name] = dict(f_total=f_total, sddmm_us=min(t_sd), spmm_forward_us=min(t_sp),
-                             ratio=min(t_sd) / min(t_sp))
+        kernel_ms, _ = alternate({"sddmm": sddmm, "spmm": spmm}, args.rounds, args.reps, 5)
+        t_sd, t_sp = min(kernel_ms["sddmm"]) * 1e3, min(kernel_ms["spmm"]) * 1e3
+        kernels[name] = dict(f_total=f_total, sddmm_us=t_sd, spmm_forward_us=t_sp, ratio=t_sd / t_sp)
 
-    name, power = _card()
+    name, power = device_record()
     print(json.dumps(dict(
         bench="support_grad", workload="cfg3", card=name, power_limit=power, learnable_graphs=len(weights),
         nnz_per_graph=[int(i.shape[1]) for i in idx],

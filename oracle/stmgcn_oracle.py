@@ -51,7 +51,7 @@ def rescaled_laplacian_dense(adj: torch.Tensor, lambda_max: float = 2.0) -> torc
     """
     d = adj.sum(dim=1).pow(-0.5)
     a_norm = d[:, None] * adj * d[None, :]
-    eye = torch.eye(adj.shape[0], dtype=adj.dtype)
+    eye = torch.eye(adj.shape[0], dtype=adj.dtype, device=adj.device)
     lap = eye - a_norm
     return (2.0 / lambda_max) * lap - eye
 
@@ -69,8 +69,9 @@ def chebyshev_supports_dense(adj: torch.Tensor, order: int, lambda_max: float = 
 
 def chain_stack_dense(mats: Sequence[torch.Tensor], order: int) -> torch.Tensor:
     """Dense stack of Chebyshev recurrence chains sharing ``T_0 = I``: ``[I, T_1(X_0)..T_K(X_0), T_1(X_1)..]`` for the
-    chain matrices ``X_c`` of ``mats`` (in their dtype), ``K = order``: the stack a support set of chains stands for."""
-    eye = torch.eye(mats[0].shape[0], dtype=mats[0].dtype)
+    chain matrices ``X_c`` of ``mats`` (in their dtype and on their device), ``K = order``: the stack a support set of
+    chains stands for."""
+    eye = torch.eye(mats[0].shape[0], dtype=mats[0].dtype, device=mats[0].device)
     out = [eye]
     for x in mats:
         polys = [eye, x]
