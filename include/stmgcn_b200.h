@@ -97,6 +97,19 @@ int32_t stmgcn_csr_sddmm(int64_t n, const int32_t* rowptr, const int32_t* colidx
                          const float* const* a, const float* const* b, const float* coef, int32_t round_b_bf16,
                          int64_t f_total, float* work, int64_t work_count, float* dvals, void* stream);
 
+/* ---- K1d: gradient of dense support slices (GCN.py:35 differentiated in A[k]) ---------------------------------------
+ *   da[k][i][j] = sum_f U_k[i][f] * x[j][f]     (dA_k = U_k x^T),   k < ks, i, j < n, f < f_total
+ * U_k = u + k * u_stride and x are (n, f_total) fp32 row-major: U_k = dL/dS_k, the gradient of the slice's product
+ * S_k = A_k x (stmgcn_proj_bwd's u, taken before the adjoint Clenshaw overwrites it), x the features it multiplied.
+ * da: (ks, n, n) row-major, OVERWRITTEN (not accumulated).  1 <= ks <= 8, 1 <= n < 2^24, 1 <= f_total < 2^31,
+ * u_stride >= 0; segments of u may overlap one another, but da shares no byte with u (its ks segments) or x (checked).
+ * 3xTF32 on the tensor cores (fp32-grade, as the projection); 16-byte loads when f_total % 4 == 0 and u, x (and, ks > 1,
+ * u_stride % 4 == 0) allow them, scalar loads otherwise; any n and f_total.  One launch.  Every element has one owner
+ * and a fixed summation order: two calls with the same inputs give bit-identical da.  A NaN in row i of U_k makes row i
+ * of dA_k NaN, a NaN in row j of x column j of every dA_k; an Inf gives NaN (inf_through_split_operands). */
+int32_t stmgcn_dense_support_grad(int64_t n, int64_t f_total, int32_t ks, const float* u, int64_t u_stride,
+                                  const float* x, float* da, void* stream);
+
 /* ---- K1c: the supports of a learnable adjacency on a fixed sparsity pattern ----------------------------------------
  * The pattern is an n x n CSR (rowptr, colidx; nnz = rowptr[n] entries, no repeated (i, j)) and its transpose's structure
  * rowptr_t, colidx_t with perm_t: CSR^T position p holds CSR entry perm_t[p].  widx (int32 per pattern entry) gives the

@@ -32,6 +32,13 @@ int32_t ensure_dyn_smem(const void* kernel, size_t bytes);   // per-(kernel, dev
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+// whether the byte ranges [p, p + pb) and [q, q + qb) share a byte (a NULL or empty range shares none): the entry points'
+// check that an output does not alias an input
+static inline bool overlaps(const void* p, int64_t pb, const void* q, int64_t qb) {
+    if (p == nullptr || q == nullptr || pb <= 0 || qb <= 0) return false;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
+    return a < b + (uintptr_t)qb && b < a + (uintptr_t)pb;
+}
 
 // ---- persistent schedule: `work` tiles dealt round-robin over at most one CTA per SM; this CTA's count and i-th tile --
 static inline int persistent_grid(int64_t work) { return (int)(work < sm_count() ? work : sm_count()); }

@@ -175,12 +175,7 @@ struct Range {
     int64_t bytes;
 };
 
-// whether the byte ranges share a byte (a NULL or empty range shares none)
-bool overlaps(const Range& x, const Range& y) {
-    if (x.p == nullptr || y.p == nullptr || x.bytes <= 0 || y.bytes <= 0) return false;
-    const uintptr_t a = reinterpret_cast<uintptr_t>(x.p), b = reinterpret_cast<uintptr_t>(y.p);
-    return a < b + (uintptr_t)y.bytes && b < a + (uintptr_t)x.bytes;
-}
+bool overlaps(const Range& x, const Range& y) { return stmgcn::overlaps(x.p, x.bytes, y.p, y.bytes); }
 
 // the checks both directions share; returns 0 or the error already reported.  outs: the ranges the call writes, ins: the
 // ranges it reads

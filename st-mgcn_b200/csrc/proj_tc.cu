@@ -25,12 +25,14 @@ constexpr int kPThreads = 256;
 constexpr int kPWarps = kPThreads / 32;
 constexpr int kMaxSeg = 8;
 
+// hi at st + off, lo at st + kLo + off (the tile pair's lo half starts kLo bytes after its hi half)
+template <uint32_t kLo = kABytes>
 __device__ __forceinline__ void split_store(uint8_t* st, uint32_t off, const float4& v) {
     float4 hi, lo;
     hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
     lo.x = tf32_lo(v.x, hi.x); lo.y = tf32_lo(v.y, hi.y); lo.z = tf32_lo(v.z, hi.z); lo.w = tf32_lo(v.w, hi.w);
     *reinterpret_cast<float4*>(st + off) = hi;
-    *reinterpret_cast<float4*>(st + kABytes + off) = lo;
+    *reinterpret_cast<float4*>(st + kLo + off) = lo;
 }
 
 // transpose-store one float4 (4 consecutive M/N indices mn..mn+3 of row k) into a K-major swizzled tile pair
@@ -338,6 +340,130 @@ __global__ void __launch_bounds__(kPThreads, 1) proj_wgrad_tc_kernel(const __gri
     }
 }
 
+// =====================================================================================================
+// Dense support gradient: da[k][i][j] = sum_f U_k[i][f] . x[j][f]   (dA_k = U_k x^T, GCN.py:35 differentiated in A)
+// Both operands are row-major (n, f) with f contiguous, i.e. K-major as they sit in HBM: every k-block of 32 f is
+// loaded row by row (float4 when f % 4 == 0 and the pointers are 16-byte aligned, scalars otherwise; rows past n and
+// columns past f read as zeros), split to tf32 hi/lo and stored swizzled, exactly as the projection's A operand.
+// Output tile 128 (i) x 256 (j): warpgroup w owns rows 64w .. 64w+63 against all 256 columns (wgmma m64n256k8, the
+// projection backward's shape).  Two shared-memory stages: the wgmma of k-block kb run while the loads of kb + 1 are in
+// flight and their split stores fill the other stage.  Persistent over (k, row tile, column tile), column tiles
+// fastest; every output element has one owner and a fixed k order (no split-K, no atomics).
+// =====================================================================================================
+constexpr int kDsgN = 256;
+using DsgCfg = PCfg<kDsgN>;
+constexpr size_t kDsgSmem = 1024 + 2 * (size_t)DsgCfg::kStageBytes;
+
+struct DsgParams {
+    const float* u;          // U_k = u + k * u_stride, (n, f) each
+    int64_t u_stride;
+    const float* x;          // (n, f)
+    float* da;               // (ks, n, n), overwritten
+    int64_t n, f;
+    int64_t n_rt, n_ct;      // row tiles of 128, column tiles of 256
+    int64_t n_tiles;         // ks * n_rt * n_ct
+    int nkb;                 // k-blocks: ceil(f / 32)
+    bool pair_store;         // n even and da 8-byte aligned: float2 stores
+};
+
+// 4 consecutive f of row `row` of a row-major (n, f) matrix, zeros past its edges
+template <bool VEC>
+__device__ __forceinline__ float4 dsg_load(const float* m, int64_t row, int64_t col, int64_t n, int64_t f) {
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (row >= n || col >= f) return v;
+    const float* src = m + row * f + col;
+    if (VEC) return *reinterpret_cast<const float4*>(src);
+    v.x = src[0];
+    if (col + 1 < f) v.y = src[1];
+    if (col + 2 < f) v.z = src[2];
+    if (col + 3 < f) v.w = src[3];
+    return v;
+}
+
+template <bool VEC>
+__global__ void __launch_bounds__(kPThreads, 1) dense_support_grad_kernel(const __grid_constant__ DsgParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* st0 = smem_raw + smem_pad1024(smem_raw);
+    const int tid = threadIdx.x;
+    const int warp = tid >> 5;
+    const int lane = tid & 31;
+    const int wg = tid >> 7;
+    const int c = tid & 7, rsub = tid >> 3;                  // float4 column of the k-block, first row
+    constexpr int kNA = kTileM / 32, kNB = kDsgN / 32;       // float4 per thread of the A / B block
+    float acc[kDsgN / 2];
+
+    for (int64_t tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+        const int64_t ct = tile % p.n_ct, rest = tile / p.n_ct;
+        const int64_t rt = rest % p.n_rt, k = rest / p.n_rt;
+        const float* uk = p.u + k * p.u_stride;
+        const int64_t i0 = rt * kTileM, j0 = ct * kDsgN;
+        float4 va[kNA], vb[kNB];
+        auto load = [&](int kb) {
+            const int64_t col = (int64_t)kb * kKB + c * 4;
+#pragma unroll
+            for (int i = 0; i < kNA; ++i) va[i] = dsg_load<VEC>(uk, i0 + rsub + 32 * i, col, p.n, p.f);
+#pragma unroll
+            for (int i = 0; i < kNB; ++i) vb[i] = dsg_load<VEC>(p.x, j0 + rsub + 32 * i, col, p.n, p.f);
+        };
+        auto store = [&](int stage) {
+            uint8_t* st = st0 + (size_t)stage * DsgCfg::kStageBytes;
+#pragma unroll
+            for (int i = 0; i < kNA; ++i) {
+                const int row = rsub + 32 * i;
+                split_store(st, (uint32_t)row * 128u + (uint32_t)((c ^ (row & 7)) << 4), va[i]);
+            }
+#pragma unroll
+            for (int i = 0; i < kNB; ++i) {
+                const int row = rsub + 32 * i;
+                split_store<DsgCfg::kBBytes>(st + 2 * kABytes, (uint32_t)row * 128u + (uint32_t)((c ^ (row & 7)) << 4), vb[i]);
+            }
+        };
+        load(0);
+        __syncthreads();                                     // both warpgroups are done with the previous tile's stages
+        store(0);
+        fence_proxy_async_smem();
+        __syncthreads();
+        for (int kb = 0; kb < p.nkb; ++kb) {
+            const uint32_t s_u = smem_u32(st0) + (uint32_t)(kb & 1) * (uint32_t)DsgCfg::kStageBytes;
+            const uint32_t a_hi = s_u + (uint32_t)wg * 64u * 128u, a_lo = a_hi + kABytes;
+            const uint32_t b_hi = s_u + 2 * kABytes, b_lo = b_hi + DsgCfg::kBBytes;
+            wg_fence_regs(acc);
+            wg_fence();
+            proj_mma<kDsgN>(acc, a_hi, a_lo, b_hi, b_lo, kb == 0);
+            wg_commit();
+            if (kb + 1 < p.nkb) {
+                load(kb + 1);
+                wg_wait<1>();                                // this warpgroup's MMAs of k-block kb - 1 are done
+                __syncthreads();                             // ... and the other's: their stage may be overwritten
+                store((kb + 1) & 1);
+                fence_proxy_async_smem();
+                __syncthreads();
+            }
+        }
+        wg_wait<0>();
+        wg_fence_regs(acc);
+        // ===================== accumulator fragment -> da[k] =====================
+        float* dak = p.da + k * p.n * p.n;
+        const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t i = i0 + r0 + 8 * h;
+            if (i >= p.n) continue;
+#pragma unroll
+            for (int j = 0; j < kDsgN / 8; ++j) {
+                const int64_t col = j0 + 8 * j + c0;
+                const float lo = acc[4 * j + 2 * h], hi = acc[4 * j + 2 * h + 1];
+                if (p.pair_store) {
+                    if (col < p.n) *reinterpret_cast<float2*>(dak + i * p.n + col) = make_float2(lo, hi);
+                } else {
+                    if (col < p.n) dak[i * p.n + col] = lo;
+                    if (col + 1 < p.n) dak[i * p.n + col + 1] = hi;
+                }
+            }
+        }
+    }
+}
+
 int32_t launch_pack_image(const float* src, int n_rows, int k_cols, int64_t rs, int64_t cs, float* img, int tile_rows,
                           cudaStream_t st) {
     pack_image_kernel<<<(n_rows * k_cols + 255) / 256, 256, 0, st>>>(src, n_rows, k_cols, rs, cs, img, tile_rows);
@@ -445,4 +571,37 @@ extern "C" int32_t stmgcn_proj_pack_tc(const float* w, int32_t ks, float* img_fw
         if (ks > 4) return launch_pack_image(w + (int64_t)256 * 64, (ks - 4) * 64, 64, 64, 1, img_bwd + 2 * 2 * 256 * 32, 256, st);
     }
     return 0;
+}
+
+extern "C" int32_t stmgcn_dense_support_grad(int64_t n, int64_t f_total, int32_t ks, const float* u, int64_t u_stride,
+                                             const float* x, float* da, void* stream) {
+    STMGCN_REQUIRE(u && x && da, STMGCN_ERR_ARG, "dense_support_grad: null pointer");
+    STMGCN_REQUIRE(ks >= 1 && ks <= 8, STMGCN_ERR_SHAPE, "dense_support_grad: ks=%d (1..8 supports)", ks);
+    STMGCN_REQUIRE(n >= 1 && n < (1 << 24), STMGCN_ERR_SHAPE, "dense_support_grad: n=%lld must be in [1, 2^24)", (long long)n);
+    STMGCN_REQUIRE(f_total >= 1 && f_total < ((int64_t)1 << 31) && n * f_total < ((int64_t)1 << 48), STMGCN_ERR_SHAPE,
+                   "dense_support_grad: f_total=%lld must be in [1, 2^31) with n * f_total below 2^48", (long long)f_total);
+    STMGCN_REQUIRE(u_stride >= 0 && u_stride < ((int64_t)1 << 48), STMGCN_ERR_ARG, "dense_support_grad: u_stride=%lld",
+                   (long long)u_stride);
+    const int64_t op_bytes = n * f_total * 4, u_bytes = ((int64_t)(ks - 1) * u_stride + n * f_total) * 4;
+    const int64_t da_bytes = (int64_t)ks * n * n * 4;
+    STMGCN_REQUIRE(!overlaps(da, da_bytes, u, u_bytes) && !overlaps(da, da_bytes, x, op_bytes), STMGCN_ERR_ARG,
+                   "dense_support_grad: da must not overlap u or x");
+    DsgParams p;
+    p.u = u;
+    p.u_stride = u_stride;
+    p.x = x;
+    p.da = da;
+    p.n = n;
+    p.f = f_total;
+    p.n_rt = ceil_div(n, kTileM);
+    p.n_ct = ceil_div(n, kDsgN);
+    p.n_tiles = (int64_t)ks * p.n_rt * p.n_ct;
+    p.nkb = (int)ceil_div(f_total, kKB);
+    p.pair_store = n % 2 == 0 && (reinterpret_cast<uintptr_t>(da) & 7u) == 0;
+    const bool vec = f_total % 4 == 0 && aligned16(u) && aligned16(x) && (ks == 1 || u_stride % 4 == 0);
+    auto kern = vec ? dense_support_grad_kernel<true> : dense_support_grad_kernel<false>;
+    if (int32_t rc = ensure_dyn_smem((const void*)kern, kDsgSmem)) return rc;
+    kern<<<persistent_grid(p.n_tiles), kPThreads, kDsgSmem, (cudaStream_t)stream>>>(p);
+    count_launch();
+    return check_launch("dense_support_grad");
 }

@@ -227,12 +227,6 @@ window_gather_kernel(const V* __restrict__ series, int64_t s_len, int64_t row, c
     }
 }
 
-// whether the byte ranges [p, p + pb) and [q, q + qb) share a byte
-bool overlaps(const void* p, int64_t pb, const void* q, int64_t qb) {
-    const uintptr_t a = reinterpret_cast<uintptr_t>(p), c = reinterpret_cast<uintptr_t>(q);
-    return a < c + (uintptr_t)qb && c < a + (uintptr_t)pb;
-}
-
 }  // namespace
 
 extern "C" {

@@ -339,13 +339,6 @@ extern "C" int32_t stmgcn_cheb_spmm_step16(int64_t n, const int32_t* rowptr, con
     return check_launch("cheb_spmm_step16");
 }
 
-// whether the byte ranges [p, p + pb) and [q, q + qb) share a byte (a NULL or empty range shares none)
-static bool overlaps(const void* p, int64_t pb, const void* q, int64_t qb) {
-    if (p == nullptr || q == nullptr || pb <= 0 || qb <= 0) return false;
-    const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
-    return a < b + (uintptr_t)qb && b < a + (uintptr_t)pb;
-}
-
 extern "C" int32_t stmgcn_csr_sddmm(int64_t n, const int32_t* rowptr, const int32_t* colidx, int64_t nnz, int32_t nterms,
                                     const float* const* a, const float* const* b, const float* coef,
                                     int32_t round_b_bf16, int64_t f_total, float* work, int64_t work_count,

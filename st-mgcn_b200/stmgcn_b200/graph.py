@@ -2,7 +2,8 @@
 
 The reference hands ``GCN.forward`` a dense ``(K+1, N, N)`` stack built once by
 ``Adj_Preprocessor.process`` (``GCN.py:57-97``; stacked ``:95``) and multiplies each slice into the
-features (``GCN.py:34-36``).  Here the stack is inspected ONCE per tensor (cached on identity + version):
+features (``GCN.py:34-36``).  Here the stack is inspected ONCE per tensor (cached on identity + version; a stack that
+requires grad at every forward, and its set carries it so the graph convolutions give it its gradient):
 
 * if it is a Chebyshev stack -- ``A[0] = I`` and ``A[k] = 2 A[1] A[k-1] - A[k-2]`` (``GCN.py:125-135``),
   checked with a random probe -- only ``L~ = A[1]`` is kept, as CSR + CSR^T on the device, and the forward
@@ -120,18 +121,26 @@ class SupportSet:
     ``values`` (optional): the source tensors of the graphs' stored values, one per graph in CSR entry order, when some
     of them require grad (a learnable :class:`SparseSupports`).  The graphs hold detached copies; the graph
     convolutions take these tensors as inputs, so their gradients reach them.
+
+    ``dense`` (optional): the dense ``(Ks, N, N)`` stack the set was converted from, when it requires grad.  The graphs
+    hold a snapshot of its slices; the graph convolutions take the stack as their one extra input and give it
+    ``dA_k = U_k x^T`` for every slice (``ops.dense_support_grad``), however the forward multiplied by it.
     """
 
     def __init__(self, mode: str, n: int, ks: int, graphs: List[GraphHandle], device: torch.device,
-                 values: Optional[List[torch.Tensor]] = None):
+                 values: Optional[List[torch.Tensor]] = None, dense: Optional[torch.Tensor] = None):
         assert mode in ("cheb", "generic")
         assert len(graphs) == ks if mode == "generic" else (ks - 1) % max(len(graphs), 1) == 0 and (ks == 1) == (not graphs)
         assert values is None or len(values) == len(graphs)
+        assert values is None or dense is None
         self.mode, self.n, self.ks, self.graphs, self.device = mode, n, ks, graphs, device
-        self.values = values
+        self.values, self.dense = values, dense
 
     def grad_values(self) -> tuple:
-        """The value tensors the graph convolutions take as inputs: ``values`` when one of them requires grad, else ()."""
+        """The tensors the graph convolutions take as inputs so that gradients reach them: ``values`` when one of them
+        requires grad, ``(dense,)`` when the dense stack requires grad, else ()."""
+        if self.dense is not None and self.dense.requires_grad:
+            return (self.dense,)
         if self.values is not None and any(v.requires_grad for v in self.values):
             return tuple(self.values)
         return ()
@@ -187,7 +196,11 @@ def support_version(a) -> tuple:
 
 
 def supports_from_dense(a: torch.Tensor) -> SupportSet:
-    """Cached conversion of a dense support stack (keyed on tensor identity + in-place version)."""
+    """Cached conversion of a dense support stack (keyed on tensor identity + in-place version).
+
+    A stack that requires grad is converted at every call and never cached: an optimizer may change it without a version
+    bump (fused optimizers, ``.data`` writes), and each forward must multiply by the values it differentiates at.  Its
+    set carries the stack (:attr:`SupportSet.dense`), so the graph convolutions give it its gradient."""
     if isinstance(a, (SparseSupports, LearnableAdjacency)):
         return a.support_set()
     if not isinstance(a, torch.Tensor) or a.dim() != 3 or a.shape[1] != a.shape[2]:
@@ -195,11 +208,21 @@ def supports_from_dense(a: torch.Tensor) -> SupportSet:
     if not a.is_cuda:
         raise RuntimeError("stmgcn_b200 has no CPU path: supports must live on a CUDA device "
                            "(the reference moves them there at Main.py:54)")
+    if a.requires_grad:
+        return _convert_dense(a, dense=a)
     key = support_version(a)
     hit = _CACHE.get(key)
     if hit is not None:
         _CACHE.move_to_end(key)
         return hit[1]
+    sset = _convert_dense(a)
+    _CACHE[key] = (a.detach(), sset)     # keep the storage alive so the data_ptr cannot be recycled under the key
+    while len(_CACHE) > _CACHE_MAX:
+        _CACHE.popitem(last=False)
+    return sset
+
+
+def _convert_dense(a: torch.Tensor, dense: Optional[torch.Tensor] = None) -> SupportSet:
     af = a.detach()
     if af.dtype != torch.float32:
         af = af.float()
@@ -207,13 +230,8 @@ def supports_from_dense(a: torch.Tensor) -> SupportSet:
     with torch.cuda.device(a.device):
         if _is_chebyshev_stack(af):
             graphs = [GraphHandle.from_dense(af[1])] if ks > 1 else []
-            sset = SupportSet("cheb", n, ks, graphs, a.device)
-        else:
-            sset = SupportSet("generic", n, ks, [GraphHandle.from_dense(af[k]) for k in range(ks)], a.device)
-    _CACHE[key] = (a, sset)          # keep `a` alive so the data_ptr cannot be recycled under the key
-    while len(_CACHE) > _CACHE_MAX:
-        _CACHE.popitem(last=False)
-    return sset
+            return SupportSet("cheb", n, ks, graphs, a.device, dense=dense)
+        return SupportSet("generic", n, ks, [GraphHandle.from_dense(af[k]) for k in range(ks)], a.device, dense=dense)
 
 
 def clear_cache() -> None:

@@ -12,8 +12,8 @@ Gradients are accumulated into ``GradBucket`` views (static addresses).  The opt
 The supports are baked in too: the graph reads the CSR tensors of the support sets converted at capture.  The step holds
 those sets (so their memory stays valid whatever happens to the conversion cache) and the supports' versions
 (``graph.support_version``); a call after any support was edited raises instead of replaying the old supports.
-Learnable supports (a ``SparseSupports`` whose values require grad) are refused at construction: their values are read
-again at every forward, which a replayed graph cannot do.
+Learnable supports (a ``SparseSupports`` whose values require grad, or a dense stack that requires grad) are refused at
+construction: their values are read again at every forward, which a replayed graph cannot do.
 
 A ``LearnableAdjacency`` is accepted: its normalisation (``ops.AdjNorm``) is captured with the step and reads ``weight``
 at its own address, so each replay runs at the weights the optimizer left there (fused optimizers included).  Its
@@ -39,6 +39,10 @@ class GraphedStep:
         if learnable:
             raise ValueError(f"GraphedStep: supports {learnable} have values that require grad; a captured step replays "
                              f"the values of capture time, so learnable supports run eagerly")
+        dense = [m for m, s in enumerate(supports) if isinstance(s, torch.Tensor) and s.requires_grad]
+        if dense:
+            raise ValueError(f"GraphedStep: the dense support stacks {dense} require grad; a captured step replays the "
+                             f"conversion of capture time, so stacks that require grad run eagerly")
         self.model, self.criterion, self.supports = model, criterion, list(supports)
         adjs = []
         for s in self.supports:

@@ -271,6 +271,36 @@ def support_value_grads(sset: SupportSet, s: torch.Tensor, u: torch.Tensor, x: O
     return grads
 
 
+def dense_support_grad(u: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+    """``dA_k = U_k x^T`` for every slice k (stmgcn_dense_support_grad): ``u`` (Ks, N, ...) the projection backward's U
+    before the adjoint Clenshaw, ``x`` (N, ...) the features the slices multiplied; both fp32 contiguous.  (Ks, N, N)."""
+    ks, n = u.shape[0], u.shape[1]
+    da = torch.empty((ks, n, n), device=u.device, dtype=torch.float32)
+    _lib.check(L.stmgcn_dense_support_grad(n, x.numel() // n, ks, u.data_ptr(), u[0].numel(), x.data_ptr(),
+                                           da.data_ptr(), _stream()), "dense_support_grad")
+    return da
+
+
+def _support_grads(ctx, s: torch.Tensor, u: Optional[torch.Tensor], x: Optional[torch.Tensor], need_dx: bool,
+                   round16: bool):
+    """The graph convolutions' shared backward tail: (dX or None, the gradients of their extra inputs).  ``u`` from the
+    projection backward (None when nothing needs it); a dense stack's gradient is taken from it before the adjoint
+    Clenshaw overwrites it, a sparse set's value gradients after."""
+    sset, need_v = ctx.sset, ctx.needs_input_grad[5:]
+    extra = [None] * len(need_v)
+    dense = sset.dense is not None and any(need_v)
+    if dense:
+        extra[0] = dense_support_grad(u, s[0] if x is None else x).to(sset.dense.dtype)
+    dx = None
+    if need_dx:
+        dx = adjoint_stack_(sset, u)
+    elif any(need_v) and not dense:
+        adjoint_stack_(sset, u, False)          # G_k into u for the value gradients only
+    if any(need_v) and not dense:
+        extra = support_value_grads(sset, s, u, x, round16, need_v)
+    return dx, extra
+
+
 NORM_KINDS = {"chebyshev": 0, "localpool": 1, "random_walk_diffusion": 2}      # STMGCN_NORM_* of the C ABI
 
 
@@ -407,8 +437,8 @@ class ObsToNodeMajor(torch.autograd.Function):
 class ChebGCN(torch.autograd.Function):
     """out (N,B,q) = act( sum_k (T_k x) W_k + b ),  x (N,B,p) node-major.
 
-    ``vals``: the support set's value tensors (``sset.grad_values()``), inputs only so that their gradients reach them:
-    the kernels read the set's own copies."""
+    ``vals``: ``sset.grad_values()``, the set's value tensors or its dense stack, inputs only so that their gradients
+    reach them: the kernels read the set's own copies."""
 
     @staticmethod
     def forward(ctx, x, w, bias, sset: SupportSet, act: int, *vals):
@@ -425,10 +455,11 @@ class ChebGCN(torch.autograd.Function):
         out = _proj_fwd(s, w, bias_c, act, None, x.shape[1], img_f)
         ctx.sset, ctx.act, ctx.has_bias = sset, act, bias is not None
         # the value gradients' B operand is what the recurrence gathered: bf16(T_{k-1}) where it read bf16 copies (asked
-        # only when a value needs grad: such a set has a graph, and a set without values runs nothing new)
-        ctx.round16 = any(ctx.needs_input_grad[5:]) and _gather16(sset, x)
+        # only when a value needs grad: such a set has a graph, and a set without values runs nothing new; a dense
+        # stack's gradient takes the fp32 x, and its set may have no graph: [I])
+        ctx.round16 = sset.dense is None and any(ctx.needs_input_grad[5:]) and _gather16(sset, x)
         if need_grad:
-            # x (generic supports' value gradients only) is saved last, and only then
+            # x (the value or dense-stack gradients of generic supports only) is saved last, and only then
             need_x = any(ctx.needs_input_grad[5:]) and sset.mode == "generic"
             ctx.save_for_backward(s, w, out, img_b, *([x] if need_x else []))
         return out
@@ -438,18 +469,12 @@ class ChebGCN(torch.autograd.Function):
         s, w, out, img_b, *x = ctx.saved_tensors
         x = x[0] if x else None
         need_dx, need_dw, need_db = ctx.needs_input_grad[:3]
-        need_v = ctx.needs_input_grad[5:]
         d_out = _f32c(d_out)
-        need_u = need_dx or any(need_v)
+        need_u = need_dx or any(ctx.needs_input_grad[5:])
         dw, db, u = _proj_bwd(s, w, ctx.act, out, d_out, None, 1.0, s.shape[2], ctx.has_bias and need_db, need_u, img_b,
                               need_w=need_dw)
-        dx = None
-        if need_dx:
-            dx = adjoint_stack_(ctx.sset, u)
-        elif need_u:
-            adjoint_stack_(ctx.sset, u, False)          # G_k into u for the value gradients only
-        dvals = support_value_grads(ctx.sset, s, u, x, ctx.round16, need_v) if any(need_v) else [None] * len(need_v)
-        return (dx, dw, db, None, None, *dvals)
+        dx, extra = _support_grads(ctx, s, u, x, need_dx, ctx.round16)
+        return (dx, dw, db, None, None, *extra)
 
 
 class TemporalPool(torch.autograd.Function):
@@ -485,18 +510,14 @@ class TemporalPool(torch.autograd.Function):
         x = x[0] if x else None
         d_pool = _f32c(d_pool)
         need_dx, need_dw, need_db = ctx.needs_input_grad[:3]
-        need_v = ctx.needs_input_grad[5:]
-        need_u = need_dx or any(need_v)
+        need_u = need_dx or any(ctx.needs_input_grad[5:])
         dw, db, u = _proj_bwd(s, w, ctx.act, out, None, d_pool, 1.0, s.shape[2], ctx.has_bias and need_db, need_u,
                               need_w=need_dw)
-        dx = None
-        if need_dx:
+        dx, extra = _support_grads(ctx, s, u, x, need_dx, False)
+        if dx is not None:
             # the GCN's dX (adjoint Clenshaw / sum_k A_k^T U_k) plus the residual's: d_pool broadcast over regions
-            dx = adjoint_stack_(ctx.sset, u) + d_pool.unsqueeze(0)
-        elif need_u:
-            adjoint_stack_(ctx.sset, u, False)          # G_k into u for the value gradients only
-        dvals = support_value_grads(ctx.sset, s, u, x, False, need_v) if any(need_v) else [None] * len(need_v)
-        return (dx, dw, db, None, None, *dvals)
+            dx = dx + d_pool.unsqueeze(0)
+        return (dx, dw, db, None, None, *extra)
 
 
 class ContextGate(torch.autograd.Function):
