@@ -110,6 +110,30 @@ int32_t stmgcn_csr_sddmm(int64_t n, const int32_t* rowptr, const int32_t* colidx
 int32_t stmgcn_dense_support_grad(int64_t n, int64_t f_total, int32_t ks, const float* u, int64_t u_stride,
                                   const float* x, float* da, void* stream);
 
+/* ---- K1e: the recurrence step with a DENSE support matrix (GCN.py:35 as the reference computes it) ------------------
+ *   Y = alpha * op(A) X + beta * Z + gamma * U      on (n, f_total) fp32 row-major X, Z, U, Y
+ * stmgcn_cheb_spmm_step's step for a matrix held dense: a (n x n) fp32 row-major with leading dimension lda >= n;
+ * op(A) = A (transpose = 0) or A^T (transpose = 1).  Z and U may be NULL (their terms vanish).  Y may BE U (the adjoint
+ * Clenshaw's y = u[k], gamma = 1) but shares no other byte with U, and none with X, Z or a (checked).
+ * 1 <= n < 2^24, lda < 2^31, 1 <= f_total < 2^31.  3xTF32 on the tensor cores with a rounded split, each 32-term block
+ * added into an fp32 register total (fp32-grade, also where the products cancel); 16-byte loads when n, lda and
+ * f_total are multiples of 4 and every pointer is 16-byte aligned, scalar loads otherwise.  One launch.  Every element has
+ * one owner and a fixed summation order: two calls with the same inputs give bit-identical y.
+ * Non-finite values: the product is dense, as the reference's einsum, so it forms 0 * NaN: a NaN in row j of X reaches
+ * every row of Y in its columns (spmm_stored_entries_only does not apply); an Inf operand gives NaN
+ * (inf_through_split_operands). */
+int32_t stmgcn_dense_mm_step(int64_t n, const float* a, int64_t lda, int32_t transpose, float alpha, const float* x,
+                             float beta, const float* z, float gamma, const float* u, float* y, int64_t f_total,
+                             void* stream);
+
+/* The same step multiplying the bf16 copy x16 (n, f_total) bf16 (the bf16-arithmetic mode, as stmgcn_cheb_spmm_step16):
+ * a bf16 value is exact in tf32, so two tensor-core passes A_hi x16 + A_lo x16; z, u, y stay fp32, and y16 (nullable)
+ * receives the bf16 copy of y (round to nearest even, as stmgcn_to_bf16).  f_total must be a multiple of 8 and x16, y,
+ * y16, z, u 16-byte aligned; y16 shares no byte with x16, y, z, u or a. */
+int32_t stmgcn_dense_mm_step16(int64_t n, const float* a, int64_t lda, int32_t transpose, float alpha, const void* x16,
+                               float beta, const float* z, float gamma, const float* u, float* y, void* y16,
+                               int64_t f_total, void* stream);
+
 /* ---- K1c: the supports of a learnable adjacency on a fixed sparsity pattern ----------------------------------------
  * The pattern is an n x n CSR (rowptr, colidx; nnz = rowptr[n] entries, no repeated (i, j)) and its transpose's structure
  * rowptr_t, colidx_t with perm_t: CSR^T position p holds CSR entry perm_t[p].  widx (int32 per pattern entry) gives the

@@ -11,6 +11,10 @@ requires grad at every forward, and its set carries it so the graph convolutions
 * otherwise (``localpool``, hand-made supports) every slice is sparsified on its own and applied
   directly (``mode == "generic"``) -- same kernels, same results as the reference's einsum.
 
+Each matrix kept (``L~``, or a generic slice) is held as CSR, or, when it is too dense to gather, as a dense snapshot
+(:class:`DenseGraph`) that the kernels multiply on the tensor cores: :func:`dense_rule` under the ``"auto"`` mode of
+``ops.dense_supports()`` (``STMGCN_DENSE_SUPPORTS``), always under ``"on"``, never under ``"off"``.
+
 ``SparseSupports`` is the sparse-native handle ``GCN.Adj_Preprocessor.process_sparse`` returns (``ChebSupports``
 for ``chebyshev``): it quacks like the reference's tensor where ``Main.py`` touches it (``.to(device)``, ``len``,
 ``.shape``) but never materialises ``N x N`` polynomials (SURVEY.md section 8(f)-1).  Its ``"cheb"`` stacks are one or
@@ -90,11 +94,15 @@ class GraphHandle:
         return new
 
     @classmethod
-    def from_dense(cls, mat: torch.Tensor) -> "GraphHandle":
+    def from_dense(cls, mat: torch.Tensor, nnz: Optional[int] = None) -> "GraphHandle":
         """Exact zeros (-0.0 included) are dropped, every other entry (NaN included) is kept verbatim: supports[1] of
-        ``Adj_Preprocessor.process`` (``GCN.py:57-97``) becomes the sparse rescaled Laplacian."""
+        ``Adj_Preprocessor.process`` (``GCN.py:57-97``) becomes the sparse rescaled Laplacian.  ``nnz``: the matrix's
+        non-zero count when the caller has it already (then no host sync here)."""
         assert mat.dtype == torch.float32 and mat.dim() == 2 and mat.shape[0] == mat.shape[1]
-        rows, cols = (mat != 0).nonzero(as_tuple=True)           # row-major order
+        if nnz is None:
+            rows, cols = (mat != 0).nonzero(as_tuple=True)           # row-major order
+        else:
+            rows, cols = torch.nonzero_static(mat != 0, size=nnz).unbind(1)
         return cls(mat.shape[0], rows, cols, mat[rows, cols])
 
     @classmethod
@@ -111,12 +119,39 @@ class GraphHandle:
         return self._csr[int(transpose)]
 
 
+class DenseGraph:
+    """One ``n x n`` support matrix held dense, for a matrix too dense to gather: the graph convolutions multiply it on
+    the tensor cores (``ops.spmm_step`` dispatches on the handle type; stmgcn_dense_mm_step), as the reference's einsum.
+
+    ``mat`` is an fp32 contiguous snapshot (a copy of what it was built from), so the forward and the backward of a step
+    multiply by one matrix and an edit of the source after the build reaches neither.  ``nnz`` is the number of stored
+    entries, ``n * n``."""
+
+    def __init__(self, mat: torch.Tensor):
+        assert mat.dim() == 2 and mat.shape[0] == mat.shape[1]
+        self.n, self.nnz, self.device = mat.shape[0], mat.shape[0] * mat.shape[0], mat.device
+        self.mat = mat.detach().to(torch.float32, copy=True).contiguous()
+
+
+# When a dense support matrix is multiplied dense (DenseGraph) instead of gathered from CSR (GraphHandle): from this
+# fraction of non-zero entries on, at n >= DENSE_MIN_N.  bench_dense_supports.py (H100, DESIGN.md K1e) puts the crossover
+# at 10-10.4 % for N = 512 .. 4096 at F = 4096 and at 10 % (N = 4096) to 16.5 % (N = 512) at F = 768: 17 % is past it
+# at every measured size and width.  Below N = 512 a step takes at most 26 us on either path, and CSR stays.
+DENSE_MIN_DENSITY = 0.17
+DENSE_MIN_N = 512
+
+
+def dense_rule(n: int, nnz: int) -> bool:
+    """Whether an ``n x n`` matrix with ``nnz`` non-zero entries is multiplied dense under the ``"auto"`` mode."""
+    return n >= DENSE_MIN_N and nnz >= DENSE_MIN_DENSITY * n * n
+
+
 class SupportSet:
     """What the kernels need to know about one ``(Ks, N, N)`` support stack.
 
     ``"cheb"``: ``graphs`` are the recurrence matrices ``X_c`` of chains that share ``T_0 = I``; chain ``c`` owns the
     segments ``1 + cK .. (c+1)K``, ``T_k(X_c)`` with ``K = (Ks - 1) / len(graphs)`` (no graph when ``Ks == 1``).
-    ``"generic"``: ``graphs[k]`` is ``A_k``.
+    ``"generic"``: ``graphs[k]`` is ``A_k``.  A graph is a :class:`GraphHandle` (CSR) or a :class:`DenseGraph`.
 
     ``values`` (optional): the source tensors of the graphs' stored values, one per graph in CSR entry order, when some
     of them require grad (a learnable :class:`SparseSupports`).  The graphs hold detached copies; the graph
@@ -210,7 +245,7 @@ def supports_from_dense(a: torch.Tensor) -> SupportSet:
                            "(the reference moves them there at Main.py:54)")
     if a.requires_grad:
         return _convert_dense(a, dense=a)
-    key = support_version(a)
+    key = _cache_key(a)
     hit = _CACHE.get(key)
     if hit is not None:
         _CACHE.move_to_end(key)
@@ -222,6 +257,27 @@ def supports_from_dense(a: torch.Tensor) -> SupportSet:
     return sset
 
 
+def _cache_key(a: torch.Tensor) -> tuple:
+    """The conversion cache's key of a dense stack: its :func:`support_version` and the dense-supports mode it was
+    converted under (a switch of the mode converts it again)."""
+    from . import ops
+    return support_version(a) + (ops.dense_supports(),)
+
+
+def _graph_from_dense(mat: torch.Tensor):
+    """The handle the kernels multiply ``mat`` through: a :class:`DenseGraph` when the dense-supports mode says so,
+    else CSR (:class:`GraphHandle`).  ``"auto"`` decides by :func:`dense_rule` on the non-zero count, the one host sync
+    of the conversion (the CSR build then takes the count and does not synchronise again)."""
+    from . import ops
+    mode = ops.dense_supports()
+    if mode == "off":
+        return GraphHandle.from_dense(mat)
+    if mode == "on":
+        return DenseGraph(mat)
+    nnz = int((mat != 0).sum())
+    return DenseGraph(mat) if dense_rule(mat.shape[0], nnz) else GraphHandle.from_dense(mat, nnz)
+
+
 def _convert_dense(a: torch.Tensor, dense: Optional[torch.Tensor] = None) -> SupportSet:
     af = a.detach()
     if af.dtype != torch.float32:
@@ -229,9 +285,9 @@ def _convert_dense(a: torch.Tensor, dense: Optional[torch.Tensor] = None) -> Sup
     ks, n, _ = af.shape
     with torch.cuda.device(a.device):
         if _is_chebyshev_stack(af):
-            graphs = [GraphHandle.from_dense(af[1])] if ks > 1 else []
+            graphs = [_graph_from_dense(af[1])] if ks > 1 else []
             return SupportSet("cheb", n, ks, graphs, a.device, dense=dense)
-        return SupportSet("generic", n, ks, [GraphHandle.from_dense(af[k]) for k in range(ks)], a.device, dense=dense)
+        return SupportSet("generic", n, ks, [_graph_from_dense(af[k]) for k in range(ks)], a.device, dense=dense)
 
 
 def clear_cache() -> None:

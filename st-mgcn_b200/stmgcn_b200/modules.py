@@ -14,7 +14,7 @@ import torch
 from torch import nn
 
 from . import _lib, ops
-from .graph import ChebSupports, supports_from_dense
+from .graph import ChebSupports, DenseGraph, supports_from_dense
 
 
 _BRANCH_STREAMS = {}
@@ -204,10 +204,10 @@ class ST_MGCN(nn.Module):
                     feats.append(self.gcn_list[m].forward_node_major(ssets[m], h_top))
                 xo.record_stream(streams[m])
                 xt.record_stream(streams[m])
-                # the CSR tensors belong to the stream that built them: once freed (their support set dropped from the
+                # the CSR tensors (a dense matrix's snapshot) belong to the stream that built them: once freed (their support set dropped from the
                 # cache), their memory must not be reused while this branch's kernels may still read it
                 for g in ssets[m].graphs:
-                    for t in g.export(False) + g.export(True):
+                    for t in (g.mat,) if isinstance(g, DenseGraph) else g.export(False) + g.export(True):
                         t.record_stream(streams[m])
             for m in range(self.M):
                 main.wait_stream(streams[m])

@@ -22,7 +22,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _lib
-from .graph import SupportSet
+from .graph import DenseGraph, SupportSet
 
 L = _lib.lib
 
@@ -44,6 +44,26 @@ def set_lstm_path(path: str) -> None:
     if path not in ("tc", "fma"):
         raise ValueError(path)
     _LSTM_PATH = path
+
+
+_DENSE_SUPPORTS = os.environ.get("STMGCN_DENSE_SUPPORTS", "auto")
+
+
+def dense_supports() -> str:
+    """How a dense support stack's matrices are multiplied: "auto" (dense on the tensor cores when ``graph.dense_rule``
+    says so, CSR gathers otherwise), "on" (always dense), "off" (always CSR).  Sparse handles always stay CSR."""
+    return _DENSE_SUPPORTS
+
+
+def set_dense_supports(mode: str) -> None:
+    global _DENSE_SUPPORTS
+    if mode not in ("auto", "on", "off"):
+        raise ValueError(f"dense supports mode {mode!r}: 'auto', 'on' or 'off'")
+    _DENSE_SUPPORTS = mode
+
+
+if _DENSE_SUPPORTS not in ("auto", "on", "off"):
+    raise ValueError(f"STMGCN_DENSE_SUPPORTS={_DENSE_SUPPORTS!r}: 'auto', 'on' or 'off'")
 
 
 # The module-level limits of the kernels, the numbers the C entry points enforce (include/stmgcn_b200.h).  The modules
@@ -108,9 +128,14 @@ def _require_cuda(*ts):
 # --------------------------------------------------------------------------------------------------
 def spmm_step(g, transpose: bool, alpha: float, x: torch.Tensor, beta: float, z: Optional[torch.Tensor],
               gamma: float, u: Optional[torch.Tensor], y: torch.Tensor) -> None:
-    """``y = alpha * op(A) x + beta * z + gamma * u`` on ``(N, F)`` views; op(A) = A, or A^T with ``transpose``."""
+    """``y = alpha * op(A) x + beta * z + gamma * u`` on ``(N, F)`` views; op(A) = A, or A^T with ``transpose``.  A
+    :class:`DenseGraph` is multiplied dense on the tensor cores, a CSR handle by the row gather."""
     n = g.n
     f_total = x.numel() // n
+    if isinstance(g, DenseGraph):
+        _lib.check(L.stmgcn_dense_mm_step(n, g.mat.data_ptr(), n, int(transpose), alpha, x.data_ptr(), beta, _p(z), gamma,
+                                          _p(u), y.data_ptr(), f_total, _stream()), "dense_mm_step")
+        return
     rowptr, colidx, vals = g.export(transpose)
     _lib.check(L.stmgcn_cheb_spmm_step(n, rowptr.data_ptr(), colidx.data_ptr(), vals.data_ptr(), alpha, x.data_ptr(),
                                        beta, _p(z), gamma, _p(u), y.data_ptr(), f_total, _stream()), "cheb_spmm_step")
@@ -120,6 +145,10 @@ def spmm_step16(g, transpose: bool, alpha: float, x16: torch.Tensor, beta: float
                 gamma: float, u: Optional[torch.Tensor], y: torch.Tensor, y16: Optional[torch.Tensor]) -> None:
     """:func:`spmm_step` with the gathered operand read from its bf16 copy ``x16``; writes the bf16 copy of ``y`` to ``y16``."""
     f_total = y.numel() // g.n
+    if isinstance(g, DenseGraph):
+        _lib.check(L.stmgcn_dense_mm_step16(g.n, g.mat.data_ptr(), g.n, int(transpose), alpha, x16.data_ptr(), beta, _p(z),
+                                            gamma, _p(u), y.data_ptr(), _p(y16), f_total, _stream()), "dense_mm_step16")
+        return
     rowptr, colidx, vals = g.export(transpose)
     _lib.check(L.stmgcn_cheb_spmm_step16(g.n, rowptr.data_ptr(), colidx.data_ptr(), vals.data_ptr(), alpha,
                                          x16.data_ptr(), beta, _p(z), gamma, _p(u), y.data_ptr(), _p(y16), f_total,
@@ -234,7 +263,10 @@ def sddmm_tiles(f_total: int) -> int:
 
 def csr_sddmm_(g, terms, dvals: torch.Tensor, round_b16: bool = False) -> None:
     """``dvals[e] += sum_t coef_t <A_t[i, :], B_t[j, :]>`` over the stored entries e = (i, j) of ``g``'s CSR, in its
-    entry order; ``terms``: (A_t, B_t, coef_t) with A_t, B_t (N, ...) fp32 contiguous.  ``round_b16``: B rounded to bf16."""
+    entry order; ``terms``: (A_t, B_t, coef_t) with A_t, B_t (N, ...) fp32 contiguous.  ``round_b16``: B rounded to bf16.
+    Sparse handles only: a dense stack's gradient is ``dense_support_grad``'s, and a sparse handle is never densified."""
+    if isinstance(g, DenseGraph):
+        raise AssertionError("csr_sddmm_ takes CSR handles only: a DenseGraph's gradient is dense_support_grad's")
     rowptr, colidx, _ = g.export(False)
     f_total = terms[0][0].numel() // g.n
     tiles = sddmm_tiles(f_total)

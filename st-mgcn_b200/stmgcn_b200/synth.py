@@ -80,6 +80,18 @@ def make_directed_adjacency(n: int, m: int, density: float) -> torch.Tensor:
     return a.to(torch.float32)
 
 
+def make_similarity_adjacency(n: int, m: int, dim: int = 16, width: float = 1.0) -> torch.Tensor:
+    """Dense float32 similarity adjacency of graph ``m``, CPU, every off-diagonal entry non-zero (a functional-similarity
+    or Gaussian-kernel distance graph nobody thresholded): ``g = torch.Generator().manual_seed(3000 + m)``; region
+    vectors ``v = rand(N, dim)``; ``A_ij = exp(-|v_i - v_j|^2 / (width * dim / 6))`` (``dim / 6`` is the mean squared
+    distance of two such vectors), zero diagonal."""
+    g = torch.Generator().manual_seed(3000 + m)
+    v = torch.rand(n, dim, generator=g, dtype=torch.float64)
+    a = torch.exp(-torch.cdist(v, v).square() / (width * dim / 6.0))
+    a.fill_diagonal_(0.0)
+    return a.to(torch.float32)
+
+
 def make_adjacency_list(w: Workload) -> List[torch.Tensor]:
     return [make_adjacency(w.n_regions, m, w.density) for m in range(w.n_graphs)]
 
