@@ -110,6 +110,22 @@ int32_t stmgcn_csr_sddmm(int64_t n, const int32_t* rowptr, const int32_t* colidx
 int32_t stmgcn_dense_support_grad(int64_t n, int64_t f_total, int32_t ks, const float* u, int64_t u_stride,
                                   const float* x, float* da, void* stream);
 
+/* ---- K1f: gradient of a DENSE Chebyshev recurrence matrix (a learnable adjacency multiplied dense) ------------------
+ *   out[i][j] = sum_t coef[t] * sum_f A_t[i][f] * B_t[j][f]      (out = sum_t coef_t A_t B_t^T),   i, j < n, f < f_total
+ * stmgcn_csr_sddmm's sum over every n x n entry: chain X with T_1 = X T_0, T_k = 2 X T_{k-1} - T_{k-2} gives
+ * dX = sum_k c_k G_k T_{k-1}^T with A_t = G_k (the total adjoint dL/dT_k), B_t = T_{k-1}, coef 1 for k = 1 and 2 after.
+ * A_t, B_t: (n, f_total) fp32 row-major, nterms = 1..8 pairs as host arrays a[nterms], b[nterms] of device pointers and
+ * coef[nterms] of host floats, read at enqueue.  round_b16 = 1 rounds every B element to bf16 (to nearest even) before
+ * the product: the operand stmgcn_dense_mm_step16 multiplied by.  out: (n, n) row-major, OVERWRITTEN.
+ * 1 <= n < 2^24, 1 <= f_total < 2^31; A_t and B_t may alias one another, out shares no byte with any (checked).
+ * 3xTF32 on the tensor cores with K1e's rounded split, each 32-term block's product added times coef_t into an fp32
+ * register total (fp32-grade where the products cancel); 16-byte loads when f_total % 4 == 0 and every A_t, B_t is
+ * 16-byte aligned, scalar loads otherwise.  One launch.  Every element has one owner and a fixed summation order (the
+ * terms in order, each over f in order): two calls with the same inputs give bit-identical out.  A NaN in row i of an
+ * A_t makes row i of out NaN, a NaN in row j of a B_t column j; an Inf gives NaN (inf_through_split_operands). */
+int32_t stmgcn_dense_chain_grad(int64_t n, int64_t f_total, int32_t nterms, const float* const* a, const float* const* b,
+                                const float* coef, int32_t round_b16, float* out, void* stream);
+
 /* ---- K1e: the recurrence step with a DENSE support matrix (GCN.py:35 as the reference computes it) ------------------
  *   Y = alpha * op(A) X + beta * Z + gamma * U      on (n, f_total) fp32 row-major X, Z, U, Y
  * stmgcn_cheb_spmm_step's step for a matrix held dense: a (n x n) fp32 row-major with leading dimension lda >= n;
@@ -168,6 +184,21 @@ int32_t stmgcn_adj_norm_bwd(int32_t kind, int64_t n, const int32_t* rowptr, cons
                             const int32_t* colidx_t, const int32_t* perm_t, int64_t nnz, const int32_t* widx, const float* w,
                             int64_t nnz_w, float scale, const float* dvals, const float* dvals_t, float* work,
                             int64_t work_count, float* dw, void* stream);
+
+/* A pattern's values <-> the dense matrix they form (a learnable adjacency multiplied dense).  The pattern: CSR rowptr
+ * (n + 1) and colidx (nnz) int32 -- a learnable adjacency's CSR, or its CSR^T (rowptr_t, colidx_t) for the values in
+ * CSR^T order (diffusion's P_f^T).  Columns may be unsorted within a row and entries repeated.
+ * scatter: dense (n x n fp32 row-major) OVERWRITTEN with the matrix: zeros, plus each entry's value added at (i, j) in
+ *   entry order (repeats add up as CSR applies them: ((0 + v_e0) + v_e1) + ...).  One launch, also when nnz == 0.
+ * gather: dvals[e] = dense[i][colidx[e]] for every entry e = (i, j), OVERWRITTEN: the values' gradient from the
+ *   matrix's.  One launch; none when nnz == 0.
+ * 1 <= n < 2^24, 0 <= nnz < 2^31; column indices in [0, n) (not checked: the caller's pattern, as for the SpMM).  The
+ * output shares no byte with the pattern or the input (checked).  Plain fp32 adds and copies: NaN and Inf pass as
+ * they are, and a stored zero is an entry like any other. */
+int32_t stmgcn_pattern_scatter(int64_t n, const int32_t* rowptr, const int32_t* colidx, int64_t nnz, const float* vals,
+                               float* dense, void* stream);
+int32_t stmgcn_pattern_gather(int64_t n, const int32_t* rowptr, const int32_t* colidx, int64_t nnz, const float* dense,
+                              float* dvals, void* stream);
 
 /* ---- input pipeline: training windows gathered from a device-resident series (Data_Container.py:114-146) ----------
  *   obs[k, t, :] = series[wrap(first + k - lags[t]), :],   y[k, :] = series[first + k, :]      (k < b, t < t_len)

@@ -95,13 +95,6 @@ __device__ __forceinline__ void ld4x4_t(float4 (&o)[4], const float* m, const ui
     o[3] = make_float4(r[0].w, r[1].w, r[2].w, r[3].w);
 }
 
-// v rounded to the nearest tf32 value (ties away from zero), exact in tf32
-__device__ __forceinline__ float tf32_rna(float v) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-    return __uint_as_float(r);
-}
-
 // 16-byte chunk k4 (k = 4 k4 .. 4 k4 + 3) of row mn of a K-major [rows][32] tile with the 128-byte swizzle
 // (sw128<4>(mn, 4 k4)); SPLIT: tf32 hi at t, lo at t + lo_off; else v as it is (a bf16 value is exact in tf32).
 // The split ROUNDS (hi = rna(v), lo = rna(v - hi): |v - hi - lo| <= 2^-24 |v|, errors of either sign) where K1d and K2

@@ -10,6 +10,8 @@
 //              P_f^T (CSR^T order) v[p] = w * inv(d_out)[i],   inv(d) = 0 where 1/d is infinite (GCN.py:100-104)
 // One warp owns one row (or one column of the transpose); its lanes take the segment's entries strided by 32 and a fixed
 // xor tree sums them: every sum has one owner and one order, no float atomics, two runs agree bit for bit.
+// When the adjacency is multiplied dense, pattern_scatter writes the values into the dense matrix and pattern_gather reads
+// the matrix's gradient back into the values' order for the backward (one warp per row as well).
 #include "common.cuh"
 #include <math.h>
 
@@ -170,6 +172,53 @@ norm_grad_rows_kernel(int64_t n, const int32_t* __restrict__ rowptr, const int32
     }
 }
 
+// pattern -> dense: row k of the n x n matrix is zeroed, then its segment's values are added in entry order.  A chunk of
+// 32 entries at a time: lanes holding the same column (a repeated entry) form a group whose lowest lane adds the
+// group's values to the element one by one in lane order, so every element is ((0 + v_e0) + v_e1) + ... over its
+// entries e0 < e1 < ..., whatever the repeats; each element has one writer per chunk and the chunks run in order.
+__global__ void __launch_bounds__(kWarps * 32)
+pattern_scatter_kernel(int64_t n, const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
+                       const float* __restrict__ vals, float* __restrict__ dense) {
+    const int lane = threadIdx.x & 31;
+    const int64_t k = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (k >= n) return;
+    float* row = dense + k * n;
+    for (int64_t j = lane; j < n; j += 32) row[j] = 0.f;
+    __syncwarp();
+    const int32_t beg = rowptr[k], end = rowptr[k + 1];
+    for (int32_t base = beg; base < end; base += 32) {
+        const int32_t e = base + lane;
+        const bool in = e < end;
+        const int32_t j = in ? __ldg(colidx + e) : -1 - lane;        // lanes past the segment: a column of their own
+        const float v = in ? __ldg(vals + e) : 0.f;
+        const unsigned grp = __match_any_sync(0xffffffffu, j);
+        const bool leader = in && lane == __ffs(grp) - 1;
+        float s = leader ? row[j] : 0.f;
+        if (__all_sync(0xffffffffu, __popc(grp) == 1)) {
+            s += v;
+        } else {
+#pragma unroll 1
+            for (int r = 0; r < 32; ++r) {
+                const float vr = __shfl_sync(0xffffffffu, v, r);
+                if ((grp >> r) & 1u) s += vr;
+            }
+        }
+        if (leader) row[j] = s;
+        __syncwarp();
+    }
+}
+
+// dense -> pattern: d vals[e] = dense[k][colidx[e]] for row k's entries (a repeated entry gets the element at each)
+__global__ void __launch_bounds__(kWarps * 32)
+pattern_gather_kernel(int64_t n, const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
+                      const float* __restrict__ dense, float* __restrict__ dvals) {
+    const int lane = threadIdx.x & 31;
+    const int64_t k = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (k >= n) return;
+    const float* row = dense + k * n;
+    for (int32_t e = rowptr[k] + lane; e < rowptr[k + 1]; e += 32) dvals[e] = __ldg(row + __ldg(colidx + e));
+}
+
 struct Range {
     const void* p;
     int64_t bytes;
@@ -278,4 +327,40 @@ extern "C" int32_t stmgcn_adj_norm_bwd(int32_t kind, int64_t n, const int32_t* r
         norm_grad_rows_kernel<false><<<grid, kWarps * 32, 0, st>>>(n, rowptr, colidx, widx, w, coef, dvals, work, dw);
     count_launch();
     return check_launch("adj_norm_bwd");
+}
+
+// the checks the pattern <-> dense entry points share: `in` (n x n, or nnz values) is read, `out` (nnz values, or n x n)
+// written, and the output shares no byte with the inputs
+static int32_t check_pattern_dense(const char* what, int64_t n, const int32_t* rowptr, const int32_t* colidx, int64_t nnz,
+                                   const void* in, int64_t in_count, const void* out, int64_t out_count) {
+    STMGCN_REQUIRE(n > 0 && n < ((int64_t)1 << 24) && nnz >= 0 && nnz < ((int64_t)1 << 31), STMGCN_ERR_SHAPE,
+                   "%s: n=%lld must be in [1, 2^24) and nnz=%lld in [0, 2^31)", what, (long long)n, (long long)nnz);
+    STMGCN_REQUIRE(rowptr, STMGCN_ERR_ARG, "%s: null rowptr", what);
+    STMGCN_REQUIRE((in || in_count == 0) && (out || out_count == 0) && (colidx || nnz == 0), STMGCN_ERR_ARG,
+                   "%s: null colidx / input / output", what);
+    const int64_t i4 = 4;
+    const Range o = {out, out_count * i4};
+    const Range ins[] = {{rowptr, (n + 1) * i4}, {colidx, nnz * i4}, {in, in_count * i4}};
+    for (const Range& r : ins)
+        STMGCN_REQUIRE(!overlaps(o, r), STMGCN_ERR_ARG, "%s: the output overlaps an input", what);
+    return 0;
+}
+
+extern "C" int32_t stmgcn_pattern_scatter(int64_t n, const int32_t* rowptr, const int32_t* colidx, int64_t nnz,
+                                          const float* vals, float* dense, void* stream) {
+    if (int32_t rc = check_pattern_dense("pattern_scatter", n, rowptr, colidx, nnz, vals, nnz, dense, n * n)) return rc;
+    pattern_scatter_kernel<<<(unsigned)ceil_div(n, kWarps), kWarps * 32, 0, (cudaStream_t)stream>>>(n, rowptr, colidx,
+                                                                                                  vals, dense);
+    count_launch();
+    return check_launch("pattern_scatter");
+}
+
+extern "C" int32_t stmgcn_pattern_gather(int64_t n, const int32_t* rowptr, const int32_t* colidx, int64_t nnz,
+                                         const float* dense, float* dvals, void* stream) {
+    if (int32_t rc = check_pattern_dense("pattern_gather", n, rowptr, colidx, nnz, dense, n * n, dvals, nnz)) return rc;
+    if (nnz == 0) return 0;            // no entry, no gradient: nothing is enqueued
+    pattern_gather_kernel<<<(unsigned)ceil_div(n, kWarps), kWarps * 32, 0, (cudaStream_t)stream>>>(n, rowptr, colidx,
+                                                                                                 dense, dvals);
+    count_launch();
+    return check_launch("pattern_gather");
 }

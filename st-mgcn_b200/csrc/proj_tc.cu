@@ -110,6 +110,7 @@ __device__ __forceinline__ void proj_mma(float (&acc)[N / 2], uint32_t a_hi, uin
         for (int k = 0; k < kKB / 8; ++k) {
             const uint32_t sc = (!first || pass > 0 || k > 0) ? 1u : 0u;
             if constexpr (N == 64) wgmma_tf32_n64(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), sc);
+            else if constexpr (N == 128) wgmma_tf32_n128(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), sc);
             else wgmma_tf32_n256(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), sc);
         }
     }
@@ -349,10 +350,23 @@ __global__ void __launch_bounds__(kPThreads, 1) proj_wgrad_tc_kernel(const __gri
 // projection backward's shape).  Two shared-memory stages: the wgmma of k-block kb run while the loads of kb + 1 are in
 // flight and their split stores fill the other stage.  Persistent over (k, row tile, column tile), column tiles
 // fastest; every output element has one owner and a fixed k order (no split-K, no atomics).
+//
+// Dense chain gradient (the same tile loop with a term loop): out[i][j] = sum_t coef_t sum_f A_t[i][f] . B_t[j][f], the
+// gradient of a dense Chebyshev recurrence matrix X (A_t = G_k, B_t = T_{k-1}, coef 1 for k = 1 and 2 after).  The k
+// blocks of all terms run as one sequence, term-major.  Its products cancel as K1e's do (a dense similarity graph's
+// T_k carry a large diagonal part), so it takes K1e's scheme: the split ROUNDS (tf32_rna) and each k-block's product,
+// accumulated by the tensor cores alone, is added times coef_t into an fp32 register total.  The total doubles the
+// accumulator, so the tile is 128 x 128 (m64n128k8); the next block's loads and split stores run under the current
+// block's wgmma.  round_b16: every B element rounded to bf16 (to nearest even) on load, the operand the bf16 forward
+// multiplied.
 // =====================================================================================================
 constexpr int kDsgN = 256;
 using DsgCfg = PCfg<kDsgN>;
 constexpr size_t kDsgSmem = 1024 + 2 * (size_t)DsgCfg::kStageBytes;
+constexpr int kDcgN = 128;
+using DcgCfg = PCfg<kDcgN>;
+constexpr size_t kDcgSmem = 1024 + 2 * (size_t)DcgCfg::kStageBytes;
+constexpr int kMaxTerms = 8;
 
 struct DsgParams {
     const float* u;          // U_k = u + k * u_stride, (n, f) each
@@ -364,6 +378,20 @@ struct DsgParams {
     int64_t n_tiles;         // ks * n_rt * n_ct
     int nkb;                 // k-blocks: ceil(f / 32)
     bool pair_store;         // n even and da 8-byte aligned: float2 stores
+};
+
+struct DcgParams {
+    const float* a[kMaxTerms];   // A_t (n, f)
+    const float* b[kMaxTerms];   // B_t (n, f)
+    float coef[kMaxTerms];
+    float* out;                  // (n, n), overwritten
+    int64_t n, f;
+    int64_t n_rt, n_ct;          // row tiles of 128, column tiles of 128
+    int64_t n_tiles;             // n_rt * n_ct
+    int nkb;                     // k-blocks per term: ceil(f / 32)
+    int nterms;
+    bool pair_store;             // n even and out 8-byte aligned: float2 stores
+    bool round_b16;
 };
 
 // 4 consecutive f of row `row` of a row-major (n, f) matrix, zeros past its edges
@@ -380,8 +408,28 @@ __device__ __forceinline__ float4 dsg_load(const float* m, int64_t row, int64_t 
     return v;
 }
 
-template <bool VEC>
-__global__ void __launch_bounds__(kPThreads, 1) dense_support_grad_kernel(const __grid_constant__ DsgParams p) {
+// v rounded to bf16 (to nearest even), widened back exactly
+__device__ __forceinline__ float round_bf16(float v) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(0.f), "f"(v));
+    return __uint_as_float(r << 16);
+}
+
+// the rounded split of split_store: hi at st + off, lo at st + kLo + off
+template <uint32_t kLo>
+__device__ __forceinline__ void split_store_rna(uint8_t* st, uint32_t off, const float4& v) {
+    float4 hi, lo;
+    hi.x = tf32_rna(v.x); hi.y = tf32_rna(v.y); hi.z = tf32_rna(v.z); hi.w = tf32_rna(v.w);
+    lo.x = tf32_rna(v.x - hi.x); lo.y = tf32_rna(v.y - hi.y); lo.z = tf32_rna(v.z - hi.z); lo.w = tf32_rna(v.w - hi.w);
+    *reinterpret_cast<float4*>(st + off) = hi;
+    *reinterpret_cast<float4*>(st + kLo + off) = lo;
+}
+
+// the tile loop both kernels run; CHAIN: the chain gradient (DcgParams), else K1d (DsgParams)
+template <bool VEC, bool CHAIN, class P>
+__device__ __forceinline__ void dsg_tiles(const P& p) {
+    constexpr int BN = CHAIN ? kDcgN : kDsgN;
+    using Cfg = PCfg<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* st0 = smem_raw + smem_pad1024(smem_raw);
     const int tid = threadIdx.x;
@@ -389,33 +437,63 @@ __global__ void __launch_bounds__(kPThreads, 1) dense_support_grad_kernel(const 
     const int lane = tid & 31;
     const int wg = tid >> 7;
     const int c = tid & 7, rsub = tid >> 3;                  // float4 column of the k-block, first row
-    constexpr int kNA = kTileM / 32, kNB = kDsgN / 32;       // float4 per thread of the A / B block
-    float acc[kDsgN / 2];
+    constexpr int kNA = kTileM / 32, kNB = BN / 32;          // float4 per thread of the A / B block
+    float acc[BN / 2];
+    float tot[CHAIN ? BN / 2 : 1];
 
     for (int64_t tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
         const int64_t ct = tile % p.n_ct, rest = tile / p.n_ct;
         const int64_t rt = rest % p.n_rt, k = rest / p.n_rt;
-        const float* uk = p.u + k * p.u_stride;
-        const int64_t i0 = rt * kTileM, j0 = ct * kDsgN;
+        const float* uk;
+        const float* xk;
+        if constexpr (CHAIN) {
+            uk = p.a[0];
+            xk = p.b[0];
+        } else {
+            uk = p.u + k * p.u_stride;
+            xk = p.x;
+        }
+        const int64_t i0 = rt * kTileM, j0 = ct * BN;
         float4 va[kNA], vb[kNB];
-        auto load = [&](int kb) {
+        // k-block q: term q / nkb (CHAIN), columns 32 (q % nkb) ..
+        auto load = [&](int q) {
+            const float* ma = uk;
+            const float* mb = xk;
+            int kb = q;
+            if constexpr (CHAIN) {
+                const int t = q / p.nkb;
+                kb = q - t * p.nkb;
+                ma = p.a[t];
+                mb = p.b[t];
+            }
             const int64_t col = (int64_t)kb * kKB + c * 4;
 #pragma unroll
-            for (int i = 0; i < kNA; ++i) va[i] = dsg_load<VEC>(uk, i0 + rsub + 32 * i, col, p.n, p.f);
+            for (int i = 0; i < kNA; ++i) va[i] = dsg_load<VEC>(ma, i0 + rsub + 32 * i, col, p.n, p.f);
 #pragma unroll
-            for (int i = 0; i < kNB; ++i) vb[i] = dsg_load<VEC>(p.x, j0 + rsub + 32 * i, col, p.n, p.f);
+            for (int i = 0; i < kNB; ++i) vb[i] = dsg_load<VEC>(mb, j0 + rsub + 32 * i, col, p.n, p.f);
+            if constexpr (CHAIN) {
+                if (p.round_b16) {
+#pragma unroll
+                    for (int i = 0; i < kNB; ++i)
+                        vb[i] = make_float4(round_bf16(vb[i].x), round_bf16(vb[i].y), round_bf16(vb[i].z), round_bf16(vb[i].w));
+                }
+            }
         };
         auto store = [&](int stage) {
-            uint8_t* st = st0 + (size_t)stage * DsgCfg::kStageBytes;
+            uint8_t* st = st0 + (size_t)stage * Cfg::kStageBytes;
 #pragma unroll
             for (int i = 0; i < kNA; ++i) {
                 const int row = rsub + 32 * i;
-                split_store(st, (uint32_t)row * 128u + (uint32_t)((c ^ (row & 7)) << 4), va[i]);
+                const uint32_t off = (uint32_t)row * 128u + (uint32_t)((c ^ (row & 7)) << 4);
+                if constexpr (CHAIN) split_store_rna<kABytes>(st, off, va[i]);
+                else split_store(st, off, va[i]);
             }
 #pragma unroll
             for (int i = 0; i < kNB; ++i) {
                 const int row = rsub + 32 * i;
-                split_store<DsgCfg::kBBytes>(st + 2 * kABytes, (uint32_t)row * 128u + (uint32_t)((c ^ (row & 7)) << 4), vb[i]);
+                const uint32_t off = (uint32_t)row * 128u + (uint32_t)((c ^ (row & 7)) << 4);
+                if constexpr (CHAIN) split_store_rna<Cfg::kBBytes>(st + 2 * kABytes, off, vb[i]);
+                else split_store<Cfg::kBBytes>(st + 2 * kABytes, off, vb[i]);
             }
         };
         load(0);
@@ -423,36 +501,71 @@ __global__ void __launch_bounds__(kPThreads, 1) dense_support_grad_kernel(const 
         store(0);
         fence_proxy_async_smem();
         __syncthreads();
-        for (int kb = 0; kb < p.nkb; ++kb) {
-            const uint32_t s_u = smem_u32(st0) + (uint32_t)(kb & 1) * (uint32_t)DsgCfg::kStageBytes;
-            const uint32_t a_hi = s_u + (uint32_t)wg * 64u * 128u, a_lo = a_hi + kABytes;
-            const uint32_t b_hi = s_u + 2 * kABytes, b_lo = b_hi + DsgCfg::kBBytes;
+        if constexpr (!CHAIN) {
+            for (int kb = 0; kb < p.nkb; ++kb) {
+                const uint32_t s_u = smem_u32(st0) + (uint32_t)(kb & 1) * (uint32_t)Cfg::kStageBytes;
+                const uint32_t a_hi = s_u + (uint32_t)wg * 64u * 128u, a_lo = a_hi + kABytes;
+                const uint32_t b_hi = s_u + 2 * kABytes, b_lo = b_hi + Cfg::kBBytes;
+                wg_fence_regs(acc);
+                wg_fence();
+                proj_mma<BN>(acc, a_hi, a_lo, b_hi, b_lo, kb == 0);
+                wg_commit();
+                if (kb + 1 < p.nkb) {
+                    load(kb + 1);
+                    wg_wait<1>();                            // this warpgroup's MMAs of k-block kb - 1 are done
+                    __syncthreads();                         // ... and the other's: their stage may be overwritten
+                    store((kb + 1) & 1);
+                    fence_proxy_async_smem();
+                    __syncthreads();
+                }
+            }
+            wg_wait<0>();
             wg_fence_regs(acc);
-            wg_fence();
-            proj_mma<kDsgN>(acc, a_hi, a_lo, b_hi, b_lo, kb == 0);
-            wg_commit();
-            if (kb + 1 < p.nkb) {
-                load(kb + 1);
-                wg_wait<1>();                                // this warpgroup's MMAs of k-block kb - 1 are done
-                __syncthreads();                             // ... and the other's: their stage may be overwritten
-                store((kb + 1) & 1);
-                fence_proxy_async_smem();
-                __syncthreads();
+        } else {
+            const int nq = p.nterms * p.nkb;
+            for (int q = 0; q < nq; ++q) {
+                const uint32_t s_u = smem_u32(st0) + (uint32_t)(q & 1) * (uint32_t)Cfg::kStageBytes;
+                const uint32_t a_hi = s_u + (uint32_t)wg * 64u * 128u, a_lo = a_hi + kABytes;
+                const uint32_t b_hi = s_u + 2 * kABytes, b_lo = b_hi + Cfg::kBBytes;
+                wg_fence_regs(acc);
+                wg_fence();
+                proj_mma<BN>(acc, a_hi, a_lo, b_hi, b_lo, true);
+                wg_commit();
+                if (q + 1 < nq) {
+                    // under this block's MMAs: the next block's loads and split stores into the other stage, whose last
+                    // reader, block q - 1's MMAs, both warpgroups waited for before the barrier that ended that iteration
+                    load(q + 1);
+                    store((q + 1) & 1);
+                    fence_proxy_async_smem();
+                }
+                wg_wait<0>();
+                wg_fence_regs(acc);
+                const float cf = p.coef[q / p.nkb];
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) tot[i] = q == 0 ? cf * acc[i] : tot[i] + cf * acc[i];
+                if (q + 1 < nq) __syncthreads();             // both stages' writes and reads of this block are done
             }
         }
-        wg_wait<0>();
-        wg_fence_regs(acc);
-        // ===================== accumulator fragment -> da[k] =====================
-        float* dak = p.da + k * p.n * p.n;
+        // ===================== accumulator fragment -> da[k] / out =====================
+        float* dak;
+        if constexpr (CHAIN) dak = p.out;
+        else dak = p.da + k * p.n * p.n;
         const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int64_t i = i0 + r0 + 8 * h;
             if (i >= p.n) continue;
 #pragma unroll
-            for (int j = 0; j < kDsgN / 8; ++j) {
+            for (int j = 0; j < BN / 8; ++j) {
                 const int64_t col = j0 + 8 * j + c0;
-                const float lo = acc[4 * j + 2 * h], hi = acc[4 * j + 2 * h + 1];
+                float lo, hi;
+                if constexpr (CHAIN) {
+                    lo = tot[4 * j + 2 * h];
+                    hi = tot[4 * j + 2 * h + 1];
+                } else {
+                    lo = acc[4 * j + 2 * h];
+                    hi = acc[4 * j + 2 * h + 1];
+                }
                 if (p.pair_store) {
                     if (col < p.n) *reinterpret_cast<float2*>(dak + i * p.n + col) = make_float2(lo, hi);
                 } else {
@@ -462,6 +575,16 @@ __global__ void __launch_bounds__(kPThreads, 1) dense_support_grad_kernel(const 
             }
         }
     }
+}
+
+template <bool VEC>
+__global__ void __launch_bounds__(kPThreads, 1) dense_support_grad_kernel(const __grid_constant__ DsgParams p) {
+    dsg_tiles<VEC, false>(p);
+}
+
+template <bool VEC>
+__global__ void __launch_bounds__(kPThreads, 1) dense_chain_grad_kernel(const __grid_constant__ DcgParams p) {
+    dsg_tiles<VEC, true>(p);
 }
 
 int32_t launch_pack_image(const float* src, int n_rows, int k_cols, int64_t rs, int64_t cs, float* img, int tile_rows,
@@ -604,4 +727,45 @@ extern "C" int32_t stmgcn_dense_support_grad(int64_t n, int64_t f_total, int32_t
     kern<<<persistent_grid(p.n_tiles), kPThreads, kDsgSmem, (cudaStream_t)stream>>>(p);
     count_launch();
     return check_launch("dense_support_grad");
+}
+
+extern "C" int32_t stmgcn_dense_chain_grad(int64_t n, int64_t f_total, int32_t nterms, const float* const* a,
+                                           const float* const* b, const float* coef, int32_t round_b16, float* out,
+                                           void* stream) {
+    STMGCN_REQUIRE(nterms >= 1 && nterms <= kMaxTerms, STMGCN_ERR_SHAPE, "dense_chain_grad: nterms=%d (1..%d)", nterms,
+                   kMaxTerms);
+    STMGCN_REQUIRE(a && b && coef && out, STMGCN_ERR_ARG, "dense_chain_grad: null pointer");
+    STMGCN_REQUIRE(round_b16 == 0 || round_b16 == 1, STMGCN_ERR_ARG, "dense_chain_grad: round_b16=%d (0 or 1)", round_b16);
+    STMGCN_REQUIRE(n >= 1 && n < (1 << 24), STMGCN_ERR_SHAPE, "dense_chain_grad: n=%lld must be in [1, 2^24)", (long long)n);
+    STMGCN_REQUIRE(f_total >= 1 && f_total < ((int64_t)1 << 31) && n * f_total < ((int64_t)1 << 48), STMGCN_ERR_SHAPE,
+                   "dense_chain_grad: f_total=%lld must be in [1, 2^31) with n * f_total below 2^48", (long long)f_total);
+    const int64_t op_bytes = n * f_total * 4, out_bytes = n * n * 4;
+    bool vec = f_total % 4 == 0;
+    for (int t = 0; t < nterms; ++t) {
+        STMGCN_REQUIRE(a[t] && b[t], STMGCN_ERR_ARG, "dense_chain_grad: null A / B of term %d", t);
+        STMGCN_REQUIRE(!overlaps(out, out_bytes, a[t], op_bytes) && !overlaps(out, out_bytes, b[t], op_bytes),
+                       STMGCN_ERR_ARG, "dense_chain_grad: out must not overlap A / B of term %d", t);
+        vec = vec && aligned16(a[t]) && aligned16(b[t]);
+    }
+    DcgParams p;
+    for (int t = 0; t < kMaxTerms; ++t) {
+        p.a[t] = t < nterms ? a[t] : nullptr;
+        p.b[t] = t < nterms ? b[t] : nullptr;
+        p.coef[t] = t < nterms ? coef[t] : 0.f;
+    }
+    p.out = out;
+    p.n = n;
+    p.f = f_total;
+    p.n_rt = ceil_div(n, kTileM);
+    p.n_ct = ceil_div(n, kDcgN);
+    p.n_tiles = p.n_rt * p.n_ct;
+    p.nkb = (int)ceil_div(f_total, kKB);
+    p.nterms = nterms;
+    p.pair_store = n % 2 == 0 && (reinterpret_cast<uintptr_t>(out) & 7u) == 0;
+    p.round_b16 = round_b16 != 0;
+    auto kern = vec ? dense_chain_grad_kernel<true> : dense_chain_grad_kernel<false>;
+    if (int32_t rc = ensure_dyn_smem((const void*)kern, kDcgSmem)) return rc;
+    kern<<<persistent_grid(p.n_tiles), kPThreads, kDcgSmem, (cudaStream_t)stream>>>(p);
+    count_launch();
+    return check_launch("dense_chain_grad");
 }

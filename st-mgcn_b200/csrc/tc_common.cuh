@@ -30,6 +30,13 @@ __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__flo
 __device__ __forceinline__ float tf32_lo(float v, float hi) {
     return __uint_as_float(__float_as_uint(v - hi) & 0xffffe000u);
 }
+// v rounded to the nearest tf32 value (ties away from zero), exact in tf32: the rounded split hi = rna(v),
+// lo = rna(v - hi) of the kernels whose products cancel (K1e, the chain gradient), |v - hi - lo| <= 2^-24 |v|
+__device__ __forceinline__ float tf32_rna(float v) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+    return __uint_as_float(r);
+}
 
 // ---- mbarrier -----------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

@@ -29,6 +29,8 @@ SIGNATURES = [
     ("stmgcn_csr_sddmm", c_int32, [c_int64, _P, _P, c_int64, c_int32, POINTER(c_void_p), POINTER(c_void_p),
                                    POINTER(c_float), c_int32, c_int64, _P, c_int64, _P, _P]),
     ("stmgcn_dense_support_grad", c_int32, [c_int64, c_int64, c_int32, _P, c_int64, _P, _P, _P]),
+    ("stmgcn_dense_chain_grad", c_int32, [c_int64, c_int64, c_int32, POINTER(c_void_p), POINTER(c_void_p),
+                                          POINTER(c_float), c_int32, _P, _P]),
     ("stmgcn_dense_mm_step", c_int32, [c_int64, _P, c_int64, c_int32, c_float, _P, c_float, _P, c_float, _P, _P, c_int64,
                                        _P]),
     ("stmgcn_dense_mm_step16", c_int32, [c_int64, _P, c_int64, c_int32, c_float, _P, c_float, _P, c_float, _P, _P, _P,
@@ -37,6 +39,8 @@ SIGNATURES = [
                                       c_int64, _P, _P, _P]),
     ("stmgcn_adj_norm_bwd", c_int32, [c_int32, c_int64, _P, _P, _P, _P, _P, c_int64, _P, _P, c_int64, c_float, _P, _P,
                                       _P, c_int64, _P, _P]),
+    ("stmgcn_pattern_scatter", c_int32, [c_int64, _P, _P, c_int64, _P, _P, _P]),
+    ("stmgcn_pattern_gather", c_int32, [c_int64, _P, _P, c_int64, _P, _P, _P]),
     ("stmgcn_window_gather", c_int32, [_P, c_int64, c_int64, POINTER(c_int32), c_int32, c_int64, c_int64, _P, _P, _P]),
     ("stmgcn_obs_to_node_major", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),
     ("stmgcn_obs_grad", c_int32, [_P, _P, _P, c_int64, c_int64, c_int64, c_int64, _P]),

@@ -124,13 +124,19 @@ class DenseGraph:
     the tensor cores (``ops.spmm_step`` dispatches on the handle type; stmgcn_dense_mm_step), as the reference's einsum.
 
     ``mat`` is an fp32 contiguous snapshot (a copy of what it was built from), so the forward and the backward of a step
-    multiply by one matrix and an edit of the source after the build reaches neither.  ``nnz`` is the number of stored
-    entries, ``n * n``."""
+    multiply by one matrix and an edit of the source after the build reaches neither.  ``copy=False`` holds ``mat``
+    itself (detached), for a caller that builds a fresh fp32 contiguous matrix at every forward and never edits it: a
+    :class:`LearnableAdjacency` multiplied dense, whose matrix is the output of its scatter.  ``nnz`` is the number of
+    stored entries, ``n * n``."""
 
-    def __init__(self, mat: torch.Tensor):
+    def __init__(self, mat: torch.Tensor, copy: bool = True):
         assert mat.dim() == 2 and mat.shape[0] == mat.shape[1]
         self.n, self.nnz, self.device = mat.shape[0], mat.shape[0] * mat.shape[0], mat.device
-        self.mat = mat.detach().to(torch.float32, copy=True).contiguous()
+        if copy:
+            self.mat = mat.detach().to(torch.float32, copy=True).contiguous()
+        else:
+            assert mat.dtype == torch.float32 and mat.is_contiguous()
+            self.mat = mat.detach()
 
 
 # When a dense support matrix is multiplied dense (DenseGraph) instead of gathered from CSR (GraphHandle): from this
@@ -153,9 +159,12 @@ class SupportSet:
     segments ``1 + cK .. (c+1)K``, ``T_k(X_c)`` with ``K = (Ks - 1) / len(graphs)`` (no graph when ``Ks == 1``).
     ``"generic"``: ``graphs[k]`` is ``A_k``.  A graph is a :class:`GraphHandle` (CSR) or a :class:`DenseGraph`.
 
-    ``values`` (optional): the source tensors of the graphs' stored values, one per graph in CSR entry order, when some
-    of them require grad (a learnable :class:`SparseSupports`).  The graphs hold detached copies; the graph
-    convolutions take these tensors as inputs, so their gradients reach them.
+    ``values`` (optional): the source tensors of the graphs' stored values, one per graph, when some of them require
+    grad: in CSR entry order for a CSR graph (a learnable :class:`SparseSupports`), the ``(N, N)`` matrix itself for a
+    :class:`DenseGraph` (a :class:`LearnableAdjacency` multiplied dense).  The graphs hold detached copies (a dense
+    matrix: the same storage, built fresh at each forward); the graph convolutions take these tensors as inputs, so their
+    gradients reach them -- the SDDMM's at the stored entries, or the whole matrix's (``ops.dense_chain_grad``, or
+    ``ops.dense_support_grad`` for a generic slice).
 
     ``dense`` (optional): the dense ``(Ks, N, N)`` stack the set was converted from, when it requires grad.  The graphs
     hold a snapshot of its slices; the graph convolutions take the stack as their one extra input and give it
@@ -418,6 +427,15 @@ class LearnableAdjacency(nn.Module):
     (``ops.AdjNorm``: no host synchronisation, fixed-order sums), so a step that learns the graph can be captured
     (``GraphedStep``) and its edge weights reduced with the model's gradients (``GradBucket(model, adjacency)``).
 
+    Each forward hands the kernels the supports' matrices as CSR, or dense when ``ops.dense_supports()`` says so for the
+    pattern (``"auto"``: :func:`dense_rule` on ``N`` and the pattern's entry count, known without a host sync; ``"on"``:
+    always; ``"off"``: never).  Dense, the normalised values are scattered into fresh ``(N, N)`` matrices
+    (``ops.PatternToDense``) that the graph convolutions multiply on the tensor cores and differentiate whole
+    (``ops.dense_chain_grad``); the matrices' gradients are read back at the pattern's entries into ``AdjNorm``'s
+    backward.  No ``N^3`` product and no polynomial stack is formed, and the forward still never synchronises.
+    Non-finite values: a dense product forms ``0 * x`` for every entry off the pattern too, as the reference's dense
+    einsum, so a NaN or Inf in the features reaches every output row (CSR: only rows with an entry in its column).
+
     Built by ``Adj_Preprocessor.process_learnable``.  The pattern -- the stored entries plus a diagonal slot in every row
     that lacks one when the kind has a diagonal term (``localpool``; ``chebyshev`` with ``2 / lambda_max != 1``) -- is
     built once, as CSR and CSR^T on the module's buffers; ``lambda_max`` is a constant.  Stands in for the support stack
@@ -529,12 +547,28 @@ class LearnableAdjacency(nn.Module):
         vals = ops.AdjNorm.apply(self.weight, self.kind, self.scale, *self.pattern())
         return list(vals) if isinstance(vals, tuple) else [vals]
 
+    def dense(self) -> bool:
+        """Whether the forward multiplies the supports' matrices dense under the current ``ops.dense_supports()`` mode
+        (``"auto"``: :func:`dense_rule` on the pattern's entry count)."""
+        from . import ops
+        mode = ops.dense_supports()
+        return mode == "on" or (mode == "auto" and dense_rule(self.n, self.colidx.numel()))
+
     def forward(self) -> SupportSet:
         """The kernels' support set at the current weights: one normalisation launch pair, then the values copied into
-        the cached structure (:meth:`SparseSupports.support_set_with`)."""
+        the cached structure (:meth:`SparseSupports.support_set_with`), or, multiplied dense (:meth:`dense`), scattered
+        into one fresh ``(N, N)`` matrix per chain (or slice): a set of :class:`DenseGraph`s whose ``values`` are those
+        matrices."""
         if not self.is_cuda:
             raise RuntimeError("LearnableAdjacency must be moved to a CUDA device before use (.to(device))")
-        return self._supports_handle().support_set_with(self._values())
+        handle = self._supports_handle()
+        if not self.dense():
+            return handle.support_set_with(self._values())
+        from . import ops
+        mats = handle.mats if handle.mode == "generic" or handle.ks > 1 else []
+        dense = [ops.PatternToDense.apply(v, rp, ci) for (rp, ci, _), v in zip(mats, self._values())]
+        return SupportSet(handle.mode, self.n, self.ks, [DenseGraph(d, copy=False) for d in dense], self.device,
+                          values=dense)
 
     def supports(self) -> SparseSupports:
         """The supports at the current weights as a fixed handle (detached copies of the values): what

@@ -12,6 +12,7 @@ Functions (reference lines they replace):
   SharedLSTM       STMGCN.py:44,47-50: modulate + 3-layer shared LSTM (lstm16.cu / lstm.cu: one call each way)
   FuseOut          STMGCN.py:116-118: sum over graphs + output FC -> (B,N,C)
   AdjNorm          GCN.py:99-111 on a fixed pattern: a learnable adjacency's weights -> its supports' stored values
+  PatternToDense   a learnable adjacency's stored values -> the dense matrix they form, when it is multiplied dense
 """
 from __future__ import annotations
 
@@ -281,26 +282,45 @@ def csr_sddmm_(g, terms, dvals: torch.Tensor, round_b16: bool = False) -> None:
 
 def support_value_grads(sset: SupportSet, s: torch.Tensor, u: torch.Tensor, x: Optional[torch.Tensor],
                         round_b16: bool, need: Sequence[bool]) -> List[Optional[torch.Tensor]]:
-    """The gradient of each graph's stored values (CSR entry order), None where ``need`` is False.  ``u`` after
-    :func:`adjoint_stack_`; ``s`` the forward stack; ``x`` the input (generic supports only).
+    """The gradient of each graph's stored values, None where ``need`` is False: CSR entry order for a CSR handle, the
+    whole ``(N, N)`` matrix for a :class:`DenseGraph`.  ``u`` after :func:`adjoint_stack_`; ``s`` the forward stack;
+    ``x`` the input (generic supports only).
 
-    cheb, chain X with terms T_0 .. T_K:  d vals[e] = sum_k c_k <G_k[i], T_{k-1}[j]>, c_1 = 1, c_k = 2 (k >= 2), one
-    SDDMM launch per chain over its own segments (``round_b16``: the bf16 copies the forward gathered from);
-    generic S_k = A_k x:  d vals_k[e] = <U_k[i], x[j]>."""
+    cheb, chain X with terms T_0 .. T_K:  dX = sum_k c_k G_k T_{k-1}^T, c_1 = 1, c_k = 2 (k >= 2): at the stored entries,
+    one SDDMM launch per chain over its own segments, or everywhere, one :func:`dense_chain_grad` launch (``round_b16``:
+    the bf16 copies the forward multiplied); generic S_k = A_k x:  dA_k = U_k x^T, at the stored entries or everywhere
+    (:func:`dense_support_grad`)."""
     grads: List[Optional[torch.Tensor]] = []
     for c, g in enumerate(sset.graphs):
         if not need[c]:
             grads.append(None)
             continue
-        dv = torch.zeros(g.nnz, device=u.device, dtype=torch.float32)
         if sset.mode == "cheb":
             seg = sset.chain_segments(c)
             terms = [(u[seg[k]], s[seg[k - 1]], 1.0 if k == 1 else 2.0) for k in range(1, len(seg))]
-            csr_sddmm_(g, terms, dv, round_b16)
         else:
-            csr_sddmm_(g, [(u[c], x, 1.0)], dv)
+            terms = [(u[c], x, 1.0)]
+        if isinstance(g, DenseGraph):
+            grads.append(dense_chain_grad(terms, round_b16) if sset.mode == "cheb"
+                         else dense_support_grad(u[c:c + 1], x)[0])
+            continue
+        dv = torch.zeros(g.nnz, device=u.device, dtype=torch.float32)
+        csr_sddmm_(g, terms, dv, round_b16 and sset.mode == "cheb")
         grads.append(dv)
     return grads
+
+
+def dense_chain_grad(terms, round_b16: bool = False) -> torch.Tensor:
+    """``sum_t coef_t A_t B_t^T`` (stmgcn_dense_chain_grad), the ``(N, N)`` gradient of a dense recurrence matrix;
+    ``terms``: (A_t, B_t, coef_t) with A_t, B_t (N, ...) fp32 contiguous.  ``round_b16``: B rounded to bf16."""
+    n = terms[0][0].shape[0]
+    out = torch.empty((n, n), device=terms[0][0].device, dtype=torch.float32)
+    a = _lib.ptr_array([t[0].data_ptr() for t in terms])
+    b = _lib.ptr_array([t[1].data_ptr() for t in terms])
+    coef = _lib.float_array([float(t[2]) for t in terms])
+    _lib.check(L.stmgcn_dense_chain_grad(n, terms[0][0].numel() // n, len(terms), a, b, coef, int(round_b16),
+                                         out.data_ptr(), _stream()), "dense_chain_grad")
+    return out
 
 
 def dense_support_grad(u: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
@@ -377,6 +397,40 @@ class AdjNorm(torch.autograd.Function):
         _lib.check(L.stmgcn_adj_norm_bwd(*_norm_args(ctx.kind, pattern, w, ctx.scale), g.data_ptr(), _p(g_t),
                                          work.data_ptr(), work.numel(), dw.data_ptr(), _stream()), "adj_norm_bwd")
         return (dw, None, None) + (None,) * len(pattern)
+
+
+def pattern_scatter(vals: torch.Tensor, rowptr: torch.Tensor, colidx: torch.Tensor) -> torch.Tensor:
+    """The ``(N, N)`` matrix of a CSR pattern's values (stmgcn_pattern_scatter): zeros off the pattern, repeated entries
+    added in entry order; ``vals`` fp32 contiguous in the order of ``(rowptr, colidx)``."""
+    n = rowptr.numel() - 1
+    dense = torch.empty((n, n), device=vals.device, dtype=torch.float32)
+    _lib.check(L.stmgcn_pattern_scatter(n, rowptr.data_ptr(), colidx.data_ptr(), colidx.numel(), vals.data_ptr(),
+                                        dense.data_ptr(), _stream()), "pattern_scatter")
+    return dense
+
+
+def pattern_gather(dense: torch.Tensor, rowptr: torch.Tensor, colidx: torch.Tensor) -> torch.Tensor:
+    """``dense[i, j]`` at every entry ``(i, j)`` of a CSR pattern, in its order (stmgcn_pattern_gather)."""
+    dv = torch.empty(colidx.numel(), device=dense.device, dtype=torch.float32)
+    _lib.check(L.stmgcn_pattern_gather(rowptr.numel() - 1, rowptr.data_ptr(), colidx.data_ptr(), colidx.numel(),
+                                       dense.data_ptr(), dv.data_ptr(), _stream()), "pattern_gather")
+    return dv
+
+
+class PatternToDense(torch.autograd.Function):
+    """The ``(N, N)`` matrix a pattern's stored values form (:func:`pattern_scatter`): ``vals`` in the order of the CSR
+    ``(rowptr, colidx)``.  Backward: the matrix's gradient read back at the entries (:func:`pattern_gather`).  A fresh
+    matrix at every call; no host synchronisation."""
+
+    @staticmethod
+    def forward(ctx, vals, rowptr, colidx):
+        _require_cuda(vals, rowptr)
+        ctx.pattern = (rowptr, colidx)
+        return pattern_scatter(_f32c(vals.detach()), rowptr, colidx)
+
+    @staticmethod
+    def backward(ctx, d_dense):
+        return pattern_gather(_f32c(d_dense), *ctx.pattern), None, None
 
 
 def _proj_images(w: torch.Tensor, ks: int, p: int, need_bwd: bool):
